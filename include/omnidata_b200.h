@@ -289,6 +289,14 @@ int odb_upsample2x_bwd(const void* dout, void* dz, int32_t b, int32_t h, int32_t
  * masked by the ReLU; the pooling gradient goes to the first maximum of each window (torch semantics). */
 int odb_stem_pool_bwd(const void* dt, const void* s0, const float* stats, const float* gamma, const float* beta, void* g_s0,
                       int32_t b, int32_t h, int32_t w, int32_t c, int32_t groups, int32_t dtype, void* stream);
+/* Gradient w.r.t. the network's input image: replaces autograd's input gradient of the hybrid stem's timm
+ * StdConv2dSame(3, 64, 7, stride 2) (TF-SAME padding (2, 3)).  ds0 `dtype` [b][h/2][w/2][64] = gradient w.r.t. the
+ * convolution's output, weight `dtype` [64][kpad] = the packed, standardised operand the forward used (column
+ * (ky*7+kx)*3+ch, odb_stem_im2col's order) -> dx fp32 NCHW [b][3][h][w], written (not accumulated).  Gather form with a
+ * fixed summation order: bit-reproducible and independent of the batch.  h, w even; kpad a multiple of 8 in
+ * [152, 1024]; ds0 16-byte and dx 8-byte aligned. */
+int odb_stem_input_grad(const void* ds0, const void* weight, float* dx, int32_t b, int32_t h, int32_t w, int32_t kpad,
+                        int32_t dtype, void* stream);
 /* DPT head tail, unfused (training): out[b][k][y][x] = relu?(bias[k] + sum_j w[k][j] a[b][y][x][j]), a has
  * channel_stride channels per pixel of which the first 32 are used; and its backward (da zero in the padding channels). */
 int odb_head_tail_fwd(const void* a, int32_t channel_stride, const float* w, const float* bias, float* out, int32_t b,

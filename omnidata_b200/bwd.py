@@ -116,6 +116,22 @@ def stem_pool_bwd(dt, s0, stats, gamma, beta, g_s0, groups: int = 32):
           s0.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), g_s0.data_ptr(), b, h, w, c, groups, _dt(s0))
 
 
+def stem_input_grad(ds0, w, dx):
+    """dx fp32 [B,3,H,W] = gradient w.r.t. the image of the 7x7 stride-2 TF-SAME stem convolution, from ds0 [B,H/2,W/2,64]
+    (gradient w.r.t. its output) and w [64, kpad] (the packed operand the forward used, same dtype as ds0)."""
+    _need(dx, torch.float32, "dx")
+    if ds0.dim() != 4 or ds0.shape[-1] != 64 or not ds0.is_contiguous():
+        raise _capi.OdbError("stem_input_grad: ds0 must be a contiguous [B,H/2,W/2,64] tensor")
+    if w.dim() != 2 or w.shape[0] != 64 or w.dtype != ds0.dtype or not w.is_contiguous():
+        raise _capi.OdbError("stem_input_grad: w must be a contiguous [64, kpad] tensor of ds0's dtype")
+    b, h2, w2, _ = ds0.shape
+    if tuple(dx.shape) != (b, 3, 2 * h2, 2 * w2) or not dx.is_contiguous():
+        raise _capi.OdbError(f"stem_input_grad: dx must be a contiguous [{b},3,{2 * h2},{2 * w2}] tensor")
+    info = {"flops": 2.0 * b * h2 * w2 * 64 * 147, "bytes": ds0.numel() * ds0.element_size() + dx.numel() * 4}
+    _call("odb_stem_input_grad", info, lib().odb_stem_input_grad, _same_device(ds0, w, dx), ds0.data_ptr(), w.data_ptr(),
+          dx.data_ptr(), b, 2 * h2, 2 * w2, w.shape[1], _dt(ds0))
+
+
 def head_tail_fwd(a, w, bias, out, relu: bool):
     b, h, wd, cs = a.shape
     _call("odb_head_tail_fwd", {}, lib().odb_head_tail_fwd, _same_device(a, w, bias, out), a.data_ptr(), cs, w.data_ptr(),
@@ -239,5 +255,5 @@ def attention_bwd(qkv, o, d_o, lse, dqkv, heads: int = 12, scale: float = 0.125)
 
 
 __all__ = ["mask_add", "gelu_fwd", "gelu_bwd", "colsum", "layernorm_bwd", "groupnorm_bwd", "upsample2x_bwd", "stem_pool_bwd",
-           "head_tail_fwd", "head_tail_bwd", "add_cast", "pack_weight", "unpack_wgrad", "conv_wgrad", "attention_bwd",
+           "stem_input_grad", "head_tail_fwd", "head_tail_bwd", "add_cast", "pack_weight", "unpack_wgrad", "conv_wgrad", "attention_bwd",
            "TAPS_1", "TAPS_3X3"]

@@ -555,6 +555,106 @@ __global__ void __launch_bounds__(256) stem_pool_bwd_kernel(const T* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------------------ stem input gradient
+// Gradient of the 7x7 stride-2 TF-SAME stem convolution (timm StdConv2dSame(3, 64, 7, stride 2), padding (2, 3)) w.r.t.
+// its fp32 NCHW input, from ds0 = the gradient w.r.t. its output [b][h/2][w/2][64] and the packed operand the forward
+// used, w [64][kpad] (column (ky*7+kx)*3+c, already standardised):
+//   dx[b][c][y][x] = sum over ky = y mod 2, kx = x mod 2, o < 64 of  w[o][(ky*7+kx)*3+c] * ds0[b][(y+2-ky)/2][(x+2-kx)/2][o]
+// restricted to ds0 pixels inside the image.  Gather form: input quad (P, Q) = pixels (2P+py, 2Q+px) reads the 4 x 4
+// ds0 pixels (P+1-i, Q+1-j), i, j < 4, through taps ky = 2i+py, kx = 2j+px (those <= 6).  Every dx element is written
+// once by one thread, summed in a fixed order (o, then j, then i): bit-reproducible and independent of the batch.
+// Block = 8 warps over a 16 x 32 quad tile, persistent over tiles; thread = two vertically adjacent quads (their 4 x 4
+// windows share 3 rows, so 20 ds0 loads and 48 weight loads feed 294 FMAs per channel).  Shared memory: the weights
+// re-laid as ws[o][i][j][py][px][c] fp32 (zero where a tap exceeds 6), staged once per block and read as warp-uniform
+// float4 broadcasts; one 16-channel chunk of the ds0 tile + halo as fp32 planes [ch][19][35], where the lanes of a
+// warp read consecutive columns of one row (no bank conflicts).
+constexpr int kSigQH = 16, kSigQW = 32, kSigKC = 16;          // quad rows / quad columns per tile, channels per chunk
+constexpr int kSigRows = kSigQH + 3, kSigCols = kSigQW + 3, kSigPlane = kSigRows * kSigCols;
+constexpr int kSigWFloats = 64 * 16 * 12;
+constexpr size_t kSigSmemBytes = (size_t)(kSigWFloats + kSigKC * kSigPlane) * sizeof(float);
+template <typename T>
+__global__ void __launch_bounds__(256, 2) stem_input_grad_kernel(const T* __restrict__ ds0, const T* __restrict__ w,
+                                                                 float* __restrict__ dx, int b, int h, int wd, int kpad) {
+  grid_dep_wait();
+  grid_dep_launch();
+  extern __shared__ float4 sig_smem[];
+  float* ws = reinterpret_cast<float*>(sig_smem);
+  float* st = ws + kSigWFloats;
+  for (int e = threadIdx.x; e < kSigWFloats; e += blockDim.x) {
+    const int c = e % 3, px = (e / 3) & 1, py = (e / 6) & 1, j = (e / 12) & 3, i = (e / 48) & 3, o = e / 192;
+    const int ky = 2 * i + py, kx = 2 * j + px;
+    ws[e] = (ky < 7 && kx < 7) ? ldf(w + (long long)o * kpad + (ky * 7 + kx) * 3 + c) : 0.f;
+  }
+  const int h2 = h / 2, w2 = wd / 2;
+  const int tiles_y = (h2 + kSigQH - 1) / kSigQH, tiles_x = (w2 + kSigQW - 1) / kSigQW;
+  const long long tiles = (long long)b * tiles_y * tiles_x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int tx = (int)(tile % tiles_x), ty = (int)((tile / tiles_x) % tiles_y);
+    const int bi = (int)(tile / ((long long)tiles_x * tiles_y));
+    const int P0 = ty * kSigQH, Q0 = tx * kSigQW;
+    const T* db = ds0 + (long long)bi * h2 * w2 * 64;
+    float acc[2][2][2][3];                                      // [quad][py][px][c]
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+      for (int k = 0; k < 12; ++k) (&acc[q][0][0][0])[k] = 0.f;
+    for (int o0 = 0; o0 < 64; o0 += kSigKC) {
+      __syncthreads();               // the previous chunk's readers (the first time: the weight staging) are done
+      // ds0 pixels (P0 - 2 + r, Q0 - 2 + col), zero outside the image; thread item = (pixel, 8 channels)
+      for (int e = threadIdx.x; e < kSigPlane * (kSigKC / 8); e += blockDim.x) {
+        const int g = e % (kSigKC / 8), pix = e / (kSigKC / 8);
+        const int r = pix / kSigCols, col = pix - r * kSigCols;
+        const int oy = P0 - 2 + r, ox = Q0 - 2 + col;
+        float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        if (oy >= 0 && oy < h2 && ox >= 0 && ox < w2) ld8(db + ((long long)oy * w2 + ox) * 64 + o0 + g * 8, v);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) st[(g * 8 + k) * kSigPlane + pix] = v[k];
+      }
+      __syncthreads();
+      for (int oc = 0; oc < kSigKC; ++oc) {
+        // rows 2*warp .. 2*warp+4 of the tile: quad q, window index i reads row 2*warp + q + 3 - i
+        const float* so = st + oc * kSigPlane + 2 * warp * kSigCols + lane + 3;
+        const float4* wo = reinterpret_cast<const float4*>(ws + (o0 + oc) * 192);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float v[5];
+#pragma unroll
+          for (int r = 0; r < 5; ++r) v[r] = so[r * kSigCols - j];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float4 wa = wo[(i * 4 + j) * 3], wb = wo[(i * 4 + j) * 3 + 1], wc = wo[(i * 4 + j) * 3 + 2];
+            const float wk[12] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w, wc.x, wc.y, wc.z, wc.w};
+#pragma unroll
+            for (int q = 0; q < 2; ++q)
+#pragma unroll
+              for (int py = 0; py < 2; ++py)
+#pragma unroll
+                for (int px = 0; px < 2; ++px) {
+                  if (2 * i + py > 6 || 2 * j + px > 6) continue;
+#pragma unroll
+                  for (int c = 0; c < 3; ++c)
+                    acc[q][py][px][c] = fmaf(wk[(py * 2 + px) * 3 + c], v[q + 3 - i], acc[q][py][px][c]);
+                }
+          }
+        }
+      }
+    }
+    const int Q = Q0 + lane;
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int P = P0 + 2 * warp + q;
+      if (P >= h2 || Q >= w2) continue;
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+#pragma unroll
+        for (int py = 0; py < 2; ++py)
+          *reinterpret_cast<float2*>(dx + (((long long)bi * 3 + c) * h + 2 * P + py) * wd + 2 * Q) =
+              make_float2(acc[q][py][0][c], acc[q][py][1][c]);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------ head tail (1x1 conv + ReLUs)
 // forward (training, unfused): out[b][k][p] = relu?(bias[k] + sum_j w[k][j] a[b][p][j]); a has `cs` channels per pixel
 // of which the first 32 are real (the 128 -> 32 conv is carried zero-padded to 64 output channels).
@@ -1143,6 +1243,40 @@ extern "C" int odb_stem_pool_bwd(const void* dt, const void* s0, const float* st
              static_cast<const T*>(dt), static_cast<const T*>(s0), stats, gamma, beta, static_cast<T*>(g_s0), h, w, c, groups));
   count_launch();
   return check_launch("stem_pool_bwd");
+}
+
+template <typename T>
+static int stem_input_grad_launch(const void* ds0, const void* w, float* dx, int b, int h, int wd, int kpad,
+                                  unsigned grid, cudaStream_t stream) {
+  static bool configured[kMaxDevices] = {};
+  const int dev_ = current_device();
+  if (!configured[dev_]) {
+    cudaError_t e = cudaFuncSetAttribute(stem_input_grad_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)kSigSmemBytes);
+    if (e != cudaSuccess) return fail_cuda(e, "stem_input_grad: cudaFuncSetAttribute");
+    configured[dev_] = true;
+  }
+  launch_pdl(stem_input_grad_kernel<T>, dim3(grid), dim3(256), kSigSmemBytes, stream, static_cast<const T*>(ds0),
+             static_cast<const T*>(w), dx, b, h, wd, kpad);
+  return ODB_OK;
+}
+
+extern "C" int odb_stem_input_grad(const void* ds0, const void* weight, float* dx, int32_t b, int32_t h, int32_t w,
+                                   int32_t kpad, int32_t dtype, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!ds0 || !weight || !dx || b < 1 || h < 2 || w < 2 || (h & 1) || (w & 1) || kpad < 152 || kpad % 8 || kpad > 1024 ||
+      !aligned16(ds0) || (reinterpret_cast<uintptr_t>(dx) & 7u))
+    return fail(ODB_ERR_INVALID, "stem_input_grad: bad argument (even h, w; kpad a multiple of 8 in [152, 1024]; "
+                                 "16-byte aligned ds0, 8-byte aligned dx)");
+  // the staged tile is fixed-size (persistent blocks loop over tiles): no limit on h or w
+  const long long tiles = (long long)b * ((h / 2 + kSigQH - 1) / kSigQH) * ((w / 2 + kSigQW - 1) / kSigQW);
+  const long long cap = (long long)num_sms() * 2;                 // two 90 KiB blocks per SM
+  const unsigned grid = (unsigned)(tiles < cap ? tiles : cap);
+  int rc = ODB_OK;
+  ODB_DT(dtype, T, "stem_input_grad", rc = stem_input_grad_launch<T>(ds0, weight, dx, b, h, w, kpad, grid, stream));
+  if (rc) return rc;
+  count_launch();
+  return check_launch("stem_input_grad");
 }
 
 constexpr int kHeadBwdBlocks = 592;

@@ -408,10 +408,11 @@ class DPTDepthModel(nn.Module):
         B, _, H, W = x.shape
         if H % 32 or W % 32 or (H // 16) * (W // 16) + 1 > 640:
             raise ValueError("H and W must be multiples of 32 with at most 639 patches (384x384 in scope)")
-        if self.training and torch.is_grad_enabled():
-            # train() mode under autograd: the differentiable forward (activations kept for the backward kernels);
-            # eval() mode, or any call under torch.no_grad(), is the inference path below and returns a tensor
-            # that is not attached to an autograd graph
+        if torch.is_grad_enabled() and (self.training or (x.requires_grad and self.backbone == "vitb_rn50_384")):
+            # train() mode under autograd, or (DPT-Hybrid) an input that requires grad in either mode: the
+            # differentiable forward (activations kept for the backward kernels).  Any other eval() call, or any call
+            # under torch.no_grad(), is the inference path below and returns a tensor that is not attached to an
+            # autograd graph
             return self._forward_autograd(x)
         x = x.detach().float().contiguous()
         sig = self._weights_signature()

@@ -11,7 +11,8 @@ layout), runs the forward keeping every activation the backward needs, and the b
     bias gradients = the kernels of csrc/bwd_ops.cu.
 `precision="fp32"` runs the same orchestration on the FP32-pipe twins: the mode the gradient-parity tests use against
 torch.autograd of the reference arithmetic.  `differentiable_forward(model, x)` wraps the engine in a
-torch.autograd.Function so that `loss(model(x)).backward()` fills `p.grad` like the reference module would.
+torch.autograd.Function so that `loss(model(x)).backward()` fills `p.grad` (and `x.grad` when x requires grad) like the
+reference module would.
 """
 from __future__ import annotations
 
@@ -429,10 +430,11 @@ class TrainEngine:
             ops.conv_gemm([dy], taps, w, dx[:, py::2, px::2, :], bias=self._zb(w))
 
     @torch.no_grad()
-    def backward(self, dout: torch.Tensor, on_ready=None):
+    def backward(self, dout: torch.Tensor, on_ready=None, dx: Optional[torch.Tensor] = None):
         """dout: gradient w.r.t. the forward's output [B,C,H,W] fp32.  Fills self.flat_grad (all 368 tensors).
         on_ready(tag) is called when a contiguous range of the flat gradient is final (plan_grad_buckets): the
-        data-parallel train step launches that range's all-reduce while the rest of the backward runs."""
+        data-parallel train step launches that range's all-reduce while the rest of the backward runs.
+        dx (optional, fp32 contiguous [B,3,H,W]) receives the gradient w.r.t. the input image."""
         ready = on_ready if on_ready is not None else (lambda tag: None)
         S, P, G, Wt, buf = self.saved, self.P, self.G, self.W, self.buf
         if S is None:
@@ -657,6 +659,8 @@ class TrainEngine:
         bwd.stem_pool_bwd(d_out, s0, st0, P[bb + "stem.norm.weight"], P[bb + "stem.norm.bias"], g_s0)
         ds0 = buf("g.stem_conv", s0.shape)
         bwd.groupnorm_bwd(g_s0, s0, st0, P[bb + "stem.norm.weight"], ds0, G[bb + "stem.norm.weight"], G[bb + "stem.norm.bias"])
+        if dx is not None:
+            bwd.stem_input_grad(ds0, self.stem_w, dx)
         gp = self.gp[: 64 * 160].view(64, 160)
         h2, w2 = H // 2, W // 2
         bwd.conv_wgrad([cols.view(B, h2, w2, 160)], bwd.TAPS_1, ds0, gp)
@@ -673,19 +677,26 @@ class _DptFunction(torch.autograd.Function):
     def forward(ctx, engine, x, *params):
         out = engine.forward(x)
         ctx.engine = engine
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         return out.clone()
 
     @staticmethod
     def backward(ctx, grad_out):
         eng = ctx.engine
-        eng.backward(grad_out)
+        dx = None
+        if ctx.needs_input_grad[1]:
+            B, _, H, W = ctx.x_shape
+            dx = torch.empty((B, 3, H, W), device=grad_out.device, dtype=torch.float32)
+        eng.backward(grad_out, dx=dx)
         grads = tuple(eng.G[n].clone() for n in eng.param_names)
-        return (None, None) + grads
+        if dx is not None:
+            dx = dx.reshape(ctx.x_shape).to(ctx.x_dtype)
+        return (None, dx) + grads
 
 
 def differentiable_forward(model: DPTDepthModel, x: torch.Tensor) -> torch.Tensor:
-    """model(x) under autograd in train() mode: returns a tensor whose backward fills p.grad of every parameter
-    (the gradient w.r.t. the input image is not produced: the reference never asks for it either)."""
+    """model(x) under autograd: returns a tensor whose backward fills p.grad of every parameter and, when x requires
+    grad, x.grad (the gradient w.r.t. the input image, in x's dtype)."""
     eng = getattr(model, "_train_engine", None)
     if eng is None or eng.fp32 != (model.precision == "fp32"):
         eng = TrainEngine(model, precision=model.precision)
