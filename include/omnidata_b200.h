@@ -297,6 +297,11 @@ int odb_stem_pool_bwd(const void* dt, const void* s0, const float* stats, const 
  * [152, 1024]; ds0 16-byte and dx 8-byte aligned. */
 int odb_stem_input_grad(const void* ds0, const void* weight, float* dx, int32_t b, int32_t h, int32_t w, int32_t kpad,
                         int32_t dtype, void* stream);
+/* Gradient of the 24 x 24 position-embedding grid through its resize to a gh x gw patch grid (modules/midas/vit.py:102-116
+ * _resize_pos_embed: F.interpolate(mode="bilinear", align_corners=False), torch's index arithmetic): dpos fp32
+ * [24*24][d] = the transpose of that map applied to dgrid fp32 [gh*gw][d], written (not accumulated).  Gather form with a
+ * fixed summation order: bit-reproducible.  gh, gw >= 1; d a multiple of 4; 16-byte aligned pointers. */
+int odb_pos_embed_resize_bwd(const float* dgrid, float* dpos, int32_t gh, int32_t gw, int32_t d, void* stream);
 /* DPT head tail, unfused (training): out[b][k][y][x] = relu?(bias[k] + sum_j w[k][j] a[b][y][x][j]), a has
  * channel_stride channels per pixel of which the first 32 are used; and its backward (da zero in the padding channels). */
 int odb_head_tail_fwd(const void* a, int32_t channel_stride, const float* w, const float* bias, float* out, int32_t b,

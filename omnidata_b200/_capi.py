@@ -137,6 +137,7 @@ _SIGNATURES = {
     "odb_upsample2x_bwd": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p]),
     "odb_stem_pool_bwd": (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 6 + [C.c_void_p]),
     "odb_stem_input_grad": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 5 + [C.c_void_p]),
+    "odb_pos_embed_resize_bwd": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p]),
     "odb_head_tail_fwd": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p]),
     "odb_head_tail_bwd_workspace_bytes": (C.c_int64, [C.c_int32]),
     "odb_head_tail_bwd": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 5 + [C.c_int32] * 7 + [C.c_void_p]),

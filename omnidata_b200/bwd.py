@@ -132,6 +132,20 @@ def stem_input_grad(ds0, w, dx):
           dx.data_ptr(), b, 2 * h2, 2 * w2, w.shape[1], _dt(ds0))
 
 
+def pos_embed_resize_bwd(dgrid, gh: int, gw: int, dpos):
+    """dpos fp32 [24*24, D] = gradient of the 24 x 24 position-embedding grid through its bilinear resize to gh x gw
+    (F.interpolate(mode="bilinear", align_corners=False)), from dgrid fp32 [gh*gw, D], the gradient at the resized rows."""
+    _need(dgrid, torch.float32, "dgrid")
+    _need(dpos, torch.float32, "dpos")
+    d = dgrid.shape[-1]
+    if dgrid.numel() != gh * gw * d or not dgrid.is_contiguous():
+        raise _capi.OdbError(f"pos_embed_resize_bwd: dgrid must be a contiguous [{gh}*{gw}, D] tensor")
+    if dpos.numel() != 24 * 24 * d or not dpos.is_contiguous():
+        raise _capi.OdbError(f"pos_embed_resize_bwd: dpos must be a contiguous [24*24, {d}] tensor")
+    _call("odb_pos_embed_resize_bwd", {"bytes": 4 * (dgrid.numel() + dpos.numel())}, lib().odb_pos_embed_resize_bwd,
+          _same_device(dgrid, dpos), dgrid.data_ptr(), dpos.data_ptr(), gh, gw, d)
+
+
 def head_tail_fwd(a, w, bias, out, relu: bool):
     b, h, wd, cs = a.shape
     _call("odb_head_tail_fwd", {}, lib().odb_head_tail_fwd, _same_device(a, w, bias, out), a.data_ptr(), cs, w.data_ptr(),
@@ -255,5 +269,5 @@ def attention_bwd(qkv, o, d_o, lse, dqkv, heads: int = 12, scale: float = 0.125)
 
 
 __all__ = ["mask_add", "gelu_fwd", "gelu_bwd", "colsum", "layernorm_bwd", "groupnorm_bwd", "upsample2x_bwd", "stem_pool_bwd",
-           "stem_input_grad", "head_tail_fwd", "head_tail_bwd", "add_cast", "pack_weight", "unpack_wgrad", "conv_wgrad", "attention_bwd",
+           "stem_input_grad", "pos_embed_resize_bwd", "head_tail_fwd", "head_tail_bwd", "add_cast", "pack_weight", "unpack_wgrad", "conv_wgrad", "attention_bwd",
            "TAPS_1", "TAPS_3X3"]

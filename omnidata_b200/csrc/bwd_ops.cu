@@ -655,6 +655,69 @@ __global__ void __launch_bounds__(256, 2) stem_input_grad_kernel(const T* __rest
   }
 }
 
+// ------------------------------------------------------------------------------------------ pos-embed resize backward
+// At a patch grid other than 24 x 24 the forward resizes the position-embedding grid (modules/midas/vit.py:102-116
+// _resize_pos_embed: F.interpolate(mode="bilinear", align_corners=False)).  On each axis torch's upsample_bilinear2d maps
+// output index j to  src = max(scale * (j + 0.5) - 0.5, 0), scale = (float)in / out;  i0 = (int)src,
+// i1 = i0 + (i0 < in - 1), l1 = src - i0, l0 = 1 - l1 (both weights land on i0 when i1 == i0).  The adjoint:
+//   dpos[iy][ix] = sum over jy, jx of  wy(iy, jy) * wx(ix, jx) * dgrid[jy][jx],   w(i, j) = l0 [i0(j) == i] + l1 [i1(j) == i].
+// i0(j) and i1(j) never decrease with j, so the j that touch source index i are one range: from the first j with
+// i1(j) >= i to the last j with i0(j) <= i (binary searches).  Gather form: block = one source pixel, thread = 4 channels
+// (float4); each dpos element is summed over jy, then jx, in a fixed order and written once (no atomics, unlike torch's
+// upsample_bilinear2d backward): bit-reproducible.
+constexpr int kPosSrc = 24;                                     // the pretrained 384 x 384 / 16 grid
+struct BilinearAxis {
+  float scale;
+  int in, out;
+  ODB_DEVINL float src(int j) const {
+    const float s = scale * (j + 0.5f) - 0.5f;
+    return s < 0.f ? 0.f : s;
+  }
+  ODB_DEVINL int i0(int j) const { return (int)src(j); }
+  ODB_DEVINL int i1(int j) const { const int a = i0(j); return a + (a < in - 1 ? 1 : 0); }
+  ODB_DEVINL float weight(int i, int j) const {
+    const float s = src(j);
+    const int a = (int)s, b = a + (a < in - 1 ? 1 : 0);
+    const float l1 = s - (float)a, l0 = 1.f - l1;
+    return (a == i ? l0 : 0.f) + (b == i ? l1 : 0.f);
+  }
+  ODB_DEVINL void range(int i, int& first, int& last) const {
+    int lo = 0, hi = out;
+    while (lo < hi) { const int m = (lo + hi) >> 1; if (i1(m) >= i) hi = m; else lo = m + 1; }
+    first = lo;
+    lo = 0; hi = out;
+    while (lo < hi) { const int m = (lo + hi) >> 1; if (i0(m) > i) hi = m; else lo = m + 1; }
+    last = lo - 1;
+  }
+};
+__global__ void __launch_bounds__(256) pos_embed_resize_bwd_kernel(const float* __restrict__ dgrid, float* __restrict__ dpos,
+                                                                   int gh, int gw, int d4) {
+  grid_dep_wait();
+  grid_dep_launch();
+  const int iy = blockIdx.x / kPosSrc, ix = blockIdx.x % kPosSrc;
+  const BilinearAxis ay{(float)kPosSrc / gh, kPosSrc, gh}, ax{(float)kPosSrc / gw, kPosSrc, gw};
+  int y0, y1, x0, x1;
+  ay.range(iy, y0, y1);
+  ax.range(ix, x0, x1);
+  const float4* g = reinterpret_cast<const float4*>(dgrid);
+  for (int c = blockIdx.y * blockDim.x + threadIdx.x; c < d4; c += gridDim.y * blockDim.x) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int jy = y0; jy <= y1; ++jy) {
+      float4 row = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int jx = x0; jx <= x1; ++jx) {
+        const float wx = ax.weight(ix, jx);
+        const float4 v = __ldg(g + ((long long)jy * gw + jx) * d4 + c);
+        row.x = fmaf(wx, v.x, row.x); row.y = fmaf(wx, v.y, row.y);
+        row.z = fmaf(wx, v.z, row.z); row.w = fmaf(wx, v.w, row.w);
+      }
+      const float wy = ay.weight(iy, jy);
+      acc.x = fmaf(wy, row.x, acc.x); acc.y = fmaf(wy, row.y, acc.y);
+      acc.z = fmaf(wy, row.z, acc.z); acc.w = fmaf(wy, row.w, acc.w);
+    }
+    reinterpret_cast<float4*>(dpos)[(long long)blockIdx.x * d4 + c] = acc;
+  }
+}
+
 // ------------------------------------------------------------------------------------------ head tail (1x1 conv + ReLUs)
 // forward (training, unfused): out[b][k][p] = relu?(bias[k] + sum_j w[k][j] a[b][p][j]); a has `cs` channels per pixel
 // of which the first 32 are real (the 128 -> 32 conv is carried zero-padded to 64 output channels).
@@ -1277,6 +1340,21 @@ extern "C" int odb_stem_input_grad(const void* ds0, const void* weight, float* d
   if (rc) return rc;
   count_launch();
   return check_launch("stem_input_grad");
+}
+
+extern "C" int odb_pos_embed_resize_bwd(const float* dgrid, float* dpos, int32_t gh, int32_t gw, int32_t d, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!dgrid || !dpos || gh < 1 || gw < 1 || d < 4 || d % 4 || !aligned16(dgrid) || !aligned16(dpos))
+    return fail(ODB_ERR_INVALID, "pos_embed_resize_bwd: bad argument (positive sizes, d a multiple of 4, 16-byte aligned "
+                                 "pointers)");
+  const int d4 = d / 4;
+  const int block = d4 >= 256 ? 256 : (d4 + 31) / 32 * 32;
+  const int chunks = (d4 + block - 1) / block;
+  const cudaError_t e = launch_pdl(pos_embed_resize_bwd_kernel, dim3(kPosSrc * kPosSrc, chunks < 64 ? chunks : 64),
+                                   dim3(block), 0, stream, dgrid, dpos, gh, gw, d4);
+  if (e != cudaSuccess) return fail_cuda(e, "pos_embed_resize_bwd");
+  count_launch();
+  return check_launch("pos_embed_resize_bwd");
 }
 
 constexpr int kHeadBwdBlocks = 592;

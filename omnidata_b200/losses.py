@@ -219,6 +219,21 @@ def normal_step_losses(normal_preds, normal_gt, mask_float):
     return {"l1_loss": l1, "cos_loss": cos, "normal_loss": total}
 
 
+def check_vnl_points(points, h: int, w: int):
+    """The VNL kernels gather at the index arrays without bounds checks: host arrays must be three equally long arrays of
+    flat indices in [0, h*w).  Device tensors (a captured step's copies of arrays checked here) are not read back."""
+    if len(points) != 3:
+        raise ValueError("points: three VNL index arrays expected")
+    if len({int(q.numel()) if isinstance(q, torch.Tensor) else int(np.size(q)) for q in points}) != 1:
+        raise ValueError("points: the three VNL index arrays must have the same length")
+    for q in points:
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            continue
+        a = np.asarray(q)
+        if a.size and (int(a.min()) < 0 or int(a.max()) >= h * w):
+            raise ValueError(f"points: VNL indices must lie in [0, {h * w}) for a {h}x{w} prediction")
+
+
 class DepthStepLoss:
     """The loss arithmetic of Depth._shared_step (train_depth.py:261-279) AND its gradient with respect to the raw
     network output, as one fixed launch sequence with no host synchronisation and no autograd graph (the train step's
@@ -248,9 +263,14 @@ class DepthStepLoss:
     def __call__(self, pred: torch.Tensor, depth_gt: torch.Tensor, mask_float: torch.Tensor, full_mix: bool = True,
                  points=None):
         """pred, depth_gt, mask_float: [B,1,H,W] fp32 CUDA.  Returns (losses fp32 [4] = (loss, ssi, reg, vn), dpred)."""
+        h, w = pred.shape[-2], pred.shape[-1]
+        if (h, w) != self.vnl.input_size:
+            raise ValueError(f"DepthStepLoss: prediction is {h}x{w}, built for {self.vnl.input_size[0]}x{self.vnl.input_size[1]}")
+        if full_mix and points is not None:
+            check_vnl_points(points, h, w)
         p, g = _f32(pred, "pred"), _f32(depth_gt, "depth_gt")
         dev = p.device
-        b, h, w = p.shape[0], p.shape[-2], p.shape[-1]
+        b = p.shape[0]
         n = b * h * w
         st = torch.cuda.current_stream(dev).cuda_stream
         pc = self._buf("pc", (b, 1, h, w), torch.float32, dev)

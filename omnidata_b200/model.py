@@ -468,17 +468,22 @@ def _debug_upsample(z: torch.Tensor) -> torch.Tensor:
     return o
 
 
+def resize_pos_grid(pos: torch.Tensor, gh: int, gw: int) -> torch.Tensor:
+    """Patch rows of the position embedding pos [1, 1 + 24*24, D] resized to a gh x gw patch grid: [gh*gw, D] (vit.py:102-116
+    _resize_pos_embed, bilinear, align_corners=False).  The train engine's backward (bwd.pos_embed_resize_bwd) is the
+    adjoint of exactly this map."""
+    g = pos[0, 1:].reshape(1, 24, 24, -1).permute(0, 3, 1, 2)
+    g = F.interpolate(g, size=(gh, gw), mode="bilinear")
+    return g.permute(0, 2, 3, 1).reshape(gh * gw, -1)
+
+
 def _pos_rows(pk, gh: int, gw: int, B: int):
     """(pos0 fp32 [D], patch rows fp32 [B, gh*gw, D]) for a gh x gw patch grid, cached in pk["pos_cache"]: they are
     derived from the weights, so they live with the packed weights.  Bilinear resize as vit.py:102-116 if needed."""
     cache = pk["pos_cache"]
     if (gh, gw) not in cache:
         pos = pk["pos"]
-        grid = pos[0, 1:]
-        if (gh, gw) != (24, 24):
-            g = grid.reshape(1, 24, 24, -1).permute(0, 3, 1, 2)
-            g = F.interpolate(g, size=(gh, gw), mode="bilinear")
-            grid = g.permute(0, 2, 3, 1).reshape(gh * gw, -1)
+        grid = pos[0, 1:] if (gh, gw) == (24, 24) else resize_pos_grid(pos, gh, gw)
         cache[(gh, gw)] = (pos[0, 0].contiguous(), grid.float().contiguous())
     pos0, grid = cache[(gh, gw)]
     pos_b = cache.get((gh, gw, B))

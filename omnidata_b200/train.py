@@ -12,6 +12,10 @@ the pre-activations of the fc1 and readout GELUs, and the unfused head's interme
   * wgrad = odb_conv_wgrad (wgmma, both operands MN-major straight from the channels-last tensors; fp32 twin);
   * attention backward = odb_attention_bwd; LayerNorm / GroupNorm / GELU / ReLU / bilinear / max-pool / head backward and
     bias gradients = the kernels of csrc/bwd_ops.cu.
+The engine takes every input size inference takes: H and W multiples of 32, at most 639 patches.  Off the pretrained
+24 x 24 patch grid the forward resizes pos_embed's patch rows from this step's fp32 master weights with the function
+inference uses (model.resize_pos_grid), and the backward takes their gradient through the adjoint of that bilinear
+resize (odb_pos_embed_resize_bwd, no atomics).
 `precision="fp32"` runs the same orchestration on the FP32-pipe twins: the mode the gradient-parity tests use against
 torch.autograd of the reference arithmetic.  `differentiable_forward(model, x)` wraps the engine in a
 torch.autograd.Function so that `loss(model(x)).backward()` fills `p.grad` (and `x.grad` when x requires grad) like the
@@ -26,7 +30,7 @@ import torch
 
 from . import bwd, ops
 from ._capi import OdbError
-from .model import _STAGES, DPTDepthModel, _Workspace, dpt_forward
+from .model import _STAGES, DPTDepthModel, _Workspace, dpt_forward, resize_pos_grid
 
 
 def _parity_dgrad_plan(mode: str):
@@ -170,10 +174,9 @@ class TrainEngine:
                 blocks.append((s, b, e))
         pk["rn_blocks"] = blocks
         pm = "pretrained.model."
-        pos = P[pm + "pos_embed"]
-        # forward() adds the (24, 24, batch) entry after its per-step copy of the replicated patch rows
+        # pos_cache: filled by every forward() with that step's rows
         pk.update(proj_w=fw("proj"), proj_b=P[pm + "patch_embed.proj.bias"], cls=P[pm + "cls_token"].view(-1),
-                  pos_cache={(24, 24): (pos[0, 0], pos[0, 1:])})
+                  pos_cache={})
         pk["vit"] = []
         for i in range(self.model.arch["depth"]):
             p = f"{pm}blocks.{i}."
@@ -266,13 +269,15 @@ class TrainEngine:
         B, _, H, W = x.shape
         if H % 32 or W % 32 or (H // 16) * (W // 16) + 1 > 640:
             raise ValueError("H and W must be multiples of 32 with at most 639 patches")
-        if (H // 16, W // 16) != (24, 24):
-            raise NotImplementedError("train step: 384x384 inputs (24x24 patch grid)")
+        gh, gw = H // 16, W // 16
         self.pack()
+        # the patch rows of this step's pos_embed (resized from the fp32 master weights as inference resizes them),
+        # replicated per image: the patch GEMM's residual operand
         pos = self.P["pretrained.model.pos_embed"]
-        pos_b = self.buf("pos_expanded", (B, 24 * 24, pos.shape[-1]), torch.float32)
-        pos_b.copy_(pos[0, 1:].unsqueeze(0).expand(B, -1, -1))
-        self.pk["pos_cache"][(24, 24, B)] = pos_b
+        grid = pos[0, 1:] if (gh, gw) == (24, 24) else resize_pos_grid(pos, gh, gw)
+        pos_b = self.buf("pos_expanded", (B, gh * gw, pos.shape[-1]), torch.float32)
+        pos_b.copy_(grid.unsqueeze(0).expand(B, -1, -1))
+        self.pk["pos_cache"] = {(gh, gw): (pos[0, 0], grid), (gh, gw, B): pos_b}
         self.saved = {}
         return dpt_forward(x, self.pk, self.model.arch, self.precision, self.non_negative, self.C, self.ws,
                            save=self.saved)
@@ -445,7 +450,13 @@ class TrainEngine:
                               dcolsum=fc2_bias)
         # ---- tokens: cls / pos_embed, patch projection
         gpos = G[pm + "pos_embed"]
-        bwd.colsum(ds.view(B, ntok * D), gpos.view(1, -1))
+        if (gh, gw) == (24, 24):
+            bwd.colsum(ds.view(B, ntok * D), gpos.view(1, -1))
+        else:                                                        # through the forward's resize of the patch rows
+            dgrid = buf("g.pos_rows", (ntok, D), f32)
+            bwd.colsum(ds.view(B, ntok * D), dgrid.view(1, -1))
+            gpos[0, 0].copy_(dgrid[0])
+            bwd.pos_embed_resize_bwd(dgrid[1:], gh, gw, gpos[0, 1:])
         G[pm + "cls_token"].view(-1).copy_(gpos[0, 0])
         g16 = ds if self.fp32 else ds16
         f3 = S["f3"]
@@ -632,7 +643,19 @@ class DepthTrainStep:
     @torch.no_grad()
     def step(self, rgb: torch.Tensor, depth_gt: torch.Tensor, mask_float: torch.Tensor, points=None,
              full_mix: Optional[bool] = None) -> torch.Tensor:
-        """-> fp32 [5] on the device: (loss, ssi, reg, vn, gradient norm before clipping); no host synchronisation."""
+        """-> fp32 [5] on the device: (loss, ssi, reg, vn, gradient norm before clipping); no host synchronisation.
+        rgb [B,3,H,W], depth_gt and mask_float [B,1,H,W] with (H, W) = the step's input_size; `points`: host index
+        arrays in [0, H*W)."""
+        from .losses import check_vnl_points
+        H, W = self.loss.vnl.input_size
+        if rgb.dim() != 4 or tuple(rgb.shape[1:]) != (3, H, W):
+            raise ValueError(f"DepthTrainStep: rgb must be [B,3,{H},{W}] (the step's input_size), got {tuple(rgb.shape)}")
+        B = rgb.shape[0]
+        for name, t in (("depth_gt", depth_gt), ("mask_float", mask_float)):
+            if tuple(t.shape[-2:]) != (H, W) or t.numel() != B * H * W:
+                raise ValueError(f"DepthTrainStep: {name} must be [{B},1,{H},{W}], got {tuple(t.shape)}")
+        if points is not None:
+            check_vnl_points(points, H, W)
         if full_mix is None:
             full_mix = self.global_step >= 15000                     # train_depth.py:274-279
         if self.use_cuda_graph and (self.dist is None or self.graph_collectives):
