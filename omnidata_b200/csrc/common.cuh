@@ -48,15 +48,12 @@ ODB_DEVINL bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 // Spin with a watchdog: a protocol bug must abort the kernel (sticky error on the host)
-// instead of hanging the GPU box.
+// instead of hanging the GPU.  Trap only, no printf: a printf is a function call, and a call
+// inlined between wgmma issue and wait makes ptxas serialise every wgmma of the kernel (C7510).
 ODB_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("odb: mbarrier watchdog block %d thread %d bar %u parity %u\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 

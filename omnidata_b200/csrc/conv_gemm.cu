@@ -250,11 +250,14 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
 
   // work units: (n tile, m tile) for a single CTA, (n tile, pair of m tiles) for a CTA pair
   const uint32_t cta_rank = PAIR ? cluster_ctarank() : 0u;
-  const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_b;
-  const int m_units = PAIR ? (m_tiles + 1) / 2 : m_tiles;
-  const int total_tiles = p.tiles_n * m_units;
-  const int unit0 = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int unit_stride = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  // the unit schedule, computed by each role after its setmaxnreg: values live across the role split must fit the
+  // producer's 40 registers, and ptxas keeps them in local memory instead
+  auto m_tiles = [&]() { return p.tiles_x * p.tiles_y * p.tiles_b; };
+  auto schedule = [&](int& total_tiles, int& unit0, int& unit_stride) {
+    total_tiles = p.tiles_n * (PAIR ? (m_tiles() + 1) / 2 : m_tiles());
+    unit0 = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
+    unit_stride = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  };
   const int num_kb = p.num_taps * p.kb_per_tap;
   const uint32_t a_bytes =
       HALO ? static_cast<uint32_t>(p.halo_w * (p.tile_h + 2)) * 128u
@@ -265,7 +268,7 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
     tn = unit % p.tiles_n;
     int m = unit / p.tiles_n;
     if (PAIR) m = 2 * m + static_cast<int>(cta_rank);
-    if (m >= m_tiles) { tx = 0; ty = 0; tb = p.tiles_b; return; }
+    if (m >= m_tiles()) { tx = 0; ty = 0; tb = p.tiles_b; return; }
     tx = m % p.tiles_x; m /= p.tiles_x;
     ty = m % p.tiles_y;
     tb = m / p.tiles_y;
@@ -290,6 +293,8 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   if (warp < 4) {
     // ------------------------------------------------------------ TMA producer (warpgroup 0, one lane)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    int total_tiles, unit0, unit_stride;
+    schedule(total_tiles, unit0, unit_stride);
     if (warp == 0 && lane == 0) {
       int stage = 0, astage = 0;
       uint32_t phase = 0, aphase = 0;
@@ -345,6 +350,8 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   } else {
     // ------------------------------------------------------------ consumers (warpgroups 1, 2): wgmma + epilogue
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    int total_tiles, unit0, unit_stride;
+    schedule(total_tiles, unit0, unit_stride);
     const int wg = (warp - 4) >> 2;                              // 64-row half of the 128-row tile
     const uint32_t a_half = static_cast<uint32_t>(wg) * 64u * 128u;
     float dacc[BLOCK_N / 2];
@@ -357,6 +364,11 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
     // the MMA half of a tile: the accumulator of tile `iter` complete in `acc`
     auto mainloop = [&](uint32_t iter) {
       if (lane == 0 && warp == 4) ODB_TRACE_TILE(iter, 0);
+      // The first wgmma of a tile ignores the accumulator (scale-d 0), but its asm operands are read-write: without
+      // this the previous tile's accumulator registers count as live through that tile's whole epilogue, and the
+      // 256-wide epilogues spill.  Overwriting them here frees each chunk's registers once it has been staged.
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) dacc[i] = 0.f;
       if constexpr (Plan::kBResident) {
         if (iter == 0) mbar_wait(bres_bar, 0);
         const uint32_t b_tap_step = static_cast<uint32_t>(p.kb_per_tap) * Plan::kBBytes;
@@ -443,13 +455,18 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
         }
       }
     };
-    auto read_row = [&](int row, int col, uint32_t* r) {
+    // v[j] = accumulator (row, col + j) + b[j] for 32 columns (b == nullptr: + 0.f).  The bias is read four values at
+    // a time after the chunk hand-over, so that beside the accumulator registers still to be staged only the 32 row
+    // values and one float4 of bias are live: the 256-wide tiles then fit without spilling.
+    auto read_row_bias = [&](int row, int col, const float* b, float* v) {
       const float4* src = reinterpret_cast<const float4*>(acc_buf + row * Acc::kPitch + col);
+      const float4* bp = reinterpret_cast<const float4*>(b);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float4 q = src[j];
-        r[4 * j + 0] = __float_as_uint(q.x); r[4 * j + 1] = __float_as_uint(q.y);
-        r[4 * j + 2] = __float_as_uint(q.z); r[4 * j + 3] = __float_as_uint(q.w);
+        const float4 b4 = b != nullptr ? __ldg(bp + j) : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[4 * j + 0] = q.x + b4.x; v[4 * j + 1] = q.y + b4.y;
+        v[4 * j + 2] = q.z + b4.z; v[4 * j + 3] = q.w + b4.w;
       }
     };
     // ------------------------------------------------------------ epilogue
@@ -459,10 +476,6 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
     const int row = quad * 32 + lane;      // accumulator row == pixel within the tile
     const bool store_leader = (ew == 0 && lane == 0);
     const int tw = p.tile_w;
-    const int rpitch = HALO ? p.halo_w : tw;            // accumulator rows per tile row
-    const int ly = row / rpitch, lx = row - ly * rpitch;
-    const bool row_in_tile = HALO ? (lx < tw && ly < p.tile_h) : (row < p.tile_w * p.tile_h);
-    const int srow = HALO ? (row_in_tile ? ly * tw + lx : 0) : row;   // dense row in the store staging tile
     if constexpr (EPI != EPI_GENERIC) {
       // ---------------------------------------------------------- specialised epilogues
       constexpr int kChunks = BLOCK_N / 64;
@@ -498,6 +511,8 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
       }
       uint32_t iter = 0;
       for (int tile = unit0; tile < total_tiles; tile += unit_stride, ++iter) {
+        mainloop(iter);      // first: the per-tile values below need no registers beside the accumulator
+        if (store_leader) ODB_TRACE_TILE(iter, 3);
         int tn, tx, ty, tb;
         decode(tile, tn, tx, ty, tb);
         const int x0 = tx * p.tile_w, y0 = ty * p.tile_h;
@@ -507,26 +522,11 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
         // EPI_GN: rows of this thread that really exist (ragged tiles)
         const int gx = x0 + (row % p.tile_w), gy = y0 + (row / p.tile_w);
         const bool valid = row < p.tile_w * p.tile_h && gx < p.out_w && gy < p.out_h && tb < p.out_b;
-        mainloop(iter);
-        if (store_leader) ODB_TRACE_TILE(iter, 3);
 #pragma unroll
         for (int c = 0; c < kChunks; ++c, ++g) {
-          uint32_t r[32];
-          float4 bv[8];
-          if constexpr (EPI != EPI_GN) {
-            const float4* bp = reinterpret_cast<const float4*>(bias + c * 64);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bv[j] = __ldg(bp + j);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bv[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
           stage_chunk_rt(c);
-          read_row(row, cofs, r);
           float v[32];
-          const float* bf = reinterpret_cast<const float*>(bv);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + bf[j];
+          read_row_bias(row, cofs, EPI == EPI_GN ? nullptr : bias + c * 64, v);
           if constexpr (EPI == EPI_BIAS_GELU) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) gelu_erf_x2(v[2 * j], v[2 * j + 1]);
@@ -624,30 +624,26 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
     const int slots = NSTAGING > 0 ? NSTAGING / bufs_per_chunk : 1;
 
     for (int tile = unit0; tile < total_tiles; tile += unit_stride, ++iter) {
+      mainloop(iter);
+      if (store_leader) ODB_TRACE_TILE(iter, 3);
+      // the row geometry is recomputed per tile: kept across the MMA loop it would not fit beside the accumulator
+      const int rpitch = HALO ? p.halo_w : tw;            // accumulator rows per tile row
+      const int ly = row / rpitch, lx = row - ly * rpitch;
+      const bool row_in_tile = HALO ? (lx < tw && ly < p.tile_h) : (row < p.tile_w * p.tile_h);
+      const int srow = HALO ? (row_in_tile ? ly * tw + lx : 0) : row;   // dense row in the store staging tile
       int tn, tx, ty, tb;
       decode(tile, tn, tx, ty, tb);
       const int x0 = tx * p.tile_w, y0 = ty * p.tile_h;
       const int x = x0 + lx, y = y0 + ly;
       const bool valid = row_in_tile && x < p.out_w && y < p.out_h && tb < p.out_b;
 
-      mainloop(iter);
-      if (store_leader) ODB_TRACE_TILE(iter, 3);
-
       if constexpr (HEAD) {
         // ---- DPT head tail: relu(conv + bias) (32 ch) -> 1x1 conv to head_c channels -> relu -> NCHW fp32
-        uint32_t r[32];
         stage_chunk_rt(0);
-        read_row(row, 0, r);
         float v[32];
+        read_row_bias(row, 0, p.bias, v);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 b4 = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias) + j)
-                             : make_float4(0.f, 0.f, 0.f, 0.f);
-          v[4 * j + 0] = fmaxf(__uint_as_float(r[4 * j + 0]) + b4.x, 0.f);
-          v[4 * j + 1] = fmaxf(__uint_as_float(r[4 * j + 1]) + b4.y, 0.f);
-          v[4 * j + 2] = fmaxf(__uint_as_float(r[4 * j + 2]) + b4.z, 0.f);
-          v[4 * j + 3] = fmaxf(__uint_as_float(r[4 * j + 3]) + b4.w, 0.f);
-        }
+        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
         if (valid) {
           for (int k = half; k < p.head_c; k += 2) {   // the two warp halves share the output channels
             const float4* wk = reinterpret_cast<const float4*>(p.head_w + k * 32);
@@ -675,11 +671,22 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
                               ? p.residual + tb * p.res_sb + y * p.res_sy + x * p.res_sx + n0 + cofs
                               : nullptr;
         constexpr int kChunks = BLOCK_N / 64;
-#pragma unroll 1
+        // unrolled: the chunk index is a compile-time constant, so the accumulator registers of a staged chunk are
+        // free for the epilogue of the chunks after it
+#pragma unroll
         for (int c = 0; c < kChunks; ++c, ++chunk_counter) {
-          uint32_t r[32];
           stage_chunk_rt(c);
-          read_row(row, cofs, r);
+          // ---- bias + activation (specialised per activation: a straight-line block keeps the 32
+          //      independent elements of a thread in flight), residual, bf16 packing
+          float v[32];
+          read_row_bias(row, cofs, bias != nullptr ? bias + c * 64 : nullptr, v);
+          if (p.act == ODB_ACT_GELU) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) gelu_erf_x2(v[2 * j], v[2 * j + 1]);
+          } else if (p.act == ODB_ACT_RELU) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+          }
           uint4 rv[4];
           if (res != nullptr) {
             const uint4* rp = reinterpret_cast<const uint4*>(res + c * 64);
@@ -689,53 +696,12 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) rv[j] = make_uint4(0, 0, 0, 0);
           }
-          float4 bv[8];
-          if (bias != nullptr) {
-            const float4* bp = reinterpret_cast<const float4*>(bias + c * 64);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bv[j] = __ldg(bp + j);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) bv[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          // ---- bias + activation (specialised per activation: a straight-line block keeps the 32
-          //      independent elements of a thread in flight), residual, bf16 packing
-          float v[32];
-          const float* bf = reinterpret_cast<const float*>(bv);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + bf[j];
-          if (p.act == ODB_ACT_GELU) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) gelu_erf_x2(v[2 * j], v[2 * j + 1]);
-          } else if (p.act == ODB_ACT_RELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          uint32_t packed[16];
           const uint32_t* ru = reinterpret_cast<const uint32_t*>(rv);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const float2 rr = unpack_bf16x2(ru[j]);
             v[2 * j] += rr.x;
             v[2 * j + 1] += rr.y;
-            packed[j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-          }
-          // ---- fused GroupNorm statistics over the unrounded fp32 values (before the bf16 store)
-          if (p.gn_partial != nullptr) {
-            float rq[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) rq[j] = valid ? v[j] : 0.f;
-            if (tb < p.out_b) {
-              const int cpg = p.gn_cpg;
-              float* dst = p.gn_partial +
-                           ((((long long)tb * (p.tiles_x * p.tiles_y) + (ty * p.tiles_x + tx)) * 4 + quad) *
-                                p.gn_groups + (n0 + c * 64 + cofs) / cpg) * 2;
-              if (cpg == 2) gn_warp_partials<2>(rq, lane, dst);
-              else if (cpg == 4) gn_warp_partials<4>(rq, lane, dst);
-              else if (cpg == 8) gn_warp_partials<8>(rq, lane, dst);
-              else if (cpg == 16) gn_warp_partials<16>(rq, lane, dst);
-              else gn_warp_partials<32>(rq, lane, dst);
-            }
           }
           // ---- staging: two slots alternate.  Slot (c & 1) was last read by the TMA store of chunk
           //      c-2, whose completion the store leader awaited before the barrier of chunk c-1, so
@@ -754,27 +720,51 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
             for (int j = 0; j < 4; ++j) {
               const uint32_t addr =
                   buf0 + rowoff + (static_cast<uint32_t>((half * 4 + j) ^ (srow & 7)) << 4);
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(packed[4 * j]),
-                           "r"(packed[4 * j + 1]), "r"(packed[4 * j + 2]), "r"(packed[4 * j + 3])
-                           : "memory");
-            }
-          }
-          if (p.has_out2 && do_store) {
-            if (p.out2_gelu) {     // the stored pre-activation `out` stays as it is; the copy is gelu of the same fp32 value
-#pragma unroll
-              for (int j = 0; j < 16; ++j) gelu_erf_x2(v[2 * j], v[2 * j + 1]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint32_t addr = buf0 + kStagingBytes + rowoff +
-                                    (static_cast<uint32_t>((half * 4 + j) ^ (srow & 7)) << 4);
               asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr),
                            "r"(pack_bf16x2(v[8 * j + 0], v[8 * j + 1])), "r"(pack_bf16x2(v[8 * j + 2], v[8 * j + 3])),
                            "r"(pack_bf16x2(v[8 * j + 4], v[8 * j + 5])), "r"(pack_bf16x2(v[8 * j + 6], v[8 * j + 7]))
                            : "memory");
+            }
+          }
+          if (p.has_out2 && do_store) {
+            // the stored pre-activation `out` stays as it is; the copy is relu / gelu of the same fp32 value, taken
+            // two elements at a time so that v stays intact for the GroupNorm statistics
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              uint32_t q[4];
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                float a = v[8 * j + 2 * i], b = v[8 * j + 2 * i + 1];
+                if (p.out2_gelu) {
+                  gelu_erf_x2(a, b);
+                } else {
+                  a = fmaxf(a, 0.f);
+                  b = fmaxf(b, 0.f);
+                }
+                q[i] = pack_bf16x2(a, b);
+              }
+              const uint32_t addr = buf0 + kStagingBytes + rowoff +
+                                    (static_cast<uint32_t>((half * 4 + j) ^ (srow & 7)) << 4);
+              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(q[0]), "r"(q[1]), "r"(q[2]),
+                           "r"(q[3])
+                           : "memory");
+            }
+          }
+          // ---- fused GroupNorm statistics over the unrounded fp32 values (before the bf16 store); v is not
+          //      needed after this, so the rows outside the output are zeroed in place
+          if (p.gn_partial != nullptr) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = valid ? v[j] : 0.f;
+            if (tb < p.out_b) {
+              const int cpg = p.gn_cpg;
+              float* dst = p.gn_partial +
+                           ((((long long)tb * (p.tiles_x * p.tiles_y) + (ty * p.tiles_x + tx)) * 4 + quad) *
+                                p.gn_groups + (n0 + c * 64 + cofs) / cpg) * 2;
+              if (cpg == 2) gn_warp_partials<2>(v, lane, dst);
+              else if (cpg == 4) gn_warp_partials<4>(v, lane, dst);
+              else if (cpg == 8) gn_warp_partials<8>(v, lane, dst);
+              else if (cpg == 16) gn_warp_partials<16>(v, lane, dst);
+              else gn_warp_partials<32>(v, lane, dst);
             }
           }
           fence_proxy_async_smem();
