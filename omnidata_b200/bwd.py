@@ -260,7 +260,21 @@ def conv_wgrad(views: Sequence[torch.Tensor], taps: Sequence[Tuple[int, int, int
 
 
 def attention_bwd(qkv, o, d_o, lse, dqkv, heads: int = 12, scale: float = 0.125):
+    """dqkv [b, T, 3*heads*64] = gradient w.r.t. qkv of o = attention(qkv), from d_o; lse fp32 [b, heads, T] (bf16 only):
+    the log2-sum-exp ops.attention wrote.  The kernels address every tensor from (b, T, heads) alone, so the shapes
+    are checked here."""
+    if qkv.dim() != 3 or qkv.shape[-1] != 3 * heads * 64 or not qkv.is_contiguous():
+        raise _capi.OdbError(f"attention_bwd: qkv must be a contiguous [b, T, {3 * heads * 64}] tensor")
     b, n, c3 = qkv.shape
+    if n > 640:
+        raise _capi.OdbError(f"attention_bwd: at most 640 tokens, got {n}")
+    _dt(qkv)
+    for name, t, shape in (("o", o, (b, n, heads * 64)), ("d_o", d_o, (b, n, heads * 64)), ("dqkv", dqkv, (b, n, c3))):
+        if tuple(t.shape) != shape or t.dtype != qkv.dtype or not t.is_contiguous():
+            raise _capi.OdbError(f"attention_bwd: {name} must be a contiguous {list(shape)} tensor of qkv's dtype")
+    if qkv.dtype == torch.bfloat16:
+        if lse is None or tuple(lse.shape) != (b, heads, n) or lse.dtype != torch.float32 or not lse.is_contiguous():
+            raise _capi.OdbError(f"attention_bwd: lse must be a contiguous fp32 [{b}, {heads}, {n}] tensor")
     need = lib().odb_attention_bwd_workspace_bytes(b, n, heads, _dt(qkv))
     ws = _scratch(need, qkv.device)
     info = {"flops": 10.0 * b * heads * n * n * 64}

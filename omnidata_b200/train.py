@@ -49,6 +49,17 @@ def _parity_dgrad_plan(mode: str):
     return plan
 
 
+def parity_dgrad_operands(wb: torch.Tensor, n_pad: int, mode: str) -> dict:
+    """Operands of the stride-2 3x3 input gradient, one small convolution per input parity plane: wb is the layer's
+    dgrad operand [c][9 * n_pad] (tap slot 8 - t holds W_t^T, odb_pack_weight).  -> {(py, px): (weight
+    [c][len(taps) * n_pad], taps)}; convolving dY with `taps` and that weight gives dX[:, py::2, px::2, :]."""
+    operands = {}
+    for plane, taps_ in _parity_dgrad_plan(mode).items():
+        cat = torch.cat([wb[:, (8 - t) * n_pad:(9 - t) * n_pad] for t, _, _ in taps_], dim=1).contiguous()
+        operands[plane] = (cat, [(0, dx, dy) for _, dy, dx in taps_])
+    return operands
+
+
 class TrainEngine:
     def __init__(self, model: DPTDepthModel, precision: str = "bf16"):
         if model.backbone != "vitb_rn50_384":
@@ -229,11 +240,9 @@ class TrainEngine:
         # stride-2 3x3 convolutions: per-parity-plane dgrad operands cut out of the rotated dgrad weight
         self.plane_w = {}
         for key, mode in (("s1b0.w2", "same"), ("s2b0.w2", "same"), ("pp4s", "sym1")):
-            _, n, c, taps, n_pad, _ = self.meta[key]
-            wb = self.W[key][1]                                    # [c][9 * n], tap slot 8 - t holds W_t^T
-            for plane, taps_ in _parity_dgrad_plan(mode).items():
-                cat = torch.cat([wb[:, (8 - t) * n_pad:(9 - t) * n_pad] for t, _, _ in taps_], dim=1).contiguous()
-                self.plane_w[(key, plane)] = (cat, [(0, dx, dy) for _, dy, dx in taps_])
+            n_pad = self.meta[key][4]
+            for plane, op in parity_dgrad_operands(self.W[key][1], n_pad, mode).items():
+                self.plane_w[(key, plane)] = op
 
     # ------------------------------------------------------------------ small helpers
     def _wgrad(self, key: str, views, taps, dy, n_rows: Optional[int] = None):
