@@ -272,13 +272,15 @@ int odb_reduce_partials(const float* partial, float* out, int32_t batches, int32
 /* LayerNorm backward on the fp32 residual stream: ds_out = ds_in + dLN(dy; x, gamma) (ds_in may be NULL), optional
  * copy of ds_out in `dtype` (the next GEMM operand), dgamma / dbeta (+)=, and optionally (dcolsum != NULL) the column
  * sums of ds_out (+)= : the bias gradient of the linear layer whose output gradient ds_out is (timm Block: attn.proj
- * after norm2's backward, the previous block's mlp.fc2 after norm1's). */
+ * after norm2's backward, the previous block's mlp.fc2 after norm1's).  dgamma = dbeta = NULL (both or neither): a frozen
+ * norm, no affine gradients and no reduction of them — one pass writing ds_out / ds_copy (and dcolsum if given). */
 int64_t odb_layernorm_bwd_workspace_bytes(int32_t cols);
 int odb_layernorm_bwd(const void* dy, const float* x, const float* gamma, const float* ds_in, float* ds_out, void* ds_copy,
                       float* dgamma, float* dbeta, float* dcolsum, void* workspace, int64_t rows, int32_t cols, float eps,
                       int32_t accumulate, int32_t dtype, void* stream);
 /* GroupNorm backward (timm GroupNormAct): g = dy * [mask > 0] (mask NULL: g = dy; the mask is the stored output of the
- * ReLU that follows the norm); dx, dgamma (+)=, dbeta (+)= from x and the forward statistics (mean, rstd). */
+ * ReLU that follows the norm); dx, dgamma (+)=, dbeta (+)= from x and the forward statistics (mean, rstd).
+ * dgamma = dbeta = NULL (both or neither): dx only (the group sums dx needs are still formed). */
 int64_t odb_groupnorm_bwd_workspace_bytes(int32_t b, int32_t hw, int32_t c, int32_t groups);
 int odb_groupnorm_bwd(const void* dy, const void* mask, const void* x, const float* stats, const float* gamma, void* dx,
                       float* dgamma, float* dbeta, void* workspace, int32_t b, int32_t hw, int32_t c, int32_t groups,
@@ -303,7 +305,8 @@ int odb_stem_input_grad(const void* ds0, const void* weight, float* dx, int32_t 
  * fixed summation order: bit-reproducible.  gh, gw >= 1; d a multiple of 4; 16-byte aligned pointers. */
 int odb_pos_embed_resize_bwd(const float* dgrid, float* dpos, int32_t gh, int32_t gw, int32_t d, void* stream);
 /* DPT head tail, unfused (training): out[b][k][y][x] = relu?(bias[k] + sum_j w[k][j] a[b][y][x][j]), a has
- * channel_stride channels per pixel of which the first 32 are used; and its backward (da zero in the padding channels). */
+ * channel_stride channels per pixel of which the first 32 are used; and its backward (da zero in the padding channels;
+ * dw = dbias = NULL, both or neither: da only). */
 int odb_head_tail_fwd(const void* a, int32_t channel_stride, const float* w, const float* bias, float* out, int32_t b,
                       int32_t h, int32_t wd, int32_t head_c, int32_t relu, int32_t dtype, void* stream);
 int64_t odb_head_tail_bwd_workspace_bytes(int32_t head_c);
@@ -397,12 +400,23 @@ int odb_normal_loss_fwd(const float* prediction, const float* target, const uint
  * clip2 = the out2 of odb_clip_grad_norm or NULL (no clipping).  step_scalars (device fp32 [2], may be NULL): when given,
  * the two step-dependent scalars (lr / (1 - beta1^step), sqrt(1 - beta2^step)) are read from device memory instead of
  * being computed from `step` — what a CUDA-graph replay of the train step needs; odb_adam_step_scalars (host function,
- * host pointer) computes them exactly as odb_adam_step does. */
+ * host pointer) computes them exactly as odb_adam_step does.
+ *
+ * The _segments variants restrict both to the elements of a device table segments int64 [num_segments][2] of [start, end)
+ * ranges of the flat buffers (1..1024 disjoint ranges, 16-byte aligned table; every start a multiple of 4, every length but
+ * the last a multiple of 4; total = the sum of the lengths): the norm of those gradients only, and no other element of
+ * params / exp_avg / exp_avg_sq is read or written.  One launch each, no host synchronisation (CUDA-graph capturable).
+ * odb_clip_grad_norm / odb_adam_step are the one-segment case [0, n) of the same kernels. */
 int64_t odb_grad_norm_workspace_bytes(void);
 int odb_clip_grad_norm(const float* grads, int64_t n, float max_norm, void* workspace, float* out2, void* stream);
+int odb_clip_grad_norm_segments(const float* grads, const int64_t* segments, int32_t num_segments, int64_t total,
+                                float max_norm, void* workspace, float* out2, void* stream);
 int odb_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
                   const float* clip2, float lr, float beta1, float beta2, float eps, int64_t step,
                   const float* step_scalars, void* stream);
+int odb_adam_step_segments(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const int64_t* segments,
+                           int32_t num_segments, int64_t total, const float* clip2, float lr, float beta1, float beta2,
+                           float eps, int64_t step, const float* step_scalars, void* stream);
 int odb_adam_step_scalars(float lr, float beta1, float beta2, int64_t step, float* out2_host);
 
 /* ---- 3-D refocus augmentation (SURVEY.md 8(f) rank 4; data/refocus_augmentation.py) ------------------------------

@@ -167,6 +167,10 @@ _SIGNATURES = {
     "odb_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,
                                 C.c_float, C.c_float, C.c_float, C.c_int64, C.c_void_p, C.c_void_p]),
     "odb_adam_step_scalars": (C.c_int, [C.c_float, C.c_float, C.c_float, C.c_int64, C.c_void_p]),
+    "odb_clip_grad_norm_segments": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]),
+    "odb_adam_step_segments": (C.c_int, [C.c_void_p] * 5 + [C.c_int32, C.c_int64, C.c_void_p] + [C.c_float] * 4 +
+                               [C.c_int64, C.c_void_p, C.c_void_p]),
     "odb_refocus_quantiles": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
                                         C.c_void_p]),
     "odb_refocus_compose": (C.c_int, [C.c_void_p] * 4 + [C.c_int32] * 4 + [C.c_void_p] * 5),

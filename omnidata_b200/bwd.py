@@ -78,7 +78,8 @@ def colsum(x, out, accumulate: bool = False, batches: int = 1):
 def layernorm_bwd(dy, x, gamma, ds_in, ds_out, ds_copy, dgamma, dbeta, eps: float = 1e-6, accumulate: bool = False,
                   dcolsum=None):
     """`dcolsum` (fp32 [cols], optional): column sums of ds_out, i.e. the bias gradient of the linear layer whose output
-    gradient ds_out is — saves a separate pass over the fp32 stream."""
+    gradient ds_out is — saves a separate pass over the fp32 stream.  dgamma = dbeta = None: a frozen norm (no affine
+    gradients)."""
     _need(x, torch.float32, "x"); _need(ds_out, torch.float32, "ds_out")
     if dcolsum is not None:
         _need(dcolsum, torch.float32, "dcolsum")
@@ -86,12 +87,13 @@ def layernorm_bwd(dy, x, gamma, ds_in, ds_out, ds_copy, dgamma, dbeta, eps: floa
     ws = _scratch(lib().odb_layernorm_bwd_workspace_bytes(cols), x.device)
     _call("odb_layernorm_bwd", {"bytes": x.numel() * (8 + dy.element_size() * 2)}, lib().odb_layernorm_bwd,
           _same_device(dy, x, gamma, ds_in, ds_out, ds_copy, dgamma, dbeta, dcolsum), dy.data_ptr(), x.data_ptr(),
-          gamma.data_ptr(), _ptr(ds_in), ds_out.data_ptr(), _ptr(ds_copy), dgamma.data_ptr(), dbeta.data_ptr(), _ptr(dcolsum),
+          gamma.data_ptr(), _ptr(ds_in), ds_out.data_ptr(), _ptr(ds_copy), _ptr(dgamma), _ptr(dbeta), _ptr(dcolsum),
           ws.data_ptr(), rows, cols, eps,
           1 if accumulate else 0, _dt(dy))
 
 
 def groupnorm_bwd(dy, x, stats, gamma, dx, dgamma, dbeta, mask=None, groups: int = 32, accumulate: bool = False):
+    """dgamma = dbeta = None: dx only (a frozen norm)."""
     b, c = x.shape[0], x.shape[-1]
     hw = x.numel() // (b * c)
     need = lib().odb_groupnorm_bwd_workspace_bytes(b, hw, c, groups)
@@ -100,7 +102,7 @@ def groupnorm_bwd(dy, x, stats, gamma, dx, dgamma, dbeta, mask=None, groups: int
     ws = _scratch(need, x.device)
     _call("odb_groupnorm_bwd", {"bytes": x.element_size() * x.numel() * (5 + 2 * (mask is not None))}, lib().odb_groupnorm_bwd,
           _same_device(dy, mask, x, stats, gamma, dx, dgamma, dbeta), dy.data_ptr(), _ptr(mask), x.data_ptr(), stats.data_ptr(),
-          gamma.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(), b, hw, c, groups,
+          gamma.data_ptr(), dx.data_ptr(), _ptr(dgamma), _ptr(dbeta), ws.data_ptr(), b, hw, c, groups,
           1 if accumulate else 0, _dt(x))
 
 
@@ -153,10 +155,11 @@ def head_tail_fwd(a, w, bias, out, relu: bool):
 
 
 def head_tail_bwd(dout, out, a, w, da, dw, dbias, relu: bool, accumulate: bool = False):
+    """dw = dbias = None: da only (a frozen head tail)."""
     b, h, wd, cs = a.shape
     ws = _scratch(lib().odb_head_tail_bwd_workspace_bytes(w.shape[0]), a.device)
     _call("odb_head_tail_bwd", {}, lib().odb_head_tail_bwd, _same_device(dout, out, a, w, da, dw, dbias), dout.data_ptr(),
-          out.data_ptr(), a.data_ptr(), cs, w.data_ptr(), da.data_ptr(), dw.data_ptr(), dbias.data_ptr(), ws.data_ptr(), b, h,
+          out.data_ptr(), a.data_ptr(), cs, w.data_ptr(), da.data_ptr(), _ptr(dw), _ptr(dbias), ws.data_ptr(), b, h,
           wd, w.shape[0], 1 if relu else 0, 1 if accumulate else 0, _dt(a))
 
 

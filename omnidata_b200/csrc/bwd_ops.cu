@@ -190,7 +190,7 @@ __global__ void __launch_bounds__(256, 1) layernorm_bwd_kernel(const T* __restri
                                                                const float* __restrict__ gamma, const float* __restrict__ ds_in,
                                                                float* __restrict__ ds_out, T* __restrict__ ds_copy,
                                                                float* __restrict__ partial, long long rows, float eps,
-                                                               int want_colsum) {
+                                                               int want_params, int want_colsum) {
   constexpr int COLS = VPL * 256;
   __shared__ float sh[8][COLS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -273,9 +273,10 @@ __global__ void __launch_bounds__(256, 1) layernorm_bwd_kernel(const T* __restri
     for (int i = 0; i < VPL; ++i) { xr[i] = xn[i]; dr[i] = dn[i]; }
     row = next;
   }
-  // block partials of dgamma / dbeta / column sums: 8 warps combined in a fixed order through shared memory
+  // block partials of dgamma / dbeta / column sums: 8 warps combined in a fixed order through shared memory (a frozen
+  // norm, want_params == 0, skips the dgamma / dbeta passes; without column sums either the kernel ends here)
   const int passes = want_colsum ? 3 : 2;
-  for (int pass = 0; pass < passes; ++pass) {
+  for (int pass = want_params ? 0 : 2; pass < passes; ++pass) {
 #pragma unroll
     for (int i = 0; i < VPL; ++i)
 #pragma unroll
@@ -290,12 +291,14 @@ __global__ void __launch_bounds__(256, 1) layernorm_bwd_kernel(const T* __restri
     __syncthreads();
   }
 }
-// dgamma / dbeta / colsum (+)= ordered sum of the block partials [blocks][3][cols]; grid ceil(passes * cols / 32)
+// dgamma / dbeta / colsum (+)= ordered sum of the block partials [blocks][3][cols]; grid ceil((passes - first) * cols / 32)
+// with first = 0, or 2 when dgamma / dbeta are not wanted (NULL)
 __global__ void __launch_bounds__(256) ln_param_reduce_kernel(const float* __restrict__ partial, float* __restrict__ dgamma,
                                                               float* __restrict__ dbeta, float* __restrict__ dcol, int blocks,
                                                               int cols, int accumulate) {
   const int passes = dcol != nullptr ? 3 : 2;
-  const int e = blockIdx.x * 32 + (threadIdx.x & 31);          // pass * cols + column
+  const int first = dgamma != nullptr ? 0 : 2;
+  const int e = (first * cols) + blockIdx.x * 32 + (threadIdx.x & 31);     // pass * cols + column
   const bool active = e < passes * cols;
   const float* src = partial + e;
   double t = ordered_sum8(blocks, active, [&](int b) { return __ldg(src + (long long)b * 3 * cols); });
@@ -399,8 +402,10 @@ __global__ void __launch_bounds__(1024) groupnorm_bwd_coef_kernel(const float* _
     const int g = ch / cpg;
     const double mean = stats[((long long)b * groups + g) * 2], rstd = stats[((long long)b * groups + g) * 2 + 1];
     cf[ch] = (float)(rstd * gamma[ch]);
-    dparam_partial[((long long)b * 2 + 0) * c + ch] = (float)(rstd * (sgx[ch] - mean * sg[ch]));   // dgamma share
-    dparam_partial[((long long)b * 2 + 1) * c + ch] = (float)sg[ch];                               // dbeta share
+    if (dparam_partial != nullptr) {                                                                // NULL: frozen norm
+      dparam_partial[((long long)b * 2 + 0) * c + ch] = (float)(rstd * (sgx[ch] - mean * sg[ch]));   // dgamma share
+      dparam_partial[((long long)b * 2 + 1) * c + ch] = (float)sg[ch];                               // dbeta share
+    }
   }
   for (int g = threadIdx.x; g < groups; g += blockDim.x) {
     const double mean = stats[((long long)b * groups + g) * 2], rstd = stats[((long long)b * groups + g) * 2 + 1];
@@ -740,7 +745,8 @@ __global__ void __launch_bounds__(256) head_tail_fwd_kernel(const T* __restrict_
   }
 }
 // backward: dpre[k] = dout[k] * [out[k] > 0] (or dout if !relu); da[j] = [a[j] > 0] * sum_k dpre[k] w[k][j];
-// per-block partials of dw[k][j] = sum dpre[k] a[j] and db[k] = sum dpre[k]  ->  partial[block][head_c][33]
+// per-block partials of dw[k][j] = sum dpre[k] a[j] and db[k] = sum dpre[k]  ->  partial[block][head_c][33] (partial NULL:
+// da only)
 template <typename T>
 __global__ void __launch_bounds__(256) head_tail_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ out,
                                                             const T* __restrict__ a, int cs, const float* __restrict__ w,
@@ -778,6 +784,7 @@ __global__ void __launch_bounds__(256) head_tail_bwd_kernel(const float* __restr
       for (int j = 4; j < cs / 8; ++j) st8(da + i * cs + j * 8, z);
     }
   }
+  if (partial == nullptr) return;                              // uniform over the block: no parameter gradient wanted
   // block reduction in a fixed order (warp shuffles, then 8 warps through shared memory)
   __shared__ float sh[8][3 * 33];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1198,18 +1205,18 @@ extern "C" int odb_layernorm_bwd(const void* dy, const float* x, const float* ga
                                  void* ds_copy, float* dgamma, float* dbeta, float* dcolsum, void* workspace, int64_t rows,
                                  int32_t cols, float eps, int32_t accumulate, int32_t dtype, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!dy || !x || !gamma || !ds_out || !dgamma || !dbeta || !workspace || rows < 1)
-    return fail(ODB_ERR_INVALID, "layernorm_bwd: bad argument");
+  if (!dy || !x || !gamma || !ds_out || !workspace || rows < 1 || (dgamma == nullptr) != (dbeta == nullptr))
+    return fail(ODB_ERR_INVALID, "layernorm_bwd: bad argument (dgamma and dbeta both NULL or both set)");
   float* partial = static_cast<float*>(workspace);
   int blocks = num_sms();
   if (blocks > kLnBwdMaxBlocks) blocks = kLnBwdMaxBlocks;
   if ((long long)blocks * 8 > rows) blocks = (int)((rows + 7) / 8);
-  const int want_colsum = dcolsum != nullptr;
+  const int want_colsum = dcolsum != nullptr, want_params = dgamma != nullptr;
 #define ODB_LN_BWD(VPL)                                                                                              \
   ODB_DT(dtype, T, "layernorm_bwd",                                                                                  \
          layernorm_bwd_kernel<VPL, T><<<blocks, 256, 0, stream>>>(static_cast<const T*>(dy), x, gamma, ds_in, ds_out, \
                                                                   static_cast<T*>(ds_copy), partial, (long long)rows, eps, \
-                                                                  want_colsum))
+                                                                  want_params, want_colsum))
   switch (cols) {
     case 256: ODB_LN_BWD(1); break;
     case 512: ODB_LN_BWD(2); break;
@@ -1219,9 +1226,12 @@ extern "C" int odb_layernorm_bwd(const void* dy, const float* x, const float* ga
   }
 #undef ODB_LN_BWD
   count_launch();
-  ln_param_reduce_kernel<<<((want_colsum ? 3 : 2) * cols + 31) / 32, 256, 0, stream>>>(partial, dgamma, dbeta, dcolsum, blocks,
-                                                                                       cols, accumulate);
-  count_launch();
+  const int reduced = (want_colsum ? 3 : 2) - (want_params ? 0 : 2);     // partial rows to reduce (0: frozen norm, no colsum)
+  if (reduced > 0) {
+    ln_param_reduce_kernel<<<(reduced * cols + 31) / 32, 256, 0, stream>>>(partial, dgamma, dbeta, dcolsum, blocks, cols,
+                                                                         accumulate);
+    count_launch();
+  }
   return check_launch("layernorm_bwd");
 }
 
@@ -1244,9 +1254,10 @@ extern "C" int odb_groupnorm_bwd(const void* dy, const void* mask, const void* x
                                  void* dx, float* dgamma, float* dbeta, void* workspace, int32_t b, int32_t hw, int32_t c,
                                  int32_t groups, int32_t accumulate, int32_t dtype, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!dy || !x || !stats || !gamma || !dx || !dgamma || !dbeta || !workspace ||
+  if (!dy || !x || !stats || !gamma || !dx || !workspace || (dgamma == nullptr) != (dbeta == nullptr) ||
       odb_groupnorm_bwd_workspace_bytes(b, hw, c, groups) < 0)
-    return fail(ODB_ERR_INVALID, "groupnorm_bwd: bad argument");
+    return fail(ODB_ERR_INVALID, "groupnorm_bwd: bad argument (dgamma and dbeta both NULL or both set)");
+  const bool want_params = dgamma != nullptr;
   int slabs, ppb;
   gn_bwd_plan(hw, c, &slabs, &ppb);
   float* partial = static_cast<float*>(workspace);
@@ -1259,7 +1270,7 @@ extern "C" int odb_groupnorm_bwd(const void* dy, const void* mask, const void* x
   count_launch();
   const int coef_lanes = 1024 / c > 1 ? 1024 / c : 1;
   groupnorm_bwd_coef_kernel<<<b, 1024, (size_t)(2 * c + 2 * groups + 2 * coef_lanes * c) * sizeof(double), stream>>>(
-      partial, stats, gamma, coef, dpar, slabs, hw, c, groups);
+      partial, stats, gamma, coef, want_params ? dpar : nullptr, slabs, hw, c, groups);
   count_launch();
   long long gx = ((long long)hw * (c / 8) + 255) / 256;
   const long long cap = ((long long)num_sms() * 8 + b - 1) / b;
@@ -1271,8 +1282,10 @@ extern "C" int odb_groupnorm_bwd(const void* dy, const void* mask, const void* x
              c, groups));
   count_launch();
   // dgamma / dbeta: ordered sum over the images
-  gn_param_reduce_kernel<<<(c + 255) / 256, 256, 0, stream>>>(dpar, dgamma, dbeta, b, c, accumulate);
-  count_launch();
+  if (want_params) {
+    gn_param_reduce_kernel<<<(c + 255) / 256, 256, 0, stream>>>(dpar, dgamma, dbeta, b, c, accumulate);
+    count_launch();
+  }
   return check_launch("groupnorm_bwd");
 }
 
@@ -1377,17 +1390,21 @@ extern "C" int odb_head_tail_bwd(const float* dout, const float* out, const void
                                  void* da, float* dw, float* dbias, void* workspace, int32_t b, int32_t h, int32_t wd,
                                  int32_t head_c, int32_t relu, int32_t accumulate, int32_t dtype, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!dout || !out || !a || !w || !da || !dw || !dbias || !workspace || b < 1 || h < 1 || wd < 1 || head_c < 1 ||
-      head_c > 3 || channel_stride < 32 || channel_stride % 8)
-    return fail(ODB_ERR_INVALID, "head_tail_bwd: bad argument (head_c <= 3)");
+  if (!dout || !out || !a || !w || !da || !workspace || (dw == nullptr) != (dbias == nullptr) || b < 1 || h < 1 ||
+      wd < 1 || head_c < 1 || head_c > 3 || channel_stride < 32 || channel_stride % 8)
+    return fail(ODB_ERR_INVALID, "head_tail_bwd: bad argument (head_c <= 3; dw and dbias both NULL or both set)");
   const long long ppi = (long long)h * wd;
-  float* partial = static_cast<float*>(workspace);
+  const bool want_params = dw != nullptr;
+  float* partial = want_params ? static_cast<float*>(workspace) : nullptr;
   ODB_DT(dtype, T, "head_tail_bwd",
          head_tail_bwd_kernel<T><<<kHeadBwdBlocks, 256, 0, stream>>>(dout, out, static_cast<const T*>(a), channel_stride, w,
                                                                      static_cast<T*>(da), partial, ppi, b, head_c, relu));
   count_launch();
-  head_param_reduce_kernel<<<(head_c * 33 + 31) / 32, 256, 0, stream>>>(partial, dw, dbias, kHeadBwdBlocks, head_c, accumulate);
-  count_launch();
+  if (want_params) {
+    head_param_reduce_kernel<<<(head_c * 33 + 31) / 32, 256, 0, stream>>>(partial, dw, dbias, kHeadBwdBlocks, head_c,
+                                                                         accumulate);
+    count_launch();
+  }
   return check_launch("head_tail_bwd");
 }
 

@@ -20,6 +20,10 @@ resize (odb_pos_embed_resize_bwd, no atomics).
 torch.autograd of the reference arithmetic.  `differentiable_forward(model, x)` wraps the engine in a
 torch.autograd.Function so that `loss(model(x)).backward()` fills `p.grad` (and `x.grad` when x requires grad) like the
 reference module would.
+requires_grad is honoured per tensor: `backward_plan` walks the network's DAG (_backward_graph) and the backward forms
+only the weight / bias / norm-affine gradients of trainable tensors and only the activation gradients that some trainable
+tensor or x.grad needs; the forward re-packs frozen operands only when they changed.  With every tensor trainable the
+launch sequence is the full one, and every gradient a partial backward forms is bit-identical to the full backward's.
 """
 from __future__ import annotations
 
@@ -60,6 +64,136 @@ def parity_dgrad_operands(wb: torch.Tensor, n_pad: int, mode: str) -> dict:
     return operands
 
 
+_BB = "pretrained.model.patch_embed.backbone."
+_PM = "pretrained.model."
+
+
+def _backward_graph() -> List[Tuple[Tuple[str, ...], Tuple[str, ...], str]]:
+    """The DPT-Hybrid forward as a DAG over the activations whose gradients the backward forms: (parameters, input
+    activations, output activation) per op, in forward order.  "x" is the input image; parameter-free ops (ReLU + add,
+    attention, upsampling, the layer_N taps) carry no parameters.  Tensors no op names (the timm classifier head, the
+    final ViT norm, refinenet4.resConfUnit1) are dead: the output does not depend on them."""
+    ops = []
+
+    def op(params, ins, out):
+        ops.append((tuple(params), tuple(ins), out))
+
+    op([_BB + "stem.conv.weight"], ["x"], "stem.s0")
+    op([_BB + "stem.norm.weight", _BB + "stem.norm.bias"], ["stem.s0"], "stem.out")
+    prev = "stem.out"
+    for s, (_, depth) in enumerate(_STAGES):
+        for b in range(depth):
+            p, t = f"{_BB}stages.{s}.blocks.{b}.", f"s{s}b{b}"
+            for i, (src, dst) in enumerate(((prev, "y1"), ("a1", "y2"), ("a2", "y3")), start=1):
+                op([p + f"conv{i}.weight"], [src if i == 1 else f"{t}.{src}"], f"{t}.{dst}")
+                op([p + f"norm{i}.weight", p + f"norm{i}.bias"], [f"{t}.{dst}"], f"{t}.{('a1', 'a2', 'r')[i - 1]}")
+            skip = prev
+            if b == 0:
+                op([p + "downsample.conv.weight"], [prev], f"{t}.d")
+                op([p + "downsample.norm.weight", p + "downsample.norm.bias"], [f"{t}.d"], f"{t}.dn")
+                skip = f"{t}.dn"
+            op([], [f"{t}.r", skip], f"{t}.out")
+            prev = f"{t}.out"
+        if s < 2:
+            op([], [prev], f"layer_{s + 1}")                        # stage outputs 0 and 1 feed the decoder
+    op([], [prev], "f3")
+    op([_PM + "patch_embed.proj.weight", _PM + "patch_embed.proj.bias", _PM + "cls_token", _PM + "pos_embed"], ["f3"],
+       "vit.x0")
+    for i in range(12):
+        p, v, x = f"{_PM}blocks.{i}.", f"vit{i}.", f"vit.x{i}"
+        op([p + "norm1.weight", p + "norm1.bias"], [x], v + "h1")
+        op([p + "attn.qkv.weight", p + "attn.qkv.bias"], [v + "h1"], v + "qkv")
+        op([], [v + "qkv"], v + "att")
+        op([p + "attn.proj.weight", p + "attn.proj.bias"], [v + "att", x], v + "xm")
+        op([p + "norm2.weight", p + "norm2.bias"], [v + "xm"], v + "h2")
+        op([p + "mlp.fc1.weight", p + "mlp.fc1.bias"], [v + "h2"], v + "u")
+        op([p + "mlp.fc2.weight", p + "mlp.fc2.bias"], [v + "u", v + "xm"], f"vit.x{i + 1}")
+    for n, tokens in ((3, "vit.x9"), (4, "vit.x12")):                # readouts hook blocks 8 and 11
+        q = f"pretrained.act_postprocess{n}."
+        op([q + "0.project.0.weight", q + "0.project.0.bias"], [tokens], f"ro{n}.r")
+        op([q + "3.weight", q + "3.bias"], [f"ro{n}.r"], f"pp{n}.o")
+    op([], ["pp3.o"], "layer_3")
+    op(["pretrained.act_postprocess4.4.weight", "pretrained.act_postprocess4.4.bias"], ["pp4.o"], "layer_4")
+    for n in (1, 2, 3, 4):
+        op([f"scratch.layer{n}_rn.weight"], [f"layer_{n}"], f"rn{n}.o")
+
+    def rcu(n, u, x, out):
+        q = f"scratch.refinenet{n}.resConfUnit{u}."
+        op([q + "conv1.weight", q + "conv1.bias"], [x], f"ff{n}.rcu{u}.t")
+        op([q + "conv2.weight", q + "conv2.bias"], [f"ff{n}.rcu{u}.t", x], out)
+    for n in (4, 3, 2, 1):
+        s_in = "rn4.o"
+        if n < 4:
+            rcu(n, 1, f"rn{n}.o", f"ff{n}.res")
+            op([], [f"ff{n}.res", f"ff{n + 1}.z"], f"ff{n}.s")
+            s_in = f"ff{n}.s"
+        rcu(n, 2, s_in, f"ff{n}.y")
+        op([f"scratch.refinenet{n}.out_conv.weight", f"scratch.refinenet{n}.out_conv.bias"], [f"ff{n}.y"], f"ff{n}.z")
+    op(["scratch.output_conv.0.weight", "scratch.output_conv.0.bias"], ["ff1.z"], "head.h1")
+    op(["scratch.output_conv.2.weight", "scratch.output_conv.2.bias"], ["head.h1"], "head.a")
+    op(["scratch.output_conv.4.weight", "scratch.output_conv.4.bias"], ["head.a"], "out")
+    return ops
+
+
+class BackwardPlan:
+    """What one backward computes.  grad(name): the parameter's gradient is formed (it is trainable); act(name): the
+    gradient w.r.t. that activation of _backward_graph is formed, which is the case iff x.grad is wanted or some
+    trainable tensor lies upstream of it.  `full`: every tensor trainable, the backward's complete launch sequence."""
+
+    def __init__(self, trainable: frozenset, acts: Dict[str, bool], full: bool, want_dx: bool):
+        self.trainable, self.acts, self.full, self.want_dx = trainable, acts, full, want_dx
+
+    def grad(self, name: str) -> bool:
+        return name in self.trainable
+
+    def act(self, name: str) -> bool:
+        return self.acts[name]
+
+
+def backward_plan(param_names, trainable=None, want_dx: bool = False) -> BackwardPlan:
+    """The backward plan for the trainable tensors `trainable` (names; None = all of param_names) and, if want_dx, the
+    gradient w.r.t. the input image."""
+    names = list(param_names)
+    ops = _backward_graph()
+    known = set(names)
+    for params, _, _ in ops:
+        for p in params:
+            if p not in known:
+                raise ValueError(f"backward_plan: parameter {p} of the DPT-Hybrid is missing from param_names")
+    T = frozenset(names) if trainable is None else frozenset(trainable)
+    unknown = T - known
+    if unknown:
+        raise ValueError(f"backward_plan: unknown parameter names {sorted(unknown)[:3]}")
+    up = {"x": bool(want_dx)}
+    for params, ins, out in ops:
+        up[out] = any(p in T for p in params) or any(up[i] for i in ins)
+    return BackwardPlan(T, up, trainable is None or T == known, bool(want_dx))
+
+
+def trainable_segments(names: List[str], sizes: List[int], trainable) -> List[Tuple[int, int]]:
+    """[start, end) ranges of the flat buffers (state_dict order, padded sizes) holding exactly the trainable tensors
+    (slices of adjacent trainable tensors merged): the segment table of the clip and Adam kernels."""
+    segs, off = [], 0
+    for n, s in zip(names, sizes):
+        if n in trainable:
+            if segs and segs[-1][1] == off:
+                segs[-1] = (segs[-1][0], off + s)
+            else:
+                segs.append((off, off + s))
+        off += s
+    return segs
+
+
+def select_buckets(buckets, names: List[str], sizes: List[int], trainable):
+    """The all-reduce buckets (plan_grad_buckets) that hold at least one trainable tensor."""
+    starts, off = [], 0
+    for n, s in zip(names, sizes):
+        if n in trainable:
+            starts.append(off)
+        off += s
+    return [(s, e, tag) for s, e, tag in buckets if any(s <= o < e for o in starts)]
+
+
 class TrainEngine:
     def __init__(self, model: DPTDepthModel, precision: str = "bf16"):
         if model.backbone != "vitb_rn50_384":
@@ -92,6 +226,12 @@ class TrainEngine:
                 self.G[name] = self.flat_grad[off:off + p.numel()].view_as(p.data)
                 off += n
         self.param_names = list(names)
+        self.params = dict(zip(names, params))                       # the model's nn.Parameters (requires_grad, _version)
+        self._plans: Dict[tuple, BackwardPlan] = {}
+        self._packed_sig: Dict[str, tuple] = {}                     # source parameter -> (version, pointer) last packed
+        self._pack_tables: Dict[tuple, bwd.PackTable] = {}
+        self._unpack_cache: Dict[frozenset, dict] = {}
+        self.plane_w = {}
         self.ws = _Workspace(self.device)
         self.bufs = self.ws.bufs
         self._build_layer_table()
@@ -160,8 +300,9 @@ class TrainEngine:
             gp = torch.zeros((n_pad, taps * c), device=self.device, dtype=torch.float32)
             self.gp_layer[k] = gp
             tag = "resnet" if "backbone" in pn else "decoder"
-            groups[tag].append((gp, self.P[pn], self.G[pn], n, c, taps, c, std))
-        self.unpack_tables = {t: bwd.UnpackTable(v) for t, v in groups.items() if v}
+            groups[tag].append((pn, (gp, self.P[pn], self.G[pn], n, c, taps, c, std)))
+        self.unpack_groups = groups
+        self.unpack_tables = {t: bwd.UnpackTable([it for _, it in v]) for t, v in groups.items() if v}
         self.zb = torch.zeros(4096, device=self.device, dtype=torch.float32)               # zero "bias" of the dgrad convs:
         #   selects the straight-line (bias / bias + residual) epilogues of the tensor-core kernel
 
@@ -212,24 +353,63 @@ class TrainEngine:
         pk["head4"] = (P["scratch.output_conv.4.weight"].view(self.C, 32), P["scratch.output_conv.4.bias"])
         return pk
 
+    def _stale(self, trainable) -> set:
+        """Source parameters whose derived forward operands must be (re)built: every trainable one (FlatAdam writes the
+        master weights through raw pointers, bumping no version counter) and every frozen one whose version counter or
+        storage changed since it was last packed (load_state_dict, copy_, re-pointed .data: DPTDepthModel's rule)."""
+        out = set()
+        for name, p in self.params.items():
+            if trainable is None or name in trainable:
+                out.add(name)
+                self._packed_sig.pop(name, None)                    # re-checked if the tensor is frozen later
+            else:
+                sig = (p._version, p.data_ptr())
+                if self._packed_sig.get(name) != sig:
+                    out.add(name)
+                    self._packed_sig[name] = sig
+        return out
+
+    def pack_table_for(self, keys: tuple) -> bwd.PackTable:
+        """The one-launch packing of the GEMM layers `keys` (cached: the table's device copy is made once, outside any
+        CUDA-graph capture)."""
+        if len(keys) == len(self.layers):
+            return self.pack_table
+        tab = self._pack_tables.get(keys)
+        if tab is None:
+            tab = self._pack_tables[keys] = bwd.PackTable(
+                [(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c, std)
+                 for k, pn, n, c, taps, n_pad, std in self.layers if k in keys], self.adt)
+        return tab
+
     @torch.no_grad()
-    def pack(self):
-        """fp32 master weights -> GEMM operands (every step: the optimizer just changed them)."""
-        self.pack_table.run()
+    def pack(self, trainable=None):
+        """fp32 master weights -> GEMM operands.  trainable None: all of them (every step: the optimizer just changed
+        them); else only those of the trainable tensors and of frozen tensors changed since their last packing."""
+        if trainable is None:
+            self._packed_sig.clear()
+        stale = None if trainable is None else self._stale(trainable)
+        fresh = (lambda name: True) if stale is None else (lambda name: name in stale)
+        keys = tuple(k for k, pn, *_ in self.layers if fresh(pn))
+        if keys:
+            self.pack_table_for(keys).run()
         P = self.P
         bb = "pretrained.model.patch_embed.backbone."
         # stem 7x7 (3 input channels): [64,3,7,7] -> standardise -> [64, (ky,kx,c)=147] padded to 160 columns
-        w = P[bb + "stem.conv.weight"]
-        std_, mean = torch.std_mean(w, dim=[1, 2, 3], keepdim=True, unbiased=False)
-        ws = ((w - mean) / (std_ + 1e-8)).permute(0, 2, 3, 1).reshape(64, 147)
-        stem = self.pk["stem_w"]
-        stem.zero_()
-        stem[:, :147].copy_(ws)
-        b2 = self.pk["head2"][1]
-        b2.zero_()
-        b2[:32].copy_(P["scratch.output_conv.2.bias"])
+        if fresh(bb + "stem.conv.weight"):
+            w = P[bb + "stem.conv.weight"]
+            std_, mean = torch.std_mean(w, dim=[1, 2, 3], keepdim=True, unbiased=False)
+            ws = ((w - mean) / (std_ + 1e-8)).permute(0, 2, 3, 1).reshape(64, 147)
+            stem = self.pk["stem_w"]
+            stem.zero_()
+            stem[:, :147].copy_(ws)
+        if fresh("scratch.output_conv.2.bias"):
+            b2 = self.pk["head2"][1]
+            b2.zero_()
+            b2[:32].copy_(P["scratch.output_conv.2.bias"])
         # ProjectReadout Linear(1536 -> 768): token half as a GEMM operand (fwd / bwd), whole matrix for the cls kernel
         for n in (3, 4):
+            if not fresh(f"pretrained.act_postprocess{n}.0.project.0.weight"):
+                continue
             wfull = P[f"pretrained.act_postprocess{n}.0.project.0.weight"]
             self.pk[f"ro{n}_wfull"].copy_(wfull)
             self.pk[f"ro{n}_wtok"].copy_(wfull[:, :768])
@@ -238,16 +418,20 @@ class TrainEngine:
             clsT = self.buf(f"w.ro{n}.clsT", (768, 768), torch.float32)
             clsT.copy_(wfull[:, 768:].t())
         # stride-2 3x3 convolutions: per-parity-plane dgrad operands cut out of the rotated dgrad weight
-        self.plane_w = {}
         for key, mode in (("s1b0.w2", "same"), ("s2b0.w2", "same"), ("pp4s", "sym1")):
+            if key not in keys:
+                continue
             n_pad = self.meta[key][4]
             for plane, op in parity_dgrad_operands(self.W[key][1], n_pad, mode).items():
                 self.plane_w[(key, plane)] = op
 
     # ------------------------------------------------------------------ small helpers
     def _wgrad(self, key: str, views, taps, dy, n_rows: Optional[int] = None):
-        """weight gradient of layer `key` into the flat gradient buffer (through the weight standardisation)."""
+        """weight gradient of layer `key` into the flat gradient buffer (through the weight standardisation); nothing
+        for a frozen weight."""
         pname, n, c, ntaps, n_pad, std = self.meta[key]
+        if not self._plan.grad(pname):
+            return
         if ntaps == 1 and not std and n_pad == n:
             # linear / 1x1 layer without weight standardisation: the packed gradient layout IS the parameter layout
             bwd.conv_wgrad(views, taps, dy, self.G[pname].view(n, c))
@@ -255,6 +439,8 @@ class TrainEngine:
         bwd.conv_wgrad(views, taps, dy, self.gp_layer[key])        # converted to parameter layout by the bucket's unpack launch
 
     def _bias_grad(self, pname: str, dy, n: Optional[int] = None):
+        if not self._plan.grad(pname):
+            return
         g = self.G[pname]
         if n is None or dy.shape[-1] == g.numel():
             bwd.colsum(dy.reshape(-1, dy.shape[-1]), g.view(1, -1))
@@ -263,15 +449,65 @@ class TrainEngine:
             bwd.colsum(dy.reshape(-1, dy.shape[-1]), tmp)
             g.copy_(tmp[0, :g.numel()])
 
+    def _param_grads(self, wname: str, bname: str):
+        """(dgamma, dbeta) outputs of a norm / the head tail: None, None when both are frozen; a frozen one of a pair
+        whose other half trains gets a scratch buffer (the kernels form both or neither)."""
+        tw, tb = self._plan.grad(wname), self._plan.grad(bname)
+        if not (tw or tb):
+            return None, None
+        G = self.G
+        dw = G[wname] if tw else self.buf(f"tmp.dparam_w{G[wname].numel()}", G[wname].shape, torch.float32)
+        db = G[bname] if tb else self.buf(f"tmp.dparam_b{G[bname].numel()}", G[bname].shape, torch.float32)
+        return dw, db
+
+    def plan_for(self, trainable, want_dx: bool) -> BackwardPlan:
+        key = (trainable, bool(want_dx))
+        plan = self._plans.get(key)
+        if plan is None:
+            plan = self._plans[key] = backward_plan(self.param_names, trainable, want_dx)
+        return plan
+
+    def _unpack(self, tag: str, plan: BackwardPlan):
+        """The packed-layout -> parameter-layout conversion of bucket `tag`, for the trainable weights only (one table per
+        trainable set, cached)."""
+        tab = self._unpack_tables_for(plan).get(tag)
+        if tab is not None:
+            tab.run()
+
+    def _unpack_tables_for(self, plan: BackwardPlan) -> dict:
+        if plan.full:
+            return self.unpack_tables
+        tabs = self._unpack_cache.get(plan.trainable)
+        if tabs is None:
+            tabs = {}
+            for tag, v in self.unpack_groups.items():
+                items = [it for pn, it in v if pn in plan.trainable]
+                if items:
+                    tabs[tag] = bwd.UnpackTable(items)
+            self._unpack_cache[plan.trainable] = tabs
+        return tabs
+
+    def prepare(self, trainable=None):
+        """Builds the packing / unpacking tables and the plans of a trainable set up front (a CUDA-graph capture cannot
+        create them)."""
+        for want_dx in (False, True):
+            plan = self.plan_for(trainable, want_dx)
+        self._unpack_tables_for(plan)
+        if trainable is not None:
+            keys = tuple(k for k, pn, *_ in self.layers if pn in trainable)
+            if keys:
+                self.pack_table_for(keys)
+
     def _zb(self, w: torch.Tensor):
         """zero bias vector for a dgrad convolution with weight `w` [n_out][K] (tensor-core path only)."""
         return None if self.fp32 else self.zb[: w.shape[0]]
 
     # ------------------------------------------------------------------ forward (activations kept)
     @torch.no_grad()
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, trainable=None) -> torch.Tensor:
         """The model's forward (the launch sequence of model.dpt_forward) on this step's weights; every activation the
-        backward reads is recorded in self.saved."""
+        backward reads is recorded in self.saved.  trainable (names; None = all): the operands of frozen tensors are
+        re-packed only when those tensors changed (pack)."""
         if not x.is_cuda or x.dim() != 4 or x.shape[1] != 3:
             raise OdbError("TrainEngine.forward: CUDA input [B,3,H,W] required")
         x = x.detach().float().contiguous()
@@ -279,7 +515,7 @@ class TrainEngine:
         if H % 32 or W % 32 or (H // 16) * (W // 16) + 1 > 640:
             raise ValueError("H and W must be multiples of 32 with at most 639 patches")
         gh, gw = H // 16, W // 16
-        self.pack()
+        self.pack(trainable)
         # the patch rows of this step's pos_embed (resized from the fp32 master weights as inference resizes them),
         # replicated per image: the patch GEMM's residual operand
         pos = self.P["pretrained.model.pos_embed"]
@@ -300,8 +536,10 @@ class TrainEngine:
             ops.conv_gemm([dy], taps, w, dx[:, py::2, px::2, :], bias=self._zb(w))
 
     @torch.no_grad()
-    def backward(self, dout: torch.Tensor, on_ready=None, dx: Optional[torch.Tensor] = None):
-        """dout: gradient w.r.t. the forward's output [B,C,H,W] fp32.  Fills self.flat_grad (all 368 tensors).
+    def backward(self, dout: torch.Tensor, on_ready=None, dx: Optional[torch.Tensor] = None, trainable=None):
+        """dout: gradient w.r.t. the forward's output [B,C,H,W] fp32.  Fills self.flat_grad: the slices of the trainable
+        tensors (`trainable`: names; None = all 368, the complete launch sequence).  The slices of frozen tensors are not
+        written, and no work is done that only they or unwanted activations need (backward_plan).
         on_ready(tag) is called when a contiguous range of the flat gradient is final (plan_grad_buckets): the
         data-parallel train step launches that range's all-reduce while the rest of the backward runs.
         dx (optional, fp32 contiguous [B,3,H,W]) receives the gradient w.r.t. the input image."""
@@ -309,108 +547,145 @@ class TrainEngine:
         S, P, G, Wt, buf = self.saved, self.P, self.G, self.W, self.buf
         if S is None:
             raise OdbError("TrainEngine.backward: call forward first")
+        plan = self._plan = self.plan_for(trainable, dx is not None)
+        need, T = plan.act, plan.grad
         B, H, W = S["B"], S["H"], S["W"]
         f32 = torch.float32
         dout = dout.detach().float().contiguous().view(B, self.C, H, W)
         hd = S["head"]
         # ---- head
-        da = buf("g.head_a", hd["a"].shape)
-        bwd.head_tail_bwd(dout, hd["out"], hd["a"], hd["w4"], da, G["scratch.output_conv.4.weight"].view(self.C, 32),
-                          G["scratch.output_conv.4.bias"], self.non_negative)
-        dh1u = buf("g.head_h1u", hd["h1u"].shape)
-        ops.conv3x3(da, Wt["head2"][1], dh1u, bias=self._zb(Wt["head2"][1]))
+        da = dh1 = dpath = None
+        w4, b4 = "scratch.output_conv.4.weight", "scratch.output_conv.4.bias"
+        if need("head.a") or T(w4) or T(b4):
+            da = buf("g.head_a", hd["a"].shape)
+            dw4, db4 = self._param_grads(w4, b4)
+            bwd.head_tail_bwd(dout, hd["out"], hd["a"], hd["w4"], da, None if dw4 is None else dw4.view(self.C, 32), db4,
+                              self.non_negative)
+        if need("head.h1"):
+            dh1u = buf("g.head_h1u", hd["h1u"].shape)
+            ops.conv3x3(da, Wt["head2"][1], dh1u, bias=self._zb(Wt["head2"][1]))
         self._wgrad("head2", [hd["h1u"]], bwd.TAPS_3X3, da)
         self._bias_grad("scratch.output_conv.2.bias", da, n=32)
-        dh1 = buf("g.head_h1", hd["h1"].shape)
-        bwd.upsample2x_bwd(dh1u, dh1)
-        dpath = buf("g.path_1", hd["path_1"].shape)
-        ops.conv3x3(dh1, Wt["head0"][1], dpath, bias=self._zb(Wt["head0"][1]))
+        if need("head.h1"):
+            dh1 = buf("g.head_h1", hd["h1"].shape)
+            bwd.upsample2x_bwd(dh1u, dh1)
+        if need("ff1.z"):
+            dpath = buf("g.path_1", hd["path_1"].shape)
+            ops.conv3x3(dh1, Wt["head0"][1], dpath, bias=self._zb(Wt["head0"][1]))
         self._wgrad("head0", [hd["path_1"]], bwd.TAPS_3X3, dh1)
         self._bias_grad("scratch.output_conv.0.bias", dh1)
 
         # ---- RefineNet fusion blocks
-        def rcu_bwd(n, u_, d_out, dx):
-            """d_out: gradient w.r.t. the RCU output; dx <- gradient w.r.t. its (pre-ReLU) input."""
+        def rcu_bwd(n, u_, d_out, dx, x_name):
+            """d_out: gradient w.r.t. the RCU output; dx <- gradient w.r.t. its (pre-ReLU) input `x_name` when needed."""
             r = S[f"ff{n}.rcu{u_}"]
             p = f"scratch.refinenet{n}.resConfUnit{u_}."
-            dt = buf(f"g.ff{n}_rcu{u_}_t", r["tmid"].shape)
-            ops.conv3x3(d_out, Wt[f"ff{n}.rcu{u_}.c2"][1], dt, bias=self._zb(Wt[f"ff{n}.rcu{u_}.c2"][1]))
+            need_t = need(f"ff{n}.rcu{u_}.t")
+            if need_t:
+                dt = buf(f"g.ff{n}_rcu{u_}_t", r["tmid"].shape)
+                ops.conv3x3(d_out, Wt[f"ff{n}.rcu{u_}.c2"][1], dt, bias=self._zb(Wt[f"ff{n}.rcu{u_}.c2"][1]))
             self._wgrad(f"ff{n}.rcu{u_}.c2", [r["tmid"]], bwd.TAPS_3X3, d_out)
             self._bias_grad(p + "conv2.bias", d_out)
-            bwd.mask_add(dt, dt, mask=r["tmid"])                        # through relu(conv1 + b1)
-            dxr = buf(f"g.ff{n}_rcu{u_}_x", r["x_raw"].shape)
-            ops.conv3x3(dt, Wt[f"ff{n}.rcu{u_}.c1"][1], dxr, bias=self._zb(Wt[f"ff{n}.rcu{u_}.c1"][1]))
-            self._wgrad(f"ff{n}.rcu{u_}.c1", [r["x_relu"]], bwd.TAPS_3X3, dt)
-            self._bias_grad(p + "conv1.bias", dt)
-            bwd.mask_add(dx, dxr, a=d_out, mask=r["x_relu"])            # skip + through relu(x)
+            if need_t:
+                bwd.mask_add(dt, dt, mask=r["tmid"])                    # through relu(conv1 + b1)
+                if need(x_name):
+                    dxr = buf(f"g.ff{n}_rcu{u_}_x", r["x_raw"].shape)
+                    ops.conv3x3(dt, Wt[f"ff{n}.rcu{u_}.c1"][1], dxr, bias=self._zb(Wt[f"ff{n}.rcu{u_}.c1"][1]))
+                self._wgrad(f"ff{n}.rcu{u_}.c1", [r["x_relu"]], bwd.TAPS_3X3, dt)
+                self._bias_grad(p + "conv1.bias", dt)
+            if need(x_name):
+                bwd.mask_add(dx, dxr, a=d_out, mask=r["x_relu"])        # skip + through relu(x)
 
-        dz = buf("g.ff1_z", S["ff1"]["z"].shape)
-        bwd.upsample2x_bwd(dpath, dz)
         d_rn = [None] * 4
+        if need("ff1.z"):
+            dz = buf("g.ff1_z", S["ff1"]["z"].shape)
+            bwd.upsample2x_bwd(dpath, dz)
         for n in (1, 2, 3, 4):
+            if not need(f"ff{n}.z"):                                    # nor anything of the later fusion blocks
+                break
             f = S[f"ff{n}"]
-            dy = buf(f"g.ff{n}_y", f["y"].shape)
-            ops.conv1x1(dz, Wt[f"ff{n}.out"][1], dy, bias=self._zb(Wt[f"ff{n}.out"][1]))
+            dy = None
+            if need(f"ff{n}.y"):
+                dy = buf(f"g.ff{n}_y", f["y"].shape)
+                ops.conv1x1(dz, Wt[f"ff{n}.out"][1], dy, bias=self._zb(Wt[f"ff{n}.out"][1]))
             self._wgrad(f"ff{n}.out", [f["y"]], bwd.TAPS_1, dz)
             self._bias_grad(f"scratch.refinenet{n}.out_conv.bias", dz)
-            ds_ = buf(f"g.ff{n}_s", f["y"].shape)
-            rcu_bwd(n, 2, dy, ds_)
+            if dy is None:
+                continue
+            s_name = "rn4.o" if n == 4 else f"ff{n}.s"
+            ds_ = buf(f"g.ff{n}_s", f["y"].shape) if need(s_name) else None
+            rcu_bwd(n, 2, dy, ds_, s_name)
             if n == 4:
                 d_rn[3] = ds_
             else:
-                dr = buf(f"g.rn{n}_raw", f["y"].shape)
-                rcu_bwd(n, 1, ds_, dr)                                  # res = RCU1(layer_rn): d res = d s
-                d_rn[n - 1] = dr
-                dz = buf(f"g.ff{n + 1}_z", S[f"ff{n + 1}"]["z"].shape)
-                bwd.upsample2x_bwd(ds_, dz)
+                if need(f"ff{n}.res"):
+                    dr = buf(f"g.rn{n}_raw", f["y"].shape) if need(f"rn{n}.o") else None
+                    rcu_bwd(n, 1, ds_, dr, f"rn{n}.o")                  # res = RCU1(layer_rn): d res = d s
+                    d_rn[n - 1] = dr
+                if need(f"ff{n + 1}.z"):
+                    dz = buf(f"g.ff{n + 1}_z", S[f"ff{n + 1}"]["z"].shape)
+                    bwd.upsample2x_bwd(ds_, dz)
         # ---- scratch.layerN_rn
-        d_layers = []
+        d_layers = [None] * 4
         for n in (1, 2, 3, 4):
             l = S["layers"][n - 1]
-            dl = buf(f"g.layer_{n}", l.shape)
-            ops.conv3x3(d_rn[n - 1], Wt[f"rn{n}"][1], dl, bias=self._zb(Wt[f"rn{n}"][1]))
+            if need(f"layer_{n}"):
+                d_layers[n - 1] = buf(f"g.layer_{n}", l.shape)
+                ops.conv3x3(d_rn[n - 1], Wt[f"rn{n}"][1], d_layers[n - 1], bias=self._zb(Wt[f"rn{n}"][1]))
             self._wgrad(f"rn{n}", [l], bwd.TAPS_3X3, d_rn[n - 1])
-            d_layers.append(dl)
         # ---- reassemble: act_postprocess4.4 (stride 2), then the two readouts
         gh, gw, ntok, D = S["gh"], S["gw"], S["ntok"], 768
         u4 = S["ro4"]["o"]
-        du4 = buf("g.pp4", u4.shape)
-        self._dgrad_s2("pp4s", d_layers[3], du4)
+        du4 = None
+        if need("pp4.o"):
+            du4 = buf("g.pp4", u4.shape)
+            self._dgrad_s2("pp4s", d_layers[3], du4)
         planes = [u4[:, py::2, px::2, :] for py in range(2) for px in range(2)]
         self._wgrad("pp4s", planes, ops._parity_taps("sym1"), d_layers[3])
         self._bias_grad("pretrained.act_postprocess4.4.bias", d_layers[3])
 
-        def readout_bwd(n, do):
-            """-> gradient w.r.t. the hooked tokens, activation type [B, ntok, D]."""
+        def readout_bwd(n, do, tokens):
+            """-> gradient w.r.t. the hooked tokens `tokens`, activation type [B, ntok, D] (None when not needed)."""
             r = S[f"ro{n}"]
             pp = f"pretrained.act_postprocess{n}."
-            dr = buf(f"g.ro{n}_r", r["r"].shape)
-            ops.conv1x1(do, Wt[f"pp{n}"][1], dr.view(B, gh, gw, D), bias=self._zb(Wt[f"pp{n}"][1]))
+            need_r = need(f"ro{n}.r")
+            if need_r:
+                dr = buf(f"g.ro{n}_r", r["r"].shape)
+                ops.conv1x1(do, Wt[f"pp{n}"][1], dr.view(B, gh, gw, D), bias=self._zb(Wt[f"pp{n}"][1]))
             self._wgrad(f"pp{n}", [r["r"].view(B, gh, gw, D)], bwd.TAPS_1, do)
             self._bias_grad(pp + "3.bias", do)
+            if not need_r:
+                return None
             bwd.gelu_bwd(dr, r["pre"], dr)
-            dtk = buf(f"g.ro{n}_tok", (B, ntok, D))
-            ops.linear(dr, self.bufs[f"w.ro{n}.tokT"], dtk[:, 1:, :].unsqueeze(1))
-            gw_ = G[pp + "0.project.0.weight"]
+            dtk = None
+            if need(tokens):
+                dtk = buf(f"g.ro{n}_tok", (B, ntok, D))
+                ops.linear(dr, self.bufs[f"w.ro{n}.tokT"], dtk[:, 1:, :].unsqueeze(1))
+            tw, wname = T(pp + "0.project.0.weight"), pp + "0.project.0.weight"
+            gw_ = G[wname]
             gp = self.gp[: D * D].view(D, D)
-            bwd.conv_wgrad([r["tk"][:, 1:, :].unsqueeze(1)], bwd.TAPS_1, dr, gp)
-            gw_[:, :D].copy_(gp)
+            if tw:
+                bwd.conv_wgrad([r["tk"][:, 1:, :].unsqueeze(1)], bwd.TAPS_1, dr, gp)
+                gw_[:, :D].copy_(gp)
             # cls half: cb[b] = W[:, D:] tok[b, 0] + bias, added to every token of image b
             dcb = buf(f"g.ro{n}_cb", (B, D), f32)
             bwd.colsum(dr.view(B, gh * gw, D), dcb, batches=B)
-            bwd.colsum(dcb, G[pp + "0.project.0.bias"].view(1, -1))
-            tok0 = buf(f"ro{n}_tok0", (B, D), f32)
-            tok0.copy_(r["tk"][:, 0, :])
-            bwd.conv_wgrad([tok0.view(1, 1, B, D)], bwd.TAPS_1, dcb.view(1, 1, B, D), gp)
-            gw_[:, D:].copy_(gp)
-            dt0 = buf(f"g.ro{n}_tok0", (B, D), f32)
-            ops.linear(dcb, self.bufs[f"w.ro{n}.clsT"], dt0)
-            dtk[:, 0, :].copy_(dt0)
+            if T(pp + "0.project.0.bias"):
+                bwd.colsum(dcb, G[pp + "0.project.0.bias"].view(1, -1))
+            if tw:
+                tok0 = buf(f"ro{n}_tok0", (B, D), f32)
+                tok0.copy_(r["tk"][:, 0, :])
+                bwd.conv_wgrad([tok0.view(1, 1, B, D)], bwd.TAPS_1, dcb.view(1, 1, B, D), gp)
+                gw_[:, D:].copy_(gp)
+            if dtk is not None:
+                dt0 = buf(f"g.ro{n}_tok0", (B, D), f32)
+                ops.linear(dcb, self.bufs[f"w.ro{n}.clsT"], dt0)
+                dtk[:, 0, :].copy_(dt0)
             return dtk
 
-        dtk4 = readout_bwd(4, du4)
-        dtk3 = readout_bwd(3, d_layers[2])
-        self.unpack_tables["decoder"].run()
+        dtk4 = readout_bwd(4, du4, "vit.x12") if need("pp4.o") else None
+        dtk3 = readout_bwd(3, d_layers[2], "vit.x9") if need("layer_3") else None
+        self._unpack("decoder", plan)
         ready("decoder")
         # ---- ViT blocks (fp32 stream gradient ds, activation-type copy ds16 for the GEMMs)
         pm = "pretrained.model."
@@ -419,63 +694,93 @@ class TrainEngine:
         ds = buf("g.vit_ds", (B, ntok, D), f32)
         ds_b = buf("g.vit_ds_b", (B, ntok, D), f32)
         ds16 = buf("g.vit_ds16", (B, ntok, D)) if not self.fp32 else None
-        bwd.add_cast(None, dtk4, ds, ds16)
+        if need("vit.x12"):
+            bwd.add_cast(None, dtk4, ds, ds16)
         hooked = (8, 11)                                             # blocks whose output gradient gets a readout gradient
         for i in range(11, -1, -1):
-            p = f"{pm}blocks.{i}."
+            p, q = f"{pm}blocks.{i}.", f"vit{i}."
             v = vit[i]
             if i == 5:
                 ready("vit_hi")
+            if not need(f"vit.x{i + 1}"):                            # nothing of this block or below is wanted
+                continue
             if i == 8:                                               # hook after block 8: tokens_8 also feed readout 3
                 bwd.add_cast(ds, dtk3, ds, ds16)
             g16 = ds if self.fp32 else ds16
             # mlp: x_{i+1} = xm + fc2(gelu(fc1(LN2(xm))))
-            dmlp = buf("g.vit_mlp", v["mlp"].shape)
-            ops.linear(g16.view(rows, -1), Wt[f"blk{i}.fc2"][1], dmlp.view(rows, -1), bias=self._zb(Wt[f"blk{i}.fc2"][1]))
+            if need(q + "u"):
+                dmlp = buf("g.vit_mlp", v["mlp"].shape)
+                ops.linear(g16.view(rows, -1), Wt[f"blk{i}.fc2"][1], dmlp.view(rows, -1), bias=self._zb(Wt[f"blk{i}.fc2"][1]))
             self._wgrad(f"blk{i}.fc2", [v["mlp"].view(rows, -1)], bwd.TAPS_1, g16.view(rows, -1))
-            if i in hooked:                                          # else: written by block i+1's norm1 backward
+            if i in hooked and T(p + "mlp.fc2.bias"):                # else: written by block i+1's norm1 backward
                 bwd.colsum(ds.view(rows, -1), G[p + "mlp.fc2.bias"].view(1, -1))
-            bwd.gelu_bwd(dmlp, v["u"], dmlp)
-            dh = buf("g.vit_h", v["h2"].shape)
-            ops.linear(dmlp.view(rows, -1), Wt[f"blk{i}.fc1"][1], dh.view(rows, -1), bias=self._zb(Wt[f"blk{i}.fc1"][1]))
-            self._wgrad(f"blk{i}.fc1", [v["h2"].view(rows, -1)], bwd.TAPS_1, dmlp.view(rows, -1))
-            self._bias_grad(p + "mlp.fc1.bias", dmlp.view(rows, -1))
+            if need(q + "u"):
+                bwd.gelu_bwd(dmlp, v["u"], dmlp)
+                if need(q + "h2"):
+                    dh = buf("g.vit_h", v["h2"].shape)
+                    ops.linear(dmlp.view(rows, -1), Wt[f"blk{i}.fc1"][1], dh.view(rows, -1),
+                               bias=self._zb(Wt[f"blk{i}.fc1"][1]))
+                self._wgrad(f"blk{i}.fc1", [v["h2"].view(rows, -1)], bwd.TAPS_1, dmlp.view(rows, -1))
+                self._bias_grad(p + "mlp.fc1.bias", dmlp.view(rows, -1))
+            if not need(q + "h2"):
+                continue
             # ds_b = gradient at attn.proj's output: its column sums are proj's bias gradient (same pass)
-            bwd.layernorm_bwd(dh, xm[i], P[p + "norm2.weight"], ds, ds_b, ds16, G[p + "norm2.weight"], G[p + "norm2.bias"],
-                              dcolsum=G[p + "attn.proj.bias"])
+            dg, db = self._param_grads(p + "norm2.weight", p + "norm2.bias")
+            bwd.layernorm_bwd(dh, xm[i], P[p + "norm2.weight"], ds, ds_b, ds16, dg, db,
+                              dcolsum=G[p + "attn.proj.bias"] if T(p + "attn.proj.bias") else None)
+            if not need(q + "xm"):
+                continue
             g16 = ds_b if self.fp32 else ds16
             # attention: xm = x_i + proj(attn(qkv(LN1(x_i))))
-            datt = buf("g.vit_att", v["att"].shape)
-            ops.linear(g16.view(rows, -1), Wt[f"blk{i}.proj"][1], datt.view(rows, -1), bias=self._zb(Wt[f"blk{i}.proj"][1]))
+            if need(q + "att"):
+                datt = buf("g.vit_att", v["att"].shape)
+                ops.linear(g16.view(rows, -1), Wt[f"blk{i}.proj"][1], datt.view(rows, -1),
+                           bias=self._zb(Wt[f"blk{i}.proj"][1]))
             self._wgrad(f"blk{i}.proj", [v["att"].view(rows, -1)], bwd.TAPS_1, g16.view(rows, -1))
+            if not need(q + "att"):
+                continue
             dqkv = buf("g.vit_qkv", v["qkv"].shape)
             bwd.attention_bwd(v["qkv"], v["att"], datt, v["lse"], dqkv, heads=12, scale=0.125)
-            ops.linear(dqkv.view(rows, -1), Wt[f"blk{i}.qkv"][1], dh.view(rows, -1), bias=self._zb(Wt[f"blk{i}.qkv"][1]))
+            if need(q + "h1"):
+                ops.linear(dqkv.view(rows, -1), Wt[f"blk{i}.qkv"][1], dh.view(rows, -1), bias=self._zb(Wt[f"blk{i}.qkv"][1]))
             self._wgrad(f"blk{i}.qkv", [v["h1"].view(rows, -1)], bwd.TAPS_1, dqkv.view(rows, -1))
             self._bias_grad(p + "attn.qkv.bias", dqkv.view(rows, -1))
+            if not need(q + "h1"):
+                continue
             # ds = gradient at block i-1's output = at its mlp.fc2 output, unless a hook adds to it first
-            fc2_bias = G[f"{pm}blocks.{i - 1}.mlp.fc2.bias"] if i >= 1 and (i - 1) not in hooked else None
-            bwd.layernorm_bwd(dh, xs[i], P[p + "norm1.weight"], ds_b, ds, ds16, G[p + "norm1.weight"], G[p + "norm1.bias"],
-                              dcolsum=fc2_bias)
+            fc2_bias = f"{pm}blocks.{i - 1}.mlp.fc2.bias"
+            fc2_bias = G[fc2_bias] if i >= 1 and (i - 1) not in hooked and T(fc2_bias) else None
+            dg, db = self._param_grads(p + "norm1.weight", p + "norm1.bias")
+            bwd.layernorm_bwd(dh, xs[i], P[p + "norm1.weight"], ds_b, ds, ds16, dg, db, dcolsum=fc2_bias)
         # ---- tokens: cls / pos_embed, patch projection
-        gpos = G[pm + "pos_embed"]
-        if (gh, gw) == (24, 24):
-            bwd.colsum(ds.view(B, ntok * D), gpos.view(1, -1))
-        else:                                                        # through the forward's resize of the patch rows
-            dgrid = buf("g.pos_rows", (ntok, D), f32)
-            bwd.colsum(ds.view(B, ntok * D), dgrid.view(1, -1))
-            gpos[0, 0].copy_(dgrid[0])
-            bwd.pos_embed_resize_bwd(dgrid[1:], gh, gw, gpos[0, 1:])
-        G[pm + "cls_token"].view(-1).copy_(gpos[0, 0])
-        g16 = ds if self.fp32 else ds16
-        f3 = S["f3"]
-        dtok = g16[:, 1:, :].unsqueeze(1)
-        df3 = buf("g.f3", f3.shape)
-        ops.linear(dtok, Wt["proj"][1], df3.view(B, 1, gh * gw, 1024), bias=self._zb(Wt["proj"][1]))
-        self._wgrad("proj", [f3.view(B, 1, gh * gw, 1024)], bwd.TAPS_1, dtok)
-        tmpb = buf("tmp.projbias", (B, D), f32)
-        bwd.colsum(ds[:, 1:, :], tmpb, batches=B)
-        bwd.colsum(tmpb, G[pm + "patch_embed.proj.bias"].view(1, -1))
+        df3 = None
+        if need("vit.x0"):
+            gpos = G[pm + "pos_embed"]
+            want_pos, want_cls = T(pm + "pos_embed"), T(pm + "cls_token")
+            if (gh, gw) == (24, 24) and want_pos:
+                bwd.colsum(ds.view(B, ntok * D), gpos.view(1, -1))
+                row0 = gpos[0, 0]
+            elif want_pos or want_cls:                               # through the forward's resize of the patch rows
+                dgrid = buf("g.pos_rows", (ntok, D), f32)
+                bwd.colsum(ds.view(B, ntok * D), dgrid.view(1, -1))
+                row0 = dgrid[0]
+                if want_pos:
+                    gpos[0, 0].copy_(dgrid[0])
+                    bwd.pos_embed_resize_bwd(dgrid[1:], gh, gw, gpos[0, 1:])
+                    row0 = gpos[0, 0]
+            if want_cls:
+                G[pm + "cls_token"].view(-1).copy_(row0)
+            g16 = ds if self.fp32 else ds16
+            f3 = S["f3"]
+            dtok = g16[:, 1:, :].unsqueeze(1)
+            if need("f3"):
+                df3 = buf("g.f3", f3.shape)
+                ops.linear(dtok, Wt["proj"][1], df3.view(B, 1, gh * gw, 1024), bias=self._zb(Wt["proj"][1]))
+            self._wgrad("proj", [f3.view(B, 1, gh * gw, 1024)], bwd.TAPS_1, dtok)
+            if T(pm + "patch_embed.proj.bias"):
+                tmpb = buf("tmp.projbias", (B, D), f32)
+                bwd.colsum(ds[:, 1:, :], tmpb, batches=B)
+                bwd.colsum(tmpb, G[pm + "patch_embed.proj.bias"].view(1, -1))
         ready("vit_lo")
 
         # ---- ResNetV2 bottlenecks, last to first
@@ -484,95 +789,129 @@ class TrainEngine:
             tag, p, stride = rec["tag"], rec["p"], rec["stride"]
             s, b = rec["s"], rec["b"]
             # stage outputs also feed the decoder
-            if (s, b) == (1, _STAGES[1][1] - 1):
+            if (s, b) == (1, _STAGES[1][1] - 1) and need("layer_2"):
                 bwd.mask_add(d_out, d_layers[1], a=d_out)
-            if (s, b) == (0, _STAGES[0][1] - 1):
+            if (s, b) == (0, _STAGES[0][1] - 1) and need("layer_1"):
                 bwd.mask_add(d_out, d_layers[0], a=d_out)
+            if not need(f"{tag}.out"):                                # nothing of this block or before it is wanted
+                continue
+            in_name = f"s{s}b{b - 1}.out" if b > 0 else (f"s{s - 1}b{_STAGES[s - 1][1] - 1}.out" if s > 0 else "stem.out")
             out, t_in = rec["out"], rec["t_in"]
             g = buf(f"g.{tag}_g", out.shape)
             bwd.mask_add(g, d_out, mask=out)                             # through the block's final ReLU
-            dy3 = buf(f"g.{tag}_y3", out.shape)
-            bwd.groupnorm_bwd(g, rec["y3"], rec["st3"], P[p + "norm3.weight"], dy3, G[p + "norm3.weight"], G[p + "norm3.bias"])
-            da2 = buf(f"g.{tag}_a2", rec["a2"].shape)
-            ops.conv1x1(dy3, Wt[tag + ".w3"][1], da2, bias=self._zb(Wt[tag + ".w3"][1]))
+            dy3 = dy2 = dy1 = None
+            if need(f"{tag}.r"):
+                dy3 = buf(f"g.{tag}_y3", out.shape)
+                dg, db = self._param_grads(p + "norm3.weight", p + "norm3.bias")
+                bwd.groupnorm_bwd(g, rec["y3"], rec["st3"], P[p + "norm3.weight"], dy3, dg, db)
+            if need(f"{tag}.a2"):
+                da2 = buf(f"g.{tag}_a2", rec["a2"].shape)
+                ops.conv1x1(dy3, Wt[tag + ".w3"][1], da2, bias=self._zb(Wt[tag + ".w3"][1]))
             self._wgrad(tag + ".w3", [rec["a2"]], bwd.TAPS_1, dy3)
-            dy2 = buf(f"g.{tag}_y2", rec["y2"].shape)
-            bwd.groupnorm_bwd(da2, rec["y2"], rec["st2"], P[p + "norm2.weight"], dy2, G[p + "norm2.weight"], G[p + "norm2.bias"],
-                              mask=rec["a2"])
-            da1 = buf(f"g.{tag}_a1", rec["a1"].shape)
+            if need(f"{tag}.a2"):
+                dy2 = buf(f"g.{tag}_y2", rec["y2"].shape)
+                dg, db = self._param_grads(p + "norm2.weight", p + "norm2.bias")
+                bwd.groupnorm_bwd(da2, rec["y2"], rec["st2"], P[p + "norm2.weight"], dy2, dg, db, mask=rec["a2"])
             a1 = rec["a1"]
+            need_a1 = need(f"{tag}.a1")
+            if need_a1:
+                da1 = buf(f"g.{tag}_a1", a1.shape)
             if stride == 1:
-                ops.conv3x3(dy2, Wt[tag + ".w2"][1], da1, bias=self._zb(Wt[tag + ".w2"][1]))
+                if need_a1:
+                    ops.conv3x3(dy2, Wt[tag + ".w2"][1], da1, bias=self._zb(Wt[tag + ".w2"][1]))
                 self._wgrad(tag + ".w2", [a1], bwd.TAPS_3X3, dy2)
             else:
-                self._dgrad_s2(tag + ".w2", dy2, da1)
+                if need_a1:
+                    self._dgrad_s2(tag + ".w2", dy2, da1)
                 planes = [a1[:, py::2, px::2, :] for py in range(2) for px in range(2)]
                 self._wgrad(tag + ".w2", planes, ops._parity_taps("same"), dy2)
-            dy1 = buf(f"g.{tag}_y1", rec["y1"].shape)
-            bwd.groupnorm_bwd(da1, rec["y1"], rec["st1"], P[p + "norm1.weight"], dy1, G[p + "norm1.weight"], G[p + "norm1.bias"],
-                              mask=a1)
-            dt_in = buf(f"g.{tag}_in", t_in.shape)
+            if need_a1:
+                dy1 = buf(f"g.{tag}_y1", rec["y1"].shape)
+                dg, db = self._param_grads(p + "norm1.weight", p + "norm1.bias")
+                bwd.groupnorm_bwd(da1, rec["y1"], rec["st1"], P[p + "norm1.weight"], dy1, dg, db, mask=a1)
+            need_in = need(in_name)
+            dt_in = buf(f"g.{tag}_in", t_in.shape) if need_in else None
             if b == 0:
-                dd = buf(f"g.{tag}_ds", rec["d"].shape)
-                bwd.groupnorm_bwd(g, rec["d"], rec["std"], P[p + "downsample.norm.weight"], dd,
-                                  G[p + "downsample.norm.weight"], G[p + "downsample.norm.bias"])
+                dd = None
+                if need(f"{tag}.dn"):
+                    dd = buf(f"g.{tag}_ds", rec["d"].shape)
+                    dg, db = self._param_grads(p + "downsample.norm.weight", p + "downsample.norm.bias")
+                    bwd.groupnorm_bwd(g, rec["d"], rec["std"], P[p + "downsample.norm.weight"], dd, dg, db)
                 if stride > 1:
-                    dt_in.zero_()
-                    ops.conv1x1(dd, Wt[tag + ".wd"][1], dt_in[:, ::stride, ::stride, :], bias=self._zb(Wt[tag + ".wd"][1]))
+                    if need_in:
+                        dt_in.zero_()
+                        ops.conv1x1(dd, Wt[tag + ".wd"][1], dt_in[:, ::stride, ::stride, :], bias=self._zb(Wt[tag + ".wd"][1]))
                     self._wgrad(tag + ".wd", [t_in[:, ::stride, ::stride, :]], bwd.TAPS_1, dd)
                 else:
-                    ops.conv1x1(dd, Wt[tag + ".wd"][1], dt_in, bias=self._zb(Wt[tag + ".wd"][1]))
+                    if need_in:
+                        ops.conv1x1(dd, Wt[tag + ".wd"][1], dt_in, bias=self._zb(Wt[tag + ".wd"][1]))
                     self._wgrad(tag + ".wd", [t_in], bwd.TAPS_1, dd)
-                ops.conv1x1(dy1, Wt[tag + ".w1"][1], dt_in, residual=dt_in, bias=self._zb(Wt[tag + ".w1"][1]))
-            else:
+                if need_in:
+                    ops.conv1x1(dy1, Wt[tag + ".w1"][1], dt_in, residual=dt_in, bias=self._zb(Wt[tag + ".w1"][1]))
+            elif need_in:
                 ops.conv1x1(dy1, Wt[tag + ".w1"][1], dt_in, residual=g, bias=self._zb(Wt[tag + ".w1"][1]))
             self._wgrad(tag + ".w1", [t_in], bwd.TAPS_1, dy1)
             d_out = dt_in
         # ---- stem
         bb = "pretrained.model.patch_embed.backbone."
-        cols, s0, st0, t = S["stem"]
-        g_s0 = buf("g.stem_gn", s0.shape)
-        bwd.stem_pool_bwd(d_out, s0, st0, P[bb + "stem.norm.weight"], P[bb + "stem.norm.bias"], g_s0)
-        ds0 = buf("g.stem_conv", s0.shape)
-        bwd.groupnorm_bwd(g_s0, s0, st0, P[bb + "stem.norm.weight"], ds0, G[bb + "stem.norm.weight"], G[bb + "stem.norm.bias"])
-        if dx is not None:
-            bwd.stem_input_grad(ds0, self.pk["stem_w"], dx)
-        gp = self.gp[: 64 * 160].view(64, 160)
-        h2, w2 = H // 2, W // 2
-        bwd.conv_wgrad([cols.view(B, h2, w2, 160)], bwd.TAPS_1, ds0, gp)
-        g147 = buf("tmp.stem_g", (64, 147), f32)
-        g147.copy_(gp[:, :147])
-        bwd.unpack_wgrad(g147, P[bb + "stem.conv.weight"], G[bb + "stem.conv.weight"], 64, 3, 49, 3, True)
-        self.unpack_tables["resnet"].run()
+        if need("stem.out"):
+            cols, s0, st0, t = S["stem"]
+            g_s0 = buf("g.stem_gn", s0.shape)
+            bwd.stem_pool_bwd(d_out, s0, st0, P[bb + "stem.norm.weight"], P[bb + "stem.norm.bias"], g_s0)
+            ds0 = buf("g.stem_conv", s0.shape)
+            dg, db = self._param_grads(bb + "stem.norm.weight", bb + "stem.norm.bias")
+            bwd.groupnorm_bwd(g_s0, s0, st0, P[bb + "stem.norm.weight"], ds0, dg, db)
+            if dx is not None:
+                bwd.stem_input_grad(ds0, self.pk["stem_w"], dx)
+            if T(bb + "stem.conv.weight"):
+                gp = self.gp[: 64 * 160].view(64, 160)
+                h2, w2 = H // 2, W // 2
+                bwd.conv_wgrad([cols.view(B, h2, w2, 160)], bwd.TAPS_1, ds0, gp)
+                g147 = buf("tmp.stem_g", (64, 147), f32)
+                g147.copy_(gp[:, :147])
+                bwd.unpack_wgrad(g147, P[bb + "stem.conv.weight"], G[bb + "stem.conv.weight"], 64, 3, 49, 3, True)
+        self._unpack("resnet", plan)
         ready("resnet")
         return self.flat_grad
+
+
+def _trainable_names(names: List[str], flags) -> Optional[frozenset]:
+    """requires-grad flags aligned with names -> the trainable set (None when every tensor trains)."""
+    flags = tuple(bool(f) for f in flags)
+    return None if all(flags) else frozenset(n for n, f in zip(names, flags) if f)
 
 
 class _DptFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, engine, x, *params):
-        out = engine.forward(x)
+        ctx.trainable = _trainable_names(engine.param_names, ctx.needs_input_grad[2:])
+        out = engine.forward(x, trainable=ctx.trainable)
         ctx.engine = engine
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         return out.clone()
 
     @staticmethod
     def backward(ctx, grad_out):
+        """Gradients of the tensors that require grad only: None (no work, no copy) for frozen ones."""
         eng = ctx.engine
+        want = ctx.needs_input_grad[2:]
+        if not ctx.needs_input_grad[1] and not any(want):
+            return (None,) * len(ctx.needs_input_grad)
         dx = None
         if ctx.needs_input_grad[1]:
             B, _, H, W = ctx.x_shape
             dx = torch.empty((B, 3, H, W), device=grad_out.device, dtype=torch.float32)
-        eng.backward(grad_out, dx=dx)
-        grads = tuple(eng.G[n].clone() for n in eng.param_names)
+        eng.backward(grad_out, dx=dx, trainable=ctx.trainable)
+        grads = tuple(eng.G[n].clone() if w else None for n, w in zip(eng.param_names, want))
         if dx is not None:
             dx = dx.reshape(ctx.x_shape).to(ctx.x_dtype)
         return (None, dx) + grads
 
 
 def differentiable_forward(model: DPTDepthModel, x: torch.Tensor) -> torch.Tensor:
-    """model(x) under autograd: returns a tensor whose backward fills p.grad of every parameter and, when x requires
-    grad, x.grad (the gradient w.r.t. the input image, in x's dtype)."""
+    """model(x) under autograd: returns a tensor whose backward fills p.grad of every parameter that requires grad and,
+    when x requires grad, x.grad (the gradient w.r.t. the input image, in x's dtype).  Only those gradients are computed
+    (backward_plan); the GEMM operands of frozen parameters are re-packed only when the parameters change."""
     eng = getattr(model, "_train_engine", None)
     if eng is None or eng.fp32 != (model.precision == "fp32"):
         eng = TrainEngine(model, precision=model.precision)
@@ -610,7 +949,13 @@ class DepthTrainStep:
     """One process per GPU.  step(rgb, depth_gt, mask_float): forward -> clamp + MiDaS SSI + gradient-matching + virtual
     normal loss -> backward -> gradient all-reduce (data parallel, as the reference's PL DDP, train_depth.py:424-426:
     mean over ranks, bucketed, overlapped with the rest of the backward on a communication stream) -> clip_grad_norm_(10)
-    -> Adam(lr) on the flat fp32 master weights (train_depth.py:381-383, Trainer(gradient_clip_val=10))."""
+    -> Adam(lr) on the flat fp32 master weights (train_depth.py:381-383, Trainer(gradient_clip_val=10)).
+
+    The trainable set is the parameters that require grad when the step is constructed (the reference's
+    `Adam(filter(lambda p: p.requires_grad, model.parameters()))`): the backward forms only their gradients, the clip
+    norm and Adam cover only them, only the all-reduce buckets holding them are reduced, and frozen parameters and
+    their moments are never written.  Changing requires_grad afterwards is an error (step() raises ValueError):
+    construct a new step for a new set."""
 
     def __init__(self, model: DPTDepthModel, lr: float = 1e-5, clip: Optional[float] = 10.0, precision: str = "bf16",
                  input_size=(384, 384)):
@@ -618,14 +963,24 @@ class DepthTrainStep:
         from .losses import DepthStepLoss
         from .optim import FlatAdam
         self.engine = TrainEngine(model, precision)
+        eng = self.engine
+        self._flag_params = [eng.params[n] for n in eng.param_names]
+        self._flags = tuple(p.requires_grad for p in self._flag_params)
+        if not any(self._flags):
+            raise ValueError("DepthTrainStep: no parameter requires grad")
+        self.trainable = _trainable_names(eng.param_names, self._flags)
+        sizes = [(eng.P[n].numel() + 3) // 4 * 4 for n in eng.param_names]
+        segments = None if self.trainable is None else trainable_segments(eng.param_names, sizes, self.trainable)
         self.loss = DepthStepLoss(input_size)
-        self.opt = FlatAdam(self.engine.flat, lr=lr)
+        self.opt = FlatAdam(self.engine.flat, lr=lr, segments=segments)
         self.clip = clip
         self.dist = dist if (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1) else None
         self.world = self.dist.get_world_size() if self.dist else 1
-        eng = self.engine
-        sizes = [(eng.P[n].numel() + 3) // 4 * 4 for n in eng.param_names]
         self.buckets = plan_grad_buckets(eng.param_names, sizes)
+        if self.trainable is not None:
+            self.buckets = select_buckets(self.buckets, eng.param_names, sizes, self.trainable)
+        eng.prepare(self.trainable)
+        self._frozen_sig = self._frozen_signature()
         self.comm_stream = torch.cuda.Stream(eng.device) if self.dist else None
         self.global_step = 0
         self.allreduce_bytes = sum(e - s for s, e, _ in self.buckets) * 4 if self.dist else 0
@@ -640,9 +995,10 @@ class DepthTrainStep:
 
     def _allreduce_bucket(self, tag: str):
         """called by the backward when the range `tag` of the flat gradient is final"""
-        if self.dist is None:
+        hit = [(s, e) for s, e, t in self.buckets if t == tag]
+        if self.dist is None or not hit:                          # (a bucket of frozen tensors is not reduced)
             return
-        s, e = next((s, e) for s, e, t in self.buckets if t == tag)
+        s, e = hit[0]
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.engine.device))
         with torch.cuda.stream(self.comm_stream):
@@ -656,6 +1012,9 @@ class DepthTrainStep:
         rgb [B,3,H,W], depth_gt and mask_float [B,1,H,W] with (H, W) = the step's input_size; `points`: host index
         arrays in [0, H*W)."""
         from .losses import check_vnl_points
+        if tuple(p.requires_grad for p in self._flag_params) != self._flags:
+            raise ValueError("DepthTrainStep: requires_grad of the model's parameters changed since the step was "
+                             "constructed; construct a new DepthTrainStep for a new trainable set")
         H, W = self.loss.vnl.input_size
         if rgb.dim() != 4 or tuple(rgb.shape[1:]) != (3, H, W):
             raise ValueError(f"DepthTrainStep: rgb must be [B,3,{H},{W}] (the step's input_size), got {tuple(rgb.shape)}")
@@ -676,9 +1035,9 @@ class DepthTrainStep:
 
     def _launch_sequence(self, rgb, depth_gt, mask_float, points, full_mix: bool, scalars_on_device: bool) -> torch.Tensor:
         eng = self.engine
-        out = eng.forward(rgb)                                        # [B,1,H,W]
+        out = eng.forward(rgb, trainable=self.trainable)              # [B,1,H,W]
         losses, dpred = self.loss(out, depth_gt, mask_float, full_mix=full_mix, points=points)
-        eng.backward(dpred, on_ready=self._allreduce_bucket)
+        eng.backward(dpred, on_ready=self._allreduce_bucket, trainable=self.trainable)
         if self.dist is not None:
             torch.cuda.current_stream(eng.device).wait_stream(self.comm_stream)
         norm = self.opt.step(eng.flat_grad, max_norm=self.clip, scalars_on_device=scalars_on_device)
@@ -725,9 +1084,21 @@ class DepthTrainStep:
         g["scratch"] = bwd._SCRATCH.buf        # the shared kernel workspace the captured launches point into stays alive
         return g
 
+    def _frozen_signature(self):
+        """(version, pointer) of every frozen parameter: the captured step packs only the trainable layers, so a change
+        of a frozen one (load_state_dict, copy_) invalidates the graphs."""
+        if self.trainable is None:
+            return None
+        return tuple((p._version, p.data_ptr()) for n, p in zip(self.engine.param_names, self._flag_params)
+                     if n not in self.trainable)
+
     def _step_graph(self, rgb, depth_gt, mask_float, points, full_mix: bool) -> torch.Tensor:
         if full_mix and points is None:
             points = self.loss.vnl.select_index()                   # host NumPy RNG, the reference's call sequence
+        sig = self._frozen_signature()
+        if sig != self._frozen_sig:
+            self._graphs.clear()                                     # re-captured below, re-packing the changed operands
+            self._frozen_sig = sig
         key = (tuple(rgb.shape), tuple(depth_gt.shape), tuple(mask_float.shape), full_mix)
         g = self._graphs.get(key)
         if g is None:
