@@ -4,7 +4,8 @@ Same constructor / call signatures as the reference modules (losses/midas_loss.p
 losses/virtual_normal_loss.py:7-27,151-194) and the loss mix of train_depth.py:261-279.  MidasLoss and VNL_Loss
 are differentiable with respect to the prediction (odb_midas_loss_bwd / odb_vnl_loss_bwd behind torch.autograd), so
 `depth_step_losses(...)["depth_loss"].backward()` yields d(loss)/d(depth_preds) — the first step of the train
-step's backward pass; so is the normal-training pair (odb_normal_loss_bwd).
+step's backward pass; so is the normal-training pair (odb_normal_loss_bwd).  DepthStepLoss and NormalStepLoss are the
+same arithmetic as one fixed, sync-free launch sequence that also returns d(loss)/d(prediction): the train steps' loss.
 """
 from __future__ import annotations
 
@@ -234,7 +235,18 @@ def check_vnl_points(points, h: int, w: int):
             raise ValueError(f"points: VNL indices must lie in [0, {h * w}) for a {h}x{w} prediction")
 
 
-class DepthStepLoss:
+class _StepBuffers:
+    """Persistent device buffers of a train step's loss, allocated at the first call at a shape and reused after it (no
+    allocation in a CUDA-graph capture or replay)."""
+
+    def _buf(self, name, shape, dtype, device):
+        t = self._bufs.get(name)
+        if t is None or tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != device:
+            t = self._bufs[name] = torch.empty(tuple(shape), dtype=dtype, device=device)
+        return t
+
+
+class DepthStepLoss(_StepBuffers):
     """The loss arithmetic of Depth._shared_step (train_depth.py:261-279) AND its gradient with respect to the raw
     network output, as one fixed launch sequence with no host synchronisation and no autograd graph (the train step's
     hot path; `depth_step_losses` above is the autograd-facing equivalent):
@@ -251,12 +263,6 @@ class DepthStepLoss:
         self.midas = MidasLoss(alpha=alpha, scales=scales)
         self.vnl = VNL_Loss(1.0, 1.0, tuple(input_size))
         self._bufs = {}
-
-    def _buf(self, name, shape, dtype, device):
-        t = self._bufs.get(name)
-        if t is None or tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != device:
-            t = self._bufs[name] = torch.empty(tuple(shape), dtype=dtype, device=device)
-        return t
 
     @_capi.on_tensor_device
     @torch.no_grad()
@@ -319,4 +325,45 @@ class DepthStepLoss:
         dpred = self._buf("dpred", (b, 1, h, w), torch.float32, dev)
         check(lib().odb_clamp01_bwd(p.data_ptr(), gm.data_ptr(), None if gv is None else gv.data_ptr(), dpred.data_ptr(), n,
                                     st), "odb_clamp01_bwd")
+        return losses, dpred
+
+
+class NormalStepLoss(_StepBuffers):
+    """The loss arithmetic of the normal model's _shared_step (train_normal.py:247-265) AND its gradient with respect to
+    the raw network output, as one fixed launch sequence with no host synchronisation, no autograd graph and no
+    allocation after the first call at a shape (the normal train step's hot path; `normal_step_losses` above is the
+    autograd-facing equivalent):
+
+        pc = clamp(pred, 0, 1); mask = make_valid_mask(mask_float) repeated over the 3 channels
+        l1 = masked_l1_loss(pc, gt, mask); cos = masked_cosine_angular_loss(pc, gt, mask)
+        loss = cos + 10 l1
+        d loss / d pred                           (through the clamp)"""
+
+    def __init__(self):
+        self._bufs = {}
+
+    @_capi.on_tensor_device
+    @torch.no_grad()
+    def __call__(self, pred: torch.Tensor, normal_gt: torch.Tensor, mask_float: torch.Tensor):
+        """pred, normal_gt: [B,3,H,W]; mask_float: [B,1,H,W]; fp32 CUDA.  Returns (losses fp32 [3] = (loss, l1, cos),
+        dpred [B,3,H,W])."""
+        if pred.dim() != 4 or pred.shape[1] != 3:
+            raise ValueError(f"NormalStepLoss: prediction must be [B,3,H,W], got {tuple(pred.shape)}")
+        b, _, h, w = pred.shape
+        if tuple(normal_gt.shape) != (b, 3, h, w):
+            raise ValueError(f"NormalStepLoss: normal_gt must be [{b},3,{h},{w}], got {tuple(normal_gt.shape)}")
+        if tuple(mask_float.shape) != (b, 1, h, w):
+            raise ValueError(f"NormalStepLoss: mask_float must be [{b},1,{h},{w}], got {tuple(mask_float.shape)}")
+        p, g, mf = _f32(pred, "pred"), _f32(normal_gt, "normal_gt"), _f32(mask_float, "mask_float")
+        dev = p.device
+        st = torch.cuda.current_stream(dev).cuda_stream
+        m = self._buf("mask", (b, h, w), torch.uint8, dev)
+        check(lib().odb_make_valid_mask(mf.data_ptr(), m.data_ptr(), b, h, w, 4, st), "odb_make_valid_mask")
+        losses = self._buf("losses", (3,), torch.float32, dev)
+        ws = self._buf("ws", (3 * b,), torch.float64, dev)
+        check(lib().odb_normal_loss_fwd(p.data_ptr(), g.data_ptr(), m.data_ptr(), b, h, w, 1, losses.data_ptr(),
+                                        ws.data_ptr(), st), "odb_normal_loss_fwd")
+        dpred = self._buf("dpred", (b, 3, h, w), torch.float32, dev)
+        check(lib().odb_normal_loss_bwd(p.data_ptr(), g.data_ptr(), m.data_ptr(), b, h, w, 1, 10.0, 1.0, ws.data_ptr(),
+                                        dpred.data_ptr(), st), "odb_normal_loss_bwd")
         return losses, dpred

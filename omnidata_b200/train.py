@@ -1,5 +1,8 @@
-"""Train step of the DPT-Hybrid depth model (train_depth.py:183-190 training_step, :261-279 _shared_step, :381-383 Adam,
-:424-426 DDP): differentiable forward + hand-written backward over the kernels of this package.
+"""Train steps of the DPT-Hybrid depth and surface-normal models (train_depth.py:183-190 training_step, :261-279
+_shared_step, :381-383 Adam, :424-426 DDP; train_normal.py:247-265 for the normal loss): differentiable forward +
+hand-written backward over the kernels of this package.  DepthTrainStep (num_channels=1) and NormalTrainStep
+(num_channels=3) differ only in their loss and inputs; engine, trainable set, all-reduce, clip + Adam and CUDA-graph
+capture are _FlatTrainStep's.
 
 `TrainEngine(model)` owns flat fp32 parameter / gradient buffers (the model's nn.Parameters become views), re-packs the
 GEMM operands from the fp32 master weights every step (odb_pack_weight: cast, ResNetV2 weight standardisation, dgrad
@@ -945,33 +948,43 @@ def plan_grad_buckets(names: List[str], sizes: List[int]) -> List[Tuple[int, int
     return [(b_tail, total, "decoder"), (b_blk6, b_tail, "vit_hi"), (b_proj, b_blk6, "vit_lo"), (0, b_proj, "resnet")]
 
 
-class DepthTrainStep:
-    """One process per GPU.  step(rgb, depth_gt, mask_float): forward -> clamp + MiDaS SSI + gradient-matching + virtual
-    normal loss -> backward -> gradient all-reduce (data parallel, as the reference's PL DDP, train_depth.py:424-426:
-    mean over ranks, bucketed, overlapped with the rest of the backward on a communication stream) -> clip_grad_norm_(10)
-    -> Adam(lr) on the flat fp32 master weights (train_depth.py:381-383, Trainer(gradient_clip_val=10)).
+class _FlatTrainStep:
+    """What the fused train steps of the DPT-Hybrid share whatever the task: one process per GPU; forward -> the task's
+    loss and its gradient w.r.t. the network output -> backward -> gradient all-reduce (data parallel, as the reference's
+    PL DDP, train_depth.py:424-426: mean over ranks, bucketed, overlapped with the rest of the backward on a
+    communication stream) -> clip_grad_norm_ -> Adam on the flat fp32 master weights.  step() returns the task's losses
+    followed by the gradient norm before clipping, fp32 on the device, with no host synchronisation.
 
     The trainable set is the parameters that require grad when the step is constructed (the reference's
     `Adam(filter(lambda p: p.requires_grad, model.parameters()))`): the backward forms only their gradients, the clip
     norm and Adam cover only them, only the all-reduce buckets holding them are reduced, and frozen parameters and
     their moments are never written.  Changing requires_grad afterwards is an error (step() raises ValueError):
-    construct a new step for a new set."""
+    construct a new step for a new set.
 
-    def __init__(self, model: DPTDepthModel, lr: float = 1e-5, clip: Optional[float] = 10.0, precision: str = "bf16",
-                 input_size=(384, 384)):
+    A task subclass sets CHANNELS (the model's num_channels it trains) and `self.loss`, validates its inputs, and
+    implements _loss_and_grad; a task with host-side inputs beyond the target tensors stages them for the captured
+    step through _stage_extra / _refill_extra."""
+
+    CHANNELS = 0
+    _RING = 4           # host staging slots: the CPU may run at most _RING - 1 replays ahead of the GPU
+
+    def __init__(self, model: DPTDepthModel, lr: float, clip: Optional[float], precision: str, input_size):
         import torch.distributed as dist
-        from .losses import DepthStepLoss
         from .optim import FlatAdam
+        name = type(self).__name__
+        if model.num_channels != self.CHANNELS:
+            raise ValueError(f"{name} trains a model with num_channels={self.CHANNELS}, got num_channels="
+                             f"{model.num_channels}")
         self.engine = TrainEngine(model, precision)
         eng = self.engine
+        self.input_size = tuple(input_size)
         self._flag_params = [eng.params[n] for n in eng.param_names]
         self._flags = tuple(p.requires_grad for p in self._flag_params)
         if not any(self._flags):
-            raise ValueError("DepthTrainStep: no parameter requires grad")
+            raise ValueError(f"{name}: no parameter requires grad")
         self.trainable = _trainable_names(eng.param_names, self._flags)
         sizes = [(eng.P[n].numel() + 3) // 4 * 4 for n in eng.param_names]
         segments = None if self.trainable is None else trainable_segments(eng.param_names, sizes, self.trainable)
-        self.loss = DepthStepLoss(input_size)
         self.opt = FlatAdam(self.engine.flat, lr=lr, segments=segments)
         self.clip = clip
         self.dist = dist if (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1) else None
@@ -986,9 +999,9 @@ class DepthTrainStep:
         self.allreduce_bytes = sum(e - s for s, e, _ in self.buckets) * 4 if self.dist else 0
         self._hooks_done: Dict[str, torch.cuda.Event] = {}
         # The eager step issues ~1150 launches from Python and is host-bound at batch 16; with use_cuda_graph the whole
-        # launch sequence (forward, loss, backward, clip, Adam) is captured once per (shape, loss mix) and replayed.
-        # Single-process by default; graph_collectives=True also captures the NCCL all-reduces (fork / join of the
-        # communication stream inside the capture).
+        # launch sequence (forward, loss, backward, clip, Adam) is captured once per input shape (and task key) and
+        # replayed.  Single-process by default; graph_collectives=True also captures the NCCL all-reduces (fork / join
+        # of the communication stream inside the capture).
         self.use_cuda_graph = False
         self.graph_collectives = False
         self._graphs: Dict[tuple, dict] = {}
@@ -1005,61 +1018,58 @@ class DepthTrainStep:
             self.comm_stream.wait_event(ev)
             self.dist.all_reduce(self.engine.flat_grad[s:e], op=self.dist.ReduceOp.AVG)
 
-    @torch.no_grad()
-    def step(self, rgb: torch.Tensor, depth_gt: torch.Tensor, mask_float: torch.Tensor, points=None,
-             full_mix: Optional[bool] = None) -> torch.Tensor:
-        """-> fp32 [5] on the device: (loss, ssi, reg, vn, gradient norm before clipping); no host synchronisation.
-        rgb [B,3,H,W], depth_gt and mask_float [B,1,H,W] with (H, W) = the step's input_size; `points`: host index
-        arrays in [0, H*W)."""
-        from .losses import check_vnl_points
+    def _check_trainable_set(self):
         if tuple(p.requires_grad for p in self._flag_params) != self._flags:
-            raise ValueError("DepthTrainStep: requires_grad of the model's parameters changed since the step was "
-                             "constructed; construct a new DepthTrainStep for a new trainable set")
-        H, W = self.loss.vnl.input_size
-        if rgb.dim() != 4 or tuple(rgb.shape[1:]) != (3, H, W):
-            raise ValueError(f"DepthTrainStep: rgb must be [B,3,{H},{W}] (the step's input_size), got {tuple(rgb.shape)}")
-        B = rgb.shape[0]
-        for name, t in (("depth_gt", depth_gt), ("mask_float", mask_float)):
-            if tuple(t.shape[-2:]) != (H, W) or t.numel() != B * H * W:
-                raise ValueError(f"DepthTrainStep: {name} must be [{B},1,{H},{W}], got {tuple(t.shape)}")
-        if points is not None:
-            check_vnl_points(points, H, W)
-        if full_mix is None:
-            full_mix = self.global_step >= 15000                     # train_depth.py:274-279
-        if self.use_cuda_graph and (self.dist is None or self.graph_collectives):
+            name = type(self).__name__
+            raise ValueError(f"{name}: requires_grad of the model's parameters changed since the step was "
+                             f"constructed; construct a new {name} for a new trainable set")
+
+    def _graph_mode(self) -> bool:
+        return self.use_cuda_graph and (self.dist is None or self.graph_collectives)
+
+    def _run(self, rgb, targets: tuple, extra, graph_key: tuple) -> torch.Tensor:
+        """One validated step: rgb and the target tensors, the task's `extra` (passed to _loss_and_grad), and what
+        besides the input shapes selects a captured graph."""
+        if self._graph_mode():
             with torch.cuda.device(self.engine.device):             # capture / replay on the engine's device and stream
-                return self._step_graph(rgb, depth_gt, mask_float, points, bool(full_mix))
-        res = self._launch_sequence(rgb, depth_gt, mask_float, points, bool(full_mix), scalars_on_device=False)
+                return self._step_graph(rgb, targets, extra, graph_key)
+        res = self._launch_sequence(rgb, targets, extra, scalars_on_device=False)
         self.global_step += 1
         return res
 
-    def _launch_sequence(self, rgb, depth_gt, mask_float, points, full_mix: bool, scalars_on_device: bool) -> torch.Tensor:
+    def _loss_and_grad(self, out: torch.Tensor, targets: tuple, extra):
+        """-> (losses fp32 [k], d loss / d out) of the network output `out`."""
+        raise NotImplementedError
+
+    def _launch_sequence(self, rgb, targets: tuple, extra, scalars_on_device: bool) -> torch.Tensor:
         eng = self.engine
-        out = eng.forward(rgb, trainable=self.trainable)              # [B,1,H,W]
-        losses, dpred = self.loss(out, depth_gt, mask_float, full_mix=full_mix, points=points)
+        out = eng.forward(rgb, trainable=self.trainable)              # [B,C,H,W]
+        losses, dpred = self._loss_and_grad(out, targets, extra)
         eng.backward(dpred, on_ready=self._allreduce_bucket, trainable=self.trainable)
         if self.dist is not None:
             torch.cuda.current_stream(eng.device).wait_stream(self.comm_stream)
         norm = self.opt.step(eng.flat_grad, max_norm=self.clip, scalars_on_device=scalars_on_device)
-        res = torch.empty(5, device=eng.device, dtype=torch.float32)
-        res[:4].copy_(losses)
-        res[4:5].copy_(norm.reshape(1) if norm is not None else torch.zeros(1, device=eng.device))
+        k = losses.numel()
+        res = torch.empty(k + 1, device=eng.device, dtype=torch.float32)
+        res[:k].copy_(losses)
+        res[k:k + 1].copy_(norm.reshape(1) if norm is not None else torch.zeros(1, device=eng.device))
         return res
 
     # ------------------------------------------------------------------ captured step
-    _RING = 4           # host staging slots: the CPU may run at most _RING - 1 replays ahead of the GPU
+    def _stage_extra(self, g: dict, extra):
+        """Capture time: device copies of the task's host inputs in graph `g` (and their pinned staging buffers in
+        g["host"]); returns the `extra` the captured launch sequence reads."""
+        return extra
 
-    def _capture(self, key, rgb, depth_gt, mask_float, points, full_mix: bool) -> dict:
+    def _refill_extra(self, g: dict, h: dict, extra):
+        """Before each replay: this step's host inputs through the staging slot `h` into graph `g`'s device copies."""
+
+    def _capture(self, rgb, targets: tuple, extra) -> dict:
         eng, dev = self.engine, self.engine.device
-        g = {"rgb": rgb.detach().float().contiguous().clone(), "gt": depth_gt.detach().float().contiguous().clone(),
-             "mask": mask_float.detach().float().contiguous().clone(), "pts": None, "slot": 0,
-             "host": [dict(scal=torch.zeros(2, dtype=torch.float32).pin_memory(), pts=None, done=None)
-                      for _ in range(self._RING)]}
-        if full_mix:
-            arrs = [np.ascontiguousarray(q, dtype=np.int32) for q in points]
-            g["pts"] = [torch.from_numpy(a).to(dev) for a in arrs]
-            for h in g["host"]:
-                h["pts"] = [torch.empty(a.shape, dtype=torch.int32).pin_memory() for a in arrs]
+        g = {"rgb": rgb.detach().float().contiguous().clone(),
+             "targets": tuple(t.detach().float().contiguous().clone() for t in targets), "slot": 0,
+             "host": [dict(scal=torch.zeros(2, dtype=torch.float32).pin_memory(), done=None) for _ in range(self._RING)]}
+        extra = self._stage_extra(g, extra)
         # one eager step first (workspaces, kernel attributes, NCCL channels): a training step changes the weights and
         # the optimizer state, so both are put back before the capture
         snap = (eng.flat.clone(), self.opt.exp_avg.clone(), self.opt.exp_avg_sq.clone(), self.opt.step_count)
@@ -1068,7 +1078,7 @@ class DepthTrainStep:
         side.wait_stream(cur)
         with torch.cuda.stream(side):
             self.opt.stage_step_scalars(g["host"][0]["scal"])
-            self._launch_sequence(g["rgb"], g["gt"], g["mask"], g["pts"], full_mix, scalars_on_device=True)
+            self._launch_sequence(g["rgb"], g["targets"], extra, scalars_on_device=True)
         cur.wait_stream(side)
         torch.cuda.synchronize(dev)
         eng.flat.copy_(snap[0]); self.opt.exp_avg.copy_(snap[1]); self.opt.exp_avg_sq.copy_(snap[2])
@@ -1079,7 +1089,7 @@ class DepthTrainStep:
         # restrict the capture's error checking to this thread
         mode = "thread_local" if self.dist is not None else "global"
         with torch.cuda.graph(graph, capture_error_mode=mode):
-            g["res"] = self._launch_sequence(g["rgb"], g["gt"], g["mask"], g["pts"], full_mix, scalars_on_device=True)
+            g["res"] = self._launch_sequence(g["rgb"], g["targets"], extra, scalars_on_device=True)
         g["graph"] = graph
         g["scratch"] = bwd._SCRATCH.buf        # the shared kernel workspace the captured launches point into stays alive
         return g
@@ -1092,33 +1102,125 @@ class DepthTrainStep:
         return tuple((p._version, p.data_ptr()) for n, p in zip(self.engine.param_names, self._flag_params)
                      if n not in self.trainable)
 
-    def _step_graph(self, rgb, depth_gt, mask_float, points, full_mix: bool) -> torch.Tensor:
-        if full_mix and points is None:
-            points = self.loss.vnl.select_index()                   # host NumPy RNG, the reference's call sequence
+    def _step_graph(self, rgb, targets: tuple, extra, graph_key: tuple) -> torch.Tensor:
         sig = self._frozen_signature()
         if sig != self._frozen_sig:
             self._graphs.clear()                                     # re-captured below, re-packing the changed operands
             self._frozen_sig = sig
-        key = (tuple(rgb.shape), tuple(depth_gt.shape), tuple(mask_float.shape), full_mix)
+        shapes = (tuple(rgb.shape),) + tuple(tuple(t.shape) for t in targets)
+        key = shapes + tuple(graph_key)
         g = self._graphs.get(key)
         if g is None:
             # the engine's activation buffers are re-allocated when the input shape changes: graphs of other shapes
             # would replay into freed memory
-            for k in [k for k in self._graphs if k[:3] != key[:3]]:
+            for k in [k for k in self._graphs if k[:len(shapes)] != shapes]:
                 del self._graphs[k]
-            g = self._graphs[key] = self._capture(key, rgb, depth_gt, mask_float, points, full_mix)
+            g = self._graphs[key] = self._capture(rgb, targets, extra)
         h = g["host"][g["slot"]]
         g["slot"] = (g["slot"] + 1) % self._RING
         if h["done"] is not None:
             h["done"].synchronize()                                 # the replay that last read this staging slot has run
-        g["rgb"].copy_(rgb); g["gt"].copy_(depth_gt); g["mask"].copy_(mask_float)
-        if full_mix:
-            for dst, hp, q in zip(g["pts"], h["pts"], points):
-                hp.copy_(torch.from_numpy(np.ascontiguousarray(q, dtype=np.int32)))
-                dst.copy_(hp, non_blocking=True)
+        g["rgb"].copy_(rgb)
+        for dst, t in zip(g["targets"], targets):
+            dst.copy_(t)
+        self._refill_extra(g, h, extra)
         self.opt.stage_step_scalars(h["scal"])
         g["graph"].replay()
         h["done"] = torch.cuda.Event()
         h["done"].record(torch.cuda.current_stream(self.engine.device))
         self.global_step += 1
         return g["res"].clone()
+
+
+class DepthTrainStep(_FlatTrainStep):
+    """The train step of the depth model (num_channels=1).  step(rgb, depth_gt, mask_float): forward -> clamp + MiDaS SSI
+    + gradient-matching + virtual normal loss (DepthStepLoss) -> backward -> bucketed gradient all-reduce ->
+    clip_grad_norm_(10) -> Adam(lr) on the flat fp32 master weights (train_depth.py:381-383,
+    Trainer(gradient_clip_val=10)).  Trainable set, data parallelism and CUDA-graph replay: _FlatTrainStep."""
+
+    CHANNELS = 1
+
+    def __init__(self, model: DPTDepthModel, lr: float = 1e-5, clip: Optional[float] = 10.0, precision: str = "bf16",
+                 input_size=(384, 384)):
+        from .losses import DepthStepLoss
+        super().__init__(model, lr, clip, precision, input_size)
+        self.loss = DepthStepLoss(input_size)
+
+    @torch.no_grad()
+    def step(self, rgb: torch.Tensor, depth_gt: torch.Tensor, mask_float: torch.Tensor, points=None,
+             full_mix: Optional[bool] = None) -> torch.Tensor:
+        """-> fp32 [5] on the device: (loss, ssi, reg, vn, gradient norm before clipping); no host synchronisation.
+        rgb [B,3,H,W], depth_gt and mask_float [B,1,H,W] with (H, W) = the step's input_size; `points`: host index
+        arrays in [0, H*W)."""
+        from .losses import check_vnl_points
+        self._check_trainable_set()
+        H, W = self.input_size
+        if rgb.dim() != 4 or tuple(rgb.shape[1:]) != (3, H, W):
+            raise ValueError(f"DepthTrainStep: rgb must be [B,3,{H},{W}] (the step's input_size), got {tuple(rgb.shape)}")
+        B = rgb.shape[0]
+        for name, t in (("depth_gt", depth_gt), ("mask_float", mask_float)):
+            if tuple(t.shape[-2:]) != (H, W) or t.numel() != B * H * W:
+                raise ValueError(f"DepthTrainStep: {name} must be [{B},1,{H},{W}], got {tuple(t.shape)}")
+        if points is not None:
+            check_vnl_points(points, H, W)
+        if full_mix is None:
+            full_mix = self.global_step >= 15000                     # train_depth.py:274-279
+        full_mix = bool(full_mix)
+        if self._graph_mode() and full_mix and points is None:
+            points = self.loss.vnl.select_index()                   # host NumPy RNG, the reference's call sequence
+        return self._run(rgb, (depth_gt, mask_float), (points, full_mix), (full_mix,))
+
+    def _loss_and_grad(self, out, targets, extra):
+        (depth_gt, mask_float), (points, full_mix) = targets, extra
+        return self.loss(out, depth_gt, mask_float, full_mix=full_mix, points=points)
+
+    def _stage_extra(self, g, extra):
+        """the VNL index arrays: device copies the captured loss gathers at, refilled through pinned slots"""
+        points, full_mix = extra
+        g["pts"] = None
+        if full_mix:
+            arrs = [np.ascontiguousarray(q, dtype=np.int32) for q in points]
+            g["pts"] = [torch.from_numpy(a).to(self.engine.device) for a in arrs]
+            for h in g["host"]:
+                h["pts"] = [torch.empty(a.shape, dtype=torch.int32).pin_memory() for a in arrs]
+        return g["pts"], full_mix
+
+    def _refill_extra(self, g, h, extra):
+        points, full_mix = extra
+        if full_mix:
+            for dst, hp, q in zip(g["pts"], h["pts"], points):
+                hp.copy_(torch.from_numpy(np.ascontiguousarray(q, dtype=np.int32)))
+                dst.copy_(hp, non_blocking=True)
+
+
+class NormalTrainStep(_FlatTrainStep):
+    """The train step of the surface-normal model (num_channels=3, hubconf.surface_normal_dpt_hybrid_384).
+    step(rgb, normal_gt, mask_float): forward -> clamp + masked L1 + masked cosine angular loss, loss = cos + 10 l1
+    (NormalStepLoss, the arithmetic of train_normal.py:247-265) -> backward -> bucketed gradient all-reduce ->
+    clip_grad_norm_(clip) -> Adam(lr) on the flat fp32 master weights.  lr and clip default to DepthTrainStep's.
+    Trainable set, data parallelism and CUDA-graph replay: _FlatTrainStep."""
+
+    CHANNELS = 3
+
+    def __init__(self, model: DPTDepthModel, lr: float = 1e-5, clip: Optional[float] = 10.0, precision: str = "bf16",
+                 input_size=(384, 384)):
+        from .losses import NormalStepLoss
+        super().__init__(model, lr, clip, precision, input_size)
+        self.loss = NormalStepLoss()
+
+    @torch.no_grad()
+    def step(self, rgb: torch.Tensor, normal_gt: torch.Tensor, mask_float: torch.Tensor) -> torch.Tensor:
+        """-> fp32 [4] on the device: (loss, l1, cos, gradient norm before clipping); no host synchronisation.
+        rgb and normal_gt [B,3,H,W], mask_float [B,1,H,W] with (H, W) = the step's input_size."""
+        self._check_trainable_set()
+        H, W = self.input_size
+        if rgb.dim() != 4 or tuple(rgb.shape[1:]) != (3, H, W):
+            raise ValueError(f"NormalTrainStep: rgb must be [B,3,{H},{W}] (the step's input_size), got {tuple(rgb.shape)}")
+        B = rgb.shape[0]
+        for name, t, c in (("normal_gt", normal_gt, 3), ("mask_float", mask_float, 1)):
+            if tuple(t.shape) != (B, c, H, W):
+                raise ValueError(f"NormalTrainStep: {name} must be [{B},{c},{H},{W}], got {tuple(t.shape)}")
+        return self._run(rgb, (normal_gt, mask_float), None, ())
+
+    def _loss_and_grad(self, out, targets, extra):
+        return self.loss(out, *targets)
