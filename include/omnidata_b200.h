@@ -299,6 +299,13 @@ int odb_stem_pool_bwd(const void* dt, const void* s0, const float* stats, const 
  * [152, 1024]; ds0 16-byte and dx 8-byte aligned. */
 int odb_stem_input_grad(const void* ds0, const void* weight, float* dx, int32_t b, int32_t h, int32_t w, int32_t kpad,
                         int32_t dtype, void* stream);
+/* Gradient w.r.t. the network's input image of the plain-ViT patch embedding: replaces autograd's input gradient of timm
+ * PatchEmbed.proj = Conv2d(3, D, patch, stride patch) (modules/midas/vit.py:131); the adjoint of odb_patchify.
+ * dcols `dtype` [b * (h/patch) * (w/patch)][3 * patch * patch] (column (c * patch + py) * patch + px) -> dx fp32 NCHW
+ * [b][3][h][w], written (not accumulated).  The patches do not overlap: every dx element is one dcols element (a
+ * permutation, bit-exact).  patch a multiple of 8 dividing h and w; 16-byte aligned pointers. */
+int odb_patch_input_grad(const void* dcols, float* dx, int32_t b, int32_t h, int32_t w, int32_t patch, int32_t dtype,
+                         void* stream);
 /* Gradient of the 24 x 24 position-embedding grid through its resize to a gh x gw patch grid (modules/midas/vit.py:102-116
  * _resize_pos_embed: F.interpolate(mode="bilinear", align_corners=False), torch's index arithmetic): dpos fp32
  * [24*24][d] = the transpose of that map applied to dgrid fp32 [gh*gw][d], written (not accumulated).  Gather form with a

@@ -134,6 +134,22 @@ def stem_input_grad(ds0, w, dx):
           dx.data_ptr(), b, 2 * h2, 2 * w2, w.shape[1], _dt(ds0))
 
 
+def patch_input_grad(dcols, dx, patch: int = 16):
+    """dx fp32 [B,3,H,W] = gradient w.r.t. the image of the plain-ViT patch embedding (the adjoint of ops.patchify), from
+    dcols [B*(H/patch)*(W/patch), 3*patch*patch], the gradient w.r.t. the patch columns."""
+    _need(dx, torch.float32, "dx")
+    b, c, h, w = dx.shape
+    if c != 3 or not dx.is_contiguous():
+        raise _capi.OdbError("patch_input_grad: dx must be a contiguous [B,3,H,W] tensor")
+    if (not dcols.is_contiguous() or h % patch or w % patch
+            or dcols.numel() != b * (h // patch) * (w // patch) * 3 * patch * patch):
+        raise _capi.OdbError(f"patch_input_grad: dcols must be a contiguous [{b}*(H/{patch})*(W/{patch}), "
+                             f"{3 * patch * patch}] tensor")
+    info = {"bytes": dcols.numel() * dcols.element_size() + dx.numel() * 4}
+    _call("odb_patch_input_grad", info, lib().odb_patch_input_grad, _same_device(dcols, dx), dcols.data_ptr(),
+          dx.data_ptr(), b, h, w, patch, _dt(dcols))
+
+
 def pos_embed_resize_bwd(dgrid, gh: int, gw: int, dpos):
     """dpos fp32 [24*24, D] = gradient of the 24 x 24 position-embedding grid through its bilinear resize to gh x gw
     (F.interpolate(mode="bilinear", align_corners=False)), from dgrid fp32 [gh*gw, D], the gradient at the resized rows."""
@@ -286,5 +302,5 @@ def attention_bwd(qkv, o, d_o, lse, dqkv, heads: int = 12, scale: float = 0.125)
 
 
 __all__ = ["mask_add", "gelu_fwd", "gelu_bwd", "colsum", "layernorm_bwd", "groupnorm_bwd", "upsample2x_bwd", "stem_pool_bwd",
-           "stem_input_grad", "pos_embed_resize_bwd", "head_tail_fwd", "head_tail_bwd", "add_cast", "pack_weight", "unpack_wgrad", "conv_wgrad", "attention_bwd",
+           "stem_input_grad", "patch_input_grad", "pos_embed_resize_bwd", "head_tail_fwd", "head_tail_bwd", "add_cast", "pack_weight", "unpack_wgrad", "conv_wgrad", "attention_bwd",
            "TAPS_1", "TAPS_3X3"]

@@ -560,6 +560,30 @@ __global__ void __launch_bounds__(256) stem_pool_bwd_kernel(const T* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------------------ patch-embedding input gradient
+// Adjoint of patchify_kernel (ops.cu; timm PatchEmbed Conv2d(3, D, p, stride p), modules/midas/vit.py:131): dcols
+// [b * gh * gw][3 * p * p] (column (c * p + py) * p + px) -> dx fp32 NCHW [b][3][h][w].  Patches do not overlap, so every
+// dx element is one dcols element: a pure permutation, written once, no sums, no atomics.  Thread = 8 consecutive x of
+// one output row: one 16-byte (bf16) or two 16-byte (fp32) loads, two 16-byte stores.
+template <typename T>
+__global__ void __launch_bounds__(256) patch_input_grad_kernel(const T* __restrict__ dcols, float* __restrict__ dx, int b,
+                                                               int h, int w, int p) {
+  grid_dep_wait();
+  grid_dep_launch();
+  const int gh = h / p, gw = w / p, w8 = w / 8;
+  const long long total = (long long)b * 3 * h * w8;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int x0 = (int)(i % w8) * 8;
+    const long long row = i / w8;                                // (bi * 3 + c) * h + y
+    const int y = (int)(row % h), c = (int)((row / h) % 3), bi = (int)(row / (3LL * h));
+    const int tx = x0 / p, px = x0 - tx * p, ty = y / p, py = y - ty * p;
+    const long long tok = ((long long)bi * gh + ty) * gw + tx;
+    float v[8];
+    ld8(dcols + tok * 3 * p * p + (c * p + py) * p + px, v);
+    st8(dx + row * w + x0, v);
+  }
+}
+
 // ------------------------------------------------------------------------------------------ stem input gradient
 // Gradient of the 7x7 stride-2 TF-SAME stem convolution (timm StdConv2dSame(3, 64, 7, stride 2), padding (2, 3)) w.r.t.
 // its fp32 NCHW input, from ds0 = the gradient w.r.t. its output [b][h/2][w/2][64] and the packed operand the forward
@@ -1353,6 +1377,21 @@ extern "C" int odb_stem_input_grad(const void* ds0, const void* weight, float* d
   if (rc) return rc;
   count_launch();
   return check_launch("stem_input_grad");
+}
+
+extern "C" int odb_patch_input_grad(const void* dcols, float* dx, int32_t b, int32_t h, int32_t w, int32_t patch,
+                                    int32_t dtype, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!dcols || !dx || b < 1 || patch < 8 || patch % 8 || h < patch || w < patch || h % patch || w % patch ||
+      !aligned16(dcols) || !aligned16(dx))
+    return fail(ODB_ERR_INVALID, "patch_input_grad: bad argument (patch a multiple of 8 dividing h and w; 16-byte aligned "
+                                 "pointers)");
+  const unsigned grid = grid_for((long long)b * 3 * h * (w / 8));
+  ODB_DT(dtype, T, "patch_input_grad",
+         launch_pdl(patch_input_grad_kernel<T>, dim3(grid), dim3(256), 0, stream, static_cast<const T*>(dcols), dx, b, h, w,
+                    patch));
+  count_launch();
+  return check_launch("patch_input_grad");
 }
 
 extern "C" int odb_pos_embed_resize_bwd(const float* dgrid, float* dpos, int32_t gh, int32_t gw, int32_t d, void* stream_) {

@@ -402,8 +402,8 @@ class DPTDepthModel(nn.Module):
         B, _, H, W = x.shape
         if H % 32 or W % 32 or (H // 16) * (W // 16) + 1 > 640:
             raise ValueError("H and W must be multiples of 32 with at most 639 patches (384x384 in scope)")
-        if torch.is_grad_enabled() and (self.training or (x.requires_grad and self.backbone == "vitb_rn50_384")):
-            # train() mode under autograd, or (DPT-Hybrid) an input that requires grad in either mode: the
+        if torch.is_grad_enabled() and (self.training or x.requires_grad):
+            # train() mode under autograd, or an input that requires grad in either mode: the
             # differentiable forward (activations kept for the backward kernels).  Any other eval() call, or any call
             # under torch.no_grad(), is the inference path below and returns a tensor that is not attached to an
             # autograd graph
@@ -633,6 +633,7 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
         cols = buf("patch_cols", (B, 1, gh * gw, 3 * 16 * 16))
         ops.patchify(x, cols.view(B * gh * gw, -1), 16)
         ops.linear(cols, pk["proj_w"], xs[0][:, 1:, :].unsqueeze(1), bias=pk["proj_b"], residual=pos_b.unsqueeze(1))
+        S["cols"] = cols
     if taps is not None:
         taps["tokens_in"] = xs[0].clone()
 

@@ -1,4 +1,4 @@
-"""Train steps of the DPT-Hybrid depth and surface-normal models (train_depth.py:183-190 training_step, :261-279
+"""Train steps of the DPT depth and surface-normal models, every backbone (train_depth.py:183-190 training_step, :261-279
 _shared_step, :381-383 Adam, :424-426 DDP; train_normal.py:247-265 for the normal loss): differentiable forward +
 hand-written backward over the kernels of this package.  DepthTrainStep (num_channels=1) and NormalTrainStep
 (num_channels=3) differ only in their loss and inputs; engine, trainable set, all-reduce, clip + Adam and CUDA-graph
@@ -14,7 +14,10 @@ the pre-activations of the fc1 and readout GELUs, and the unfused head's interme
     stride-2 convolutions scatter through parity-plane output views;
   * wgrad = odb_conv_wgrad (wgmma, both operands MN-major straight from the channels-last tensors; fp32 twin);
   * attention backward = odb_attention_bwd; LayerNorm / GroupNorm / GELU / ReLU / bilinear / max-pool / head backward and
-    bias gradients = the kernels of csrc/bwd_ops.cu.
+    bias gradients = the kernels of csrc/bwd_ops.cu;
+  * the plain ViTs' ConvTranspose reassembles: one dgrad and one wgrad with k taps on k row views of the output gradient.
+The DPT-Hybrid (vitb_rn50_384), DPT-Large (vitl16_384) and the plain ViT-B DPT (vitb16_384) share this engine: only the
+front end (ResNetV2 + stem vs patch embedding) and the reassemble of layer_1 / layer_2 are backbone-specific.
 The engine takes every input size inference takes: H and W multiples of 32, at most 639 patches.  Off the pretrained
 24 x 24 patch grid the forward resizes pos_embed's patch rows from this step's fp32 master weights with the function
 inference uses (model.resize_pos_grid), and the backward takes their gradient through the adjoint of that bilinear
@@ -37,7 +40,7 @@ import torch
 
 from . import bwd, ops
 from ._capi import OdbError
-from .model import _STAGES, DPTDepthModel, _Workspace, dpt_forward, resize_pos_grid
+from .model import _ARCH, _STAGES, DPTDepthModel, _Workspace, dpt_forward, resize_pos_grid
 
 
 def _parity_dgrad_plan(mode: str):
@@ -71,16 +74,47 @@ _BB = "pretrained.model.patch_embed.backbone."
 _PM = "pretrained.model."
 
 
-def _backward_graph() -> List[Tuple[Tuple[str, ...], Tuple[str, ...], str]]:
-    """The DPT-Hybrid forward as a DAG over the activations whose gradients the backward forms: (parameters, input
-    activations, output activation) per op, in forward order.  "x" is the input image; parameter-free ops (ReLU + add,
-    attention, upsampling, the layer_N taps) carry no parameters.  Tensors no op names (the timm classifier head, the
-    final ViT norm, refinenet4.resConfUnit1) are dead: the output does not depend on them."""
+def _backward_graph(arch: dict) -> List[Tuple[Tuple[str, ...], Tuple[str, ...], str]]:
+    """The DPT forward of backbone `arch` (model._ARCH) as a DAG over the activations whose gradients the backward forms:
+    (parameters, input activations, output activation) per op, in forward order.  "x" is the input image; parameter-free
+    ops (ReLU + add, attention, upsampling, the layer_N taps) carry no parameters.  Tensors no op names (the timm
+    classifier head, the final ViT norm, refinenet4.resConfUnit1) are dead: the output does not depend on them."""
     ops = []
 
     def op(params, ins, out):
         ops.append((tuple(params), tuple(ins), out))
 
+    if arch["hybrid"]:
+        _resnet_graph(op)
+    else:
+        op([_PM + "patch_embed.proj.weight", _PM + "patch_embed.proj.bias", _PM + "cls_token", _PM + "pos_embed"], ["x"],
+           "vit.x0")
+    for i in range(arch["depth"]):
+        p, v, x = f"{_PM}blocks.{i}.", f"vit{i}.", f"vit.x{i}"
+        op([p + "norm1.weight", p + "norm1.bias"], [x], v + "h1")
+        op([p + "attn.qkv.weight", p + "attn.qkv.bias"], [v + "h1"], v + "qkv")
+        op([], [v + "qkv"], v + "att")
+        op([p + "attn.proj.weight", p + "attn.proj.bias"], [v + "att", x], v + "xm")
+        op([p + "norm2.weight", p + "norm2.bias"], [v + "xm"], v + "h2")
+        op([p + "mlp.fc1.weight", p + "mlp.fc1.bias"], [v + "h2"], v + "u")
+        op([p + "mlp.fc2.weight", p + "mlp.fc2.bias"], [v + "u", v + "xm"], f"vit.x{i + 1}")
+    readouts = (3, 4) if arch["hybrid"] else (1, 2, 3, 4)
+    for n, hook in zip(readouts, arch["hooks"]):
+        q = f"pretrained.act_postprocess{n}."
+        op([q + "0.project.0.weight", q + "0.project.0.bias"], [f"vit.x{hook + 1}"], f"ro{n}.r")
+        op([q + "3.weight", q + "3.bias"], [f"ro{n}.r"], f"pp{n}.o")
+    if not arch["hybrid"]:                                           # the ConvTranspose reassembles of layer_1 / layer_2
+        for n in (1, 2):
+            q = f"pretrained.act_postprocess{n}."
+            op([q + "4.weight", q + "4.bias"], [f"pp{n}.o"], f"layer_{n}")
+    op([], ["pp3.o"], "layer_3")
+    op(["pretrained.act_postprocess4.4.weight", "pretrained.act_postprocess4.4.bias"], ["pp4.o"], "layer_4")
+    _decoder_graph(op)
+    return ops
+
+
+def _resnet_graph(op):
+    """The DPT-Hybrid's ResNetV2 stem and stages, then its 1x1 patch projection (the front end of _backward_graph)."""
     op([_BB + "stem.conv.weight"], ["x"], "stem.s0")
     op([_BB + "stem.norm.weight", _BB + "stem.norm.bias"], ["stem.s0"], "stem.out")
     prev = "stem.out"
@@ -102,21 +136,10 @@ def _backward_graph() -> List[Tuple[Tuple[str, ...], Tuple[str, ...], str]]:
     op([], [prev], "f3")
     op([_PM + "patch_embed.proj.weight", _PM + "patch_embed.proj.bias", _PM + "cls_token", _PM + "pos_embed"], ["f3"],
        "vit.x0")
-    for i in range(12):
-        p, v, x = f"{_PM}blocks.{i}.", f"vit{i}.", f"vit.x{i}"
-        op([p + "norm1.weight", p + "norm1.bias"], [x], v + "h1")
-        op([p + "attn.qkv.weight", p + "attn.qkv.bias"], [v + "h1"], v + "qkv")
-        op([], [v + "qkv"], v + "att")
-        op([p + "attn.proj.weight", p + "attn.proj.bias"], [v + "att", x], v + "xm")
-        op([p + "norm2.weight", p + "norm2.bias"], [v + "xm"], v + "h2")
-        op([p + "mlp.fc1.weight", p + "mlp.fc1.bias"], [v + "h2"], v + "u")
-        op([p + "mlp.fc2.weight", p + "mlp.fc2.bias"], [v + "u", v + "xm"], f"vit.x{i + 1}")
-    for n, tokens in ((3, "vit.x9"), (4, "vit.x12")):                # readouts hook blocks 8 and 11
-        q = f"pretrained.act_postprocess{n}."
-        op([q + "0.project.0.weight", q + "0.project.0.bias"], [tokens], f"ro{n}.r")
-        op([q + "3.weight", q + "3.bias"], [f"ro{n}.r"], f"pp{n}.o")
-    op([], ["pp3.o"], "layer_3")
-    op(["pretrained.act_postprocess4.4.weight", "pretrained.act_postprocess4.4.bias"], ["pp4.o"], "layer_4")
+
+
+def _decoder_graph(op):
+    """scratch.layerN_rn, the RefineNet fusion blocks and the head (the back end of _backward_graph)."""
     for n in (1, 2, 3, 4):
         op([f"scratch.layer{n}_rn.weight"], [f"layer_{n}"], f"rn{n}.o")
 
@@ -135,7 +158,6 @@ def _backward_graph() -> List[Tuple[Tuple[str, ...], Tuple[str, ...], str]]:
     op(["scratch.output_conv.0.weight", "scratch.output_conv.0.bias"], ["ff1.z"], "head.h1")
     op(["scratch.output_conv.2.weight", "scratch.output_conv.2.bias"], ["head.h1"], "head.a")
     op(["scratch.output_conv.4.weight", "scratch.output_conv.4.bias"], ["head.a"], "out")
-    return ops
 
 
 class BackwardPlan:
@@ -153,16 +175,16 @@ class BackwardPlan:
         return self.acts[name]
 
 
-def backward_plan(param_names, trainable=None, want_dx: bool = False) -> BackwardPlan:
-    """The backward plan for the trainable tensors `trainable` (names; None = all of param_names) and, if want_dx, the
-    gradient w.r.t. the input image."""
+def backward_plan(param_names, trainable=None, want_dx: bool = False, backbone: str = "vitb_rn50_384") -> BackwardPlan:
+    """The backward plan of the DPT with encoder `backbone` for the trainable tensors `trainable` (names; None = all of
+    param_names) and, if want_dx, the gradient w.r.t. the input image."""
     names = list(param_names)
-    ops = _backward_graph()
+    ops = _backward_graph(_ARCH[backbone])
     known = set(names)
     for params, _, _ in ops:
         for p in params:
             if p not in known:
-                raise ValueError(f"backward_plan: parameter {p} of the DPT-Hybrid is missing from param_names")
+                raise ValueError(f"backward_plan: parameter {p} of the {backbone} DPT is missing from param_names")
     T = frozenset(names) if trainable is None else frozenset(trainable)
     unknown = T - known
     if unknown:
@@ -199,11 +221,14 @@ def select_buckets(buckets, names: List[str], sizes: List[int], trainable):
 
 class TrainEngine:
     def __init__(self, model: DPTDepthModel, precision: str = "bf16"):
-        if model.backbone != "vitb_rn50_384":
-            raise NotImplementedError("the train step is built for the DPT-Hybrid depth / normal model (vitb_rn50_384)")
         if precision not in ("bf16", "fp32"):
             raise ValueError("precision must be 'bf16' or 'fp32'")
         self.model = model
+        self.backbone, self.hybrid = model.backbone, model.arch["hybrid"]
+        self.D, self.heads, self.depth, self.hooks = (model.arch[k] for k in ("embed", "heads", "depth", "hooks"))
+        self.rn_in, self.rn_pad = model.arch["rn_in"], model._rn_pad
+        # the readouts the hooked blocks feed, in hook order (act_postprocess1..4; the hybrid's layer_1/2 come from ResNetV2)
+        self.readouts = (3, 4) if self.hybrid else (1, 2, 3, 4)
         self.precision = precision
         self.fp32 = precision == "fp32"
         self.adt = torch.float32 if self.fp32 else torch.bfloat16
@@ -247,63 +272,78 @@ class TrainEngine:
 
     # ------------------------------------------------------------------ weight table / per-step packing
     def _build_layer_table(self):
-        """(key, param name, n, c, taps, n_pad, standardize) for every GEMM weight; fwd [n_pad][taps*c],
-        bwd [c][taps*n_pad] operand buffers are allocated once and re-filled every step."""
+        """(key, param name, n, c, taps, n_pad, c_pad, standardize) for every GEMM weight, the parameter read as
+        [n][c][taps]; fwd [n_pad][taps*c_pad], bwd [c_pad][taps*n_pad] operand buffers are allocated once and re-filled
+        every step.  Padded rows / columns are zero and their gradients are dropped by the unpack pass."""
         T = []
-        bb = "pretrained.model.patch_embed.backbone."
-        cin = 64
-        for s, (cout, depth) in enumerate(_STAGES):
-            mid = cout // 4
-            for b in range(depth):
-                p = f"{bb}stages.{s}.blocks.{b}."
-                if b == 0:
-                    T.append((f"s{s}b{b}.wd", p + "downsample.conv.weight", cout, cin, 1, cout, True))
-                T.append((f"s{s}b{b}.w1", p + "conv1.weight", mid, cin if b == 0 else cout, 1, mid, True))
-                T.append((f"s{s}b{b}.w2", p + "conv2.weight", mid, mid, 9, mid, True))
-                T.append((f"s{s}b{b}.w3", p + "conv3.weight", cout, mid, 1, cout, True))
-            cin = cout
         pm = "pretrained.model."
-        T.append(("proj", pm + "patch_embed.proj.weight", 768, 1024, 1, 768, False))
-        for i in range(12):
+        D = self.D
+        if self.hybrid:
+            bb = "pretrained.model.patch_embed.backbone."
+            cin = 64
+            for s, (cout, depth) in enumerate(_STAGES):
+                mid = cout // 4
+                for b in range(depth):
+                    p = f"{bb}stages.{s}.blocks.{b}."
+                    if b == 0:
+                        T.append((f"s{s}b{b}.wd", p + "downsample.conv.weight", cout, cin, 1, cout, cin, True))
+                    c1 = cin if b == 0 else cout
+                    T.append((f"s{s}b{b}.w1", p + "conv1.weight", mid, c1, 1, mid, c1, True))
+                    T.append((f"s{s}b{b}.w2", p + "conv2.weight", mid, mid, 9, mid, mid, True))
+                    T.append((f"s{s}b{b}.w3", p + "conv3.weight", cout, mid, 1, cout, mid, True))
+                cin = cout
+            T.append(("proj", pm + "patch_embed.proj.weight", D, 1024, 1, D, 1024, False))
+        else:                                                        # Conv2d(3, D, 16, stride 16) over patchify's columns
+            T.append(("proj", pm + "patch_embed.proj.weight", D, 768, 1, D, 768, False))
+        for i in range(self.depth):
             p = f"{pm}blocks.{i}."
-            T.append((f"blk{i}.qkv", p + "attn.qkv.weight", 2304, 768, 1, 2304, False))
-            T.append((f"blk{i}.proj", p + "attn.proj.weight", 768, 768, 1, 768, False))
-            T.append((f"blk{i}.fc1", p + "mlp.fc1.weight", 3072, 768, 1, 3072, False))
-            T.append((f"blk{i}.fc2", p + "mlp.fc2.weight", 768, 3072, 1, 768, False))
-        for n in (3, 4):
-            T.append((f"pp{n}", f"pretrained.act_postprocess{n}.3.weight", 768, 768, 1, 768, False))
-        T.append(("pp4s", "pretrained.act_postprocess4.4.weight", 768, 768, 9, 768, False))
-        for n, c in zip((1, 2, 3, 4), (256, 512, 768, 768)):
-            T.append((f"rn{n}", f"scratch.layer{n}_rn.weight", 256, c, 9, 256, False))
+            T.append((f"blk{i}.qkv", p + "attn.qkv.weight", 3 * D, D, 1, 3 * D, D, False))
+            T.append((f"blk{i}.proj", p + "attn.proj.weight", D, D, 1, D, D, False))
+            T.append((f"blk{i}.fc1", p + "mlp.fc1.weight", 4 * D, D, 1, 4 * D, D, False))
+            T.append((f"blk{i}.fc2", p + "mlp.fc2.weight", D, 4 * D, 1, D, 4 * D, False))
+        for n in self.readouts:
+            c, cp = self.rn_in[n - 1], self.rn_pad[n - 1]
+            T.append((f"pp{n}", f"pretrained.act_postprocess{n}.3.weight", c, D, 1, cp, D, False))
+        if not self.hybrid:
+            # ConvTranspose2d(c, c, k, stride k), weight [in][out][k][k] read as n = in, c = out, taps = (ky, kx): fwd
+            # [in][(ky, kx, out)] is the input-gradient operand, bwd's tap blocks are the forward's per-phase 1x1 operands
+            for n, k in ((1, 4), (2, 2)):
+                c, cp = self.rn_in[n - 1], self.rn_pad[n - 1]
+                T.append((f"pp{n}t", f"pretrained.act_postprocess{n}.4.weight", c, c, k * k, cp, cp, False))
+        T.append(("pp4s", "pretrained.act_postprocess4.4.weight", D, D, 9, D, D, False))
+        for n in (1, 2, 3, 4):
+            c, cp = self.rn_in[n - 1], self.rn_pad[n - 1]
+            T.append((f"rn{n}", f"scratch.layer{n}_rn.weight", 256, c, 9, 256, cp, False))
         for n in (1, 2, 3, 4):
             p = f"scratch.refinenet{n}."
-            T.append((f"ff{n}.out", p + "out_conv.weight", 256, 256, 1, 256, False))
+            T.append((f"ff{n}.out", p + "out_conv.weight", 256, 256, 1, 256, 256, False))
             for u in ((2,) if n == 4 else (1, 2)):
                 for cv in (1, 2):
-                    T.append((f"ff{n}.rcu{u}.c{cv}", f"{p}resConfUnit{u}.conv{cv}.weight", 256, 256, 9, 256, False))
-        T.append(("head0", "scratch.output_conv.0.weight", 128, 256, 9, 128, False))
-        T.append(("head2", "scratch.output_conv.2.weight", 32, 128, 9, 64, False))     # carried zero-padded to 64
+                    T.append((f"ff{n}.rcu{u}.c{cv}", f"{p}resConfUnit{u}.conv{cv}.weight", 256, 256, 9, 256, 256, False))
+        T.append(("head0", "scratch.output_conv.0.weight", 128, 256, 9, 128, 256, False))
+        T.append(("head2", "scratch.output_conv.2.weight", 32, 128, 9, 64, 128, False))     # carried zero-padded to 64
         self.layers = T
         self.W: Dict[str, Tuple[torch.Tensor, torch.Tensor]] = {}
-        for key, pname, n, c, taps, n_pad, std in T:
-            fwd = torch.zeros((n_pad, taps * c), device=self.device, dtype=self.adt)
-            bwd_ = torch.zeros((c, taps * n_pad), device=self.device, dtype=self.adt)
+        for key, pname, n, c, taps, n_pad, c_pad, std in T:
+            fwd = torch.zeros((n_pad, taps * c_pad), device=self.device, dtype=self.adt)
+            bwd_ = torch.zeros((c_pad, taps * n_pad), device=self.device, dtype=self.adt)
             self.W[key] = (fwd, bwd_)
-        self.meta = {key: (pname, n, c, taps, n_pad, std) for key, pname, n, c, taps, n_pad, std in T}
-        self.gp = torch.empty(768 * 9 * 768, device=self.device, dtype=torch.float32)     # packed-layout wgrad scratch
+        self.meta = {key: (pname, n, c, taps, n_pad, c_pad, std) for key, pname, n, c, taps, n_pad, c_pad, std in T}
+        # packed-layout wgrad scratch (the readouts' Linear halves, the stem)
+        self.gp = torch.empty(D * 9 * D, device=self.device, dtype=torch.float32)
         # one-launch packing of all layers; packed-layout gradient buffers of the layers that need the unpack pass
-        # (3x3 taps or weight standardisation), converted by ONE launch per all-reduce bucket
-        self.pack_table = bwd.PackTable([(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c, std)
-                                         for k, pn, n, c, taps, n_pad, std in T], self.adt)
+        # (3x3 taps, weight standardisation or padding), converted by ONE launch per all-reduce bucket
+        self.pack_table = bwd.PackTable([(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c_pad, std)
+                                         for k, pn, n, c, taps, n_pad, c_pad, std in T], self.adt)
         self.gp_layer: Dict[str, torch.Tensor] = {}
         groups = {"decoder": [], "resnet": []}
-        for k, pn, n, c, taps, n_pad, std in T:
-            if taps == 1 and not std and n_pad == n:
+        for k, pn, n, c, taps, n_pad, c_pad, std in T:
+            if taps == 1 and not std and n_pad == n and c_pad == c:
                 continue                                           # written straight into the flat gradient
-            gp = torch.zeros((n_pad, taps * c), device=self.device, dtype=torch.float32)
+            gp = torch.zeros((n_pad, taps * c_pad), device=self.device, dtype=torch.float32)
             self.gp_layer[k] = gp
             tag = "resnet" if "backbone" in pn else "decoder"
-            groups[tag].append((pn, (gp, self.P[pn], self.G[pn], n, c, taps, c, std)))
+            groups[tag].append((pn, (gp, self.P[pn], self.G[pn], n, c, taps, c_pad, std)))
         self.unpack_groups = groups
         self.unpack_tables = {t: bwd.UnpackTable([it for _, it in v]) for t, v in groups.items() if v}
         self.zb = torch.zeros(4096, device=self.device, dtype=torch.float32)               # zero "bias" of the dgrad convs:
@@ -314,36 +354,44 @@ class TrainEngine:
         operands pack() refills in place, and views of the flat fp32 master weights (biases, norm affines, cls, pos)."""
         P = self.P
         fw = lambda key: self.W[key][0]
-        bb = "pretrained.model.patch_embed.backbone."
-        pk = {"stem_w": self.buf("w.stem", (64, 160)), "stem_g": P[bb + "stem.norm.weight"],
-              "stem_b": P[bb + "stem.norm.bias"]}
-        blocks = []
-        for s, (cout, depth) in enumerate(_STAGES):
-            for b in range(depth):
-                p, tag = f"{bb}stages.{s}.blocks.{b}.", f"s{s}b{b}"
-                e = {"stride": 2 if (b == 0 and s > 0) else 1, "cout": cout, "mid": cout // 4}
-                if b == 0:
-                    e.update(wd=fw(tag + ".wd"), gd=P[p + "downsample.norm.weight"], bd=P[p + "downsample.norm.bias"])
-                for i in (1, 2, 3):
-                    e.update({f"w{i}": fw(f"{tag}.w{i}"), f"g{i}": P[p + f"norm{i}.weight"], f"b{i}": P[p + f"norm{i}.bias"]})
-                blocks.append((s, b, e))
-        pk["rn_blocks"] = blocks
+        pk = {}
+        if self.hybrid:
+            bb = "pretrained.model.patch_embed.backbone."
+            pk = {"stem_w": self.buf("w.stem", (64, 160)), "stem_g": P[bb + "stem.norm.weight"],
+                  "stem_b": P[bb + "stem.norm.bias"]}
+            blocks = []
+            for s, (cout, depth) in enumerate(_STAGES):
+                for b in range(depth):
+                    p, tag = f"{bb}stages.{s}.blocks.{b}.", f"s{s}b{b}"
+                    e = {"stride": 2 if (b == 0 and s > 0) else 1, "cout": cout, "mid": cout // 4}
+                    if b == 0:
+                        e.update(wd=fw(tag + ".wd"), gd=P[p + "downsample.norm.weight"], bd=P[p + "downsample.norm.bias"])
+                    for i in (1, 2, 3):
+                        e.update({f"w{i}": fw(f"{tag}.w{i}"), f"g{i}": P[p + f"norm{i}.weight"], f"b{i}": P[p + f"norm{i}.bias"]})
+                    blocks.append((s, b, e))
+            pk["rn_blocks"] = blocks
         pm = "pretrained.model."
         # pos_cache: filled by every forward() with that step's rows
         pk.update(proj_w=fw("proj"), proj_b=P[pm + "patch_embed.proj.bias"], cls=P[pm + "cls_token"].view(-1),
                   pos_cache={})
         pk["vit"] = []
-        for i in range(self.model.arch["depth"]):
+        for i in range(self.depth):
             p = f"{pm}blocks.{i}."
             lin = lambda name, bias: (fw(f"blk{i}.{name}"), P[p + bias])
             pk["vit"].append({"ln1": (P[p + "norm1.weight"], P[p + "norm1.bias"]), "qkv": lin("qkv", "attn.qkv.bias"),
                               "proj": lin("proj", "attn.proj.bias"), "ln2": (P[p + "norm2.weight"], P[p + "norm2.bias"]),
                               "fc1": lin("fc1", "mlp.fc1.bias"), "fc2": lin("fc2", "mlp.fc2.bias")})
-        D = self.model.arch["embed"]
-        for n in (3, 4):
+        D = self.D
+        for n in self.readouts:
             p = f"pretrained.act_postprocess{n}."
             pk.update({f"ro{n}_wfull": self.buf(f"w.ro{n}.full", (D, 2 * D)), f"ro{n}_wtok": self.buf(f"w.ro{n}.tok", (D, D)),
-                       f"ro{n}_b": P[p + "0.project.0.bias"], f"pp{n}_w": fw(f"pp{n}"), f"pp{n}_b": P[p + "3.bias"]})
+                       f"ro{n}_b": P[p + "0.project.0.bias"], f"pp{n}_w": fw(f"pp{n}"), f"pp{n}_b": self._padded_bias(p + "3.bias", n)})
+        if not self.hybrid:
+            for n, k in ((1, 4), (2, 2)):
+                cp = self.rn_pad[n - 1]
+                phases = self.buf(f"w.pp{n}t.phases", (k * k, cp, cp))     # filled by pack() from the dgrad operand
+                pk[f"pp{n}t_w"] = [[phases[dy * k + dx] for dx in range(k)] for dy in range(k)]
+                pk[f"pp{n}t_b"] = self._padded_bias(f"pretrained.act_postprocess{n}.4.bias", n)
         pk["pp4s_w"], pk["pp4s_b"] = fw("pp4s"), P["pretrained.act_postprocess4.4.bias"]
         for n in (1, 2, 3, 4):
             p = f"scratch.refinenet{n}."
@@ -355,6 +403,13 @@ class TrainEngine:
         pk["head2"] = (fw("head2"), self.buf("head_b2pad", (64,), torch.float32))    # carried zero-padded to 64
         pk["head4"] = (P["scratch.output_conv.4.weight"].view(self.C, 32), P["scratch.output_conv.4.bias"])
         return pk
+
+    def _padded_bias(self, pname: str, n: int) -> torch.Tensor:
+        """The reassemble bias `pname` of layer_n as the forward reads it: the master weights' view, or, for a width
+        carried zero-padded (vitb16_384's 96-wide layer_1), a zero-padded copy that pack() refreshes."""
+        if self.rn_pad[n - 1] == self.rn_in[n - 1]:
+            return self.P[pname]
+        return self.buf(f"w.pad.{pname}", (self.rn_pad[n - 1],), torch.float32)
 
     def _stale(self, trainable) -> set:
         """Source parameters whose derived forward operands must be (re)built: every trainable one (FlatAdam writes the
@@ -380,8 +435,8 @@ class TrainEngine:
         tab = self._pack_tables.get(keys)
         if tab is None:
             tab = self._pack_tables[keys] = bwd.PackTable(
-                [(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c, std)
-                 for k, pn, n, c, taps, n_pad, std in self.layers if k in keys], self.adt)
+                [(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c_pad, std)
+                 for k, pn, n, c, taps, n_pad, c_pad, std in self.layers if k in keys], self.adt)
         return tab
 
     @torch.no_grad()
@@ -398,7 +453,7 @@ class TrainEngine:
         P = self.P
         bb = "pretrained.model.patch_embed.backbone."
         # stem 7x7 (3 input channels): [64,3,7,7] -> standardise -> [64, (ky,kx,c)=147] padded to 160 columns
-        if fresh(bb + "stem.conv.weight"):
+        if self.hybrid and fresh(bb + "stem.conv.weight"):
             w = P[bb + "stem.conv.weight"]
             std_, mean = torch.std_mean(w, dim=[1, 2, 3], keepdim=True, unbiased=False)
             ws = ((w - mean) / (std_ + 1e-8)).permute(0, 2, 3, 1).reshape(64, 147)
@@ -409,17 +464,31 @@ class TrainEngine:
             b2 = self.pk["head2"][1]
             b2.zero_()
             b2[:32].copy_(P["scratch.output_conv.2.bias"])
-        # ProjectReadout Linear(1536 -> 768): token half as a GEMM operand (fwd / bwd), whole matrix for the cls kernel
-        for n in (3, 4):
+        # ProjectReadout Linear(2D -> D): token half as a GEMM operand (fwd / bwd), whole matrix for the cls kernel
+        D = self.D
+        for n in self.readouts:
             if not fresh(f"pretrained.act_postprocess{n}.0.project.0.weight"):
                 continue
             wfull = P[f"pretrained.act_postprocess{n}.0.project.0.weight"]
             self.pk[f"ro{n}_wfull"].copy_(wfull)
-            self.pk[f"ro{n}_wtok"].copy_(wfull[:, :768])
-            tokb = self.buf(f"w.ro{n}.tokT", (768, 768))
-            tokb.copy_(wfull[:, :768].t())
-            clsT = self.buf(f"w.ro{n}.clsT", (768, 768), torch.float32)
-            clsT.copy_(wfull[:, 768:].t())
+            self.pk[f"ro{n}_wtok"].copy_(wfull[:, :D])
+            tokb = self.buf(f"w.ro{n}.tokT", (D, D))
+            tokb.copy_(wfull[:, :D].t())
+            clsT = self.buf(f"w.ro{n}.clsT", (D, D), torch.float32)
+            clsT.copy_(wfull[:, D:].t())
+        if not self.hybrid:
+            for n, k in ((1, 4), (2, 2)):
+                cp = self.rn_pad[n - 1]
+                for pname, key in ((f"pretrained.act_postprocess{n}.3.bias", f"pp{n}_b"),
+                                   (f"pretrained.act_postprocess{n}.4.bias", f"pp{n}t_b")):
+                    if cp != self.rn_in[n - 1] and fresh(pname):
+                        self.pk[key].zero_()
+                        self.pk[key][:self.rn_in[n - 1]].copy_(P[pname])
+                if f"pp{n}t" in keys:
+                    # the forward's per-phase operands W[:, :, ky, kx]^T [out][in] = the tap blocks of the dgrad
+                    # operand, bwd[out][(k*k-1-t)*cp + in]
+                    phases = self.buf(f"w.pp{n}t.phases", (k * k, cp, cp))
+                    phases.copy_(self.W[f"pp{n}t"][1].view(cp, k * k, cp).permute(1, 0, 2).flip(0))
         # stride-2 3x3 convolutions: per-parity-plane dgrad operands cut out of the rotated dgrad weight
         for key, mode in (("s1b0.w2", "same"), ("s2b0.w2", "same"), ("pp4s", "sym1")):
             if key not in keys:
@@ -432,23 +501,23 @@ class TrainEngine:
     def _wgrad(self, key: str, views, taps, dy, n_rows: Optional[int] = None):
         """weight gradient of layer `key` into the flat gradient buffer (through the weight standardisation); nothing
         for a frozen weight."""
-        pname, n, c, ntaps, n_pad, std = self.meta[key]
+        pname, n, c, ntaps, n_pad, c_pad, std = self.meta[key]
         if not self._plan.grad(pname):
             return
-        if ntaps == 1 and not std and n_pad == n:
+        if key not in self.gp_layer:
             # linear / 1x1 layer without weight standardisation: the packed gradient layout IS the parameter layout
             bwd.conv_wgrad(views, taps, dy, self.G[pname].view(n, c))
             return
         bwd.conv_wgrad(views, taps, dy, self.gp_layer[key])        # converted to parameter layout by the bucket's unpack launch
 
-    def _bias_grad(self, pname: str, dy, n: Optional[int] = None):
+    def _bias_grad(self, pname: str, dy):
         if not self._plan.grad(pname):
             return
         g = self.G[pname]
-        if n is None or dy.shape[-1] == g.numel():
+        if dy.shape[-1] == g.numel():
             bwd.colsum(dy.reshape(-1, dy.shape[-1]), g.view(1, -1))
-        else:                                                   # padded output channels (head conv2)
-            tmp = self.buf("tmp.bias", (1, dy.shape[-1]), torch.float32)
+        else:                                                   # padded output channels (head conv2, vitb16 layer_1)
+            tmp = self.buf(f"tmp.bias{dy.shape[-1]}", (1, dy.shape[-1]), torch.float32)
             bwd.colsum(dy.reshape(-1, dy.shape[-1]), tmp)
             g.copy_(tmp[0, :g.numel()])
 
@@ -467,7 +536,7 @@ class TrainEngine:
         key = (trainable, bool(want_dx))
         plan = self._plans.get(key)
         if plan is None:
-            plan = self._plans[key] = backward_plan(self.param_names, trainable, want_dx)
+            plan = self._plans[key] = backward_plan(self.param_names, trainable, want_dx, self.backbone)
         return plan
 
     def _unpack(self, tag: str, plan: BackwardPlan):
@@ -538,6 +607,23 @@ class TrainEngine:
             w, taps = self.plane_w[(key, (py, px))]
             ops.conv_gemm([dy], taps, w, dx[:, py::2, px::2, :], bias=self._zb(w))
 
+    def _conv_transpose_bwd(self, n: int, k: int, dout, u):
+        """Backward of layer_n's ConvTranspose2d(c, c, k, stride k) (plain ViTs), out[b, k*y+ky, k*x+kx, o] =
+        sum_i u[b, y, x, i] W[i, o, ky, kx] + bias[o].  Row k*y+ky of the channels-last dout is contiguous over (kx, o),
+        so dout is k views [B, gh, gw, k*c], one per ky: the input gradient is one convolution with k taps (K = k*k*c)
+        and the weight gradient one wgrad with k taps, no scatter.  -> gradient w.r.t. u (None when not needed)."""
+        B, H, W, cp = dout.shape
+        views = [dout.view(B, H // k, k, W // k, k * cp)[:, :, ky] for ky in range(k)]
+        taps = [(ky, 0, 0) for ky in range(k)]
+        du = None
+        if self._plan.act(f"pp{n}.o"):
+            w = self.W[f"pp{n}t"][0]                                  # [in][(ky, kx, out)]
+            du = self.buf(f"g.pp{n}", u.shape)
+            ops.conv_gemm(views, taps, w, du, bias=self._zb(w))
+        self._wgrad(f"pp{n}t", views, taps, u)                         # [in][(ky, kx, out)] = the parameter's layout
+        self._bias_grad(f"pretrained.act_postprocess{n}.4.bias", dout)
+        return du
+
     @torch.no_grad()
     def backward(self, dout: torch.Tensor, on_ready=None, dx: Optional[torch.Tensor] = None, trainable=None):
         """dout: gradient w.r.t. the forward's output [B,C,H,W] fp32.  Fills self.flat_grad: the slices of the trainable
@@ -568,7 +654,7 @@ class TrainEngine:
             dh1u = buf("g.head_h1u", hd["h1u"].shape)
             ops.conv3x3(da, Wt["head2"][1], dh1u, bias=self._zb(Wt["head2"][1]))
         self._wgrad("head2", [hd["h1u"]], bwd.TAPS_3X3, da)
-        self._bias_grad("scratch.output_conv.2.bias", da, n=32)
+        self._bias_grad("scratch.output_conv.2.bias", da)
         if need("head.h1"):
             dh1 = buf("g.head_h1", hd["h1"].shape)
             bwd.upsample2x_bwd(dh1u, dh1)
@@ -636,8 +722,9 @@ class TrainEngine:
                 d_layers[n - 1] = buf(f"g.layer_{n}", l.shape)
                 ops.conv3x3(d_rn[n - 1], Wt[f"rn{n}"][1], d_layers[n - 1], bias=self._zb(Wt[f"rn{n}"][1]))
             self._wgrad(f"rn{n}", [l], bwd.TAPS_3X3, d_rn[n - 1])
-        # ---- reassemble: act_postprocess4.4 (stride 2), then the two readouts
-        gh, gw, ntok, D = S["gh"], S["gw"], S["ntok"], 768
+        # ---- reassemble: act_postprocess4.4 (stride 2), the ConvTransposes of layer_1 / layer_2 (plain ViTs), then the
+        # readouts
+        gh, gw, ntok, D = S["gh"], S["gw"], S["ntok"], self.D
         u4 = S["ro4"]["o"]
         du4 = None
         if need("pp4.o"):
@@ -646,6 +733,11 @@ class TrainEngine:
         planes = [u4[:, py::2, px::2, :] for py in range(2) for px in range(2)]
         self._wgrad("pp4s", planes, ops._parity_taps("sym1"), d_layers[3])
         self._bias_grad("pretrained.act_postprocess4.4.bias", d_layers[3])
+        d_pp = {3: d_layers[2], 4: du4}                              # gradient w.r.t. act_postprocessN.3's output
+        if not self.hybrid:
+            for n, k in ((2, 2), (1, 4)):
+                if need(f"layer_{n}"):
+                    d_pp[n] = self._conv_transpose_bwd(n, k, d_layers[n - 1], S[f"ro{n}"]["o"])
 
         def readout_bwd(n, do, tokens):
             """-> gradient w.r.t. the hooked tokens `tokens`, activation type [B, ntok, D] (None when not needed)."""
@@ -686,8 +778,10 @@ class TrainEngine:
                 dtk[:, 0, :].copy_(dt0)
             return dtk
 
-        dtk4 = readout_bwd(4, du4, "vit.x12") if need("pp4.o") else None
-        dtk3 = readout_bwd(3, d_layers[2], "vit.x9") if need("layer_3") else None
+        dtk = {}                                                     # hooked block -> gradient w.r.t. its output tokens
+        for n, hook in reversed(list(zip(self.readouts, self.hooks))):
+            if need(f"pp{n}.o"):
+                dtk[hook] = readout_bwd(n, d_pp[n], f"vit.x{hook + 1}")
         self._unpack("decoder", plan)
         ready("decoder")
         # ---- ViT blocks (fp32 stream gradient ds, activation-type copy ds16 for the GEMMs)
@@ -697,18 +791,18 @@ class TrainEngine:
         ds = buf("g.vit_ds", (B, ntok, D), f32)
         ds_b = buf("g.vit_ds_b", (B, ntok, D), f32)
         ds16 = buf("g.vit_ds16", (B, ntok, D)) if not self.fp32 else None
-        if need("vit.x12"):
-            bwd.add_cast(None, dtk4, ds, ds16)
-        hooked = (8, 11)                                             # blocks whose output gradient gets a readout gradient
-        for i in range(11, -1, -1):
+        hooked, depth = self.hooks, self.depth                       # blocks whose output gradient gets a readout gradient
+        if need(f"vit.x{depth}"):                                    # every backbone hooks its last block
+            bwd.add_cast(None, dtk[depth - 1], ds, ds16)
+        for i in range(depth - 1, -1, -1):
             p, q = f"{pm}blocks.{i}.", f"vit{i}."
             v = vit[i]
-            if i == 5:
+            if i == depth // 2 - 1:
                 ready("vit_hi")
             if not need(f"vit.x{i + 1}"):                            # nothing of this block or below is wanted
                 continue
-            if i == 8:                                               # hook after block 8: tokens_8 also feed readout 3
-                bwd.add_cast(ds, dtk3, ds, ds16)
+            if i in hooked and i != depth - 1:                       # the hooked tokens also feed a readout
+                bwd.add_cast(ds, dtk[i], ds, ds16)
             g16 = ds if self.fp32 else ds16
             # mlp: x_{i+1} = xm + fc2(gelu(fc1(LN2(xm))))
             if need(q + "u"):
@@ -743,7 +837,7 @@ class TrainEngine:
             if not need(q + "att"):
                 continue
             dqkv = buf("g.vit_qkv", v["qkv"].shape)
-            bwd.attention_bwd(v["qkv"], v["att"], datt, v["lse"], dqkv, heads=12, scale=0.125)
+            bwd.attention_bwd(v["qkv"], v["att"], datt, v["lse"], dqkv, heads=self.heads, scale=0.125)
             if need(q + "h1"):
                 ops.linear(dqkv.view(rows, -1), Wt[f"blk{i}.qkv"][1], dh.view(rows, -1), bias=self._zb(Wt[f"blk{i}.qkv"][1]))
             self._wgrad(f"blk{i}.qkv", [v["h1"].view(rows, -1)], bwd.TAPS_1, dqkv.view(rows, -1))
@@ -774,17 +868,27 @@ class TrainEngine:
             if want_cls:
                 G[pm + "cls_token"].view(-1).copy_(row0)
             g16 = ds if self.fp32 else ds16
-            f3 = S["f3"]
             dtok = g16[:, 1:, :].unsqueeze(1)
-            if need("f3"):
-                df3 = buf("g.f3", f3.shape)
-                ops.linear(dtok, Wt["proj"][1], df3.view(B, 1, gh * gw, 1024), bias=self._zb(Wt["proj"][1]))
-            self._wgrad("proj", [f3.view(B, 1, gh * gw, 1024)], bwd.TAPS_1, dtok)
+            if self.hybrid:
+                f3 = S["f3"]
+                if need("f3"):
+                    df3 = buf("g.f3", f3.shape)
+                    ops.linear(dtok, Wt["proj"][1], df3.view(B, 1, gh * gw, 1024), bias=self._zb(Wt["proj"][1]))
+                self._wgrad("proj", [f3.view(B, 1, gh * gw, 1024)], bwd.TAPS_1, dtok)
+            else:                                                    # Conv2d(3, D, 16, stride 16) = GEMM over patchify's columns
+                cols = S["cols"]
+                if dx is not None:
+                    dcols = buf("g.patch_cols", cols.shape)
+                    ops.linear(dtok, Wt["proj"][1], dcols, bias=self._zb(Wt["proj"][1]))
+                    bwd.patch_input_grad(dcols.view(B * gh * gw, -1), dx)
+                self._wgrad("proj", [cols], bwd.TAPS_1, dtok)
             if T(pm + "patch_embed.proj.bias"):
                 tmpb = buf("tmp.projbias", (B, D), f32)
                 bwd.colsum(ds[:, 1:, :], tmpb, batches=B)
                 bwd.colsum(tmpb, G[pm + "patch_embed.proj.bias"].view(1, -1))
         ready("vit_lo")
+        if not self.hybrid:
+            return self.flat_grad
 
         # ---- ResNetV2 bottlenecks, last to first
         d_out = df3
@@ -927,9 +1031,11 @@ def differentiable_forward(model: DPTDepthModel, x: torch.Tensor) -> torch.Tenso
 # ====================================================================================== the train step
 def plan_grad_buckets(names: List[str], sizes: List[int]) -> List[Tuple[int, int, str]]:
     """Contiguous [start, end) ranges of the flat gradient buffer (state_dict order, padded sizes) in the order the
-    backward COMPLETES them, so that each range can be all-reduced while the rest of the backward still runs:
-      decoder + reassemble (scratch.*, act_postprocess*) -> ViT blocks 6..11 -> ViT blocks 0..5 + patch projection ->
-      cls / pos_embed + the ResNetV2 stem and stages.
+    backward COMPLETES them, so that each range can be all-reduced while the rest of the backward still runs, for a
+    model of `depth` ViT blocks:
+      DPT-Hybrid: decoder + reassemble (scratch.*, act_postprocess*) -> ViT blocks depth/2.. -> ViT blocks ..depth/2-1 +
+      patch projection -> cls / pos_embed + the ResNetV2 stem and stages;
+      plain ViTs: decoder + reassemble -> ViT blocks depth/2.. -> cls / pos_embed, patch embedding, ViT blocks ..depth/2-1.
     Returns (start, end, ready_after) with ready_after in {"decoder", "vit_hi", "vit_lo", "resnet"}."""
     offs, off = {}, 0
     for n, s in zip(names, sizes):
@@ -939,13 +1045,17 @@ def plan_grad_buckets(names: List[str], sizes: List[int]) -> List[Tuple[int, int
 
     def first(pred):
         return min(offs[n][0] for n in names if pred(n))
+    block = lambda n: int(n.split(".")[3]) if n.startswith("pretrained.model.blocks.") else -1
+    depth = max(block(n) for n in names) + 1
     b_blocks = first(lambda n: n.startswith("pretrained.model.blocks."))
     b_proj = first(lambda n: n.startswith("pretrained.model.patch_embed.proj."))
-    b_blk6 = first(lambda n: n.startswith("pretrained.model.blocks.6."))
+    b_half = first(lambda n: block(n) >= depth // 2)
     b_tail = first(lambda n: n.startswith("pretrained.model.norm.") or n.startswith("pretrained.act_postprocess") or
                    n.startswith("scratch."))
-    assert b_proj < b_blocks < b_blk6 < b_tail
-    return [(b_tail, total, "decoder"), (b_blk6, b_tail, "vit_hi"), (b_proj, b_blk6, "vit_lo"), (0, b_proj, "resnet")]
+    assert b_proj < b_blocks < b_half < b_tail
+    if not any(n.startswith(_BB) for n in names):                    # plain ViT: nothing precedes the patch embedding
+        return [(b_tail, total, "decoder"), (b_half, b_tail, "vit_hi"), (0, b_half, "vit_lo")]
+    return [(b_tail, total, "decoder"), (b_half, b_tail, "vit_hi"), (b_proj, b_half, "vit_lo"), (0, b_proj, "resnet")]
 
 
 class _FlatTrainStep:
