@@ -21,6 +21,11 @@ from typing import Dict, Optional
 import torch
 import torch.nn.functional as F
 
+from .gemm_oracle import attention_bf16
+
+# the wgmma attention kernel's rounding points, defined once in gemm_oracle (kept under this name for its callers)
+_attention_bf16 = attention_bf16
+
 P = "pretrained.model."
 BB = P + "patch_embed.backbone."
 
@@ -168,18 +173,6 @@ def forward_fp32(sd: Dict[str, torch.Tensor], x: torch.Tensor, taps: Optional[di
 
 
 # ----------------------------------------------------------------------------- product rounding points
-def _attention_bf16(q, k, v):
-    """The wgmma attention kernel's arithmetic (omnidata_b200/csrc/attention_tc.cu): exact two-pass
-    softmax in the log2 domain, p = exp2(s*c - max(s)*c); the probabilities are rounded to bf16 for the
-    PV product while the row sum uses the unrounded fp32 values.  Equal to softmax(qk^T/8)v in real
-    arithmetic."""
-    c = float(torch.tensor(0.125, dtype=torch.float32) * torch.tensor(1.4426950408889634, dtype=torch.float32))
-    s_ = q @ k.transpose(-2, -1)
-    m = s_.amax(dim=-1, keepdim=True)
-    p = torch.exp2(s_ * c - m * c)
-    return (_bf16(p) @ v) / p.sum(dim=-1, keepdim=True)
-
-
 def _attention_online_bf16(q, k, v, chunk: int = 64):
     """Arithmetic of the legacy mma.sync kernel (attention.cu): flash-style online softmax over
     64-key chunks, P of a chunk rounded to bf16, fp32 running row sum of the unrounded values."""
@@ -268,7 +261,7 @@ def forward_bf16(sd: Dict[str, torch.Tensor], x: torch.Tensor, taps: Optional[di
         qkv = r(F.linear(h, wq(g(p + "attn.qkv.weight")), g(p + "attn.qkv.bias")))
         N = qkv.shape[1]
         q, k, v = qkv.reshape(B, N, 3, 12, 64).permute(2, 0, 3, 1, 4)
-        a = _attention_bf16(q, k, v)
+        a = attention_bf16(q, k, v)
         a = r(a.transpose(1, 2).reshape(B, N, 768))
         tok = tok + F.linear(a, wq(g(p + "attn.proj.weight")), g(p + "attn.proj.bias"))
         h = r(F.layer_norm(tok, (768,), g(p + "norm2.weight"), g(p + "norm2.bias"), 1e-6))

@@ -73,6 +73,48 @@ def checked_launch(bufs: Sequence[Guarded], outs: Sequence[torch.Tensor], launch
     return first
 
 
+def _extent(t: torch.Tensor) -> int:
+    return 1 + sum((s - 1) * st for s, st in zip(t.shape, t.stride())) if t.numel() else 0
+
+
+def geometry(tensors: dict):
+    """Tensors of one launch (name -> tensor or None) -> (groups, specs), hashable: one group per storage, spanning only
+    what the tensors cover (plus the base's offset within 256 bytes, so alignment is kept); each tensor as (group,
+    shape, stride, element offset in the group).  Aliasing between the tensors (in-place outputs, views of one
+    buffer) is part of the geometry."""
+    by_storage = {}
+    for t in tensors.values():
+        if t is not None:
+            by_storage.setdefault(t.untyped_storage().data_ptr(), []).append(t)
+    groups, where = [], {}
+    for key, ts in by_storage.items():
+        assert len({t.dtype for t in ts}) == 1
+        es, base = ts[0].element_size(), min(t.data_ptr() for t in ts)
+        lead = (base % 256) // es
+        where[key] = (len(groups), base, lead, es)
+        groups.append((max(lead + (t.data_ptr() - base) // es + _extent(t) for t in ts), ts[0].dtype))
+    specs = []
+    for name, t in tensors.items():
+        if t is None:
+            specs.append((name, None))
+            continue
+        gi, base, lead, es = where[t.untyped_storage().data_ptr()]
+        specs.append((name, (gi, tuple(t.shape), tuple(t.stride()), lead + (t.data_ptr() - base) // es)))
+    return tuple(groups), tuple(specs)
+
+
+def materialize(geom, gen: torch.Generator):
+    """A geometry -> (Guarded buffers, name -> tensor), every tensor at its recorded place in a fresh guarded buffer
+    of seeded random values, so that the tensors alias each other exactly as they did when recorded."""
+    groups, specs = geom
+    bufs = [Guarded(n, dtype, gen) for n, dtype in groups]
+    return bufs, {name: None if s is None else bufs[s[0]].view(s[1], s[2], s[3]) for name, s in specs}
+
+
+def same_storage(a: torch.Tensor, b: torch.Tensor) -> bool:
+    return a is not None and b is not None and a.untyped_storage().data_ptr() == b.untyped_storage().data_ptr()
+
+
 def ulp_bf16(x: torch.Tensor) -> torch.Tensor:
     """Spacing of bf16 values at |x| (8 significant bits), for |x| in the normal range; float64."""
     _, e = torch.frexp(x.double().abs().clamp_min(2.0 ** -126))

@@ -277,14 +277,19 @@ def test_patch_proj_style_pos_residual():
     assert float(tokens[:, 0, :].abs().max()) == 0.0
 
 
+# the four widths the LayerNorm kernels are instantiated for (VPL = cols / 256); DPT-Large runs 1024
+LN_COLS = [256, 512, 768, 1024]
+
+
 def test_layernorm():
     o = ops()
-    x = (rnd(4 * 577, 768) * 3 + 0.5).to(torch.bfloat16)
-    g, bta = rnd(768) * 0.1 + 1, rnd(768) * 0.1
-    out = torch.empty_like(x)
-    o.layernorm(x, g, bta, out, 1e-6)
-    torch.cuda.synchronize()
-    check(out, F.layer_norm(x.float(), (768,), g, bta, 1e-6), "layernorm")
+    for cols in LN_COLS:
+        x = (rnd(4 * 577, cols) * 3 + 0.5).to(torch.bfloat16)
+        g, bta = rnd(cols) * 0.1 + 1, rnd(cols) * 0.1
+        out = torch.empty_like(x)
+        o.layernorm(x, g, bta, out, 1e-6)
+        torch.cuda.synchronize()
+        check(out, F.layer_norm(x.float(), (cols,), g, bta, 1e-6), f"layernorm {cols}")
 
 
 @pytest.mark.parametrize("b,tokens", [(2, 577), (1, 64), (1, 100), (13, 257), (33, 577)])
@@ -298,9 +303,9 @@ def test_attention(b, tokens):
     torch.cuda.synchronize()
     q, k, v = qkv.float().view(b, tokens, 3, 12, 64).permute(2, 0, 3, 1, 4)
     s = q @ k.transpose(-1, -2) * 0.125
-    # the kernel's own definition of where P is rounded to bf16 (see oracle/dpt_oracle.py)
-    from oracle.dpt_oracle import _attention_bf16
-    ref = _attention_bf16(q, k, v)   # plain torch ops, on the GPU
+    # the kernel's own definition of where P is rounded to bf16 (see oracle/gemm_oracle.py)
+    from oracle.gemm_oracle import attention_bf16
+    ref = attention_bf16(q, k, v)    # plain torch ops, on the GPU
     check(out, ref.transpose(1, 2).reshape(b, tokens, 768), f"attention b{b} n{tokens}", tol=1e-3)
     exact = (torch.softmax(s, dim=-1) @ v).transpose(1, 2).reshape(b, tokens, 768)
     assert rel_l2(out.float(), exact) < 4e-3
@@ -578,12 +583,13 @@ def test_patch_proj_fp32_tokens():
 
 def test_layernorm_fp32_stream_and_cast():
     o = ops()
-    x = rnd(4 * 577, 768) * 3 + 0.5
-    g, bta = rnd(768) * 0.1 + 1, rnd(768) * 0.1
-    out = torch.empty_like(x, dtype=torch.bfloat16)
-    o.layernorm(x, g, bta, out, 1e-6)
-    xb = torch.empty_like(out)
-    o.cast_f32_bf16(x, xb)
-    torch.cuda.synchronize()
-    check(out, F.layer_norm(x, (768,), g, bta, 1e-6), "layernorm fp32 in")
-    assert torch.equal(xb, x.to(torch.bfloat16))
+    for cols in LN_COLS:
+        x = rnd(4 * 577, cols) * 3 + 0.5
+        g, bta = rnd(cols) * 0.1 + 1, rnd(cols) * 0.1
+        out = torch.empty_like(x, dtype=torch.bfloat16)
+        o.layernorm(x, g, bta, out, 1e-6)
+        xb = torch.empty_like(out)
+        o.cast_f32_bf16(x, xb)
+        torch.cuda.synchronize()
+        check(out, F.layer_norm(x, (cols,), g, bta, 1e-6), f"layernorm fp32 in {cols}")
+        assert torch.equal(xb, x.to(torch.bfloat16)), cols

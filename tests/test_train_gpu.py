@@ -47,8 +47,13 @@ def _setup(lib_built):
 
 # ------------------------------------------------------------------------------------------ kernels (fp32 storage)
 def test_layernorm_bwd_kernel():
+    for c in (256, 512, 768, 1024):                          # the kernel's four instances (VPL = c / 256)
+        _check_layernorm_bwd(c)
+
+
+def _check_layernorm_bwd(c):
     from omnidata_b200 import bwd
-    rows, c = 4 * 577, 768
+    rows = 4 * 577
     x, dy, g, ds_in = rnd(rows, c) * 2 + 0.3, rnd(rows, c, seed=1), rnd(c) * 0.1 + 1, rnd(rows, c, seed=2)
     xd = x.double().requires_grad_(True); gd = g.double().requires_grad_(True); bd = torch.zeros(c, device=dev(), dtype=torch.float64, requires_grad=True)
     y = F.layer_norm(xd, (c,), gd, bd, 1e-6)
