@@ -4,7 +4,8 @@
 //   warpgroups 1-2  consumers: each issues the wgmma of 64 of the 128 tile rows, then all eight warps run the
 //                   epilogue (accumulator chunk -> shared memory -> one row per thread -> bias/act/residual
 //                   -> bf16 -> swizzled smem -> TMA store), two warps per 32-row quarter, each owning 32 of
-//                   the 64 columns of a chunk
+//                   the 64 columns of a chunk (EPI_BIAS_RES_F32: each thread adds its accumulator fragment
+//                   into the staged fp32 residual instead)
 //
 // The A operand of the GEMM (rows = output pixels, K = taps x input channels) is never
 // materialised: each K block is a 4-D TMA box {64 ch, tile_w, tile_h, 1} of the channels-last
@@ -88,8 +89,9 @@ ODB_DEVINL unsigned long long global_ns() {
 // convolutions: ~4x fewer instructions per 64-column chunk, and (EPI_BIAS_RES) the residual fetched by TMA into the output
 // staging slot a few chunks ahead instead of 1024 scattered 16-byte loads per chunk.
 // EPI_BIAS_RES_F32: fp32 residual in, fp32 out (the ViT residual stream: attn.proj / mlp.fc2 / patch proj).  A
-// 64-column chunk is two 128-row x 32-fp32 TMA boxes (128-byte swizzled rows), one per epilogue warp half, so a
-// chunk occupies TWO 16 KiB staging units.
+// 64-column chunk is two 128-row x 32-fp32 TMA boxes (128-byte swizzled rows), so a chunk occupies TWO 16 KiB staging
+// units.  Each consumer thread adds its own accumulator fragment elements into the staged residual in place: this
+// epilogue needs no accumulator chunk buffer, and the shared memory it frees holds one more operand stage.
 enum : int { EPI_GENERIC = 0, EPI_BIAS = 1, EPI_BIAS_RELU = 2, EPI_BIAS_GELU = 3, EPI_BIAS_RES = 4, EPI_GN = 5,
              EPI_BIAS_RES_F32 = 6 };
 
@@ -173,7 +175,8 @@ struct AccChunk {
   static constexpr int kBytes = kTileRows * kPitch * 4;
 };
 
-template <int BLOCK_N, int STAGES, int NSTAGING, bool HALO, bool HEAD>
+// ACC_BUF = false (EPI_BIAS_RES_F32): no accumulator chunk buffer
+template <int BLOCK_N, int STAGES, int NSTAGING, bool HALO, bool HEAD, bool ACC_BUF>
 struct SmemPlan {
   static constexpr bool kBResident = HALO && HEAD;
   static constexpr int kBBytes = BLOCK_N * 128;
@@ -183,7 +186,7 @@ struct SmemPlan {
   static constexpr int kBOff = kAStages * kAStageBytes;
   static constexpr int kCOff = kBOff + (kBResident ? kResidentBTiles : STAGES) * kBBytes;
   static constexpr int kAccOff = kCOff + NSTAGING * kStagingBytes;
-  static constexpr int kBarOff = kAccOff + AccChunk<BLOCK_N>::kBytes;
+  static constexpr int kBarOff = kAccOff + (ACC_BUF ? AccChunk<BLOCK_N>::kBytes : 0);
   // full[STAGES], empty[STAGES], a_full[8], a_empty[8], res_full[4], b_resident
   static constexpr int kBarBytes = (2 * STAGES + 2 * kMaxAStages + 4 + 1) * 8;
   static constexpr int kTotal = kBarOff + kBarBytes + 1024;  // +1024: manual 1 KiB alignment
@@ -204,7 +207,7 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   static_assert(EPI == EPI_GENERIC || (!HEAD && !HALO && NSTAGING >= 2), "fast epilogues: plain tiles only");
   static_assert(!PAIR || !HEAD, "CTA pairs: no head tail");
   static_assert(EPI != EPI_BIAS_RES_F32 || NSTAGING >= 4, "fp32 epilogue: two staging slots of two 16 KiB units");
-  using Plan = SmemPlan<BLOCK_N, STAGES, NSTAGING, HALO, HEAD>;
+  using Plan = SmemPlan<BLOCK_N, STAGES, NSTAGING, HALO, HEAD, EPI != EPI_BIAS_RES_F32>;
   using Acc = AccChunk<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -469,6 +472,41 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
         v[4 * j + 2] = q.z + b4.z; v[4 * j + 3] = q.w + b4.w;
       }
     };
+    // EPI_BIAS_RES_F32: the accumulator columns [C0, C0 + 64) of this thread's fragment (rows r and r + 8 of its
+    // warpgroup's 64-row half) added in place into the fp32 residual chunk staged at `buf`, two 32-column TMA boxes
+    // of 128-byte rows whose 16-byte unit u sits at u ^ (row & 7).  The sum is res + (acc + bias), as the row
+    // epilogues round it.  A quad covers 32 contiguous bytes of a row: 8-byte accesses.
+    auto add_frag_res_f32 = [&](auto c0_tag, uint32_t buf, const float* b) {
+      constexpr int C0 = decltype(c0_tag)::value;
+      const int r = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+      const uint32_t rbase = buf + static_cast<uint32_t>(r) * 128u + (static_cast<uint32_t>(lane & 1) << 3);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 b2 = __ldg(reinterpret_cast<const float2*>(b + C0 + 8 * j + 2 * (lane & 3)));
+        const uint32_t unit = static_cast<uint32_t>(2 * (j & 3) + ((lane & 3) >> 1));
+        const uint32_t addr = rbase + static_cast<uint32_t>(j >> 2) * kStagingBytes + ((unit ^ (r & 7)) << 4);
+        const float* a = dacc + 4 * (C0 / 8 + j);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {                   // rows r, r + 8
+          const uint32_t ad = addr + h * 8u * 128u;
+          float q0, q1;
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(q0), "=f"(q1) : "r"(ad) : "memory");
+          q0 += a[2 * h] + b2.x;
+          q1 += a[2 * h + 1] + b2.y;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(ad), "f"(q0), "f"(q1) : "memory");
+        }
+      }
+    };
+    auto add_frag_res_f32_rt = [&](int c, uint32_t buf, const float* b) {   // run-time chunk index
+      if (c == 0) add_frag_res_f32(std::integral_constant<int, 0>{}, buf, b);
+      if constexpr (BLOCK_N > 64) {
+        if (c == 1) add_frag_res_f32(std::integral_constant<int, 64>{}, buf, b);
+      }
+      if constexpr (BLOCK_N > 128) {
+        if (c == 2) add_frag_res_f32(std::integral_constant<int, 128>{}, buf, b);
+        else if (c == 3) add_frag_res_f32(std::integral_constant<int, 192>{}, buf, b);
+      }
+    };
     // ------------------------------------------------------------ epilogue
     const int ew = warp - 4;               // epilogue warp 0..7
     const int quad = (ew + 2) & 3;         // 32-row quarter of the tile this warp owns
@@ -517,16 +555,19 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
         decode(tile, tn, tx, ty, tb);
         const int x0 = tx * p.tile_w, y0 = ty * p.tile_h;
         const int n0 = tn * BLOCK_N;
-        const float* bias = EPI == EPI_GN ? nullptr
-                                          : p.bias + static_cast<long long>(tb < p.out_b ? tb : 0) * p.bias_sb + n0 + cofs;
+        const float* bias_n0 = EPI == EPI_GN ? nullptr
+                                             : p.bias + static_cast<long long>(tb < p.out_b ? tb : 0) * p.bias_sb + n0;
+        const float* bias = EPI == EPI_GN ? nullptr : bias_n0 + cofs;
         // EPI_GN: rows of this thread that really exist (ragged tiles)
         const int gx = x0 + (row % p.tile_w), gy = y0 + (row / p.tile_w);
         const bool valid = row < p.tile_w * p.tile_h && gx < p.out_w && gy < p.out_h && tb < p.out_b;
 #pragma unroll
         for (int c = 0; c < kChunks; ++c, ++g) {
-          stage_chunk_rt(c);
           float v[32];
-          read_row_bias(row, cofs, EPI == EPI_GN ? nullptr : bias + c * 64, v);
+          if constexpr (!F32) {
+            stage_chunk_rt(c);
+            read_row_bias(row, cofs, EPI == EPI_GN ? nullptr : bias + c * 64, v);
+          }
           if constexpr (EPI == EPI_BIAS_GELU) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) gelu_erf_x2(v[2 * j], v[2 * j + 1]);
@@ -537,19 +578,8 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
           const uint32_t slot = g % NS;
           const uint32_t buf = smem_base + Plan::kCOff + slot * kSlotBytes;
           if constexpr (F32) {
-            // fp32 residual + fp32 result: this warp half owns the 32-column (128-byte) sub-tile `half` of the slot
             mbar_wait(rfull_bar(slot), (g / NS) & 1u);
-            const uint32_t sub = buf + static_cast<uint32_t>(half) * kStagingBytes + rowoff;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint32_t addr = sub + (static_cast<uint32_t>(j ^ (row & 7)) << 4);
-              float q0, q1, q2, q3;
-              asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                           : "=f"(q0), "=f"(q1), "=f"(q2), "=f"(q3) : "r"(addr) : "memory");
-              q0 += v[4 * j + 0]; q1 += v[4 * j + 1]; q2 += v[4 * j + 2]; q3 += v[4 * j + 3];
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(q0), "f"(q1), "f"(q2), "f"(q3)
-                           : "memory");
-            }
+            add_frag_res_f32_rt(c, buf, bias_n0);
           } else {
           if constexpr (EPI == EPI_BIAS_RES) {
             // the residual rows of this chunk were TMA-loaded into the staging slot (same swizzled
@@ -813,7 +843,7 @@ static int encode_view_map(CUtensorMap* map, const odb_view& v, int box_c, int b
 
 template <int BLOCK_N, int STAGES, int NSTAGING, bool HEAD, bool HALO, int EPI = EPI_GENERIC, bool PAIR = false>
 static int launch_instance(const ConvGemmParams& p, long long units, cudaStream_t stream) {
-  using Plan = SmemPlan<BLOCK_N, STAGES, NSTAGING, HALO, HEAD>;
+  using Plan = SmemPlan<BLOCK_N, STAGES, NSTAGING, HALO, HEAD, EPI != EPI_BIAS_RES_F32>;
   auto kernel = conv_gemm_kernel<BLOCK_N, STAGES, NSTAGING, HEAD, HALO, PAIR, EPI>;
   static bool configured[kMaxDevices] = {};      // the opt-in is per device
   const int dev = current_device();
@@ -858,12 +888,13 @@ static int launch_instance(const ConvGemmParams& p, long long units, cudaStream_
 template <int EPI>
 static int launch_fast(const ConvGemmParams& p, int block_n, bool pair, long long units, cudaStream_t stream) {
   if constexpr (EPI == EPI_BIAS_RES_F32) {
-    // fp32 residual stream: a chunk needs two 16 KiB staging units
-    if (pair && block_n == 128) return launch_instance<128, 3, 4, false, false, EPI, true>(p, units, stream);
-    if (pair) return launch_instance<256, 2, 4, false, false, EPI, true>(p, units, stream);
+    // fp32 residual stream: a chunk needs two 16 KiB staging units, and there is no accumulator chunk buffer
+    // (256 wide: 3 x 48 KiB of operands + 64 KiB of staging = 208 KiB)
+    if (pair && block_n == 128) return launch_instance<128, 4, 4, false, false, EPI, true>(p, units, stream);
+    if (pair) return launch_instance<256, 3, 4, false, false, EPI, true>(p, units, stream);
     switch (block_n) {
-      case 256: return launch_instance<256, 2, 4, false, false, EPI>(p, units, stream);
-      case 128: return launch_instance<128, 3, 4, false, false, EPI>(p, units, stream);
+      case 256: return launch_instance<256, 3, 4, false, false, EPI>(p, units, stream);
+      case 128: return launch_instance<128, 4, 4, false, false, EPI>(p, units, stream);
       default: return launch_instance<64, 4, 4, false, false, EPI>(p, units, stream);
     }
   } else {
