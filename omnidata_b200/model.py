@@ -15,7 +15,7 @@ head `dpt_depth.py:91-99`; encoder arithmetic is timm 0.4.12 `vit_base_resnet50_
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -41,18 +41,106 @@ _ARCH = {
 }
 
 
-def _pad_to(t: torch.Tensor, dim: int, size: int) -> torch.Tensor:
-    """zero-pad `t` along `dim` up to `size` (weights / biases of layers whose width is not a multiple of 64)."""
-    if t.shape[dim] == size:
-        return t
-    shape = list(t.shape)
-    shape[dim] = size - t.shape[dim]
-    return torch.cat([t, torch.zeros(shape, dtype=t.dtype, device=t.device)], dim=dim)
-
-
 def _rn_pad(arch: dict) -> Tuple[int, ...]:
     """reassemble widths, zero-padded to the GEMM's N granularity"""
     return tuple((c + 63) // 64 * 64 for c in arch["rn_in"])
+
+
+class GemmLayer(NamedTuple):
+    """One GEMM layer of the DPT.  Parameter `weight` is read as [n][c][taps]; its forward operand is
+    [n_pad][taps * c_pad], tap-major, the padded rows / columns zero.  `bias` names the bias parameter (None: no bias);
+    `standardize`: timm StdConv2dSame weight standardisation (the ResNetV2 convolutions)."""
+    key: str
+    weight: str
+    bias: Optional[str]
+    n: int
+    c: int
+    taps: int
+    n_pad: int
+    c_pad: int
+    standardize: bool
+
+
+def _rcu_layers(n: int, u: int) -> List[GemmLayer]:
+    p = f"scratch.refinenet{n}.resConfUnit{u}."
+    return [GemmLayer(f"ff{n}.rcu{u}.c{cv}", f"{p}conv{cv}.weight", f"{p}conv{cv}.bias", 256, 256, 9, 256, 256, False)
+            for cv in (1, 2)]
+
+
+def gemm_layers(arch: dict) -> List[GemmLayer]:
+    """Every GEMM layer of the DPT with encoder `arch` (an `_ARCH` entry) whose operands the packers build from a weight
+    of the state dict, in the order of the train engine's packing tables.  Not listed: the hybrid's 7x7 stem (im2col
+    operand) and the readout Linear layers (split into token and cls halves)."""
+    L = []
+    pm, D = "pretrained.model.", arch["embed"]
+    rn_in, rn_pad = arch["rn_in"], _rn_pad(arch)
+    if arch["hybrid"]:
+        bb = pm + "patch_embed.backbone."
+        cin = 64
+        for s, (cout, depth) in enumerate(_STAGES):
+            mid = cout // 4
+            for b in range(depth):
+                p = f"{bb}stages.{s}.blocks.{b}."
+                if b == 0:
+                    L.append(GemmLayer(f"s{s}b{b}.wd", p + "downsample.conv.weight", None, cout, cin, 1, cout, cin,
+                                       True))
+                c1 = cin if b == 0 else cout
+                L.append(GemmLayer(f"s{s}b{b}.w1", p + "conv1.weight", None, mid, c1, 1, mid, c1, True))
+                L.append(GemmLayer(f"s{s}b{b}.w2", p + "conv2.weight", None, mid, mid, 9, mid, mid, True))
+                L.append(GemmLayer(f"s{s}b{b}.w3", p + "conv3.weight", None, cout, mid, 1, cout, mid, True))
+            cin = cout
+        c_proj = 1024
+    else:
+        c_proj = 3 * 16 * 16                        # Conv2d(3, D, 16, stride 16) over patchify's columns
+    L.append(GemmLayer("proj", pm + "patch_embed.proj.weight", pm + "patch_embed.proj.bias", D, c_proj, 1, D, c_proj,
+                       False))
+    for i in range(arch["depth"]):
+        p = f"{pm}blocks.{i}."
+        for key, name, n, c in (("qkv", "attn.qkv", 3 * D, D), ("proj", "attn.proj", D, D),
+                                ("fc1", "mlp.fc1", 4 * D, D), ("fc2", "mlp.fc2", D, 4 * D)):
+            L.append(GemmLayer(f"blk{i}.{key}", p + name + ".weight", p + name + ".bias", n, c, 1, n, c, False))
+    for n in ((3, 4) if arch["hybrid"] else (1, 2, 3, 4)):
+        p = f"pretrained.act_postprocess{n}."
+        L.append(GemmLayer(f"pp{n}", p + "3.weight", p + "3.bias", rn_in[n - 1], D, 1, rn_pad[n - 1], D, False))
+    if not arch["hybrid"]:
+        # ConvTranspose2d(c, c, k, stride k), weight [in][out][k][k] read as n = in, c = out, taps = (ky, kx): the
+        # forward operand [in][(ky, kx, out)] is the input-gradient operand, the dgrad operand's tap blocks the
+        # forward's per-phase 1x1 operands
+        for n, k in ((1, 4), (2, 2)):
+            p, c, cp = f"pretrained.act_postprocess{n}.", rn_in[n - 1], rn_pad[n - 1]
+            L.append(GemmLayer(f"pp{n}t", p + "4.weight", p + "4.bias", c, c, k * k, cp, cp, False))
+    L.append(GemmLayer("pp4s", "pretrained.act_postprocess4.4.weight", "pretrained.act_postprocess4.4.bias",
+                       D, D, 9, D, D, False))
+    for n in (1, 2, 3, 4):
+        L.append(GemmLayer(f"rn{n}", f"scratch.layer{n}_rn.weight", None, 256, rn_in[n - 1], 9, 256, rn_pad[n - 1],
+                           False))
+    for n in (1, 2, 3, 4):
+        p = f"scratch.refinenet{n}."
+        L.append(GemmLayer(f"ff{n}.out", p + "out_conv.weight", p + "out_conv.bias", 256, 256, 1, 256, 256, False))
+        for u in ((2,) if n == 4 else (1, 2)):      # refinenet4.resConfUnit1 is dead (blocks.py:328-330)
+            L += _rcu_layers(n, u)
+    L.append(GemmLayer("head0", "scratch.output_conv.0.weight", "scratch.output_conv.0.bias", 128, 256, 9, 128, 256,
+                       False))
+    # the train forward carries head conv2's 32 channels zero-padded to 64 (its unfused ReLU output feeds the backward)
+    L.append(GemmLayer("head2", "scratch.output_conv.2.weight", "scratch.output_conv.2.bias", 32, 128, 9, 64, 128,
+                       False))
+    return L
+
+
+def _forward_vectors(backbone: str) -> List[str]:
+    """The parameters besides the GEMM layers' biases that dpt_forward reads as fp32 tensors: the norm affines, the cls
+    token, the readout Linear biases and the head's final 1x1 conv (32 -> num_channels)."""
+    return [k for k, _ in state_dict_spec(backbone=backbone)
+            if (".norm" in k and not k.startswith("pretrained.model.norm."))   # the final ViT norm is dead (vit.py:153)
+            or k.endswith(("cls_token", "0.project.0.bias")) or k.startswith("scratch.output_conv.4.")]
+
+
+def _gemm_operand(w: torch.Tensor, layer: GemmLayer) -> torch.Tensor:
+    """Forward operand of `layer`, fp32 [n_pad][taps * c_pad], from its weight `w`: standardised if the layer says so,
+    read as [n][c][taps], zero-padded to [n_pad][c_pad], taken tap-major."""
+    w = _std_weight(w) if layer.standardize else w.float()
+    w = F.pad(w.reshape(layer.n, layer.c, layer.taps), (0, 0, 0, layer.c_pad - layer.c, 0, layer.n_pad - layer.n))
+    return w.permute(0, 2, 1).reshape(layer.n_pad, -1)
 
 
 def _decoder_spec(add, num_channels: int, features: int, rn_in) -> None:
@@ -311,86 +399,37 @@ class DPTDepthModel(nn.Module):
     # ------------------------------------------------------------------ weight pre-pack (one-time)
     @torch.no_grad()
     def _prepack(self, device) -> dict:
+        """The forward's operand table (schema: dpt_forward) from the state dict, in its own storage: packed state never
+        aliases a parameter."""
         sd = {k: v.detach().to(device) for k, v in self.state_dict().items()}
-        f32 = lambda k: sd[k].float().clone().contiguous()      # own storage: packed state never aliases a parameter
-        wdt = torch.float32 if self._precision == "fp32" else torch.bfloat16
-        bf = lambda t: t.to(wdt).contiguous()                      # operand storage type of the GEMM weights
-        _pack = ops.pack_conv_weight
-        pack_w = lambda w: _pack(w, wdt)
-        pk: dict = {}
-        pm = "pretrained.model."
-        D, depth = self.arch["embed"], self.arch["depth"]
+        wdt = torch.float32 if self._precision == "fp32" else torch.bfloat16    # operand storage type of the GEMMs
+        gemm = {}
+        vec = {k: sd[k].float().clone() for k in _forward_vectors(self.backbone)}
+        # refinenet4.resConfUnit1 is dead in the forward but packed (and broadcast) with the other decoder layers
+        for layer in gemm_layers(self.arch) + _rcu_layers(4, 1):
+            if layer.key == "head2":
+                layer = layer._replace(n_pad=layer.n)      # unpadded: the fused head tail launches at block_n 32
+            w = _gemm_operand(sd[layer.weight], layer)
+            if layer.key in ("pp1t", "pp2t"):
+                # ConvTranspose2d(c, c, k, stride k) (vit.py:216-225, 240-249): k*k independent 1x1 convolutions, one
+                # per output phase t = (dy, dx): phases[t] = weight[:, :, dy, dx]^T, [out][in]
+                w = w.view(layer.n_pad, layer.taps, layer.c_pad).permute(1, 2, 0)
+                gemm[layer.key + ".phases"] = w.to(wdt).contiguous()
+            else:
+                gemm[layer.key] = w.to(wdt).contiguous()
+            if layer.bias is not None:
+                vec[layer.bias] = F.pad(sd[layer.bias].float(), (0, layer.n_pad - layer.n))
         if self.arch["hybrid"]:
-            bb = pm + "patch_embed.backbone."
             # stem 7x7: [64,3,7,7] -> [64, (ky,kx,c)=147] padded to 160 columns
-            w = _std_weight(sd[bb + "stem.conv.weight"]).permute(0, 2, 3, 1).reshape(64, 147)
-            pk["stem_w"] = bf(F.pad(w, (0, 13)))
-            pk["stem_g"], pk["stem_b"] = f32(bb + "stem.norm.weight"), f32(bb + "stem.norm.bias")
-            blocks = []
-            for s, (cout, dep) in enumerate(_STAGES):
-                for b in range(dep):
-                    p = f"{bb}stages.{s}.blocks.{b}."
-                    e = {"stride": 2 if (b == 0 and s > 0) else 1, "cout": cout, "mid": cout // 4}
-                    if b == 0:
-                        e["wd"] = pack_w(_std_weight(sd[p + "downsample.conv.weight"]))
-                        e["gd"], e["bd"] = f32(p + "downsample.norm.weight"), f32(p + "downsample.norm.bias")
-                    for i in (1, 2, 3):
-                        e[f"w{i}"] = pack_w(_std_weight(sd[p + f"conv{i}.weight"]))
-                        e[f"g{i}"], e[f"b{i}"] = f32(p + f"norm{i}.weight"), f32(p + f"norm{i}.bias")
-                    blocks.append((s, b, e))
-            pk["rn_blocks"] = blocks
-            pk["proj_w"] = pack_w(sd[pm + "patch_embed.proj.weight"])
-        else:
-            # PatchEmbed conv [D,3,16,16]: its row-major flattening is the GEMM weight for odb_patchify's columns
-            pk["proj_w"] = bf(sd[pm + "patch_embed.proj.weight"].reshape(D, -1))
-        pk["proj_b"] = f32(pm + "patch_embed.proj.bias")
-        pk["cls"] = f32(pm + "cls_token").reshape(-1)
-        pk["pos"] = f32(pm + "pos_embed")                       # [1,577,D] fp32 master copy
-        vit = []
-        for i in range(depth):
-            p = f"{pm}blocks.{i}."
-            vit.append({
-                "ln1": (f32(p + "norm1.weight"), f32(p + "norm1.bias")),
-                "qkv": (bf(sd[p + "attn.qkv.weight"]), f32(p + "attn.qkv.bias")),
-                "proj": (bf(sd[p + "attn.proj.weight"]), f32(p + "attn.proj.bias")),
-                "ln2": (f32(p + "norm2.weight"), f32(p + "norm2.bias")),
-                "fc1": (bf(sd[p + "mlp.fc1.weight"]), f32(p + "mlp.fc1.bias")),
-                "fc2": (bf(sd[p + "mlp.fc2.weight"]), f32(p + "mlp.fc2.bias")),
-            })
-        pk["vit"] = vit
+            w = _std_weight(sd["pretrained.model.patch_embed.backbone.stem.conv.weight"]).permute(0, 2, 3, 1)
+            gemm["stem"] = F.pad(w.reshape(64, 147), (0, 13)).to(wdt).contiguous()
+        D = self.arch["embed"]
         for n in ((3, 4) if self.arch["hybrid"] else (1, 2, 3, 4)):
-            p = f"pretrained.act_postprocess{n}."
-            wfull = bf(sd[p + "0.project.0.weight"])               # [D, 2D]
-            pk[f"ro{n}_wfull"] = wfull
-            pk[f"ro{n}_wtok"] = wfull[:, :D].contiguous()          # token half of the split Linear
-            pk[f"ro{n}_b"] = f32(p + "0.project.0.bias")
-            cp = self._rn_pad[n - 1]
-            pk[f"pp{n}_w"] = pack_w(_pad_to(sd[p + "3.weight"], 0, cp))
-            pk[f"pp{n}_b"] = _pad_to(f32(p + "3.bias"), 0, cp)
-        pk["pp4s_w"] = pack_w(sd["pretrained.act_postprocess4.4.weight"])
-        pk["pp4s_b"] = f32("pretrained.act_postprocess4.4.bias")
-        if not self.arch["hybrid"]:
-            # ConvTranspose2d(c, c, k, stride k) (vit.py:216-225, 240-249): k*k independent 1x1 convolutions,
-            # one per output phase (dy, dx): W_phase[out][in] = weight[in][out][dy][dx]
-            for n, k in ((1, 4), (2, 2)):
-                cp = self._rn_pad[n - 1]
-                w = _pad_to(_pad_to(sd[f"pretrained.act_postprocess{n}.4.weight"].float(), 0, cp), 1, cp)
-                pk[f"pp{n}t_w"] = [[bf(w[:, :, dy, dx].t()) for dx in range(k)] for dy in range(k)]
-                pk[f"pp{n}t_b"] = _pad_to(f32(f"pretrained.act_postprocess{n}.4.bias"), 0, cp)
-        for n in (1, 2, 3, 4):
-            pk[f"rn{n}_w"] = pack_w(_pad_to(sd[f"scratch.layer{n}_rn.weight"], 1, self._rn_pad[n - 1]))
-            p = f"scratch.refinenet{n}."
-            pk[f"ff{n}_out"] = (pack_w(sd[p + "out_conv.weight"]), f32(p + "out_conv.bias"))
-            for u in (1, 2):
-                pk[f"ff{n}_rcu{u}"] = tuple(
-                    (pack_w(sd[f"{p}resConfUnit{u}.conv{cv}.weight"]),
-                     f32(f"{p}resConfUnit{u}.conv{cv}.bias")) for cv in (1, 2))
-        pk["head0"] = (pack_w(sd["scratch.output_conv.0.weight"]), f32("scratch.output_conv.0.bias"))
-        pk["head2"] = (pack_w(sd["scratch.output_conv.2.weight"]), f32("scratch.output_conv.2.bias"))
-        pk["head4"] = (sd["scratch.output_conv.4.weight"].float().reshape(self.num_channels, 32).contiguous(),
-                       f32("scratch.output_conv.4.bias"))
-        pk["pos_cache"] = {}
-        return pk
+            wfull = sd[f"pretrained.act_postprocess{n}.0.project.0.weight"].to(wdt, copy=True)     # [D, 2D]
+            gemm[f"ro{n}.full"] = wfull
+            gemm[f"ro{n}.tok"] = wfull[:, :D].contiguous()                                # token half of the Linear
+        pos = sd["pretrained.model.pos_embed"].float().clone()                              # [1,577,D] fp32 master copy
+        return {"gemm": gemm, "vec": vec, "pos": pos, "pos_cache": {}}
 
     # ------------------------------------------------------------------ forward
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -521,46 +560,51 @@ def _resnet_features(x, pk, ws, buf, fp32: bool, taps, S):
     cols = buf("stem_cols", (B * h2 * w2, 160))
     ops.stem_im2col(x, cols)
     s0 = buf("stem_conv", (B, h2, w2, 64))
-    st = conv_stats(ops.conv1x1, cols.view(B, h2, w2, 160), pk["stem_w"], out=s0)
+    gemm, vec = pk["gemm"], pk["vec"]
+    bb = "pretrained.model.patch_embed.backbone."
+    st = conv_stats(ops.conv1x1, cols.view(B, h2, w2, 160), gemm["stem"], out=s0)
     t = buf("stem_pool", (B, h2 // 2, w2 // 2, 64))
-    ops.stem_gn_relu_maxpool(s0, st, pk["stem_g"], pk["stem_b"], t)
+    ops.stem_gn_relu_maxpool(s0, st, vec[bb + "stem.norm.weight"], vec[bb + "stem.norm.bias"], t)
     S["stem"] = (cols, s0, st, t)
     if taps is not None:
         taps["stem_conv"], taps["stem_pool"] = s0, t
     feats, blocks = [], []
     hh, ww = h2 // 2, w2 // 2
-    for s, b, e in pk["rn_blocks"]:
-        stride, cout, mid = e["stride"], e["cout"], e["mid"]
+    for s, b in [(s, b) for s, (_, depth) in enumerate(_STAGES) for b in range(depth)]:
+        cout, mid, stride = _STAGES[s][0], _STAGES[s][0] // 4, (2 if b == 0 and s > 0 else 1)
         ho, wo = hh // stride, ww // stride
-        tag = f"s{s}b{b}"
+        tag, p = f"s{s}b{b}", f"{bb}stages.{s}.blocks.{b}."
+        gn = lambda norm: (vec[p + norm + ".weight"], vec[p + norm + ".bias"])      # GroupNorm affine
         # p: the block's parameter-name prefix, for the backward's gradient lookups
-        rec = {"tag": tag, "p": f"pretrained.model.patch_embed.backbone.stages.{s}.blocks.{b}.", "stride": stride,
-               "t_in": t, "b": b, "s": s}
+        rec = {"tag": tag, "p": p, "stride": stride, "t_in": t, "b": b, "s": s}
         shortcut, sc_stats = t, None
         if b == 0:
             d = buf(tag + "_ds", (B, ho, wo, cout))
-            sc_stats = conv_stats(ops.conv1x1, t[:, ::stride, ::stride, :] if stride > 1 else t, e["wd"], out=d)
+            sc_stats = conv_stats(ops.conv1x1, t[:, ::stride, ::stride, :] if stride > 1 else t, gemm[tag + ".wd"],
+                                  out=d)
             shortcut = d
             rec.update(d=d, std=sc_stats)
         y1 = buf(tag + "_y1", (B, hh, ww, mid))
-        st1 = conv_stats(ops.conv1x1, t, e["w1"], out=y1)
+        st1 = conv_stats(ops.conv1x1, t, gemm[tag + ".w1"], out=y1)
         a1 = buf(tag + "_a1", (B, hh, ww, mid))
-        ops.groupnorm_apply(y1, st1, e["g1"], e["b1"], a1, relu=True)
+        ops.groupnorm_apply(y1, st1, *gn("norm1"), a1, relu=True)
         y2 = buf(tag + "_y2", (B, ho, wo, mid))
         if stride == 1:
-            st2 = conv_stats(ops.conv3x3, a1, e["w2"], out=y2)
+            st2 = conv_stats(ops.conv3x3, a1, gemm[tag + ".w2"], out=y2)
         else:
-            st2 = conv_stats(lambda a, w_, o, **kw: ops.conv3x3_s2(a, w_, o, "same", **kw), a1, e["w2"], out=y2)
+            st2 = conv_stats(lambda a, w_, o, **kw: ops.conv3x3_s2(a, w_, o, "same", **kw), a1, gemm[tag + ".w2"],
+                             out=y2)
         a2 = buf(tag + "_a2", (B, ho, wo, mid))
-        ops.groupnorm_apply(y2, st2, e["g2"], e["b2"], a2, relu=True)
+        ops.groupnorm_apply(y2, st2, *gn("norm2"), a2, relu=True)
         y3 = buf(tag + "_y3", (B, ho, wo, cout))
-        st3 = conv_stats(ops.conv1x1, a2, e["w3"], out=y3)
+        st3 = conv_stats(ops.conv1x1, a2, gemm[tag + ".w3"], out=y3)
         out = buf(tag + "_out", (B, ho, wo, cout))
         if b == 0:
-            ops.groupnorm_apply(y3, st3, e["g3"], e["b3"], out, relu=True, res=shortcut,
-                                res_stats=sc_stats, res_gamma=e["gd"], res_beta=e["bd"])
+            gd, bd = gn("downsample.norm")
+            ops.groupnorm_apply(y3, st3, *gn("norm3"), out, relu=True, res=shortcut, res_stats=sc_stats, res_gamma=gd,
+                                res_beta=bd)
         else:
-            ops.groupnorm_apply(y3, st3, e["g3"], e["b3"], out, relu=True, res=shortcut)
+            ops.groupnorm_apply(y3, st3, *gn("norm3"), out, relu=True, res=shortcut)
         rec.update(y1=y1, st1=st1, a1=a1, y2=y2, st2=st2, a2=a2, y3=y3, st3=st3, out=out)
         blocks.append(rec)
         t, hh, ww = out, ho, wo
@@ -576,11 +620,18 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
                 ws: _Workspace, taps: Optional[dict] = None, save: Optional[dict] = None) -> torch.Tensor:
     """The launch sequence of one DPT forward, for inference (`DPTDepthModel`) and training (`train.TrainEngine`).
 
-    `pk` holds the operands in the schema of `DPTDepthModel._prepack`, `ws` owns the activations, `taps` (inference
-    diagnostics) receives named intermediates.  `x` is fp32 contiguous [B,3,H,W]; returns the fp32 NCHW output buffer.
-    With `save` given, every activation the hand-written backward reads is kept and recorded in it.  That changes the
-    sequence at five points, marked (1)-(5) below: the backward needs each ViT block's activations, the attention's
-    log-sum-exp, the pre-activations of the GELUs, and the head's intermediates that the fused epilogue never stores."""
+    `pk` is the operand table both packers fill (`DPTDepthModel._prepack`, `train.TrainEngine`):
+      pk["gemm"]  GEMM operands by layer key: those of `gemm_layers(arch)` (the ConvTransposes "pp{n}t" are read as
+                  "pp{n}t.phases" [k*k][c][c], one [out][in] 1x1 operand per output phase), the hybrid's "stem"
+                  [64][160] (im2col columns), the readout Linear "ro{n}.full" [D][2D] and its token half "ro{n}.tok";
+      pk["vec"]   fp32 tensors by parameter name: the layers' biases, zero-padded to n_pad where the forward reads the
+                  layer padded, and the norm affines, cls token, readout biases and the head's last 1x1 conv;
+      pk["pos"]   pos_embed in fp32 (inference), and pk["pos_cache"] the patch rows resized to a grid (`_pos_rows`).
+    `ws` owns the activations, `taps` (inference diagnostics) receives named intermediates.  `x` is fp32 contiguous
+    [B,3,H,W]; returns the fp32 NCHW output buffer.  With `save` given, every activation the hand-written backward reads
+    is kept and recorded in it.  That changes the sequence at five points, marked (1)-(5) below: the backward needs each
+    ViT block's activations, the attention's log-sum-exp, the pre-activations of the GELUs, and the head's intermediates
+    that the fused epilogue never stores."""
     B, _, H, W = x.shape
     fp32 = precision == "fp32"
     adt = torch.float32 if fp32 else torch.bfloat16            # activation storage type
@@ -590,6 +641,8 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
     S.update(x=x, B=B, H=H, W=W)
 
     D, heads, depth, hooks = arch["embed"], arch["heads"], arch["depth"], arch["hooks"]
+    gemm, vec = pk["gemm"], pk["vec"]
+    pm = "pretrained.model."
     if arch["hybrid"]:
         layer_1, layer_2, f3 = _resnet_features(x, pk, ws, buf, fp32, taps, S)
         gh, gw = f3.shape[1], f3.shape[2]
@@ -625,57 +678,62 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
 
     # ---------------- tokens: patch proj + cls + pos (vit.py:131-147)
     pos0, pos_b = _pos_rows(pk, gh, gw, B)
-    ops.write_cls_row(xs[0], pk["cls"], pos0)
+    ops.write_cls_row(xs[0], vec[pm + "cls_token"].view(-1), pos0)
+    proj_b = vec[pm + "patch_embed.proj.bias"]
     if arch["hybrid"]:
-        ops.linear(f3.view(B, 1, gh * gw, 1024), pk["proj_w"], xs[0][:, 1:, :].unsqueeze(1), bias=pk["proj_b"],
+        ops.linear(f3.view(B, 1, gh * gw, 1024), gemm["proj"], xs[0][:, 1:, :].unsqueeze(1), bias=proj_b,
                    residual=pos_b.unsqueeze(1))
     else:
         cols = buf("patch_cols", (B, 1, gh * gw, 3 * 16 * 16))
         ops.patchify(x, cols.view(B * gh * gw, -1), 16)
-        ops.linear(cols, pk["proj_w"], xs[0][:, 1:, :].unsqueeze(1), bias=pk["proj_b"], residual=pos_b.unsqueeze(1))
+        ops.linear(cols, gemm["proj"], xs[0][:, 1:, :].unsqueeze(1), bias=proj_b, residual=pos_b.unsqueeze(1))
         S["cols"] = cols
     if taps is not None:
         taps["tokens_in"] = xs[0].clone()
 
     # ---------------- ViT blocks (vit.py:150-151); final norm is dead compute and skipped
-    for i, (blk, v) in enumerate(zip(pk["vit"], vit)):
-        ops.layernorm(xs[i], blk["ln1"][0], blk["ln1"][1], v["h1"])
-        ops.linear(v["h1"].view(rows, -1), blk["qkv"][0], v["qkv"].view(rows, -1), bias=blk["qkv"][1])
+    for i, v in enumerate(vit):
+        p, blk = f"{pm}blocks.{i}.", f"blk{i}."
+        ops.layernorm(xs[i], vec[p + "norm1.weight"], vec[p + "norm1.bias"], v["h1"])
+        ops.linear(v["h1"].view(rows, -1), gemm[blk + "qkv"], v["qkv"].view(rows, -1), bias=vec[p + "attn.qkv.bias"])
         ops.attention(v["qkv"], v["att"], heads=heads, scale=0.125, lse=v["lse"])
-        ops.linear(v["att"].view(rows, -1), blk["proj"][0], xm[i].view(rows, -1), bias=blk["proj"][1],
+        ops.linear(v["att"].view(rows, -1), gemm[blk + "proj"], xm[i].view(rows, -1), bias=vec[p + "attn.proj.bias"],
                    residual=xs[i].view(rows, -1))
-        ops.layernorm(xm[i], blk["ln2"][0], blk["ln2"][1], v["h2"])
+        ops.layernorm(xm[i], vec[p + "norm2.weight"], vec[p + "norm2.bias"], v["h2"])
         h2, mlp = v["h2"].view(rows, -1), v["mlp"].view(rows, -1)
+        fc1, fc1_b = gemm[blk + "fc1"], vec[p + "mlp.fc1.bias"]
         if save is None:
-            ops.linear(h2, blk["fc1"][0], mlp, bias=blk["fc1"][1], act=ops.ACT_GELU)
+            ops.linear(h2, fc1, mlp, bias=fc1_b, act=ops.ACT_GELU)
         elif fp32:      # (3) the backward needs the pre-activation u as well as gelu(u)
-            ops.linear(h2, blk["fc1"][0], v["u"].view(rows, -1), bias=blk["fc1"][1])
+            ops.linear(h2, fc1, v["u"].view(rows, -1), bias=fc1_b)
             bwd.gelu_fwd(v["u"], v["mlp"])
         else:           # (3) one pass: the pre-activation and gelu of the same fp32 value
-            ops.linear(h2, blk["fc1"][0], v["u"].view(rows, -1), bias=blk["fc1"][1], out2=mlp, out2_act=ops.ACT_GELU)
-        ops.linear(mlp, blk["fc2"][0], xs[i + 1].view(rows, -1), bias=blk["fc2"][1], residual=xm[i].view(rows, -1))
+            ops.linear(h2, fc1, v["u"].view(rows, -1), bias=fc1_b, out2=mlp, out2_act=ops.ACT_GELU)
+        ops.linear(mlp, gemm[blk + "fc2"], xs[i + 1].view(rows, -1), bias=vec[p + "mlp.fc2.bias"],
+                   residual=xm[i].view(rows, -1))
         if taps is not None:
             taps[f"tokens_{i}"] = xs[i + 1].clone()
     hooked = [xs[hk + 1] for hk in hooks]
 
     # ---------------- reassemble (vit.py:66-97, 185-290 / 431-462)
     def readout(tk32, n, cout):
+        p = f"pretrained.act_postprocess{n}."
         tk = tk32
         if not fp32:                                   # the hooked activation leaves the fp32 stream as a bf16 operand
             tk = buf(f"ro{n}_tok", (B, ntok, D))
             ops.cast_f32_bf16(tk32, tk)
         cb = buf(f"ro{n}_cb", (B, D), f32)
-        ops.readout_cls_bias(pk[f"ro{n}_wfull"], pk[f"ro{n}_b"], tk, cb)
+        ops.readout_cls_bias(gemm[f"ro{n}.full"], vec[p + "0.project.0.bias"], tk, cb)
         r = buf(f"ro{n}_r", (B, 1, gh * gw, D))
         pre = None
         if save is None:
-            ops.linear(tk[:, 1:, :].unsqueeze(1), pk[f"ro{n}_wtok"], r, bias=cb, bias_per_image=True, act=ops.ACT_GELU)
+            ops.linear(tk[:, 1:, :].unsqueeze(1), gemm[f"ro{n}.tok"], r, bias=cb, bias_per_image=True, act=ops.ACT_GELU)
         else:           # (4) the backward needs the pre-activation: GELU by a separate kernel
             pre = buf(f"ro{n}_pre", (B, 1, gh * gw, D))
-            ops.linear(tk[:, 1:, :].unsqueeze(1), pk[f"ro{n}_wtok"], pre, bias=cb, bias_per_image=True)
+            ops.linear(tk[:, 1:, :].unsqueeze(1), gemm[f"ro{n}.tok"], pre, bias=cb, bias_per_image=True)
             bwd.gelu_fwd(pre, r)
         o = buf(f"pp{n}", (B, gh, gw, cout))
-        ops.conv1x1(r.view(B, gh, gw, D), pk[f"pp{n}_w"], o, bias=pk[f"pp{n}_b"])
+        ops.conv1x1(r.view(B, gh, gw, D), gemm[f"pp{n}"], o, bias=vec[p + "3.bias"])
         S[f"ro{n}"] = dict(tk=tk, tk32=tk32, pre=pre, r=r, o=o)
         return o
 
@@ -684,9 +742,10 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
         input, stored through a strided view of the output (no scatter kernel)."""
         c = t.shape[3]
         o = buf(f"pp{n}t", (B, gh * k, gw * k, c))
+        phases, bias = gemm[f"pp{n}t.phases"], vec[f"pretrained.act_postprocess{n}.4.bias"]
         for dy in range(k):
             for dx in range(k):
-                ops.conv1x1(t, pk[f"pp{n}t_w"][dy][dx], o[:, dy::k, dx::k, :], bias=pk[f"pp{n}t_b"])
+                ops.conv1x1(t, phases[dy * k + dx], o[:, dy::k, dx::k, :], bias=bias)
         return o
 
     rn_in = _rn_pad(arch)
@@ -699,7 +758,7 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
         layer_3 = readout(hooked[2], 3, rn_in[2])
         u4 = readout(hooked[3], 4, rn_in[3])
     layer_4 = buf("pp4s", (B, gh // 2, gw // 2, rn_in[3]))
-    ops.conv3x3_s2(u4, pk["pp4s_w"], layer_4, "sym1", bias=pk["pp4s_b"])
+    ops.conv3x3_s2(u4, gemm["pp4s"], layer_4, "sym1", bias=vec["pretrained.act_postprocess4.4.bias"])
     S["layers"] = (layer_1, layer_2, layer_3, layer_4)
 
     # ---------------- scratch.layerN_rn (dpt_depth.py:73-76): raw + relu copies feed the RCUs
@@ -707,17 +766,17 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
     for n, l in zip((1, 2, 3, 4), S["layers"]):
         shp = (B, l.shape[1], l.shape[2], _FEATURES)
         raw, rl = buf(f"rn{n}_raw", shp), buf(f"rn{n}_relu", shp)
-        ops.conv3x3(l, pk[f"rn{n}_w"], raw, out2=rl)
+        ops.conv3x3(l, gemm[f"rn{n}"], raw, out2=rl)
         rn_raw.append(raw)
         rn_relu.append(rl)
     S.update(rn_raw=rn_raw, rn_relu=rn_relu)
 
     # ---------------- RefineNet fusion (dpt_depth.py:78-81; blocks.py:263-341)
     def rcu(n, u, x_raw, x_relu, out):
-        (w1, b1), (w2, b2) = pk[f"ff{n}_rcu{u}"]
+        key, p = f"ff{n}.rcu{u}.c", f"scratch.refinenet{n}.resConfUnit{u}.conv"
         tmid = buf(f"ff{n}_rcu{u}_t", x_raw.shape)
-        ops.conv3x3(x_relu, w1, tmid, bias=b1, act=ops.ACT_RELU)       # relu(conv1(relu(x)))
-        ops.conv3x3(tmid, w2, out, bias=b2, residual=x_raw)             # conv2(.) + x
+        ops.conv3x3(x_relu, gemm[key + "1"], tmid, bias=vec[p + "1.bias"], act=ops.ACT_RELU)   # relu(conv1(relu(x)))
+        ops.conv3x3(tmid, gemm[key + "2"], out, bias=vec[p + "2.bias"], residual=x_raw)       # conv2(.) + x
         S[f"ff{n}.rcu{u}"] = dict(x_raw=x_raw, x_relu=x_relu, tmid=tmid)
 
     def fusion_tail(n, s_raw, s_relu):
@@ -726,8 +785,7 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
         y = buf(f"ff{n}_y", s_raw.shape)
         rcu(n, 2, s_raw, s_relu, y)
         z = buf(f"ff{n}_z", s_raw.shape)
-        w, bias = pk[f"ff{n}_out"]
-        ops.conv1x1(y, w, z, bias=bias)
+        ops.conv1x1(y, gemm[f"ff{n}.out"], z, bias=vec[f"scratch.refinenet{n}.out_conv.bias"])
         S[f"ff{n}"] = dict(y=y, z=z)
         return z
 
@@ -747,13 +805,13 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
     ops.upsample2x_add(z, path_1)
 
     # ---------------- head (dpt_depth.py:91-99)
-    w0, b0 = pk["head0"]
     h1 = buf("head_h1", (B, path_1.shape[1], path_1.shape[2], _FEATURES // 2))
-    ops.conv3x3(path_1, w0, h1, bias=b0)
+    ops.conv3x3(path_1, gemm["head0"], h1, bias=vec["scratch.output_conv.0.bias"])
     h1u = buf("head_h1u", (B, H, W, _FEATURES // 2))
     ops.upsample2x_add(h1, h1u)
     out = buf("out", (B, num_channels, H, W), f32)
-    (w2, b2), (w4, b4) = pk["head2"], pk["head4"]
+    w2, b2 = gemm["head2"], vec["scratch.output_conv.2.bias"]
+    w4, b4 = vec["scratch.output_conv.4.weight"].view(num_channels, 32), vec["scratch.output_conv.4.bias"]
     if save is not None:
         # (5) unfused: the backward needs relu(conv2) (32 channels carried zero-padded to 64) and the output map
         a = buf("head_a", (B, H, W, 64))

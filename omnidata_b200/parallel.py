@@ -73,18 +73,13 @@ def broadcast_state_dict(module: torch.nn.Module, src: int = 0, bucket_bytes: in
     return total
 
 
-def _packed_tensors(obj, prefix=""):
-    """Deterministic (path, tensor) walk of a packed-weights structure (dicts / lists / tuples of tensors)."""
-    if torch.is_tensor(obj):
-        yield prefix, obj
-    elif isinstance(obj, dict):
-        for k in sorted(obj, key=str):
-            if k == "pos_cache":
-                continue
-            yield from _packed_tensors(obj[k], f"{prefix}.{k}")
-    elif isinstance(obj, (list, tuple)):
-        for i, v in enumerate(obj):
-            yield from _packed_tensors(v, f"{prefix}[{i}]")
+def _packed_tensors(pk):
+    """Deterministic (name, tensor) walk of a packed operand table (schema: model.dpt_forward): pos_embed, then the
+    GEMM operands and the fp32 vectors in key order.  The pos_cache derived from pos_embed is left out."""
+    yield "pos", pk["pos"]
+    for table in ("gemm", "vec"):
+        for k in sorted(pk[table]):
+            yield f"{table}.{k}", pk[table][k]
 
 
 def broadcast_packed_weights(model, device, src: int = 0) -> int:

@@ -40,7 +40,8 @@ import torch
 
 from . import bwd, ops
 from ._capi import OdbError
-from .model import _ARCH, _STAGES, DPTDepthModel, _Workspace, dpt_forward, resize_pos_grid
+from .model import (_ARCH, _STAGES, DPTDepthModel, _forward_vectors, _Workspace, dpt_forward, gemm_layers,
+                    resize_pos_grid)
 
 
 def _parity_dgrad_plan(mode: str):
@@ -272,144 +273,63 @@ class TrainEngine:
 
     # ------------------------------------------------------------------ weight table / per-step packing
     def _build_layer_table(self):
-        """(key, param name, n, c, taps, n_pad, c_pad, standardize) for every GEMM weight, the parameter read as
-        [n][c][taps]; fwd [n_pad][taps*c_pad], bwd [c_pad][taps*n_pad] operand buffers are allocated once and re-filled
-        every step.  Padded rows / columns are zero and their gradients are dropped by the unpack pass."""
-        T = []
-        pm = "pretrained.model."
-        D = self.D
-        if self.hybrid:
-            bb = "pretrained.model.patch_embed.backbone."
-            cin = 64
-            for s, (cout, depth) in enumerate(_STAGES):
-                mid = cout // 4
-                for b in range(depth):
-                    p = f"{bb}stages.{s}.blocks.{b}."
-                    if b == 0:
-                        T.append((f"s{s}b{b}.wd", p + "downsample.conv.weight", cout, cin, 1, cout, cin, True))
-                    c1 = cin if b == 0 else cout
-                    T.append((f"s{s}b{b}.w1", p + "conv1.weight", mid, c1, 1, mid, c1, True))
-                    T.append((f"s{s}b{b}.w2", p + "conv2.weight", mid, mid, 9, mid, mid, True))
-                    T.append((f"s{s}b{b}.w3", p + "conv3.weight", cout, mid, 1, cout, mid, True))
-                cin = cout
-            T.append(("proj", pm + "patch_embed.proj.weight", D, 1024, 1, D, 1024, False))
-        else:                                                        # Conv2d(3, D, 16, stride 16) over patchify's columns
-            T.append(("proj", pm + "patch_embed.proj.weight", D, 768, 1, D, 768, False))
-        for i in range(self.depth):
-            p = f"{pm}blocks.{i}."
-            T.append((f"blk{i}.qkv", p + "attn.qkv.weight", 3 * D, D, 1, 3 * D, D, False))
-            T.append((f"blk{i}.proj", p + "attn.proj.weight", D, D, 1, D, D, False))
-            T.append((f"blk{i}.fc1", p + "mlp.fc1.weight", 4 * D, D, 1, 4 * D, D, False))
-            T.append((f"blk{i}.fc2", p + "mlp.fc2.weight", D, 4 * D, 1, D, 4 * D, False))
-        for n in self.readouts:
-            c, cp = self.rn_in[n - 1], self.rn_pad[n - 1]
-            T.append((f"pp{n}", f"pretrained.act_postprocess{n}.3.weight", c, D, 1, cp, D, False))
-        if not self.hybrid:
-            # ConvTranspose2d(c, c, k, stride k), weight [in][out][k][k] read as n = in, c = out, taps = (ky, kx): fwd
-            # [in][(ky, kx, out)] is the input-gradient operand, bwd's tap blocks are the forward's per-phase 1x1 operands
-            for n, k in ((1, 4), (2, 2)):
-                c, cp = self.rn_in[n - 1], self.rn_pad[n - 1]
-                T.append((f"pp{n}t", f"pretrained.act_postprocess{n}.4.weight", c, c, k * k, cp, cp, False))
-        T.append(("pp4s", "pretrained.act_postprocess4.4.weight", D, D, 9, D, D, False))
-        for n in (1, 2, 3, 4):
-            c, cp = self.rn_in[n - 1], self.rn_pad[n - 1]
-            T.append((f"rn{n}", f"scratch.layer{n}_rn.weight", 256, c, 9, 256, cp, False))
-        for n in (1, 2, 3, 4):
-            p = f"scratch.refinenet{n}."
-            T.append((f"ff{n}.out", p + "out_conv.weight", 256, 256, 1, 256, 256, False))
-            for u in ((2,) if n == 4 else (1, 2)):
-                for cv in (1, 2):
-                    T.append((f"ff{n}.rcu{u}.c{cv}", f"{p}resConfUnit{u}.conv{cv}.weight", 256, 256, 9, 256, 256, False))
-        T.append(("head0", "scratch.output_conv.0.weight", 128, 256, 9, 128, 256, False))
-        T.append(("head2", "scratch.output_conv.2.weight", 32, 128, 9, 64, 128, False))     # carried zero-padded to 64
-        self.layers = T
+        """The GEMM layers (model.gemm_layers): fwd [n_pad][taps*c_pad], bwd [c_pad][taps*n_pad] operand buffers are
+        allocated once and re-filled every step.  Padded rows / columns are zero and their gradients are dropped by the
+        unpack pass."""
+        self.layers = gemm_layers(self.model.arch)
+        self.layer = {L.key: L for L in self.layers}
         self.W: Dict[str, Tuple[torch.Tensor, torch.Tensor]] = {}
-        for key, pname, n, c, taps, n_pad, c_pad, std in T:
-            fwd = torch.zeros((n_pad, taps * c_pad), device=self.device, dtype=self.adt)
-            bwd_ = torch.zeros((c_pad, taps * n_pad), device=self.device, dtype=self.adt)
-            self.W[key] = (fwd, bwd_)
-        self.meta = {key: (pname, n, c, taps, n_pad, c_pad, std) for key, pname, n, c, taps, n_pad, c_pad, std in T}
+        for L in self.layers:
+            fwd = torch.zeros((L.n_pad, L.taps * L.c_pad), device=self.device, dtype=self.adt)
+            bwd_ = torch.zeros((L.c_pad, L.taps * L.n_pad), device=self.device, dtype=self.adt)
+            self.W[L.key] = (fwd, bwd_)
         # packed-layout wgrad scratch (the readouts' Linear halves, the stem)
+        D = self.D
         self.gp = torch.empty(D * 9 * D, device=self.device, dtype=torch.float32)
         # one-launch packing of all layers; packed-layout gradient buffers of the layers that need the unpack pass
         # (3x3 taps, weight standardisation or padding), converted by ONE launch per all-reduce bucket
-        self.pack_table = bwd.PackTable([(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c_pad, std)
-                                         for k, pn, n, c, taps, n_pad, c_pad, std in T], self.adt)
+        self.pack_table = self._new_pack_table(self.layers)
         self.gp_layer: Dict[str, torch.Tensor] = {}
         groups = {"decoder": [], "resnet": []}
-        for k, pn, n, c, taps, n_pad, c_pad, std in T:
-            if taps == 1 and not std and n_pad == n and c_pad == c:
+        for L in self.layers:
+            if L.taps == 1 and not L.standardize and L.n_pad == L.n and L.c_pad == L.c:
                 continue                                           # written straight into the flat gradient
-            gp = torch.zeros((n_pad, taps * c_pad), device=self.device, dtype=torch.float32)
-            self.gp_layer[k] = gp
-            tag = "resnet" if "backbone" in pn else "decoder"
-            groups[tag].append((pn, (gp, self.P[pn], self.G[pn], n, c, taps, c_pad, std)))
+            gp = torch.zeros((L.n_pad, L.taps * L.c_pad), device=self.device, dtype=torch.float32)
+            self.gp_layer[L.key] = gp
+            tag = "resnet" if "backbone" in L.weight else "decoder"
+            groups[tag].append((L.weight, (gp, self.P[L.weight], self.G[L.weight], L.n, L.c, L.taps, L.c_pad,
+                                           L.standardize)))
         self.unpack_groups = groups
         self.unpack_tables = {t: bwd.UnpackTable([it for _, it in v]) for t, v in groups.items() if v}
         self.zb = torch.zeros(4096, device=self.device, dtype=torch.float32)               # zero "bias" of the dgrad convs:
         #   selects the straight-line (bias / bias + residual) epilogues of the tensor-core kernel
 
+    def _new_pack_table(self, layers) -> bwd.PackTable:
+        return bwd.PackTable([(self.P[L.weight], *self.W[L.key], L.n, L.c, L.taps, L.n_pad, L.c_pad, L.standardize)
+                              for L in layers], self.adt)
+
     def _forward_operands(self) -> dict:
-        """The forward's operands in the schema of DPTDepthModel._prepack, as the engine's persistent tensors: the GEMM
-        operands pack() refills in place, and views of the flat fp32 master weights (biases, norm affines, cls, pos)."""
-        P = self.P
-        fw = lambda key: self.W[key][0]
-        pk = {}
+        """The forward's operand table (schema: model.dpt_forward) as the engine's persistent tensors: the GEMM operands
+        pack() refills in place, and views of the flat fp32 master weights, or zero-padded copies that pack() refreshes
+        where the forward reads a bias padded (head conv2, vitb16_384's 96-wide layer_1)."""
+        gemm = {L.key: self.W[L.key][0] for L in self.layers}
+        vec = {name: self.P[name] for name in _forward_vectors(self.backbone)}
+        for L in self.layers:
+            if L.bias is not None:
+                padded = L.n_pad != L.n
+                vec[L.bias] = self.buf(f"w.pad.{L.bias}", (L.n_pad,), torch.float32) if padded else self.P[L.bias]
         if self.hybrid:
-            bb = "pretrained.model.patch_embed.backbone."
-            pk = {"stem_w": self.buf("w.stem", (64, 160)), "stem_g": P[bb + "stem.norm.weight"],
-                  "stem_b": P[bb + "stem.norm.bias"]}
-            blocks = []
-            for s, (cout, depth) in enumerate(_STAGES):
-                for b in range(depth):
-                    p, tag = f"{bb}stages.{s}.blocks.{b}.", f"s{s}b{b}"
-                    e = {"stride": 2 if (b == 0 and s > 0) else 1, "cout": cout, "mid": cout // 4}
-                    if b == 0:
-                        e.update(wd=fw(tag + ".wd"), gd=P[p + "downsample.norm.weight"], bd=P[p + "downsample.norm.bias"])
-                    for i in (1, 2, 3):
-                        e.update({f"w{i}": fw(f"{tag}.w{i}"), f"g{i}": P[p + f"norm{i}.weight"], f"b{i}": P[p + f"norm{i}.bias"]})
-                    blocks.append((s, b, e))
-            pk["rn_blocks"] = blocks
-        pm = "pretrained.model."
-        # pos_cache: filled by every forward() with that step's rows
-        pk.update(proj_w=fw("proj"), proj_b=P[pm + "patch_embed.proj.bias"], cls=P[pm + "cls_token"].view(-1),
-                  pos_cache={})
-        pk["vit"] = []
-        for i in range(self.depth):
-            p = f"{pm}blocks.{i}."
-            lin = lambda name, bias: (fw(f"blk{i}.{name}"), P[p + bias])
-            pk["vit"].append({"ln1": (P[p + "norm1.weight"], P[p + "norm1.bias"]), "qkv": lin("qkv", "attn.qkv.bias"),
-                              "proj": lin("proj", "attn.proj.bias"), "ln2": (P[p + "norm2.weight"], P[p + "norm2.bias"]),
-                              "fc1": lin("fc1", "mlp.fc1.bias"), "fc2": lin("fc2", "mlp.fc2.bias")})
+            gemm["stem"] = self.buf("w.stem", (64, 160))
         D = self.D
         for n in self.readouts:
-            p = f"pretrained.act_postprocess{n}."
-            pk.update({f"ro{n}_wfull": self.buf(f"w.ro{n}.full", (D, 2 * D)), f"ro{n}_wtok": self.buf(f"w.ro{n}.tok", (D, D)),
-                       f"ro{n}_b": P[p + "0.project.0.bias"], f"pp{n}_w": fw(f"pp{n}"), f"pp{n}_b": self._padded_bias(p + "3.bias", n)})
+            gemm[f"ro{n}.full"] = self.buf(f"w.ro{n}.full", (D, 2 * D))
+            gemm[f"ro{n}.tok"] = self.buf(f"w.ro{n}.tok", (D, D))
         if not self.hybrid:
-            for n, k in ((1, 4), (2, 2)):
+            for n, k in ((1, 4), (2, 2)):                           # filled by pack() from the dgrad operand
                 cp = self.rn_pad[n - 1]
-                phases = self.buf(f"w.pp{n}t.phases", (k * k, cp, cp))     # filled by pack() from the dgrad operand
-                pk[f"pp{n}t_w"] = [[phases[dy * k + dx] for dx in range(k)] for dy in range(k)]
-                pk[f"pp{n}t_b"] = self._padded_bias(f"pretrained.act_postprocess{n}.4.bias", n)
-        pk["pp4s_w"], pk["pp4s_b"] = fw("pp4s"), P["pretrained.act_postprocess4.4.bias"]
-        for n in (1, 2, 3, 4):
-            p = f"scratch.refinenet{n}."
-            pk[f"rn{n}_w"] = fw(f"rn{n}")
-            pk[f"ff{n}_out"] = (fw(f"ff{n}.out"), P[p + "out_conv.bias"])
-            for u in ((2,) if n == 4 else (1, 2)):                  # refinenet4.resConfUnit1 is dead
-                pk[f"ff{n}_rcu{u}"] = tuple((fw(f"ff{n}.rcu{u}.c{cv}"), P[f"{p}resConfUnit{u}.conv{cv}.bias"]) for cv in (1, 2))
-        pk["head0"] = (fw("head0"), P["scratch.output_conv.0.bias"])
-        pk["head2"] = (fw("head2"), self.buf("head_b2pad", (64,), torch.float32))    # carried zero-padded to 64
-        pk["head4"] = (P["scratch.output_conv.4.weight"].view(self.C, 32), P["scratch.output_conv.4.bias"])
-        return pk
-
-    def _padded_bias(self, pname: str, n: int) -> torch.Tensor:
-        """The reassemble bias `pname` of layer_n as the forward reads it: the master weights' view, or, for a width
-        carried zero-padded (vitb16_384's 96-wide layer_1), a zero-padded copy that pack() refreshes."""
-        if self.rn_pad[n - 1] == self.rn_in[n - 1]:
-            return self.P[pname]
-        return self.buf(f"w.pad.{pname}", (self.rn_pad[n - 1],), torch.float32)
+                gemm[f"pp{n}t.phases"] = self.buf(f"w.pp{n}t.phases", (k * k, cp, cp))
+        # pos_cache: filled by every forward() with that step's rows
+        return {"gemm": gemm, "vec": vec, "pos_cache": {}}
 
     def _stale(self, trainable) -> set:
         """Source parameters whose derived forward operands must be (re)built: every trainable one (FlatAdam writes the
@@ -434,9 +354,7 @@ class TrainEngine:
             return self.pack_table
         tab = self._pack_tables.get(keys)
         if tab is None:
-            tab = self._pack_tables[keys] = bwd.PackTable(
-                [(self.P[pn], self.W[k][0], self.W[k][1], n, c, taps, n_pad, c_pad, std)
-                 for k, pn, n, c, taps, n_pad, c_pad, std in self.layers if k in keys], self.adt)
+            tab = self._pack_tables[keys] = self._new_pack_table([L for L in self.layers if L.key in keys])
         return tab
 
     @torch.no_grad()
@@ -447,66 +365,59 @@ class TrainEngine:
             self._packed_sig.clear()
         stale = None if trainable is None else self._stale(trainable)
         fresh = (lambda name: True) if stale is None else (lambda name: name in stale)
-        keys = tuple(k for k, pn, *_ in self.layers if fresh(pn))
+        keys = tuple(L.key for L in self.layers if fresh(L.weight))
         if keys:
             self.pack_table_for(keys).run()
-        P = self.P
+        P, gemm, vec = self.P, self.pk["gemm"], self.pk["vec"]
         bb = "pretrained.model.patch_embed.backbone."
         # stem 7x7 (3 input channels): [64,3,7,7] -> standardise -> [64, (ky,kx,c)=147] padded to 160 columns
         if self.hybrid and fresh(bb + "stem.conv.weight"):
             w = P[bb + "stem.conv.weight"]
             std_, mean = torch.std_mean(w, dim=[1, 2, 3], keepdim=True, unbiased=False)
             ws = ((w - mean) / (std_ + 1e-8)).permute(0, 2, 3, 1).reshape(64, 147)
-            stem = self.pk["stem_w"]
+            stem = gemm["stem"]
             stem.zero_()
             stem[:, :147].copy_(ws)
-        if fresh("scratch.output_conv.2.bias"):
-            b2 = self.pk["head2"][1]
-            b2.zero_()
-            b2[:32].copy_(P["scratch.output_conv.2.bias"])
+        for L in self.layers:                                        # the biases the forward reads zero-padded
+            if L.bias is not None and L.n_pad != L.n and fresh(L.bias):
+                vec[L.bias].zero_()
+                vec[L.bias][:L.n].copy_(P[L.bias])
         # ProjectReadout Linear(2D -> D): token half as a GEMM operand (fwd / bwd), whole matrix for the cls kernel
         D = self.D
         for n in self.readouts:
             if not fresh(f"pretrained.act_postprocess{n}.0.project.0.weight"):
                 continue
             wfull = P[f"pretrained.act_postprocess{n}.0.project.0.weight"]
-            self.pk[f"ro{n}_wfull"].copy_(wfull)
-            self.pk[f"ro{n}_wtok"].copy_(wfull[:, :D])
+            gemm[f"ro{n}.full"].copy_(wfull)
+            gemm[f"ro{n}.tok"].copy_(wfull[:, :D])
             tokb = self.buf(f"w.ro{n}.tokT", (D, D))
             tokb.copy_(wfull[:, :D].t())
             clsT = self.buf(f"w.ro{n}.clsT", (D, D), torch.float32)
             clsT.copy_(wfull[:, D:].t())
         if not self.hybrid:
             for n, k in ((1, 4), (2, 2)):
-                cp = self.rn_pad[n - 1]
-                for pname, key in ((f"pretrained.act_postprocess{n}.3.bias", f"pp{n}_b"),
-                                   (f"pretrained.act_postprocess{n}.4.bias", f"pp{n}t_b")):
-                    if cp != self.rn_in[n - 1] and fresh(pname):
-                        self.pk[key].zero_()
-                        self.pk[key][:self.rn_in[n - 1]].copy_(P[pname])
                 if f"pp{n}t" in keys:
                     # the forward's per-phase operands W[:, :, ky, kx]^T [out][in] = the tap blocks of the dgrad
                     # operand, bwd[out][(k*k-1-t)*cp + in]
-                    phases = self.buf(f"w.pp{n}t.phases", (k * k, cp, cp))
-                    phases.copy_(self.W[f"pp{n}t"][1].view(cp, k * k, cp).permute(1, 0, 2).flip(0))
+                    cp = self.rn_pad[n - 1]
+                    gemm[f"pp{n}t.phases"].copy_(self.W[f"pp{n}t"][1].view(cp, k * k, cp).permute(1, 0, 2).flip(0))
         # stride-2 3x3 convolutions: per-parity-plane dgrad operands cut out of the rotated dgrad weight
         for key, mode in (("s1b0.w2", "same"), ("s2b0.w2", "same"), ("pp4s", "sym1")):
             if key not in keys:
                 continue
-            n_pad = self.meta[key][4]
-            for plane, op in parity_dgrad_operands(self.W[key][1], n_pad, mode).items():
+            for plane, op in parity_dgrad_operands(self.W[key][1], self.layer[key].n_pad, mode).items():
                 self.plane_w[(key, plane)] = op
 
     # ------------------------------------------------------------------ small helpers
     def _wgrad(self, key: str, views, taps, dy, n_rows: Optional[int] = None):
         """weight gradient of layer `key` into the flat gradient buffer (through the weight standardisation); nothing
         for a frozen weight."""
-        pname, n, c, ntaps, n_pad, c_pad, std = self.meta[key]
-        if not self._plan.grad(pname):
+        L = self.layer[key]
+        if not self._plan.grad(L.weight):
             return
         if key not in self.gp_layer:
             # linear / 1x1 layer without weight standardisation: the packed gradient layout IS the parameter layout
-            bwd.conv_wgrad(views, taps, dy, self.G[pname].view(n, c))
+            bwd.conv_wgrad(views, taps, dy, self.G[L.weight].view(L.n, L.c))
             return
         bwd.conv_wgrad(views, taps, dy, self.gp_layer[key])        # converted to parameter layout by the bucket's unpack launch
 
@@ -566,7 +477,7 @@ class TrainEngine:
             plan = self.plan_for(trainable, want_dx)
         self._unpack_tables_for(plan)
         if trainable is not None:
-            keys = tuple(k for k, pn, *_ in self.layers if pn in trainable)
+            keys = tuple(L.key for L in self.layers if L.weight in trainable)
             if keys:
                 self.pack_table_for(keys)
 
@@ -600,6 +511,19 @@ class TrainEngine:
                            save=self.saved)
 
     # ------------------------------------------------------------------ backward
+    def _gemm_bwd(self, key: str, dy, x, dx=None, bias: bool = True):
+        """Backward of GEMM layer `key` (one input view, the taps of its table entry) with output gradient dy and input
+        x: the input gradient into dx (skipped when dx is None), the weight gradient and, unless `bias` is False (formed
+        elsewhere), the bias gradient."""
+        L = self.layer[key]
+        taps = bwd.TAPS_1 if L.taps == 1 else bwd.TAPS_3X3
+        if dx is not None:
+            w = self.W[key][1]
+            ops.conv_gemm([dy], taps, w, dx, bias=self._zb(w))
+        self._wgrad(key, [x], taps, dy)
+        if bias and L.bias is not None:
+            self._bias_grad(L.bias, dy)
+
     def _dgrad_s2(self, key: str, dy, dx):
         """gradient w.r.t. the input of a stride-2 3x3 convolution: one small convolution per input parity plane,
         stored through a strided view of dx."""
@@ -650,38 +574,26 @@ class TrainEngine:
             dw4, db4 = self._param_grads(w4, b4)
             bwd.head_tail_bwd(dout, hd["out"], hd["a"], hd["w4"], da, None if dw4 is None else dw4.view(self.C, 32), db4,
                               self.non_negative)
-        if need("head.h1"):
-            dh1u = buf("g.head_h1u", hd["h1u"].shape)
-            ops.conv3x3(da, Wt["head2"][1], dh1u, bias=self._zb(Wt["head2"][1]))
-        self._wgrad("head2", [hd["h1u"]], bwd.TAPS_3X3, da)
-        self._bias_grad("scratch.output_conv.2.bias", da)
+        dh1u = buf("g.head_h1u", hd["h1u"].shape) if need("head.h1") else None
+        self._gemm_bwd("head2", da, hd["h1u"], dh1u)
         if need("head.h1"):
             dh1 = buf("g.head_h1", hd["h1"].shape)
             bwd.upsample2x_bwd(dh1u, dh1)
         if need("ff1.z"):
             dpath = buf("g.path_1", hd["path_1"].shape)
-            ops.conv3x3(dh1, Wt["head0"][1], dpath, bias=self._zb(Wt["head0"][1]))
-        self._wgrad("head0", [hd["path_1"]], bwd.TAPS_3X3, dh1)
-        self._bias_grad("scratch.output_conv.0.bias", dh1)
+        self._gemm_bwd("head0", dh1, hd["path_1"], dpath)
 
         # ---- RefineNet fusion blocks
         def rcu_bwd(n, u_, d_out, dx, x_name):
             """d_out: gradient w.r.t. the RCU output; dx <- gradient w.r.t. its (pre-ReLU) input `x_name` when needed."""
             r = S[f"ff{n}.rcu{u_}"]
-            p = f"scratch.refinenet{n}.resConfUnit{u_}."
             need_t = need(f"ff{n}.rcu{u_}.t")
-            if need_t:
-                dt = buf(f"g.ff{n}_rcu{u_}_t", r["tmid"].shape)
-                ops.conv3x3(d_out, Wt[f"ff{n}.rcu{u_}.c2"][1], dt, bias=self._zb(Wt[f"ff{n}.rcu{u_}.c2"][1]))
-            self._wgrad(f"ff{n}.rcu{u_}.c2", [r["tmid"]], bwd.TAPS_3X3, d_out)
-            self._bias_grad(p + "conv2.bias", d_out)
+            dt = buf(f"g.ff{n}_rcu{u_}_t", r["tmid"].shape) if need_t else None
+            self._gemm_bwd(f"ff{n}.rcu{u_}.c2", d_out, r["tmid"], dt)
             if need_t:
                 bwd.mask_add(dt, dt, mask=r["tmid"])                    # through relu(conv1 + b1)
-                if need(x_name):
-                    dxr = buf(f"g.ff{n}_rcu{u_}_x", r["x_raw"].shape)
-                    ops.conv3x3(dt, Wt[f"ff{n}.rcu{u_}.c1"][1], dxr, bias=self._zb(Wt[f"ff{n}.rcu{u_}.c1"][1]))
-                self._wgrad(f"ff{n}.rcu{u_}.c1", [r["x_relu"]], bwd.TAPS_3X3, dt)
-                self._bias_grad(p + "conv1.bias", dt)
+                dxr = buf(f"g.ff{n}_rcu{u_}_x", r["x_raw"].shape) if need(x_name) else None
+                self._gemm_bwd(f"ff{n}.rcu{u_}.c1", dt, r["x_relu"], dxr)
             if need(x_name):
                 bwd.mask_add(dx, dxr, a=d_out, mask=r["x_relu"])        # skip + through relu(x)
 
@@ -693,12 +605,8 @@ class TrainEngine:
             if not need(f"ff{n}.z"):                                    # nor anything of the later fusion blocks
                 break
             f = S[f"ff{n}"]
-            dy = None
-            if need(f"ff{n}.y"):
-                dy = buf(f"g.ff{n}_y", f["y"].shape)
-                ops.conv1x1(dz, Wt[f"ff{n}.out"][1], dy, bias=self._zb(Wt[f"ff{n}.out"][1]))
-            self._wgrad(f"ff{n}.out", [f["y"]], bwd.TAPS_1, dz)
-            self._bias_grad(f"scratch.refinenet{n}.out_conv.bias", dz)
+            dy = buf(f"g.ff{n}_y", f["y"].shape) if need(f"ff{n}.y") else None
+            self._gemm_bwd(f"ff{n}.out", dz, f["y"], dy)
             if dy is None:
                 continue
             s_name = "rn4.o" if n == 4 else f"ff{n}.s"
@@ -720,8 +628,7 @@ class TrainEngine:
             l = S["layers"][n - 1]
             if need(f"layer_{n}"):
                 d_layers[n - 1] = buf(f"g.layer_{n}", l.shape)
-                ops.conv3x3(d_rn[n - 1], Wt[f"rn{n}"][1], d_layers[n - 1], bias=self._zb(Wt[f"rn{n}"][1]))
-            self._wgrad(f"rn{n}", [l], bwd.TAPS_3X3, d_rn[n - 1])
+            self._gemm_bwd(f"rn{n}", d_rn[n - 1], l, d_layers[n - 1])
         # ---- reassemble: act_postprocess4.4 (stride 2), the ConvTransposes of layer_1 / layer_2 (plain ViTs), then the
         # readouts
         gh, gw, ntok, D = S["gh"], S["gw"], S["ntok"], self.D
@@ -743,13 +650,9 @@ class TrainEngine:
             """-> gradient w.r.t. the hooked tokens `tokens`, activation type [B, ntok, D] (None when not needed)."""
             r = S[f"ro{n}"]
             pp = f"pretrained.act_postprocess{n}."
-            need_r = need(f"ro{n}.r")
-            if need_r:
-                dr = buf(f"g.ro{n}_r", r["r"].shape)
-                ops.conv1x1(do, Wt[f"pp{n}"][1], dr.view(B, gh, gw, D), bias=self._zb(Wt[f"pp{n}"][1]))
-            self._wgrad(f"pp{n}", [r["r"].view(B, gh, gw, D)], bwd.TAPS_1, do)
-            self._bias_grad(pp + "3.bias", do)
-            if not need_r:
+            dr = buf(f"g.ro{n}_r", r["r"].shape) if need(f"ro{n}.r") else None
+            self._gemm_bwd(f"pp{n}", do, r["r"].view(B, gh, gw, D), None if dr is None else dr.view(B, gh, gw, D))
+            if dr is None:
                 return None
             bwd.gelu_bwd(dr, r["pre"], dr)
             dtk = None
@@ -805,20 +708,16 @@ class TrainEngine:
                 bwd.add_cast(ds, dtk[i], ds, ds16)
             g16 = ds if self.fp32 else ds16
             # mlp: x_{i+1} = xm + fc2(gelu(fc1(LN2(xm))))
-            if need(q + "u"):
-                dmlp = buf("g.vit_mlp", v["mlp"].shape)
-                ops.linear(g16.view(rows, -1), Wt[f"blk{i}.fc2"][1], dmlp.view(rows, -1), bias=self._zb(Wt[f"blk{i}.fc2"][1]))
-            self._wgrad(f"blk{i}.fc2", [v["mlp"].view(rows, -1)], bwd.TAPS_1, g16.view(rows, -1))
+            dmlp = buf("g.vit_mlp", v["mlp"].shape) if need(q + "u") else None
+            self._gemm_bwd(f"blk{i}.fc2", g16.view(rows, -1), v["mlp"].view(rows, -1),
+                           None if dmlp is None else dmlp.view(rows, -1), bias=False)
             if i in hooked and T(p + "mlp.fc2.bias"):                # else: written by block i+1's norm1 backward
                 bwd.colsum(ds.view(rows, -1), G[p + "mlp.fc2.bias"].view(1, -1))
             if need(q + "u"):
                 bwd.gelu_bwd(dmlp, v["u"], dmlp)
-                if need(q + "h2"):
-                    dh = buf("g.vit_h", v["h2"].shape)
-                    ops.linear(dmlp.view(rows, -1), Wt[f"blk{i}.fc1"][1], dh.view(rows, -1),
-                               bias=self._zb(Wt[f"blk{i}.fc1"][1]))
-                self._wgrad(f"blk{i}.fc1", [v["h2"].view(rows, -1)], bwd.TAPS_1, dmlp.view(rows, -1))
-                self._bias_grad(p + "mlp.fc1.bias", dmlp.view(rows, -1))
+                dh = buf("g.vit_h", v["h2"].shape) if need(q + "h2") else None
+                self._gemm_bwd(f"blk{i}.fc1", dmlp.view(rows, -1), v["h2"].view(rows, -1),
+                               None if dh is None else dh.view(rows, -1))
             if not need(q + "h2"):
                 continue
             # ds_b = gradient at attn.proj's output: its column sums are proj's bias gradient (same pass)
@@ -829,19 +728,15 @@ class TrainEngine:
                 continue
             g16 = ds_b if self.fp32 else ds16
             # attention: xm = x_i + proj(attn(qkv(LN1(x_i))))
-            if need(q + "att"):
-                datt = buf("g.vit_att", v["att"].shape)
-                ops.linear(g16.view(rows, -1), Wt[f"blk{i}.proj"][1], datt.view(rows, -1),
-                           bias=self._zb(Wt[f"blk{i}.proj"][1]))
-            self._wgrad(f"blk{i}.proj", [v["att"].view(rows, -1)], bwd.TAPS_1, g16.view(rows, -1))
+            datt = buf("g.vit_att", v["att"].shape) if need(q + "att") else None
+            self._gemm_bwd(f"blk{i}.proj", g16.view(rows, -1), v["att"].view(rows, -1),
+                           None if datt is None else datt.view(rows, -1), bias=False)
             if not need(q + "att"):
                 continue
             dqkv = buf("g.vit_qkv", v["qkv"].shape)
             bwd.attention_bwd(v["qkv"], v["att"], datt, v["lse"], dqkv, heads=self.heads, scale=0.125)
-            if need(q + "h1"):
-                ops.linear(dqkv.view(rows, -1), Wt[f"blk{i}.qkv"][1], dh.view(rows, -1), bias=self._zb(Wt[f"blk{i}.qkv"][1]))
-            self._wgrad(f"blk{i}.qkv", [v["h1"].view(rows, -1)], bwd.TAPS_1, dqkv.view(rows, -1))
-            self._bias_grad(p + "attn.qkv.bias", dqkv.view(rows, -1))
+            self._gemm_bwd(f"blk{i}.qkv", dqkv.view(rows, -1), v["h1"].view(rows, -1),
+                           dh.view(rows, -1) if need(q + "h1") else None)
             if not need(q + "h1"):
                 continue
             # ds = gradient at block i-1's output = at its mlp.fc2 output, unless a hook adds to it first
@@ -869,19 +764,18 @@ class TrainEngine:
                 G[pm + "cls_token"].view(-1).copy_(row0)
             g16 = ds if self.fp32 else ds16
             dtok = g16[:, 1:, :].unsqueeze(1)
+            # the bias gradient sums the patch rows of ds (below)
             if self.hybrid:
                 f3 = S["f3"]
-                if need("f3"):
-                    df3 = buf("g.f3", f3.shape)
-                    ops.linear(dtok, Wt["proj"][1], df3.view(B, 1, gh * gw, 1024), bias=self._zb(Wt["proj"][1]))
-                self._wgrad("proj", [f3.view(B, 1, gh * gw, 1024)], bwd.TAPS_1, dtok)
+                df3 = buf("g.f3", f3.shape) if need("f3") else None
+                self._gemm_bwd("proj", dtok, f3.view(B, 1, gh * gw, 1024),
+                               None if df3 is None else df3.view(B, 1, gh * gw, 1024), bias=False)
             else:                                                    # Conv2d(3, D, 16, stride 16) = GEMM over patchify's columns
                 cols = S["cols"]
+                dcols = buf("g.patch_cols", cols.shape) if dx is not None else None
+                self._gemm_bwd("proj", dtok, cols, dcols, bias=False)
                 if dx is not None:
-                    dcols = buf("g.patch_cols", cols.shape)
-                    ops.linear(dtok, Wt["proj"][1], dcols, bias=self._zb(Wt["proj"][1]))
                     bwd.patch_input_grad(dcols.view(B * gh * gw, -1), dx)
-                self._wgrad("proj", [cols], bwd.TAPS_1, dtok)
             if T(pm + "patch_embed.proj.bias"):
                 tmpb = buf("tmp.projbias", (B, D), f32)
                 bwd.colsum(ds[:, 1:, :], tmpb, batches=B)
@@ -911,22 +805,17 @@ class TrainEngine:
                 dy3 = buf(f"g.{tag}_y3", out.shape)
                 dg, db = self._param_grads(p + "norm3.weight", p + "norm3.bias")
                 bwd.groupnorm_bwd(g, rec["y3"], rec["st3"], P[p + "norm3.weight"], dy3, dg, db)
-            if need(f"{tag}.a2"):
-                da2 = buf(f"g.{tag}_a2", rec["a2"].shape)
-                ops.conv1x1(dy3, Wt[tag + ".w3"][1], da2, bias=self._zb(Wt[tag + ".w3"][1]))
-            self._wgrad(tag + ".w3", [rec["a2"]], bwd.TAPS_1, dy3)
+            da2 = buf(f"g.{tag}_a2", rec["a2"].shape) if need(f"{tag}.a2") else None
+            self._gemm_bwd(tag + ".w3", dy3, rec["a2"], da2)
             if need(f"{tag}.a2"):
                 dy2 = buf(f"g.{tag}_y2", rec["y2"].shape)
                 dg, db = self._param_grads(p + "norm2.weight", p + "norm2.bias")
                 bwd.groupnorm_bwd(da2, rec["y2"], rec["st2"], P[p + "norm2.weight"], dy2, dg, db, mask=rec["a2"])
             a1 = rec["a1"]
             need_a1 = need(f"{tag}.a1")
-            if need_a1:
-                da1 = buf(f"g.{tag}_a1", a1.shape)
+            da1 = buf(f"g.{tag}_a1", a1.shape) if need_a1 else None
             if stride == 1:
-                if need_a1:
-                    ops.conv3x3(dy2, Wt[tag + ".w2"][1], da1, bias=self._zb(Wt[tag + ".w2"][1]))
-                self._wgrad(tag + ".w2", [a1], bwd.TAPS_3X3, dy2)
+                self._gemm_bwd(tag + ".w2", dy2, a1, da1)
             else:
                 if need_a1:
                     self._dgrad_s2(tag + ".w2", dy2, da1)
@@ -944,19 +833,17 @@ class TrainEngine:
                     dd = buf(f"g.{tag}_ds", rec["d"].shape)
                     dg, db = self._param_grads(p + "downsample.norm.weight", p + "downsample.norm.bias")
                     bwd.groupnorm_bwd(g, rec["d"], rec["std"], P[p + "downsample.norm.weight"], dd, dg, db)
-                if stride > 1:
+                if stride > 1:                                       # the strided 1x1 conv: through strided views
                     if need_in:
                         dt_in.zero_()
                         ops.conv1x1(dd, Wt[tag + ".wd"][1], dt_in[:, ::stride, ::stride, :], bias=self._zb(Wt[tag + ".wd"][1]))
                     self._wgrad(tag + ".wd", [t_in[:, ::stride, ::stride, :]], bwd.TAPS_1, dd)
                 else:
-                    if need_in:
-                        ops.conv1x1(dd, Wt[tag + ".wd"][1], dt_in, bias=self._zb(Wt[tag + ".wd"][1]))
-                    self._wgrad(tag + ".wd", [t_in], bwd.TAPS_1, dd)
-                if need_in:
-                    ops.conv1x1(dy1, Wt[tag + ".w1"][1], dt_in, residual=dt_in, bias=self._zb(Wt[tag + ".w1"][1]))
-            elif need_in:
-                ops.conv1x1(dy1, Wt[tag + ".w1"][1], dt_in, residual=g, bias=self._zb(Wt[tag + ".w1"][1]))
+                    self._gemm_bwd(tag + ".wd", dd, t_in, dt_in)
+            # w1: its input gradient adds to the shortcut's (b = 0) or to the skip connection's (b > 0)
+            if need_in:
+                w1 = Wt[tag + ".w1"][1]
+                ops.conv1x1(dy1, w1, dt_in, residual=dt_in if b == 0 else g, bias=self._zb(w1))
             self._wgrad(tag + ".w1", [t_in], bwd.TAPS_1, dy1)
             d_out = dt_in
         # ---- stem
@@ -969,7 +856,7 @@ class TrainEngine:
             dg, db = self._param_grads(bb + "stem.norm.weight", bb + "stem.norm.bias")
             bwd.groupnorm_bwd(g_s0, s0, st0, P[bb + "stem.norm.weight"], ds0, dg, db)
             if dx is not None:
-                bwd.stem_input_grad(ds0, self.pk["stem_w"], dx)
+                bwd.stem_input_grad(ds0, self.pk["gemm"]["stem"], dx)
             if T(bb + "stem.conv.weight"):
                 gp = self.gp[: 64 * 160].view(64, 160)
                 h2, w2 = H // 2, W // 2

@@ -102,6 +102,21 @@ def test_plain_vit_state_dict_layout_is_the_reference_layout(backbone, golden):
         assert [[k, list(v.shape)] for k, v in ref.state_dict().items()] == spec
 
 
+@pytest.mark.parametrize("backbone", ["vitb_rn50_384", "vitl16_384", "vitb16_384"])
+def test_gemm_layer_table_matches_the_state_dict(backbone):
+    """Every GEMM layer reads its whole weight as [n][c][taps], pads without truncating and names a bias of the
+    model."""
+    import math
+    from omnidata_b200.model import _ARCH, gemm_layers, state_dict_spec
+    spec = dict(state_dict_spec(1, backbone=backbone))
+    layers = gemm_layers(_ARCH[backbone])
+    assert len({L.key for L in layers}) == len(layers)
+    for L in layers:
+        assert L.n * L.c * L.taps == math.prod(spec[L.weight]), L.key
+        assert L.n_pad >= L.n and L.c_pad >= L.c, L.key
+        assert L.bias is None or spec.get(L.bias) == (L.n,), L.key
+
+
 def test_every_host_module_refuses_cpu_tensors():
     """No CPU / eager fallback anywhere: the host mirrors raise instead of computing on the CPU."""
     if torch.cuda.is_available():

@@ -405,7 +405,7 @@ def _record(backbone, size, precision, batch=2):
         eng.backward(dout)
     torch.cuda.synchronize()
     # every layer's weight gradient, each readout's token and cls halves and (hybrid) the stem go through conv_wgrad
-    dest = {(eng.gp_layer[k] if k in eng.gp_layer else eng.G[pn]).data_ptr(): k for k, pn, *_ in eng.layers}
+    dest = {(eng.gp_layer[L.key] if L.key in eng.gp_layer else eng.G[L.weight]).data_ptr(): L.key for L in eng.layers}
     missing = sorted(k for p, k in dest.items() if p not in wgrad_outs)
     expected_calls = len(eng.layers) + 2 * len(eng.readouts) + int(eng.hybrid)
     del eng, model

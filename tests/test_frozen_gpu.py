@@ -93,7 +93,7 @@ def test_frozen_backward_is_the_full_backwards_bits(case, pattern):
 def _wgrad_count(eng, trainable):
     """conv_wgrad calls of a backward: one per trainable GEMM weight (engine layer table and the stem), two per
     trainable readout projection (its token and cls halves)."""
-    gemm = {pn for _, pn, *_ in eng.layers} | {BB + "stem.conv.weight"}
+    gemm = {L.weight for L in eng.layers} | {BB + "stem.conv.weight"}
     ro = {f"pretrained.act_postprocess{n}.0.project.0.weight" for n in (3, 4)}
     return sum(1 for n in trainable if n in gemm) + 2 * sum(1 for n in trainable if n in ro)
 
@@ -134,7 +134,7 @@ def test_frozen_slices_are_not_written(sd, pattern, monkeypatch):
     assert n_frozen < n_full
 
 
-def test_frozen_operands_are_packed_only_when_they_change(sd, monkeypatch):
+def test_frozen_layer_operands_are_packed_only_when_they_change(sd, monkeypatch):
     from omnidata_b200 import bwd
     from oracle import weights
     x, R = _inputs((384, 384))
@@ -145,7 +145,8 @@ def test_frozen_operands_are_packed_only_when_they_change(sd, monkeypatch):
     runs = []
     real = bwd.PackTable.run
     monkeypatch.setattr(bwd.PackTable, "run", lambda self, *a, **k: (runs.append(1), real(self, *a, **k)))
-    derived = [eng.pk["stem_w"], eng.pk["head2"][1], eng.pk["ro3_wfull"], eng.bufs["w.ro4.tokT"]]
+    derived = [eng.pk["gemm"]["stem"], eng.pk["vec"]["scratch.output_conv.2.bias"], eng.pk["gemm"]["ro3.full"],
+               eng.bufs["w.ro4.tokT"]]
     versions = [t._version for t in derived]
     xi = x.clone().requires_grad_(True)
     out = model(xi)

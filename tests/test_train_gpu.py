@@ -187,6 +187,37 @@ def test_pack_table_multi(dtype):
         assert torch.equal(bk.view(c_pad, taps, n_pad), fwd.view(n_pad, taps, c_pad).permute(2, 1, 0).flip(1))
 
 
+@pytest.mark.parametrize("precision", ["bf16", "fp32"])
+@pytest.mark.parametrize("backbone", ["vitb_rn50_384", "vitl16_384", "vitb16_384"])
+def test_engine_and_inference_operand_tables_agree(backbone, precision):
+    """The train engine and inference hand dpt_forward operand tables with the same keys, shapes and dtypes, but for the
+    documented differences: head conv2 (operand and bias) padded to 64 rows in training, the ConvTransposes' table
+    operands (engine only; inference reads their per-phase operands), the dead refinenet4.resConfUnit1 (inference
+    only)."""
+    from omnidata_b200.model import DPTDepthModel
+    from omnidata_b200.train import TrainEngine
+    model = DPTDepthModel(backbone=backbone).to(dev())
+    model.precision = precision
+    inf = model._prepack(dev())
+    eng = TrainEngine(model, precision).pk
+    spec = lambda table: {k: (tuple(t.shape), t.dtype) for k, t in table.items()}
+    adt = torch.float32 if precision == "fp32" else torch.bfloat16
+    g_eng, g_inf = spec(eng["gemm"]), spec(inf["gemm"])
+    assert g_eng.pop("head2") == ((64, 9 * 128), adt) and g_inf.pop("head2") == ((32, 9 * 128), adt)
+    for cv in (1, 2):
+        assert g_inf.pop(f"ff4.rcu1.c{cv}") == ((256, 9 * 256), adt)
+    if not model.arch["hybrid"]:
+        for n in (1, 2):
+            assert g_eng.pop(f"pp{n}t")[1] == adt
+    assert g_eng == g_inf and all(dt == adt for _, dt in g_eng.values())
+    v_eng, v_inf = spec(eng["vec"]), spec(inf["vec"])
+    b2 = "scratch.output_conv.2.bias"
+    assert v_eng.pop(b2) == ((64,), torch.float32) and v_inf.pop(b2) == ((32,), torch.float32)
+    for cv in (1, 2):
+        assert v_inf.pop(f"scratch.refinenet4.resConfUnit1.conv{cv}.bias") == ((256,), torch.float32)
+    assert v_eng == v_inf and all(dt == torch.float32 for _, dt in v_eng.values())
+
+
 def test_stem_and_head_bwd_kernels():
     from omnidata_b200 import bwd, ops
     b, h, w, c = 2, 32, 48, 64
