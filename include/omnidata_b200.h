@@ -141,12 +141,15 @@ int odb_layernorm(const void* x, const float* gamma, const float* beta, void* y,
 /* Fused multi-head attention (timm Attention.forward): qkv bf16 [b][tokens][3][heads][64] as written
  * by the qkv linear; out bf16 [b][tokens][heads*64]; softmax(q k^T * scale) v.  wgmma kernel:
  * S and O accumulate in registers, exact two-pass fp32 softmax (global row maximum), P rounded to bf16
- * for the PV product, fp32 row sum of the unrounded P.  tokens <= 640.  lse (optional, training): fp32
- * [b][heads][tokens] = log2 of the row's sum of exp2(s * scale * log2 e), what odb_attention_bwd re-normalises with. */
+ * for the PV product, fp32 row sum of the unrounded P.  tokens <= 4097 (a 64 x 64 patch grid + cls): up to 640
+ * tokens K and V of an (image, head) stay resident in shared memory, above that they stream through it per
+ * 128-query tile (same arithmetic); more tokens return ODB_ERR_UNSUPPORTED.  lse (optional): fp32
+ * [b][heads][tokens] = log2 of the row's sum of exp2(s * scale * log2 e), what odb_attention_bwd re-normalises with
+ * (the backward itself takes at most 640 tokens). */
 int odb_attention(const void* qkv, void* out, float* lse, int32_t b, int32_t tokens, int32_t heads, float scale,
                   void* stream);
 /* fp32 correctness mode of odb_attention: qkv fp32 [b][tokens][3][heads][64], out fp32 [b][tokens][heads*64];
- * dot products and the PV sum in fp64, exp / division exact (no fast-math). */
+ * dot products and the PV sum in fp64, exp / division exact (no fast-math).  tokens <= 4097. */
 int odb_attention_f32(const float* qkv, float* out, int32_t b, int32_t tokens, int32_t heads, float scale,
                       void* stream);
 

@@ -1,9 +1,15 @@
-// wgmma fused attention for the ViT-B/16 blocks of DPT-Hybrid (<= 640 tokens, d = 64):
+// wgmma fused attention for the ViT blocks of the DPTs (d = 64, up to 4 097 tokens):
 //   out = softmax(q k^T * scale) v        (timm Attention.forward; block loop at M/vit.py:150-151)
 //
-// One persistent CTA per SM; a work unit is one (image, head).  K and V of the unit (5 blocks of
-// 128 keys x 64 d each) are TMA-loaded once into shared memory and stay resident; the 128-query
-// tiles of the unit stream through a double-buffered Q slot.
+// Two instances of one kernel, chosen by the host from the token count:
+//   resident (<= 640 tokens)  one persistent CTA per SM; a work unit is one (image, head).  K and V of the unit
+//                             (<= 5 blocks of 128 keys x 64 d each) are TMA-loaded once into shared memory and stay
+//                             resident; the 128-query tiles of the unit stream through a double-buffered Q slot.
+//   streaming (> 640 tokens)  a work item is one (image, head, 128-query tile), items of one (image, head) adjacent so
+//                             that the CTAs running at the same time share K and V through L2.  K and V blocks stream
+//                             through a ring of 10 slots of 128 keys (the shared memory of the resident K and V) in
+//                             the order the consumers read them: K_0..K_{n-1} for pass 1, then K_j, V_j for pass 2.
+//                             Every query tile reads K twice and V once from L2.
 //   warpgroup 0      TMA producer (K, V blocks; Q tiles)
 //   warpgroups 1, 2  64 query rows of the tile each:  S = Q K_j^T  (wgmma M=64, N=128, K=64, both operands K-major)
 //                                                     O += P_j V_j (M=64, N=64, K=128, P from registers,
@@ -12,7 +18,7 @@
 // turns them into P = exp2(s*c - m*c) (bf16, straight from the accumulator registers into the A-operand registers
 // of the PV product) and accumulates the fp32 row sum of the unrounded P.  O therefore never needs rescaling and
 // stays in registers until the epilogue.  A row of S lives in the four lanes of a quad: row reductions are two
-// shuffles.
+// shuffles.  Both instances compute the same function with the same rounding points; only the data movement differs.
 #include "common.cuh"
 #include "host_util.h"
 #include "wgmma.cuh"
@@ -21,7 +27,9 @@
 namespace odb {
 
 constexpr int kTcBlk = 128;         // queries per tile == keys per block
-constexpr int kTcMaxBlocks = 5;     // 640 keys
+constexpr int kTcMaxBlocks = 5;     // 640 keys: the resident instance
+constexpr int kTcStreamMaxTokens = 4097;   // 64 x 64 patches + cls: the streaming instance
+constexpr int kTcRing = 2 * kTcMaxBlocks;  // streaming K / V ring slots: the resident K and V space
 constexpr int kTcTileBytes = kTcBlk * 128;   // 128 rows x 64 bf16
 constexpr int kTcThreads = 384;
 constexpr int kTcConsumerWarps = 8;
@@ -57,6 +65,7 @@ ODB_DEVINL float fast_exp2_tc(float x) {
   return y;
 }
 
+template <bool STREAM>
 __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -68,14 +77,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
   // instead of after the whole 160 KiB, the rest of the fetch hides behind pass 1
   auto k_full = [&](int j) { return bar0 + 136u + 8u * j; };
   auto v_full = [&](int j) { return bar0 + 176u + 8u * j; };
+  // streaming: slot i of the K / V ring at sbase + i * kTcTileBytes, full / empty barrier pair of its own
+  auto ring_full = [&](uint32_t i) { return bar0 + 48u + 8u * i; };
+  auto ring_empty = [&](uint32_t i) { return bar0 + 128u + 8u * i; };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nblk = (p.tokens + kTcBlk - 1) / kTcBlk;     // key blocks == query tiles
   const int units = p.batch * p.heads;
+  const int items = units * nblk;                         // streaming work items: (image, head, query tile)
 
   if (threadIdx.x == 0) {
-    mbar_init(kv_empty, kTcConsumerWarps);
-    for (int j = 0; j < kTcMaxBlocks; ++j) { mbar_init(k_full(j), 1); mbar_init(v_full(j), 1); }
+    if constexpr (STREAM) {
+      for (uint32_t i = 0; i < kTcRing; ++i) { mbar_init(ring_full(i), 1); mbar_init(ring_empty(i), kTcConsumerWarps); }
+    } else {
+      mbar_init(kv_empty, kTcConsumerWarps);
+      for (int j = 0; j < kTcMaxBlocks; ++j) { mbar_init(k_full(j), 1); mbar_init(v_full(j), 1); }
+    }
     for (int i = 0; i < 2; ++i) { mbar_init(q_full(i), 1); mbar_init(q_empty(i), kTcConsumerWarps); }
     mbar_fence_init();
     tma_prefetch_desc(&p.qkv_map);
@@ -88,23 +105,46 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
     // ------------------------------------------------------------------ TMA producer
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 0 && lane == 0) {
-      uint32_t u_iter = 0, qt_iter = 0;
-      for (int unit = blockIdx.x; unit < units; unit += gridDim.x, ++u_iter) {
-        const int b = unit / p.heads, h = unit % p.heads;
-        mbar_wait(kv_empty, (u_iter & 1u) ^ 1u);
-        for (int j = 0; j < nblk; ++j) {
-          mbar_expect_tx(k_full(j), kTcTileBytes);
-          tma_load_4d(sbase + kTcOffK + j * kTcTileBytes, &p.qkv_map, k_full(j), 0, p.heads + h, j * kTcBlk, b);
-        }
-        for (int j = 0; j < nblk; ++j) {
-          mbar_expect_tx(v_full(j), kTcTileBytes);
-          tma_load_4d(sbase + kTcOffV + j * kTcTileBytes, &p.qkv_map, v_full(j), 0, 2 * p.heads + h, j * kTcBlk, b);
-        }
-        for (int qt = 0; qt < nblk; ++qt, ++qt_iter) {
+      if constexpr (STREAM) {
+        uint32_t slot = 0, phase = 0, qt_iter = 0;
+        auto ring_load = [&](int row, int j, int b) {
+          mbar_wait(ring_empty(slot), phase ^ 1u);
+          mbar_expect_tx(ring_full(slot), kTcTileBytes);
+          tma_load_4d(sbase + slot * kTcTileBytes, &p.qkv_map, ring_full(slot), 0, row, j * kTcBlk, b);
+          if (++slot == kTcRing) { slot = 0; phase ^= 1u; }
+        };
+        for (int item = blockIdx.x; item < items; item += gridDim.x, ++qt_iter) {
+          const int unit = item / nblk, qt = item - unit * nblk;
+          const int b = unit / p.heads, h = unit % p.heads;
           const int qb = qt_iter & 1u;
           mbar_wait(q_empty(qb), ((qt_iter >> 1) & 1u) ^ 1u);
           mbar_expect_tx(q_full(qb), kTcTileBytes);
           tma_load_4d(sbase + kTcOffQ + qb * kTcTileBytes, &p.qkv_map, q_full(qb), 0, h, qt * kTcBlk, b);
+          for (int j = 0; j < nblk; ++j) ring_load(p.heads + h, j, b);             // pass 1: K
+          for (int j = 0; j < nblk; ++j) {                                         // pass 2: K, V
+            ring_load(p.heads + h, j, b);
+            ring_load(2 * p.heads + h, j, b);
+          }
+        }
+      } else {
+        uint32_t u_iter = 0, qt_iter = 0;
+        for (int unit = blockIdx.x; unit < units; unit += gridDim.x, ++u_iter) {
+          const int b = unit / p.heads, h = unit % p.heads;
+          mbar_wait(kv_empty, (u_iter & 1u) ^ 1u);
+          for (int j = 0; j < nblk; ++j) {
+            mbar_expect_tx(k_full(j), kTcTileBytes);
+            tma_load_4d(sbase + kTcOffK + j * kTcTileBytes, &p.qkv_map, k_full(j), 0, p.heads + h, j * kTcBlk, b);
+          }
+          for (int j = 0; j < nblk; ++j) {
+            mbar_expect_tx(v_full(j), kTcTileBytes);
+            tma_load_4d(sbase + kTcOffV + j * kTcTileBytes, &p.qkv_map, v_full(j), 0, 2 * p.heads + h, j * kTcBlk, b);
+          }
+          for (int qt = 0; qt < nblk; ++qt, ++qt_iter) {
+            const int qb = qt_iter & 1u;
+            mbar_wait(q_empty(qb), ((qt_iter >> 1) & 1u) ^ 1u);
+            mbar_expect_tx(q_full(qb), kTcTileBytes);
+            tma_load_4d(sbase + kTcOffQ + qb * kTcTileBytes, &p.qkv_map, q_full(qb), 0, h, qt * kTcBlk, b);
+          }
         }
       }
     }
@@ -117,9 +157,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
     const float c = p.scale_log2e;
     uint32_t u_iter = 0, qt_iter = 0;
     float s[64];
-    auto compute_s = [&](int j, uint32_t qb) {
+    auto compute_s = [&](uint32_t koff, uint32_t qb) {
       const uint64_t adesc = gmma_desc_sw128(sbase + kTcOffQ + qb * kTcTileBytes + static_cast<uint32_t>(wg) * 8192u);
-      const uint64_t bdesc = gmma_desc_sw128(sbase + kTcOffK + j * kTcTileBytes);
+      const uint64_t bdesc = gmma_desc_sw128(sbase + koff);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) Wgmma<128>::ss<0, 0>(s, adesc + 2u * k, bdesc + 2u * k, k != 0 ? 1u : 0u);
@@ -127,16 +167,36 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
       wgmma_wait<0>();
       wgmma_fence_regs<64>(s);
     };
-    for (int unit = blockIdx.x; unit < units; unit += gridDim.x, ++u_iter) {
-      const int b = unit / p.heads, h = unit % p.heads;
-      for (int qt = 0; qt < nblk; ++qt, ++qt_iter) {
+    // streaming: the next ring slot in the producer's order, released once this warp's MMAs have read it
+    uint32_t r_slot = 0, r_phase = 0;
+    auto ring_acquire = [&]() {
+      mbar_wait(ring_full(r_slot), r_phase);
+      return r_slot;
+    };
+    auto ring_release = [&](uint32_t slot) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(ring_empty(slot));
+      if (++r_slot == kTcRing) { r_slot = 0; r_phase ^= 1u; }
+    };
+    // resident: work unit = (image, head), all its query tiles; streaming: work item = one query tile
+    for (int unit = blockIdx.x; unit < (STREAM ? items : units); unit += gridDim.x, ++u_iter) {
+      const int bh = STREAM ? unit / nblk : unit;
+      const int b = bh / p.heads, h = bh % p.heads;
+      const int qt_end = STREAM ? unit - bh * nblk + 1 : nblk;
+      for (int qt = STREAM ? qt_end - 1 : 0; qt < qt_end; ++qt, ++qt_iter) {
         const uint32_t qb = qt_iter & 1u;
         mbar_wait(q_full(qb), (qt_iter >> 1) & 1u);
         // ---- pass 1: row maximum over all valid keys
         float mx0 = -INFINITY, mx1 = -INFINITY;
         for (int j = 0; j < nblk; ++j) {
-          mbar_wait(k_full(j), u_iter & 1u);
-          compute_s(j, qb);
+          if constexpr (STREAM) {
+            const uint32_t slot = ring_acquire();
+            compute_s(slot * kTcTileBytes, qb);
+            ring_release(slot);
+          } else {
+            mbar_wait(k_full(j), u_iter & 1u);
+            compute_s(kTcOffK + j * kTcTileBytes, qb);
+          }
           if (j == 0) ODB_ATRACE(qt_iter, 0);
           const int key0 = j * kTcBlk + cl;
 #pragma unroll
@@ -160,7 +220,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
         float o[32];
         float l0 = 0.f, l1 = 0.f;
         for (int j = 0; j < nblk; ++j) {
-          compute_s(j, qb);
+          if constexpr (STREAM) {
+            const uint32_t slot = ring_acquire();
+            compute_s(slot * kTcTileBytes, qb);
+            ring_release(slot);
+          } else {
+            compute_s(kTcOffK + j * kTcTileBytes, qb);
+          }
           const int key0 = j * kTcBlk + cl;
           uint32_t a[32];
 #pragma unroll
@@ -177,16 +243,23 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
             a[4 * (jj >> 1) + 2 * (jj & 1) + 0] = pack_bf16x2(p00, p01);
             a[4 * (jj >> 1) + 2 * (jj & 1) + 1] = pack_bf16x2(p10, p11);
           }
-          mbar_wait(v_full(j), u_iter & 1u);
+          uint32_t voff, vslot = 0;
+          if constexpr (STREAM) {
+            vslot = ring_acquire();
+            voff = vslot * kTcTileBytes;
+          } else {
+            mbar_wait(v_full(j), u_iter & 1u);
+            voff = kTcOffV + j * kTcTileBytes;
+          }
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < 8; ++kk)   // B = V_j rows 16 kk.. (MN-major: +16 rows = 2048 B)
-            Wgmma<64>::rs<1>(o, a + 4 * kk, gmma_desc_sw128(sbase + kTcOffV + j * kTcTileBytes + kk * 2048),
-                             (j | kk) != 0 ? 1u : 0u);
+            Wgmma<64>::rs<1>(o, a + 4 * kk, gmma_desc_sw128(sbase + voff + kk * 2048), (j | kk) != 0 ? 1u : 0u);
           wgmma_commit();
           wgmma_wait<0>();
           wgmma_fence_regs<32>(o);
-          ODB_ATRACE(qt_iter, 2 + j);
+          if constexpr (STREAM) ring_release(vslot);
+          if (!STREAM || j < kTcMaxBlocks) ODB_ATRACE(qt_iter, 2 + j);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(q_empty(qb));                 // this warp no longer reads the Q tile
@@ -215,8 +288,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) attention_tc_kernel(const __gri
         }
         ODB_ATRACE(qt_iter, 9);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(kv_empty);                      // K / V of this unit are no longer read
+      if constexpr (!STREAM) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(kv_empty);                    // K / V of this unit are no longer read
+      }
     }
   }
 }
@@ -230,7 +305,11 @@ extern "C" int odb_attention(const void* qkv, void* out, float* lse, int32_t b, 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!qkv || !out || b < 1 || heads < 1 || tokens < 1)
     return fail(ODB_ERR_INVALID, "attention: bad argument");
-  if (tokens > kTcBlk * kTcMaxBlocks) return fail(ODB_ERR_UNSUPPORTED, "attention: at most 640 tokens");
+  if (tokens > kTcStreamMaxTokens) return fail(ODB_ERR_UNSUPPORTED, "attention: at most 4097 tokens");
+  const bool stream_kv = tokens > kTcBlk * kTcMaxBlocks;   // K / V no longer fit in shared memory
+  const long long units = (long long)b * heads;
+  const long long items = stream_kv ? units * ((tokens + kTcBlk - 1) / kTcBlk) : units;
+  if (items > 0x7fffffffLL) return fail(ODB_ERR_UNSUPPORTED, "attention: too many (image, head, query tile) items");
   if (reinterpret_cast<uintptr_t>(qkv) & 15u) return fail(ODB_ERR_INVALID, "attention: qkv must be 16-byte aligned");
   AttnTcParams p;
   memset(&p, 0, sizeof(p));
@@ -248,17 +327,16 @@ extern "C" int odb_attention(const void* qkv, void* out, float* lse, int32_t b, 
   p.tokens = tokens; p.heads = heads; p.batch = b;
   p.scale_log2e = scale * 1.4426950408889634f;
   p.trace = debug_trace();
-  static bool configured[kMaxDevices] = {};
+  static bool configured[2][kMaxDevices] = {};
   const int dev_ = current_device();
-  if (!configured[dev_]) {
-    cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         kTcSmemBytes);
+  const auto kernel = stream_kv ? attention_tc_kernel<true> : attention_tc_kernel<false>;
+  if (!configured[stream_kv][dev_]) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes);
     if (e != cudaSuccess) return fail_cuda(e, "attention: cudaFuncSetAttribute");
-    configured[dev_] = true;
+    configured[stream_kv][dev_] = true;
   }
-  const int units = b * heads;
-  const int grid = units < num_sms() ? units : num_sms();
-  cudaError_t le = launch_pdl(attention_tc_kernel, dim3(grid), dim3(kTcThreads), kTcSmemBytes, stream, p);
+  const int grid = items < num_sms() ? (int)items : num_sms();
+  cudaError_t le = launch_pdl(kernel, dim3(grid), dim3(kTcThreads), kTcSmemBytes, stream, p);
   count_launch();
   if (le != cudaSuccess) return fail_cuda(le, "attention_tc: launch");
   return check_launch("attention_tc");

@@ -199,6 +199,70 @@ __global__ void __launch_bounds__(256) attention_f32_kernel(const float* __restr
   }
 }
 
+
+// Above 640 tokens: the same arithmetic with the S rows [Q][tokens] in dynamic shared memory sized from tokens; Q = 16
+// while they fit in 227 KiB, 8 above (8 x 4 097 x 4 B = 128 KiB).  The <= 640-token launch keeps the kernel above.
+constexpr int kAttStreamMaxTok = 4097;
+constexpr int kAttSmemLimit = 232448;    // 227 KiB of shared memory per block
+
+template <int Q>
+__global__ void __launch_bounds__(256) attention_f32_dyn_kernel(const float* __restrict__ qkv, float* __restrict__ out,
+                                                                int tokens, int heads, float scale) {
+  __shared__ float q_s[Q][64];
+  __shared__ float l_s[Q];
+  extern __shared__ float s_dyn[];                 // [Q][tokens]
+  auto s_s = [&](int r) { return s_dyn + r * tokens; };
+  const int t = threadIdx.x;
+  const int q0 = blockIdx.x * Q, h = blockIdx.y, b = blockIdx.z;
+  const long long row_stride = 3LL * heads * 64;
+  const float* base = qkv + (long long)b * tokens * row_stride + h * 64;
+  for (int i = t; i < Q * 64; i += 256) {
+    const int r = i >> 6, d = i & 63;
+    q_s[r][d] = (q0 + r < tokens) ? base[(long long)(q0 + r) * row_stride + d] : 0.f;
+  }
+  __syncthreads();
+  // S = (q k^T) * scale
+  for (int idx = t; idx < Q * tokens; idx += 256) {
+    const int r = idx & (Q - 1), j = idx / Q;
+    const float* kr = base + (long long)j * row_stride + heads * 64;
+    double acc = 0.0;
+#pragma unroll 16
+    for (int d = 0; d < 64; ++d) acc += (double)q_s[r][d] * (double)kr[d];
+    s_s(r)[j] = (float)acc * scale;
+  }
+  __syncthreads();
+  // softmax rows: warp w owns rows w, w + 8, ...
+  const int warp = t >> 5, lane = t & 31;
+  for (int r = warp; r < Q; r += 8) {
+    float mx = -INFINITY;
+    for (int j = lane; j < tokens; j += 32) mx = fmaxf(mx, s_s(r)[j]);
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    double sum = 0.0;
+    for (int j = lane; j < tokens; j += 32) {
+      const float e = expf(s_s(r)[j] - mx);
+      s_s(r)[j] = e;
+      sum += (double)e;
+    }
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (lane == 0) l_s[r] = (float)sum;
+  }
+  __syncthreads();
+  // O = P V / l: 16 threads per row
+  const int r = t >> 4, d4 = (t & 15) * 4;
+  if (r < Q && q0 + r < tokens) {
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    const float* vb = base + 2 * heads * 64 + d4;
+    for (int j = 0; j < tokens; ++j) {
+      const double pj = (double)s_s(r)[j];
+      const float4 v = *reinterpret_cast<const float4*>(vb + (long long)j * row_stride);
+      a0 += pj * (double)v.x; a1 += pj * (double)v.y; a2 += pj * (double)v.z; a3 += pj * (double)v.w;
+    }
+    const double inv = 1.0 / (double)l_s[r];
+    float* o = out + ((long long)b * tokens + q0 + r) * (heads * 64) + h * 64 + d4;
+    *reinterpret_cast<float4*>(o) = make_float4((float)(a0 * inv), (float)(a1 * inv), (float)(a2 * inv), (float)(a3 * inv));
+  }
+}
+
 // ------------------------------------------------------------------------------------------ head tail
 __global__ void __launch_bounds__(256) head_tail_f32_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                             const float* __restrict__ bias, float* __restrict__ out,
@@ -297,11 +361,31 @@ extern "C" int odb_attention_f32(const float* qkv, float* out, int32_t b, int32_
                                  void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!qkv || !out || b < 1 || heads < 1 || tokens < 1) return fail(ODB_ERR_INVALID, "attention_f32: bad argument");
-  if (tokens > kAttMaxTok) return fail(ODB_ERR_UNSUPPORTED, "attention_f32: at most 640 tokens");
+  if (tokens > kAttStreamMaxTok) return fail(ODB_ERR_UNSUPPORTED, "attention_f32: at most 4097 tokens");
   if ((reinterpret_cast<uintptr_t>(qkv) & 15u) || (reinterpret_cast<uintptr_t>(out) & 15u))
     return fail(ODB_ERR_INVALID, "attention_f32: pointers must be 16-byte aligned");
-  dim3 grid((tokens + kAttQ - 1) / kAttQ, heads, b);
-  attention_f32_kernel<<<grid, 256, 0, stream>>>(qkv, out, tokens, heads, scale);
+  if (heads > 65535 || b > 65535) return fail(ODB_ERR_UNSUPPORTED, "attention_f32: at most 65535 heads and images");
+  if (tokens <= kAttMaxTok) {
+    dim3 grid((tokens + kAttQ - 1) / kAttQ, heads, b);
+    attention_f32_kernel<<<grid, 256, 0, stream>>>(qkv, out, tokens, heads, scale);
+  } else {
+    // 16 rows while 16 rows of S and the static q / l rows fit in 227 KiB, 8 above
+    const size_t static_bytes = (size_t)kAttQ * 64 * 4 + kAttQ * 4;     // q_s, l_s of the Q = 16 instance
+    const bool q16 = (size_t)kAttQ * tokens * 4 + static_bytes <= (size_t)kAttSmemLimit;
+    const int q = q16 ? kAttQ : kAttQ / 2;
+    const size_t smem = (size_t)q * tokens * 4;
+    const auto kernel = q16 ? attention_f32_dyn_kernel<kAttQ> : attention_f32_dyn_kernel<kAttQ / 2>;
+    static bool configured[2][kMaxDevices] = {};
+    const int dev_ = current_device();
+    if (!configured[q16][dev_]) {
+      cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           kAttSmemLimit - (int)static_bytes);
+      if (e != cudaSuccess) return fail_cuda(e, "attention_f32: cudaFuncSetAttribute");
+      configured[q16][dev_] = true;
+    }
+    dim3 grid((tokens + q - 1) / q, heads, b);
+    kernel<<<grid, 256, smem, stream>>>(qkv, out, tokens, heads, scale);
+  }
   count_launch();
   return check_launch("attention_f32");
 }

@@ -40,6 +40,30 @@ _ARCH = {
                        rn_in=(96, 192, 384, 768)),
 }
 
+# Input sizes (H, W multiples of 32).  Inference takes up to MAX_PATCHES patches: the attention kernels take up to
+# 4 097 tokens.  Training and x.grad take up to MAX_TRAIN_PATCHES: the attention backward materialises P and dS per
+# (image, head) for up to 640 tokens.
+MAX_PATCHES = 4096
+MAX_TRAIN_PATCHES = 639
+STEM_MAX_W = 1792          # DPT-Hybrid: the stem im2col stages 21 input rows of W + 5 floats in shared memory
+
+
+def check_input_size(H: int, W: int, hybrid: bool, autograd: bool) -> None:
+    """Raises ValueError, before anything is launched, for an input size the launch sequence cannot take: the
+    differentiable forward (autograd) up to MAX_TRAIN_PATCHES patches, inference up to MAX_PATCHES."""
+    patches = (H // 16) * (W // 16)
+    if H % 32 or W % 32 or patches > MAX_TRAIN_PATCHES:
+        if autograd:
+            raise ValueError(f"H and W must be multiples of 32 with at most {MAX_TRAIN_PATCHES} patches for training "
+                             f"and x.grad, got {H}x{W}")
+        if H % 32 or W % 32 or patches > MAX_PATCHES:
+            raise ValueError(f"H and W must be multiples of 32 with at most {MAX_PATCHES} patches, got {H}x{W}")
+        # sizes beyond 639 patches: what the kernels of the launch sequence take
+        if min(H, W) < 64:
+            raise ValueError(f"H and W must be at least 64 (the 1/32 decoder map is upsampled from 2x2), got {H}x{W}")
+        if hybrid and W > STEM_MAX_W:
+            raise ValueError(f"DPT-Hybrid: W must be at most {STEM_MAX_W} (stem convolution), got {W}")
+
 
 def _rn_pad(arch: dict) -> Tuple[int, ...]:
     """reassemble widths, zero-padded to the GEMM's N granularity"""
@@ -439,9 +463,9 @@ class DPTDepthModel(nn.Module):
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
         B, _, H, W = x.shape
-        if H % 32 or W % 32 or (H // 16) * (W // 16) + 1 > 640:
-            raise ValueError("H and W must be multiples of 32 with at most 639 patches (384x384 in scope)")
-        if torch.is_grad_enabled() and (self.training or x.requires_grad):
+        autograd = torch.is_grad_enabled() and (self.training or x.requires_grad)
+        check_input_size(H, W, self.arch["hybrid"], autograd)
+        if autograd:
             # train() mode under autograd, or an input that requires grad in either mode: the
             # differentiable forward (activations kept for the backward kernels).  Any other eval() call, or any call
             # under torch.no_grad(), is the inference path below and returns a tensor that is not attached to an
@@ -540,7 +564,11 @@ def _resnet_features(x, pk, ws, buf, fp32: bool, taps, S):
     stats_pool = buf("gn_stats", (n_gn, B, 32, 2), torch.float32)
     gn_scratch = ws.bufs.get("gn_scratch")
     if gn_scratch is None:                             # zeroed once; the kernel leaves it zeroed
-        gn_scratch = ws.bufs["gn_scratch"] = torch.zeros(4 << 20, dtype=torch.uint8, device=x.device)
+        # fp32 mode's statistics partials grow with B * H * W: the stem (64 ch at H/2) and stage 0 (256 ch at H/4)
+        # need the most (4 MiB covers B = 56 at 384x384, B = 7 at 1024x1024)
+        need = max(int(ops.lib().odb_groupnorm_scratch_bytes(B, hw, c, 32))
+                   for hw, c in ((h2 * w2, 64), ((H // 4) * (W // 4), 256)))
+        gn_scratch = ws.bufs["gn_scratch"] = torch.zeros(max(4 << 20, need), dtype=torch.uint8, device=x.device)
     stat_i = iter(range(n_gn))
     # fused statistics: the conv epilogue writes per-warp partial sums here (largest layer:
     # stage 0 at 96x96 -> 72 tiles x 4 quadrants x 32 groups x 2 per image)

@@ -18,7 +18,7 @@ the pre-activations of the fc1 and readout GELUs, and the unfused head's interme
   * the plain ViTs' ConvTranspose reassembles: one dgrad and one wgrad with k taps on k row views of the output gradient.
 The DPT-Hybrid (vitb_rn50_384), DPT-Large (vitl16_384) and the plain ViT-B DPT (vitb16_384) share this engine: only the
 front end (ResNetV2 + stem vs patch embedding) and the reassemble of layer_1 / layer_2 are backbone-specific.
-The engine takes every input size inference takes: H and W multiples of 32, at most 639 patches.  Off the pretrained
+The engine takes H and W multiples of 32 with at most 639 patches (inference takes up to 4 096).  Off the pretrained
 24 x 24 patch grid the forward resizes pos_embed's patch rows from this step's fp32 master weights with the function
 inference uses (model.resize_pos_grid), and the backward takes their gradient through the adjoint of that bilinear
 resize (odb_pos_embed_resize_bwd, no atomics).
@@ -40,8 +40,8 @@ import torch
 
 from . import bwd, ops
 from ._capi import OdbError
-from .model import (_ARCH, _STAGES, DPTDepthModel, _forward_vectors, _Workspace, dpt_forward, gemm_layers,
-                    resize_pos_grid)
+from .model import (_ARCH, _STAGES, MAX_TRAIN_PATCHES, DPTDepthModel, _forward_vectors, _Workspace, check_input_size,
+                    dpt_forward, gemm_layers, resize_pos_grid)
 
 
 def _parity_dgrad_plan(mode: str):
@@ -495,8 +495,7 @@ class TrainEngine:
             raise OdbError("TrainEngine.forward: CUDA input [B,3,H,W] required")
         x = x.detach().float().contiguous()
         B, _, H, W = x.shape
-        if H % 32 or W % 32 or (H // 16) * (W // 16) + 1 > 640:
-            raise ValueError("H and W must be multiples of 32 with at most 639 patches")
+        check_input_size(H, W, self.model.arch["hybrid"], autograd=True)
         gh, gw = H // 16, W // 16
         self.pack(trainable)
         # the patch rows of this step's pos_embed (resized from the fp32 master weights as inference resizes them),
@@ -906,6 +905,8 @@ def differentiable_forward(model: DPTDepthModel, x: torch.Tensor) -> torch.Tenso
     """model(x) under autograd: returns a tensor whose backward fills p.grad of every parameter that requires grad and,
     when x requires grad, x.grad (the gradient w.r.t. the input image, in x's dtype).  Only those gradients are computed
     (backward_plan); the GEMM operands of frozen parameters are re-packed only when the parameters change."""
+    if x.dim() == 4:
+        check_input_size(x.shape[2], x.shape[3], model.arch["hybrid"], autograd=True)
     eng = getattr(model, "_train_engine", None)
     if eng is None or eng.fp32 != (model.precision == "fp32"):
         eng = TrainEngine(model, precision=model.precision)
@@ -969,6 +970,9 @@ class _FlatTrainStep:
         import torch.distributed as dist
         from .optim import FlatAdam
         name = type(self).__name__
+        if (input_size[0] // 16) * (input_size[1] // 16) > MAX_TRAIN_PATCHES:
+            raise ValueError(f"{name}: training takes at most {MAX_TRAIN_PATCHES} patches, got input_size "
+                             f"{tuple(input_size)}")
         if model.num_channels != self.CHANNELS:
             raise ValueError(f"{name} trains a model with num_channels={self.CHANNELS}, got num_channels="
                              f"{model.num_channels}")
