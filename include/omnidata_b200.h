@@ -41,8 +41,10 @@ typedef enum odb_act { ODB_ACT_NONE = 0, ODB_ACT_RELU = 1, ODB_ACT_GELU = 2 } od
 
 /* Storage type of an activation tensor.  bf16 is the production format; fp32 carries the ViT residual stream
  * (the reference adds every block's output to an fp32 stream: timm Block.forward `x = x + ...`) and every
- * activation of the fp32 correctness mode (SURVEY.md 8c: the reference itself is fp32-only). */
-typedef enum odb_dtype { ODB_DTYPE_BF16 = 0, ODB_DTYPE_F32 = 1 } odb_dtype;
+ * activation of the fp32 correctness mode (SURVEY.md 8c: the reference itself is fp32-only).  e4m3 (FP8, 1 byte,
+ * OCP E4M3FN: finite range +-448) is the operand type of the fp8 inference mode's ViT linear layers, always paired with
+ * fp32 scale vectors (odb_conv_gemm_scaled, odb_layernorm_e4m3, odb_rowquant_e4m3). */
+typedef enum odb_dtype { ODB_DTYPE_BF16 = 0, ODB_DTYPE_F32 = 1, ODB_DTYPE_E4M3 = 2 } odb_dtype;
 
 /* A strided channels-last view [b][h][w][c] (bf16 storage unless the owning descriptor says fp32; strides in
  * elements of the storage type). */
@@ -133,10 +135,29 @@ int odb_conv_gemm(const odb_conv_gemm_desc* desc, void* stream);
  * CTA pair, bit 1 = halo mode. */
 int odb_conv_gemm_plan(const odb_conv_gemm_desc* desc, int32_t* out4);
 
+/* The fp8 inference mode's ViT linear layers (nn.Linear in timm Attention/Mlp, loop M/vit.py:150-151: attn.qkv,
+ * attn.proj, mlp.fc1, mlp.fc2) on e4m3 wgmma.  desc as for odb_conv_gemm with in_dtype = ODB_DTYPE_E4M3: views[0] and
+ * weight are e4m3 (channels and strides multiples of 16), one view, one tap at offset 0, the input extent equal to
+ * the output extent, a bias, no head / halo / CTA pair / gn_partial / out2.  With q_a, q_w the e4m3 operands:
+ *   v[r][c] = (sum_k q_a[r][k] * q_w[c][k]) * (row_scale[r] * col_scale[c]) + bias[c]      (fp32, one fma)
+ * then the layer's epilogue: bf16 out = act(v) (act NONE or GELU), or fp32 out = residual + v (out_dtype F32,
+ * residual fp32).  row_scale fp32 [b][h][w] (one per row of the input), col_scale fp32 [n] (16-byte aligned). */
+int odb_conv_gemm_scaled(const odb_conv_gemm_desc* desc, const float* row_scale, const float* col_scale, void* stream);
+
 /* LayerNorm over the last dim (timm Block.norm1/norm2, eps 1e-6): y = (x-mean)/sqrt(var+eps)*g + b.
  * x, y bf16 [rows][cols] (cols multiple of 256, <= 1024); gamma/beta fp32. */
 int odb_layernorm(const void* x, const float* gamma, const float* beta, void* y, int64_t rows,
                   int32_t cols, float eps, int32_t x_dtype, int32_t y_dtype, void* stream);
+/* odb_layernorm (timm Block.norm1/norm2 in the fp8 inference mode) with an e4m3 output quantised per row from the fp32
+ * result z of odb_layernorm's arithmetic: amax = max_k |z[k]|, row_scale = amax / 448, q = cvt.rn.satfinite.e4m3(z *
+ * (448 / amax)) (IEEE division); an all-zero row gets row_scale 1 and q 0.  x fp32 or bf16 [rows][cols] (x_dtype),
+ * y e4m3 [rows][cols], row_scale fp32 [rows]. */
+int odb_layernorm_e4m3(const void* x, const float* gamma, const float* beta, void* y, float* row_scale, int64_t rows,
+                       int32_t cols, float eps, int32_t x_dtype, void* stream);
+/* The same per-row quantisation of a bf16 tensor: x bf16 [rows][cols] -> y e4m3 [rows][cols], row_scale fp32 [rows];
+ * cols in {768, 1024, 3072, 4096}, 16-byte aligned pointers.  Feeds attn.proj from odb_attention's output and mlp.fc2
+ * from mlp.fc1's GELU output in the fp8 inference mode (timm Attention.proj / Mlp.fc2 inputs, M/vit.py:150-151). */
+int odb_rowquant_e4m3(const void* x, void* y, float* row_scale, int64_t rows, int32_t cols, void* stream);
 
 /* Fused multi-head attention (timm Attention.forward): qkv bf16 [b][tokens][3][heads][64] as written
  * by the qkv linear; out bf16 [b][tokens][heads*64]; softmax(q k^T * scale) v.  wgmma kernel:

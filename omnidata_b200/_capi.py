@@ -14,7 +14,7 @@ LIB_PATH = Path(__file__).resolve().parent / "lib" / "libomnidata_b200.so"
 ODB_MAX_VIEWS = 4
 ODB_MAX_TAPS = 9
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
-DTYPE_BF16, DTYPE_F32 = 0, 1
+DTYPE_BF16, DTYPE_F32, DTYPE_E4M3 = 0, 1, 2
 
 
 class OdbError(RuntimeError):
@@ -96,6 +96,9 @@ class WgradDesc(C.Structure):
 _SIGNATURES = {
     "odb_conv_gemm": (C.c_int, [C.POINTER(ConvGemmDesc), C.c_void_p]),
     "odb_conv_gemm_plan": (C.c_int, [C.POINTER(ConvGemmDesc), C.POINTER(C.c_int32)]),
+    "odb_conv_gemm_scaled": (C.c_int, [C.POINTER(ConvGemmDesc), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "odb_layernorm_e4m3": (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_int32, C.c_float, C.c_int32, C.c_void_p]),
+    "odb_rowquant_e4m3": (C.c_int, [C.c_void_p] * 3 + [C.c_int64, C.c_int32, C.c_void_p]),
     "odb_groupnorm_finalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                          C.c_float, C.c_void_p]),
     "odb_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,

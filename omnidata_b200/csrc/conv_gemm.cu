@@ -66,6 +66,14 @@ struct ConvGemmParams {
   unsigned long long* trace;  // diagnostics (odb_debug_conv_trace): kTraceSlots globaltimer stamps per CTA
 };
 
+// Parameters of the e4m3 instances (odb_conv_gemm_scaled).  `trace` is hidden by a null constant: the diagnostics
+// trace is compiled out of these instances, whose bookkeeping would not fit beside the accumulator without spilling.
+struct ConvGemmParamsFp8 : ConvGemmParams {
+  const float* row_scale;     // fp32 [rows]: the A operand's per-row dequantisation scale
+  const float* col_scale;     // fp32 [n]: the weight's per-output-channel dequantisation scale
+  static constexpr unsigned long long* trace = nullptr;
+};
+
 // trace slots per CTA: 0 prologue done, 1 dependency wait done, 2 kernel end, 3 tiles of this CTA;
 // per tile i < kTraceTiles at 8 + 5 i: MMA start, first stage full, accumulator complete, epilogue start, epilogue end
 constexpr int kTraceTiles = 24;
@@ -193,6 +201,86 @@ struct SmemPlan {
   static_assert(kTotal <= 232448, "shared memory plan exceeds 227 KiB");
 };
 
+// ---- FP8 epilogue pieces (conv_gemm_kernel<..., FP8 = true>).  The scaled GEMM takes [rows][C] operands (h = b = 1):
+// tile row r is output row x0 + r; rows outside the output get scale 0.
+ODB_DEVINL float fp8_row_scale(const ConvGemmParamsFp8& p, int x0, int r) {
+  return r < p.tile_w && x0 + r < p.out_w ? __ldg(p.row_scale + x0 + r) : 0.f;
+}
+// v[j] = src[j] * (sa * cs[j]) + b[j] for the 32 staged accumulator values of one row (the row-per-thread epilogues).
+// The scale products are formed in v first, so that the column scales and the bias are never in registers together
+// beside the accumulator columns still to be staged.
+ODB_DEVINL void fp8_read_row_scaled(const float* src_row, const float* b, const float* cs, float sa, float* v) {
+  const float4* src = reinterpret_cast<const float4*>(src_row);
+  const float4* bp = reinterpret_cast<const float4*>(b);
+  const float4* sp = reinterpret_cast<const float4*>(cs);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 s4 = __ldg(sp + j);
+    v[4 * j + 0] = sa * s4.x; v[4 * j + 1] = sa * s4.y; v[4 * j + 2] = sa * s4.z; v[4 * j + 3] = sa * s4.w;
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 q = src[j];
+    const float4 b4 = __ldg(bp + j);
+    v[4 * j + 0] = fmaf(q.x, v[4 * j + 0], b4.x); v[4 * j + 1] = fmaf(q.y, v[4 * j + 1], b4.y);
+    v[4 * j + 2] = fmaf(q.z, v[4 * j + 2], b4.z); v[4 * j + 3] = fmaf(q.w, v[4 * j + 3], b4.w);
+  }
+}
+// EPI_BIAS_RES_F32 with e4m3 operands: as the kernel's add_frag_res_f32 (same fragment rows, columns and swizzled
+// staging addresses), adding res + (acc * (sa[h] * cs[c]) + bias[c]); sa[h] = the scales of rows r and r + 8.
+template <int C0>
+ODB_DEVINL void fp8_add_frag_res_f32(const float* dacc, uint32_t buf, const float* b, const float* cs, const float* sa,
+                                     int r, int lane) {
+  const uint32_t rbase = buf + static_cast<uint32_t>(r) * 128u + (static_cast<uint32_t>(lane & 1) << 3);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float2 b2 = __ldg(reinterpret_cast<const float2*>(b + C0 + 8 * j + 2 * (lane & 3)));
+    const float2 s2 = __ldg(reinterpret_cast<const float2*>(cs + C0 + 8 * j + 2 * (lane & 3)));
+    const uint32_t unit = static_cast<uint32_t>(2 * (j & 3) + ((lane & 3) >> 1));
+    const uint32_t addr = rbase + static_cast<uint32_t>(j >> 2) * kStagingBytes + ((unit ^ (r & 7)) << 4);
+    const float* a = dacc + 4 * (C0 / 8 + j);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {                   // rows r, r + 8
+      const uint32_t ad = addr + h * 8u * 128u;
+      float q0, q1;
+      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(q0), "=f"(q1) : "r"(ad) : "memory");
+      q0 += fmaf(a[2 * h], sa[h] * s2.x, b2.x);
+      q1 += fmaf(a[2 * h + 1], sa[h] * s2.y, b2.y);
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(ad), "f"(q0), "f"(q1) : "memory");
+    }
+  }
+}
+template <int BLOCK_N>
+ODB_DEVINL void fp8_add_frag_res_f32_rt(int c, const float* dacc, uint32_t buf, const float* b, const float* cs,
+                                        const float* sa, int r, int lane) {   // run-time chunk index
+  if (c == 0) fp8_add_frag_res_f32<0>(dacc, buf, b, cs, sa, r, lane);
+  if constexpr (BLOCK_N > 64) {
+    if (c == 1) fp8_add_frag_res_f32<64>(dacc, buf, b, cs, sa, r, lane);
+  }
+  if constexpr (BLOCK_N > 128) {
+    if (c == 2) fp8_add_frag_res_f32<128>(dacc, buf, b, cs, sa, r, lane);
+    else if (c == 3) fp8_add_frag_res_f32<192>(dacc, buf, b, cs, sa, r, lane);
+  }
+}
+
+// The row scales of one thread's rows for a tile, read once per tile: x = the row of the row-per-thread epilogues, or
+// (x, y) = the fragment rows r and r + 8 (EPI_BIAS_RES_F32).  bf16 instances get an empty object.
+struct Fp8NoScale {};
+template <bool FP8, bool F32, typename P>
+ODB_DEVINL auto fp8_tile_scales(const P& p, int x0, int row, int frag_row) {
+  if constexpr (!FP8) {
+    return Fp8NoScale{};
+  } else if constexpr (F32) {
+    return make_float2(fp8_row_scale(p, x0, frag_row), fp8_row_scale(p, x0, frag_row + 8));
+  } else {
+    return make_float2(fp8_row_scale(p, x0, row), 0.f);
+  }
+}
+
+// K elements per 128-byte operand row: 64 bf16, 128 e4m3.  (A class constant: a constexpr local in the kernel
+// body changes the register allocation of the bf16 instances.)
+template <bool FP8> struct KBlock { static constexpr int value = FP8 ? 2 * kKBlock : kKBlock; };
+
 // Named barriers of the consumer warpgroups (barrier 0 is __syncthreads)
 constexpr uint32_t kBarEpilogue = 1;   // staging slot hand-over to the TMA store
 constexpr uint32_t kBarAccChunk = 2;   // accumulator chunk buffer written / read
@@ -201,12 +289,22 @@ constexpr uint32_t kBarAccChunk = 2;   // accumulator chunk buffer written / rea
 // CTA TMA-loads its own A rows and HALF of the B rows, multicast into both CTAs, so the pair reads each weight tile
 // from L2 once.  A B stage is refilled only after the consumers of BOTH CTAs released it (each consumer warp arrives
 // on the empty barrier of both CTAs).  The MMAs and their order are those of the single-CTA kernel.
-template <int BLOCK_N, int STAGES, int NSTAGING, bool HEAD, bool HALO, bool PAIR, int EPI = EPI_GENERIC>
+//
+// FP8 = true (odb_conv_gemm_scaled, the ViT blocks' linear layers in the fp8 inference mode): e4m3 operands.  A
+// 128-byte swizzled row holds 128 e4m3 elements instead of 64 bf16 ones, so a stage has the same bytes and layout and
+// carries twice the K; each of its four wgmma steps is one m64nNk32 e4m3 instruction (32 bytes, as k16 bf16).  The
+// epilogue dequantises before the bias: v = acc * (row_scale[r] * col_scale[c]) + bias[c] (one fma), then the
+// layer's epilogue as in bf16.  1-tap linear layers with EPI_BIAS / EPI_BIAS_GELU / EPI_BIAS_RES_F32 only.  Every
+// FP8 difference sits in an `if constexpr (FP8)` branch: the FP8 = false instances are the code they were before.
+template <int BLOCK_N, int STAGES, int NSTAGING, bool HEAD, bool HALO, bool PAIR, int EPI = EPI_GENERIC,
+          bool FP8 = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
-conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
+conv_gemm_kernel(const __grid_constant__ std::conditional_t<FP8, ConvGemmParamsFp8, ConvGemmParams> p) {
   static_assert(EPI == EPI_GENERIC || (!HEAD && !HALO && NSTAGING >= 2), "fast epilogues: plain tiles only");
   static_assert(!PAIR || !HEAD, "CTA pairs: no head tail");
   static_assert(EPI != EPI_BIAS_RES_F32 || NSTAGING >= 4, "fp32 epilogue: two staging slots of two 16 KiB units");
+  static_assert(!FP8 || (!PAIR && (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RES_F32)),
+                "e4m3 operands: single-CTA linear layers with a bias, bias + GELU or fp32-residual epilogue");
   using Plan = SmemPlan<BLOCK_N, STAGES, NSTAGING, HALO, HEAD, EPI != EPI_BIAS_RES_F32>;
   using Acc = AccChunk<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
@@ -342,8 +440,8 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
             for (int kb = 0; kb < p.kb_per_tap; ++kb) {
               mbar_wait(empty_bar(stage), phase ^ 1u);
               mbar_expect_tx(full_bar(stage), a_bytes + Plan::kBBytes);
-              tma_load_4d(smem_base + Plan::kAOff + stage * kABytes, amap, full_bar(stage), kb * kKBlock, ax, ay, tb);
-              load_b(stage, (tap * p.kb_per_tap + kb) * kKBlock, tn);
+              tma_load_4d(smem_base + Plan::kAOff + stage * kABytes, amap, full_bar(stage), kb * KBlock<FP8>::value, ax, ay, tb);
+              load_b(stage, (tap * p.kb_per_tap + kb) * KBlock<FP8>::value, tn);
               if (++stage == STAGES) { stage = 0; phase ^= 1u; }
             }
           }
@@ -425,8 +523,12 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
           const uint64_t bdesc = gmma_desc_sw128(smem_base + Plan::kBOff + stage * Plan::kBBytes);
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kKBlock / 16; ++k)   // +32 bytes (= 2 in 16-byte units) per K step of 16
-            Wgmma<BLOCK_N>::template ss<0, 0>(dacc, adesc + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+          for (int k = 0; k < kKBlock / 16; ++k) {  // +32 bytes (= 2 in 16-byte units) per K step of 16 (FP8: 32)
+            if constexpr (FP8)
+              WgmmaE4M3<BLOCK_N>::ss(dacc, adesc + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+            else
+              Wgmma<BLOCK_N>::template ss<0, 0>(dacc, adesc + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+          }
           wgmma_commit();
           wgmma_wait<1>();
           if (prev >= 0 && lane == 0) release_b(prev);
@@ -561,12 +663,17 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
         // EPI_GN: rows of this thread that really exist (ragged tiles)
         const int gx = x0 + (row % p.tile_w), gy = y0 + (row / p.tile_w);
         const bool valid = row < p.tile_w * p.tile_h && gx < p.out_w && gy < p.out_h && tb < p.out_b;
+        [[maybe_unused]] const auto sa = fp8_tile_scales<FP8, F32>(p, x0, row, wg * 64 + 16 * (warp & 3) + (lane >> 2));
 #pragma unroll
         for (int c = 0; c < kChunks; ++c, ++g) {
           float v[32];
           if constexpr (!F32) {
             stage_chunk_rt(c);
-            read_row_bias(row, cofs, EPI == EPI_GN ? nullptr : bias + c * 64, v);
+            if constexpr (FP8)
+              fp8_read_row_scaled(acc_buf + row * Acc::kPitch + cofs, bias + c * 64, p.col_scale + n0 + cofs + c * 64,
+                                  sa.x, v);
+            else
+              read_row_bias(row, cofs, EPI == EPI_GN ? nullptr : bias + c * 64, v);
           }
           if constexpr (EPI == EPI_BIAS_GELU) {
 #pragma unroll
@@ -579,7 +686,13 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
           const uint32_t buf = smem_base + Plan::kCOff + slot * kSlotBytes;
           if constexpr (F32) {
             mbar_wait(rfull_bar(slot), (g / NS) & 1u);
-            add_frag_res_f32_rt(c, buf, bias_n0);
+            if constexpr (FP8) {
+              const int r = wg * 64 + 16 * (warp & 3) + (lane >> 2);      // the fragment rows r and r + 8
+              const float sa2[2] = {sa.x, sa.y};
+              fp8_add_frag_res_f32_rt<BLOCK_N>(c, dacc, buf, bias_n0, p.col_scale + n0, sa2, r, lane);
+            } else {
+              add_frag_res_f32_rt(c, buf, bias_n0);
+            }
           } else {
           if constexpr (EPI == EPI_BIAS_RES) {
             // the residual rows of this chunk were TMA-loaded into the staging slot (same swizzled
@@ -819,13 +932,13 @@ conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
 
 // ------------------------------------------------------------------------------------------ host
 
+// esz: element size in bytes, 2 = bf16, 4 = fp32, 1 = e4m3 (encoded as UINT8: TMA moves bytes)
 static int encode_view_map(CUtensorMap* map, const odb_view& v, int box_c, int box_w, int box_h,
-                           CUtensorMapSwizzle swz, bool f32 = false) {
+                           CUtensorMapSwizzle swz, int esz = 2) {
   if (v.ptr == nullptr) return fail(ODB_ERR_INVALID, "conv_gemm: null view pointer");
   if ((reinterpret_cast<uintptr_t>(v.ptr) & 15u) != 0)
     return fail(ODB_ERR_INVALID, "conv_gemm: view pointer must be 16-byte aligned");
   if (v.c % 8 != 0) return fail(ODB_ERR_INVALID, "conv_gemm: channel count must be a multiple of 8");
-  const int esz = f32 ? 4 : 2;
   cuuint64_t dims[4] = {(cuuint64_t)v.c, (cuuint64_t)v.w, (cuuint64_t)v.h, (cuuint64_t)v.b};
   // strides of dims 1..3 in bytes; a unit extent may carry any (16B-multiple) stride
   long long sx = v.sx, sy = v.sy, sb = v.sb;
@@ -834,17 +947,22 @@ static int encode_view_map(CUtensorMap* map, const odb_view& v, int box_c, int b
   if (v.b == 1 && sb == 0) sb = (long long)v.h * sy;
   if (sx % 8 != 0 || sy % 8 != 0 || sb % 8 != 0 || sx <= 0 || sy <= 0 || sb <= 0)
     return fail(ODB_ERR_INVALID, "conv_gemm: view strides must be positive multiples of 8 elements");
+  if (esz == 1 && (sx % 16 != 0 || sy % 16 != 0 || sb % 16 != 0 || v.c % 16 != 0))
+    return fail(ODB_ERR_INVALID, "conv_gemm: e4m3 views need channel counts and strides that are multiples of 16");
   cuuint64_t strides[3] = {(cuuint64_t)sx * esz, (cuuint64_t)sy * esz, (cuuint64_t)sb * esz};
   cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  return encode_tiled(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
-                      const_cast<void*>(v.ptr), dims, strides, box, estr, swz);
+  const CUtensorMapDataType dt = esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                 : esz == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  return encode_tiled(map, dt, 4, const_cast<void*>(v.ptr), dims, strides, box, estr, swz);
 }
 
-template <int BLOCK_N, int STAGES, int NSTAGING, bool HEAD, bool HALO, int EPI = EPI_GENERIC, bool PAIR = false>
-static int launch_instance(const ConvGemmParams& p, long long units, cudaStream_t stream) {
+template <int BLOCK_N, int STAGES, int NSTAGING, bool HEAD, bool HALO, int EPI = EPI_GENERIC, bool PAIR = false,
+          bool FP8 = false>
+static int launch_instance(const std::conditional_t<FP8, ConvGemmParamsFp8, ConvGemmParams>& p, long long units,
+                           cudaStream_t stream) {
   using Plan = SmemPlan<BLOCK_N, STAGES, NSTAGING, HALO, HEAD, EPI != EPI_BIAS_RES_F32>;
-  auto kernel = conv_gemm_kernel<BLOCK_N, STAGES, NSTAGING, HEAD, HALO, PAIR, EPI>;
+  auto kernel = conv_gemm_kernel<BLOCK_N, STAGES, NSTAGING, HEAD, HALO, PAIR, EPI, FP8>;
   static bool configured[kMaxDevices] = {};      // the opt-in is per device
   const int dev = current_device();
   if (!configured[dev]) {
@@ -905,6 +1023,21 @@ static int launch_fast(const ConvGemmParams& p, int block_n, bool pair, long lon
       case 128: return launch_instance<128, 4, 2, false, false, EPI>(p, units, stream);
       default: return launch_instance<64, 4, 4, false, false, EPI>(p, units, stream);
     }
+  }
+}
+
+// the e4m3 instances (odb_conv_gemm_scaled): the bf16 instances' shared-memory plans, each stage carrying twice the K.
+// EPI_BIAS has no 256-wide instance (it does not fit in registers without spilling); the host plans it at 128.
+template <int EPI>
+static int launch_fp8(const ConvGemmParamsFp8& p, int block_n, long long units, cudaStream_t stream) {
+  constexpr int NS = EPI == EPI_BIAS_RES_F32 ? 4 : 2;
+  if constexpr (EPI != EPI_BIAS) {
+    if (block_n == 256) return launch_instance<256, 3, NS, false, false, EPI, false, true>(p, units, stream);
+  }
+  switch (block_n) {
+    case 128: return launch_instance<128, 4, NS, false, false, EPI, false, true>(p, units, stream);
+    case 64: return launch_instance<64, 4, 4, false, false, EPI, false, true>(p, units, stream);
+    default: return fail(ODB_ERR_UNSUPPORTED, "conv_gemm_scaled: no instance for this block_n");
   }
 }
 
@@ -1082,9 +1215,9 @@ extern "C" int odb_conv_gemm(const odb_conv_gemm_desc* d, void* stream_) {
       return fail(ODB_ERR_UNSUPPORTED, "conv_gemm: fp32 output needs bias + fp32 residual and no act/out2/gn/head/halo");
     if (d->out.c != N || d->residual.c != N || d->residual.w < ow || d->residual.h < oh || d->residual.b < ob)
       return fail(ODB_ERR_INVALID, "conv_gemm: fp32 out/residual extent mismatch");
-    rc = encode_view_map(&p.out_map, d->out, 32, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, true);
+    rc = encode_view_map(&p.out_map, d->out, 32, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, 4);
     if (rc) return rc;
-    rc = encode_view_map(&p.res_map, d->residual, 32, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, true);
+    rc = encode_view_map(&p.res_map, d->residual, 32, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, 4);
     if (rc) return rc;
     p.out2_map = p.out_map;
     p.bias = d->bias;
@@ -1183,4 +1316,87 @@ extern "C" int odb_conv_gemm(const odb_conv_gemm_desc* d, void* stream_) {
       return launch_instance<32, 8, 0, true, false>(p, total, stream);
   }
   return fail(ODB_ERR_INVALID, "conv_gemm: unreachable");
+}
+
+
+extern "C" int odb_conv_gemm_scaled(const odb_conv_gemm_desc* d, const float* row_scale, const float* col_scale,
+                                    void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (d == nullptr || d->in_dtype != ODB_DTYPE_E4M3)
+    return fail(ODB_ERR_INVALID, "conv_gemm_scaled: needs a descriptor with in_dtype ODB_DTYPE_E4M3");
+  if (row_scale == nullptr || col_scale == nullptr || (reinterpret_cast<uintptr_t>(row_scale) & 3u) != 0 ||
+      (reinterpret_cast<uintptr_t>(col_scale) & 15u) != 0)
+    return fail(ODB_ERR_INVALID, "conv_gemm_scaled: row_scale (4-byte) and col_scale (16-byte aligned) are required");
+  if (d->num_views != 1 || d->num_taps != 1 || d->tap_view[0] != 0 || d->tap_dx[0] != 0 || d->tap_dy[0] != 0)
+    return fail(ODB_ERR_UNSUPPORTED, "conv_gemm_scaled: linear layers only (one view, one tap at offset 0)");
+  if (d->views[0].w != d->out.w || d->views[0].h != 1 || d->views[0].b != 1 || d->out.h != 1 || d->out.b != 1)
+    return fail(ODB_ERR_INVALID, "conv_gemm_scaled: [rows][C] operands (h = b = 1) with equal input and output rows");
+  if (d->head_out != nullptr || d->halo == 1 || d->cta_pair == 1 || d->gn_partial != nullptr || d->out2.ptr != nullptr ||
+      d->bias == nullptr || d->epilogue != 0)
+    return fail(ODB_ERR_UNSUPPORTED, "conv_gemm_scaled: needs a bias; no head, halo, CTA pair, GroupNorm or out2");
+  const bool out_f32 = d->out_dtype == ODB_DTYPE_F32;
+  if (out_f32 ? (d->act != ODB_ACT_NONE || d->residual.ptr == nullptr)
+              : (d->out_dtype != ODB_DTYPE_BF16 || d->residual.ptr != nullptr ||
+                 (d->act != ODB_ACT_NONE && d->act != ODB_ACT_GELU)))
+    return fail(ODB_ERR_UNSUPPORTED,
+                "conv_gemm_scaled: bf16 output with bias [+ GELU], or fp32 output with bias + fp32 residual");
+  HostPlan hp;
+  int rc = make_plan(d, &hp);
+  if (rc) return rc;
+  if (d->out.ptr == nullptr) return fail(ODB_ERR_INVALID, "conv_gemm_scaled: null output");
+  if (d->weight == nullptr || (reinterpret_cast<uintptr_t>(d->weight) & 15u) != 0)
+    return fail(ODB_ERR_INVALID, "conv_gemm_scaled: weight must be non-null and 16-byte aligned");
+  const bool bias_only = !out_f32 && d->act == ODB_ACT_NONE;
+  if (bias_only && hp.block_n == 256) {
+    if (d->block_n == 256) return fail(ODB_ERR_UNSUPPORTED, "conv_gemm_scaled: bias-only epilogue: block_n 64 or 128");
+    hp.block_n = 128;
+  }
+  const int C = d->views[0].c, N = d->n, tw = hp.tw, th = hp.th, block_n = hp.block_n;
+  if (block_n < 64) return fail(ODB_ERR_UNSUPPORTED, "conv_gemm_scaled: block_n must be 64, 128 or 256");
+  const int ow = d->out.w, oh = d->out.h, ob = d->out.b;
+
+  ConvGemmParamsFp8 p;
+  memset(&p, 0, sizeof(p));
+  p.tile_w = tw; p.tile_h = th;
+  p.tiles_x = hp.tiles_x; p.tiles_y = hp.tiles_y; p.tiles_b = ob;
+  p.out_w = ow; p.out_h = oh; p.out_b = ob; p.n_total = N;
+  p.tiles_n = N / block_n;
+  const long long units = hp.m_tiles * p.tiles_n;
+  p.num_taps = 1;
+  p.kb_per_tap = (C + 127) / 128;        // 128 e4m3 elements per K block
+  for (int v = 0; v < ODB_MAX_VIEWS; ++v) {
+    rc = encode_view_map(&p.a_map[v], d->views[0], 128, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, 1);
+    if (rc) return rc;
+  }
+  {
+    cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)N};
+    cuuint64_t strides[1] = {(cuuint64_t)C};
+    cuuint32_t box[2] = {128u, (cuuint32_t)block_n};
+    cuuint32_t estr[2] = {1, 1};
+    rc = encode_tiled(&p.b_map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(d->weight), dims, strides, box,
+                      estr, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  }
+  if (d->out.c != N) return fail(ODB_ERR_INVALID, "conv_gemm_scaled: out.c must equal n");
+  p.bias = d->bias;
+  p.bias_sb = d->bias_sb;
+  p.row_scale = row_scale;
+  p.col_scale = col_scale;
+  if (out_f32) {
+    if (d->residual.c != N || d->residual.w < ow || d->residual.h < oh || d->residual.b < ob)
+      return fail(ODB_ERR_INVALID, "conv_gemm_scaled: fp32 out/residual extent mismatch");
+    rc = encode_view_map(&p.out_map, d->out, 32, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, 4);
+    if (rc) return rc;
+    rc = encode_view_map(&p.res_map, d->residual, 32, tw, th, CU_TENSOR_MAP_SWIZZLE_128B, 4);
+    if (rc) return rc;
+    p.out2_map = p.out_map;
+    return launch_fp8<EPI_BIAS_RES_F32>(p, block_n, units, stream);
+  }
+  rc = encode_view_map(&p.out_map, d->out, 64, tw, th, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  p.out2_map = p.out_map;
+  p.res_map = p.out_map;
+  p.act = d->act;
+  return d->act == ODB_ACT_GELU ? launch_fp8<EPI_BIAS_GELU>(p, block_n, units, stream)
+                                : launch_fp8<EPI_BIAS>(p, block_n, units, stream);
 }

@@ -35,15 +35,37 @@ ODB_DEVINL void store8(float* p, const float* v) {
 ODB_DEVINL void store1(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
 ODB_DEVINL void store1(float* p, float v) { *p = v; }
 
+// ---- e4m3 storage (the fp8 inference mode's GEMM operands), quantised per row:
+//   amax = max |z|, scale = amax / 448, q = cvt.rn.satfinite.e4m3(z * (448 / amax)); an all-zero row: scale 1, q = z * 0.
+// Both divisions are IEEE round-to-nearest (__fdiv_rn) although this file is built with fast math.
+struct e4m3_t { uint8_t bits; };
+ODB_DEVINL float e4m3_inv_scale(float amax) { return amax > 0.f ? __fdiv_rn(448.f, amax) : 0.f; }
+ODB_DEVINL float e4m3_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f; }
+// eight values times inv -> eight e4m3 bytes, v[0] in the lowest byte
+ODB_DEVINL uint2 quant8_e4m3(const float* v, float inv) {
+  uint32_t w[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    uint16_t h;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h) : "f"(__fmul_rn(v[2 * k + 1], inv)),
+        "f"(__fmul_rn(v[2 * k], inv)));
+    w[k] = h;
+  }
+  return make_uint2(w[0] | (w[1] << 16), w[2] | (w[3] << 16));
+}
+
 // ------------------------------------------------------------------------------------------
 // LayerNorm: each warp normalises TWO rows held in registers (cols <= 1024 -> <= 4 vectors per lane
 // and row), so six to eight 16-byte loads are in flight per lane before the first reduction.
+// TO = e4m3_t: the fp32 results stay in registers until the row's amax is known, then are quantised as above and
+// the row scale goes to row_scale[row] (unused otherwise).
 template <int VPL, typename TI, typename TO>  // 8-element items per lane and row; cols = VPL * 256
 __global__ void __launch_bounds__(256) layernorm_kernel(const TI* __restrict__ x,
                                                         const float* __restrict__ gamma,
                                                         const float* __restrict__ beta,
                                                         TO* __restrict__ y, long long rows,
-                                                        float eps) {
+                                                        float eps, float* __restrict__ row_scale) {
+  constexpr bool E4M3 = std::is_same<TO, e4m3_t>::value;
   grid_dep_wait();
   grid_dep_launch();
   constexpr int COLS = VPL * 256;
@@ -78,6 +100,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const TI* __restrict__ x
       }
     const float rstd = rsqrtf(warp_sum(q) * (1.0f / COLS) + eps);
     TO* yr = y + (row0 + r) * COLS;
+    float amax = 0.f;
 #pragma unroll
     for (int i = 0; i < VPL; ++i) {
       const int c0 = (i * 32 + lane) * 8;
@@ -90,9 +113,70 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const TI* __restrict__ x
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[r][i][j] - mean) * rstd * g[j] + bb[j];
-      store8(yr + c0, o);
+      if constexpr (E4M3) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          v[r][i][j] = o[j];
+          amax = fmaxf(amax, fabsf(o[j]));
+        }
+      } else {
+        store8(yr + c0, o);
+      }
+    }
+    if constexpr (E4M3) {
+      amax = warp_max(amax);
+      const float inv = e4m3_inv_scale(amax);
+#pragma unroll
+      for (int i = 0; i < VPL; ++i)
+        *reinterpret_cast<uint2*>(yr + (i * 32 + lane) * 8) = quant8_e4m3(v[r][i], inv);
+      if (lane == 0) row_scale[row0 + r] = e4m3_row_scale(amax);
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------
+// Per-row e4m3 quantisation of a bf16 [rows][cols] tensor (the inputs of attn.proj and mlp.fc2 in the fp8 mode): one
+// warp per row, the row held in registers as VPL 16-byte vectors per lane (cols = VPL * 256) between the amax
+// reduction and the quantisation; 8-byte e4m3 stores.
+template <int VPL>
+__global__ void __launch_bounds__(256) rowquant_e4m3_kernel(const bf16* __restrict__ x, e4m3_t* __restrict__ y,
+                                                            float* __restrict__ row_scale, long long rows) {
+  grid_dep_wait();
+  grid_dep_launch();
+  constexpr int COLS = VPL * 256;
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const bf16* xr = x + row * COLS;
+  uint4 u[VPL];
+#pragma unroll
+  for (int i = 0; i < VPL; ++i) u[i] = __ldg(reinterpret_cast<const uint4*>(xr + (i * 32 + lane) * 8));
+  float amax = 0.f;
+#pragma unroll
+  for (int i = 0; i < VPL; ++i) {
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(&u[i]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 f = unpack_bf16x2(w[k]);
+      amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+    }
+  }
+  amax = warp_max(amax);
+  const float inv = e4m3_inv_scale(amax);
+  e4m3_t* yr = y + row * COLS;
+#pragma unroll
+  for (int i = 0; i < VPL; ++i) {
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(&u[i]);
+    float f[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 t = unpack_bf16x2(w[k]);
+      f[2 * k] = t.x;
+      f[2 * k + 1] = t.y;
+    }
+    *reinterpret_cast<uint2*>(yr + (i * 32 + lane) * 8) = quant8_e4m3(f, inv);
+  }
+  if (lane == 0) row_scale[row] = e4m3_row_scale(amax);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -580,16 +664,16 @@ using namespace odb;
 
 template <typename TI, typename TO>
 static int layernorm_launch(const void* x, const float* gamma, const float* beta, void* y, int64_t rows, int32_t cols,
-                            float eps, cudaStream_t stream) {
+                            float eps, cudaStream_t stream, float* rs = nullptr) {
   const int rpb = 16;   // 8 warps x 2 rows
   const unsigned grid = (unsigned)((rows + rpb - 1) / rpb);
   const TI* xp = static_cast<const TI*>(x);
   TO* yp = static_cast<TO*>(y);
   switch (cols) {
-    case 256: launch_pdl(layernorm_kernel<1, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps); break;
-    case 512: launch_pdl(layernorm_kernel<2, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps); break;
-    case 768: launch_pdl(layernorm_kernel<3, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps); break;
-    case 1024: launch_pdl(layernorm_kernel<4, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps); break;
+    case 256: launch_pdl(layernorm_kernel<1, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps, rs); break;
+    case 512: launch_pdl(layernorm_kernel<2, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps, rs); break;
+    case 768: launch_pdl(layernorm_kernel<3, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps, rs); break;
+    case 1024: launch_pdl(layernorm_kernel<4, TI, TO>, dim3(grid), dim3(256), 0, stream, xp, gamma, beta, yp, (long long)rows, eps, rs); break;
     default: return fail(ODB_ERR_UNSUPPORTED, "layernorm: cols must be 256/512/768/1024");
   }
   count_launch();
@@ -605,6 +689,38 @@ extern "C" int odb_layernorm(const void* x, const float* gamma, const float* bet
   if (x_dtype == ODB_DTYPE_F32 && y_dtype == ODB_DTYPE_BF16) return layernorm_launch<float, bf16>(x, gamma, beta, y, rows, cols, eps, stream);
   if (x_dtype == ODB_DTYPE_F32 && y_dtype == ODB_DTYPE_F32) return layernorm_launch<float, float>(x, gamma, beta, y, rows, cols, eps, stream);
   return fail(ODB_ERR_INVALID, "layernorm: (x, y) dtypes must be (bf16, bf16), (f32, bf16) or (f32, f32)");
+}
+
+extern "C" int odb_layernorm_e4m3(const void* x, const float* gamma, const float* beta, void* y, float* row_scale,
+                                  int64_t rows, int32_t cols, float eps, int32_t x_dtype, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!x || !gamma || !beta || !y || !row_scale || rows < 0) return fail(ODB_ERR_INVALID, "layernorm_e4m3: bad argument");
+  if ((reinterpret_cast<uintptr_t>(y) & 7u) != 0) return fail(ODB_ERR_INVALID, "layernorm_e4m3: y must be 8-byte aligned");
+  if (rows == 0) return ODB_OK;
+  if (x_dtype == ODB_DTYPE_F32) return layernorm_launch<float, e4m3_t>(x, gamma, beta, y, rows, cols, eps, stream, row_scale);
+  if (x_dtype == ODB_DTYPE_BF16) return layernorm_launch<bf16, e4m3_t>(x, gamma, beta, y, rows, cols, eps, stream, row_scale);
+  return fail(ODB_ERR_INVALID, "layernorm_e4m3: x_dtype must be ODB_DTYPE_F32 or ODB_DTYPE_BF16");
+}
+
+extern "C" int odb_rowquant_e4m3(const void* x, void* y, float* row_scale, int64_t rows, int32_t cols, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!x || !y || !row_scale || rows < 0) return fail(ODB_ERR_INVALID, "rowquant_e4m3: bad argument");
+  if (((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) != 0)
+    return fail(ODB_ERR_INVALID, "rowquant_e4m3: x and y must be 16-byte aligned");
+  if (rows == 0) return ODB_OK;
+  const unsigned grid = (unsigned)((rows + 7) / 8);       // 8 warps, one row each
+  const bf16* xp = static_cast<const bf16*>(x);
+  e4m3_t* yp = static_cast<e4m3_t*>(y);
+  const long long n = rows;
+  switch (cols) {
+    case 768: launch_pdl(rowquant_e4m3_kernel<3>, dim3(grid), dim3(256), 0, stream, xp, yp, row_scale, n); break;
+    case 1024: launch_pdl(rowquant_e4m3_kernel<4>, dim3(grid), dim3(256), 0, stream, xp, yp, row_scale, n); break;
+    case 3072: launch_pdl(rowquant_e4m3_kernel<12>, dim3(grid), dim3(256), 0, stream, xp, yp, row_scale, n); break;
+    case 4096: launch_pdl(rowquant_e4m3_kernel<16>, dim3(grid), dim3(256), 0, stream, xp, yp, row_scale, n); break;
+    default: return fail(ODB_ERR_UNSUPPORTED, "rowquant_e4m3: cols must be 768, 1024, 3072 or 4096");
+  }
+  count_launch();
+  return check_launch("rowquant_e4m3");
 }
 
 static int gn_args_ok(int b, int hw, int c, int groups) {

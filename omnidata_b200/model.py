@@ -167,6 +167,23 @@ def _gemm_operand(w: torch.Tensor, layer: GemmLayer) -> torch.Tensor:
     return w.permute(0, 2, 1).reshape(layer.n_pad, -1)
 
 
+def quantize_rows_e4m3(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(q e4m3 [n][k], s fp32 [n]) with w ~= q * s[:, None], per row n: amax = max |w[n]|, s = amax / 448,
+    q = e4m3_rn_satfinite(w * (448 / amax)); an all-zero row gets s = 1 and q = 0.  The rule the fp8 mode's kernels
+    apply to each token of a GEMM input, here for the weights (fp32 ops in torch)."""
+    w = w.float()
+    amax = w.abs().amax(dim=1)
+    nz = amax > 0
+    # tensor-by-tensor divisions: IEEE round-to-nearest quotients (a division by a Python scalar may be evaluated as a
+    # product with its rounded reciprocal)
+    c448 = torch.full_like(amax, 448.0)
+    safe = torch.where(nz, amax, torch.ones_like(amax))
+    s = torch.where(nz, safe / c448, torch.ones_like(amax))
+    inv = torch.where(nz, c448 / safe, torch.zeros_like(amax))
+    q = (w * inv[:, None]).clamp(-448.0, 448.0).to(torch.float8_e4m3fn)
+    return q.contiguous(), s.contiguous()
+
+
 def _decoder_spec(add, num_channels: int, features: int, rn_in) -> None:
     for n, c in zip((1, 2, 3, 4), rn_in):
         add(f"scratch.layer{n}_rn.weight", features, c, 3, 3)
@@ -342,7 +359,9 @@ class DPTDepthModel(nn.Module):
         self.taps: Dict[str, torch.Tensor] = {}
         # "bf16": wgmma tensor-core path (bf16 operands / storage, fp32 accumulation, fp32 ViT residual stream);
         # "fp32": correctness mode — every operand and activation fp32, contractions on the FP32 pipe with fp64
-        #         combination of partial sums (the reference is fp32-only: requirements.txt:4, no autocast anywhere)
+        #         combination of partial sums (the reference is fp32-only: requirements.txt:4, no autocast anywhere);
+        # "fp8":  inference only — the bf16 path with the ViT blocks' four linear layers on e4m3 wgmma (per-token
+        #         activation and per-channel weight scales; DESIGN.md §3 "Rounding points")
         self._precision = "bf16"
         self._packed = None
         self._packed_sig = None
@@ -389,8 +408,8 @@ class DPTDepthModel(nn.Module):
 
     @precision.setter
     def precision(self, value: str):
-        if value not in ("bf16", "fp32"):
-            raise ValueError("precision must be 'bf16' or 'fp32'")
+        if value not in ("bf16", "fp32", "fp8"):
+            raise ValueError("precision must be 'bf16', 'fp32' or 'fp8'")
         if value != self._precision:
             self._precision = value
             self._invalidate()
@@ -434,7 +453,10 @@ class DPTDepthModel(nn.Module):
             if layer.key == "head2":
                 layer = layer._replace(n_pad=layer.n)      # unpadded: the fused head tail launches at block_n 32
             w = _gemm_operand(sd[layer.weight], layer)
-            if layer.key in ("pp1t", "pp2t"):
+            if self._precision == "fp8" and layer.key.startswith("blk"):
+                # the ViT blocks' qkv / proj / fc1 / fc2: e4m3 with a per-output-channel scale
+                gemm[layer.key], vec[layer.key + ".scale"] = quantize_rows_e4m3(w)
+            elif layer.key in ("pp1t", "pp2t"):
                 # ConvTranspose2d(c, c, k, stride k) (vit.py:216-225, 240-249): k*k independent 1x1 convolutions, one
                 # per output phase t = (dy, dx): phases[t] = weight[:, :, dy, dx]^T, [out][in]
                 w = w.view(layer.n_pad, layer.taps, layer.c_pad).permute(1, 2, 0)
@@ -464,6 +486,9 @@ class DPTDepthModel(nn.Module):
             raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
         B, _, H, W = x.shape
         autograd = torch.is_grad_enabled() and (self.training or x.requires_grad)
+        if autograd and self._precision == "fp8":
+            raise ValueError("precision 'fp8' is inference-only: call the model under torch.no_grad() in eval() with "
+                             "an input that does not require grad, or switch to 'bf16' / 'fp32' to train")
         check_input_size(H, W, self.arch["hybrid"], autograd)
         if autograd:
             # train() mode under autograd, or an input that requires grad in either mode: the
@@ -654,6 +679,9 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
                   [64][160] (im2col columns), the readout Linear "ro{n}.full" [D][2D] and its token half "ro{n}.tok";
       pk["vec"]   fp32 tensors by parameter name: the layers' biases, zero-padded to n_pad where the forward reads the
                   layer padded, and the norm affines, cls token, readout biases and the head's last 1x1 conv;
+                  precision "fp8": pk["gemm"]["blk{i}.qkv" / ".proj" / ".fc1" / ".fc2"] are e4m3 [n][c]
+                  (`quantize_rows_e4m3`) and pk["vec"]["blk{i}.<layer>.scale"] their fp32 per-output-channel scales;
+                  every other operand is as in "bf16";
       pk["pos"]   pos_embed in fp32 (inference), and pk["pos_cache"] the patch rows resized to a grid (`_pos_rows`).
     `ws` owns the activations, `taps` (inference diagnostics) receives named intermediates.  `x` is fp32 contiguous
     [B,3,H,W]; returns the fp32 NCHW output buffer.  With `save` given, every activation the hand-written backward reads
@@ -661,8 +689,10 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
     ViT block's activations, the attention's log-sum-exp, the pre-activations of the GELUs, and the head's intermediates
     that the fused epilogue never stores."""
     B, _, H, W = x.shape
-    fp32 = precision == "fp32"
-    adt = torch.float32 if fp32 else torch.bfloat16            # activation storage type
+    fp32, fp8 = precision == "fp32", precision == "fp8"
+    if fp8 and save is not None:
+        raise ValueError("precision 'fp8' is inference-only: the train forward takes 'bf16' or 'fp32'")
+    adt = torch.float32 if fp32 else torch.bfloat16            # activation storage type (fp8: bf16 outside the GEMMs)
     f32 = torch.float32
     buf = lambda name, shape, dtype=None: ws.get(name, shape, adt if dtype is None else dtype)
     S = {} if save is None else save
@@ -720,8 +750,30 @@ def dpt_forward(x: torch.Tensor, pk: dict, arch: dict, precision: str, non_negat
         taps["tokens_in"] = xs[0].clone()
 
     # ---------------- ViT blocks (vit.py:150-151); final norm is dead compute and skipped
+    if fp8:
+        # the e4m3 GEMM inputs and their row scales: one buffer each, every input consumed before the next is made
+        qbuf, qs = buf("vit_q", (rows * 4 * D,), torch.float8_e4m3fn), buf("vit_qs", (rows,), f32)
+        q1, q4 = qbuf[:rows * D].view(rows, D), qbuf.view(rows, 4 * D)
     for i, v in enumerate(vit):
         p, blk = f"{pm}blocks.{i}.", f"blk{i}."
+        if fp8:
+            ops.layernorm_e4m3(xs[i], vec[p + "norm1.weight"], vec[p + "norm1.bias"], q1.view(B, ntok, D), qs)
+            ops.linear_fp8(q1, qs, gemm[blk + "qkv"], vec[blk + "qkv.scale"], v["qkv"].view(rows, -1),
+                           bias=vec[p + "attn.qkv.bias"])
+            ops.attention(v["qkv"], v["att"], heads=heads, scale=0.125)
+            ops.rowquant_e4m3(v["att"].view(rows, -1), q1, qs)
+            ops.linear_fp8(q1, qs, gemm[blk + "proj"], vec[blk + "proj.scale"], xm[i].view(rows, -1),
+                           bias=vec[p + "attn.proj.bias"], residual=xs[i].view(rows, -1))
+            ops.layernorm_e4m3(xm[i], vec[p + "norm2.weight"], vec[p + "norm2.bias"], q1.view(B, ntok, D), qs)
+            mlp = v["mlp"].view(rows, -1)
+            ops.linear_fp8(q1, qs, gemm[blk + "fc1"], vec[blk + "fc1.scale"], mlp, bias=vec[p + "mlp.fc1.bias"],
+                           act=ops.ACT_GELU)
+            ops.rowquant_e4m3(mlp, q4, qs)
+            ops.linear_fp8(q4, qs, gemm[blk + "fc2"], vec[blk + "fc2.scale"], xs[i + 1].view(rows, -1),
+                           bias=vec[p + "mlp.fc2.bias"], residual=xm[i].view(rows, -1))
+            if taps is not None:
+                taps[f"tokens_{i}"] = xs[i + 1].clone()
+            continue
         ops.layernorm(xs[i], vec[p + "norm1.weight"], vec[p + "norm1.bias"], v["h1"])
         ops.linear(v["h1"].view(rows, -1), gemm[blk + "qkv"], v["qkv"].view(rows, -1), bias=vec[p + "attn.qkv.bias"])
         ops.attention(v["qkv"], v["att"], heads=heads, scale=0.125, lse=v["lse"])

@@ -12,10 +12,11 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _capi
-from ._capi import ACT_GELU, ACT_NONE, ACT_RELU, DTYPE_BF16, DTYPE_F32, ConvGemmDesc, View, check, lib
+from ._capi import ACT_GELU, ACT_NONE, ACT_RELU, DTYPE_BF16, DTYPE_E4M3, DTYPE_F32, ConvGemmDesc, View, check, lib
 
 __all__ = [
     "ACT_NONE", "ACT_RELU", "ACT_GELU", "conv_gemm", "linear", "conv1x1", "conv3x3", "conv3x3_s2",
+    "linear_fp8", "layernorm_e4m3", "rowquant_e4m3",
     "layernorm", "attention", "groupnorm_stats", "groupnorm_apply", "stem_gn_relu_maxpool",
     "stem_im2col", "patchify", "upsample2x_add", "write_cls_row", "readout_cls_bias", "pack_conv_weight",
     "cast_f32_bf16", "head_tail_f32",
@@ -190,6 +191,87 @@ def conv_gemm(views: Sequence[torch.Tensor], taps: Sequence[Tuple[int, int, int]
     count = float(d.out.w) * float(d.out.h) * (d.n // gn_groups)
     _call("odb_groupnorm_finalize", {}, lib().odb_groupnorm_finalize, dev, partial.data_ptr(), stats.data_ptr(),
           d.out.b, part_rows, gn_groups, count, gn_eps)
+
+
+E4M3 = torch.float8_e4m3fn
+
+
+def _rows_operand(t: torch.Tensor, dtype, name: str, cols: Optional[int] = None) -> Tuple[int, int]:
+    """(rows, cols) of a contiguous 2-D [rows, cols] operand of `dtype`, 16-byte aligned; raises otherwise."""
+    _need(t, dtype, name)
+    if t.dim() != 2 or not t.is_contiguous() or t.data_ptr() % 16 != 0:
+        raise _capi.OdbError(f"{name}: need a contiguous, 16-byte aligned [rows, cols] tensor, got {tuple(t.shape)}")
+    if cols is not None and t.shape[1] != cols:
+        raise _capi.OdbError(f"{name}: expected {cols} columns, got {t.shape[1]}")
+    return t.shape[0], t.shape[1]
+
+
+def _row_scale(s: torch.Tensor, rows: int, name: str = "row_scale"):
+    _need(s, torch.float32, name)
+    if s.dim() != 1 or s.shape[0] != rows or not s.is_contiguous():
+        raise _capi.OdbError(f"{name}: need a contiguous fp32 [{rows}] tensor, got {tuple(s.shape)}")
+
+
+def linear_fp8(x, row_scale, weight, col_scale, out, *, bias, residual=None, act: int = ACT_NONE,
+               block_n: int = 0) -> None:
+    """The fp8 mode's linear layer: out = epilogue((x @ weight^T) * (row_scale[r] * col_scale[c]) + bias[c]).
+    x e4m3 [rows, K] with row_scale fp32 [rows]; weight e4m3 [N, K] with col_scale fp32 [N]; bias fp32 [N].
+    out bf16 [rows, N] (act ACT_NONE or ACT_GELU), or fp32 [rows, N] = residual (fp32 [rows, N]) + the value."""
+    rows, k = _rows_operand(x, E4M3, "x")
+    n, _ = _rows_operand(weight, E4M3, "weight", k)
+    _row_scale(row_scale, rows)
+    _row_scale(col_scale, n, "col_scale")
+    _need(bias, torch.float32, "bias")
+    if bias.numel() != n or not bias.is_contiguous() or col_scale.data_ptr() % 16 != 0:
+        raise _capi.OdbError("linear_fp8: bias [N] contiguous and col_scale 16-byte aligned required")
+    f32 = out.dtype == torch.float32
+    _rows_operand(out, torch.float32 if f32 else torch.bfloat16, "out", n)
+    if out.shape[0] != rows:
+        raise _capi.OdbError("linear_fp8: out must have x's rows")
+    if f32 != (residual is not None) or (f32 and act != ACT_NONE) or act not in (ACT_NONE, ACT_GELU):
+        raise _capi.OdbError("linear_fp8: bf16 out with bias [+ GELU], or fp32 out with an fp32 residual")
+    d = ConvGemmDesc()
+    d.in_dtype = DTYPE_E4M3
+    d.num_views = 1
+    d.views[0] = View(x.data_ptr(), k, rows, 1, 1, k, 0, 0)
+    d.num_taps = 1
+    d.weight = weight.data_ptr()
+    d.n = n
+    d.out_dtype = DTYPE_F32 if f32 else DTYPE_BF16
+    d.out = _view4(out, "out", out.dtype)
+    d.bias = bias.data_ptr()
+    if residual is not None:
+        _rows_operand(residual, torch.float32, "residual", n)
+        d.residual = _view4(residual, "residual", torch.float32)
+    d.act = act
+    d.block_n = block_n
+    info = {"m": rows, "n": n, "k": k, "taps": 1, "w": rows, "h": 1, "f32": False, "fp8": True}
+    _call("odb_conv_gemm_scaled", info, lib().odb_conv_gemm_scaled, _same_device(x, weight, out, bias, residual),
+          C.byref(d), row_scale.data_ptr(), col_scale.data_ptr())
+
+
+def layernorm_e4m3(x, gamma, beta, out, row_scale, eps: float = 1e-6):
+    """LayerNorm of x (fp32 or bf16 [.., cols]) quantised per row to e4m3 `out` with its fp32 row scales."""
+    _need(gamma, torch.float32, "gamma"); _need(beta, torch.float32, "beta")
+    _need(out, E4M3, "out")
+    if not (x.is_contiguous() and out.is_contiguous()) or out.shape != x.shape:
+        raise _capi.OdbError("layernorm_e4m3: contiguous x and out of one shape required")
+    rows = x.numel() // x.shape[-1]
+    _row_scale(row_scale, rows)
+    _call("odb_layernorm_e4m3", {"bytes": x.element_size() * x.numel() + out.numel() + 4 * rows},
+          lib().odb_layernorm_e4m3, _same_device(x, gamma, beta, out, row_scale), x.data_ptr(), gamma.data_ptr(),
+          beta.data_ptr(), out.data_ptr(), row_scale.data_ptr(), rows, x.shape[-1], eps, _dt(x, "x"))
+
+
+def rowquant_e4m3(x, out, row_scale):
+    """Per-row e4m3 quantisation of x bf16 [rows, cols] into out e4m3 [rows, cols] and row_scale fp32 [rows]."""
+    rows, cols = _rows_operand(x, torch.bfloat16, "x")
+    _rows_operand(out, E4M3, "out", cols)
+    if out.shape[0] != rows:
+        raise _capi.OdbError("rowquant_e4m3: out must have x's shape")
+    _row_scale(row_scale, rows)
+    _call("odb_rowquant_e4m3", {"bytes": 3 * x.numel() + 4 * rows, "cols": cols}, lib().odb_rowquant_e4m3,
+          _same_device(x, out, row_scale), x.data_ptr(), out.data_ptr(), row_scale.data_ptr(), rows, cols)
 
 
 TAPS_1 = [(0, 0, 0)]

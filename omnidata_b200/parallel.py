@@ -98,8 +98,9 @@ def broadcast_packed_weights(model, device, src: int = 0) -> int:
     items = list(_packed_tensors(model._packed))
     total = 0
     with torch.no_grad():
-        for dtype in (torch.bfloat16, torch.float32):
-            group = [t for _, t in items if t.dtype == dtype]
+        # precision "fp8": the e4m3 operands travel as their bytes (uint8 views)
+        for dtype in (torch.bfloat16, torch.float32, torch.float8_e4m3fn):
+            group = [t if dtype != torch.float8_e4m3fn else t.view(torch.uint8) for _, t in items if t.dtype == dtype]
             if not group:
                 continue
             flat = torch.cat([t.reshape(-1) for t in group])

@@ -222,6 +222,8 @@ def select_buckets(buckets, names: List[str], sizes: List[int], trainable):
 
 class TrainEngine:
     def __init__(self, model: DPTDepthModel, precision: str = "bf16"):
+        if precision == "fp8":
+            raise ValueError("precision 'fp8' is inference-only: training and gradients take 'bf16' or 'fp32'")
         if precision not in ("bf16", "fp32"):
             raise ValueError("precision must be 'bf16' or 'fp32'")
         self.model = model
