@@ -3,7 +3,9 @@
 
     python demo.py --task {normal,depth} --img_path FILE-or-DIR --output_path DIR
 
-writes <name>_<task>.png and <name>_rgb.png.  Weights: ./pretrained_models/omnidata_dpt_{normal,depth}_v2.ckpt
+writes <name>_<task>.png and <name>_rgb.png.  `--full_res` predicts at the image's own size instead of a 384 centre crop
+(omnidata_b200.tiled.TiledPredictor: overlapping 384 x 384 tiles, depth tiles aligned in scale and shift, blended) and
+writes <name>_<task>.png at the input resolution.  Weights: ./pretrained_models/omnidata_dpt_{normal,depth}_v2.ckpt
 (reference checkpoint names, demo.py:62,80); `--synthetic_weights` substitutes seeded random weights
 when no checkpoint is available (offline).  Inference runs on cuda:0 through the sm_90a kernels —
 there is no CPU path.
@@ -85,6 +87,7 @@ def main(argv=None):
     parser.add_argument("--output_path", dest="output_path", help="path to where output image should be stored")
     parser.add_argument("--synthetic_weights", action="store_true")
     parser.add_argument("--weights_dir", default="./pretrained_models/")
+    parser.add_argument("--full_res", action="store_true", help="predict at the input resolution with overlapping tiles")
     args = parser.parse_args(argv)
     if args.task not in ("normal", "depth"):
         print("task should be one of the following: normal, depth")
@@ -99,7 +102,24 @@ def main(argv=None):
     from omnidata_b200 import imageproc
     preprocess = imageproc.DevicePreprocessor(args.task, image_size, device)
 
+    def save_full_res(img_path, name):
+        from omnidata_b200.tiled import TiledPredictor
+        save_path = os.path.join(args.output_path, f"{name}_{args.task}.png")
+        print(f"Reading input {img_path} ...")
+        t = to_tensor(Image.open(img_path).convert("RGB"))
+        if args.task == "depth":
+            t = (t - 0.5) / 0.5                                       # Normalize(0.5, 0.5), demo.py:92-95
+        output = TiledPredictor(model, tile=(image_size, image_size), overlap=64)(t.unsqueeze(0).to(device))
+        if args.task == "depth":
+            depth = 1.0 - output[0].clamp(0, 1)                       # demo.py:140-145 without the 512 resize
+            Image.fromarray(viridis(depth.cpu().numpy())).save(save_path)
+        else:
+            Image.fromarray(imageproc.to_uint8_hwc(output[0], clamp01=True).cpu().numpy()).save(save_path)
+        print(f"Writing output {save_path} ...")
+
     def save_outputs(img_path, name):
+        if args.full_res:
+            return save_full_res(img_path, name)
         with torch.no_grad():
             save_path = os.path.join(args.output_path, f"{name}_{args.task}.png")
             print(f"Reading input {img_path} ...")

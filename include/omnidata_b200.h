@@ -503,6 +503,41 @@ int odb_bicubic_resize_f32(const float* in, int32_t planes, int32_t in_h, int32_
 int odb_f32_chw_to_u8_hwc(const float* in, int32_t c, int32_t h, int32_t w, int32_t clamp01, void* out,
                           void* stream);
 
+/* ---- tiled inference: merging overlapping tile predictions (omnidata_b200/tiled.py TiledPredictor) ------------
+ *
+ * The reference predicts one 384 x 384 crop per image (demo.py:74-76 Resize + CenterCrop, then DPT.forward,
+ * M/dpt_depth.py:67-85,107).  These entry points cut an image of any size into tiles the forward accepts and merge the
+ * tiles' predictions back at the image's own size.  Tile grid per axis (length L, tile t, overlap v, 0 <= 2 v < t):
+ * L <= t: one tile at 0; else n = ceil((L - v) / (t - v)) tiles at o_k = round(k (L - t) / (n - 1)), halves rounded up.
+ * Tiles are numbered row-major (i = ty * nx + tx, T = ny * nx <= ODB_TILE_MAX_TILES per image).  Pairs: the ny (nx - 1)
+ * horizontal neighbour pairs row-major, then the (ny - 1) nx vertical ones; "a" is the left / upper tile's prediction,
+ * "b" the other's.  tile_h, tile_w: multiples of 32; b, h, w <= 65535.
+ *
+ * odb_tile_gather: tiles fp32 [b * T][3][tile_h][tile_w] (16-byte aligned) from image fp32 [b][3][h][w], replicating
+ * the last row / column where the image is smaller than a tile.
+ * odb_tile_overlap_moments (depth): moments fp64 [b][pairs][6] = (n, Sa, Sb, Saa, Sbb, Sab) over each pair's overlap
+ * inside the image, from pred fp32 [b * T][tile_h][tile_w]; no launch for a single tile.
+ * odb_tile_align_solve (depth): scale_shift fp64 [b][T][2] = (s_i, t_i) minimising
+ *   sum_pairs sum_overlap (s_i a + t_i - s_j b - t_j)^2 + 1e-3 Nbar sum_i ((s_i - 1)^2 + t_i^2)
+ * (Nbar = the mean overlap pixel count, at least 1) — the per-image scale-and-shift least squares of
+ * L/midas_loss.py:10-30 (compute_scale_and_shift) solved for all tiles of an image jointly.  Banded fp64 Cholesky, one
+ * CTA per image; workspace: odb_tile_align_workspace_bytes(b, tiles_y, tiles_x) bytes (0: none needed; negative:
+ * refused).  moments may be NULL for a single tile.
+ * odb_tile_blend: out fp32 [b][c][h][w] (the forward's output layout) = sum_i w_i (s_i d_i + t_i) / sum_i w_i over the
+ * tiles covering each pixel, row-major, fp32; pred fp32 [b * T][c][tile_h][tile_w]; scale_shift NULL: s = 1, t = 0.
+ * w_i = rho(dy) rho(dx), rho(d) = min(1, (d + 1) / (overlap + 1)), d = the distance to the tile's nearest edge that is
+ * not on the image border.  All four are deterministic and batch-independent. */
+#define ODB_TILE_MAX_TILES 1024
+int odb_tile_gather(const float* image, int32_t b, int32_t h, int32_t w, int32_t tile_h, int32_t tile_w,
+                    int32_t overlap, float* tiles, void* stream);
+int odb_tile_overlap_moments(const float* pred, int32_t b, int32_t h, int32_t w, int32_t tile_h, int32_t tile_w,
+                             int32_t overlap, double* moments, void* stream);
+int64_t odb_tile_align_workspace_bytes(int32_t b, int32_t tiles_y, int32_t tiles_x);
+int odb_tile_align_solve(const double* moments, int32_t b, int32_t tiles_y, int32_t tiles_x, void* workspace,
+                         double* scale_shift, void* stream);
+int odb_tile_blend(const float* pred, const double* scale_shift, int32_t b, int32_t c, int32_t h, int32_t w,
+                   int32_t tile_h, int32_t tile_w, int32_t overlap, float* out, void* stream);
+
 /* Introspection (no GPU needed). */
 int odb_abi_version(void);
 const char* odb_last_error(void);

@@ -15,6 +15,7 @@ ODB_MAX_VIEWS = 4
 ODB_MAX_TAPS = 9
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 DTYPE_BF16, DTYPE_F32, DTYPE_E4M3 = 0, 1, 2
+TILE_MAX_TILES = 1024  # include/omnidata_b200.h: ODB_TILE_MAX_TILES
 
 
 class OdbError(RuntimeError):
@@ -188,6 +189,11 @@ _SIGNATURES = {
     "odb_bicubic_resize_f32": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          C.c_void_p, C.c_void_p]),
     "odb_f32_chw_to_u8_hwc": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "odb_tile_gather": (C.c_int, [C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p]),
+    "odb_tile_overlap_moments": (C.c_int, [C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p]),
+    "odb_tile_align_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
+    "odb_tile_align_solve": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
+    "odb_tile_blend": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 7 + [C.c_void_p] * 2),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -19,7 +19,7 @@ __all__ = [
     "linear_fp8", "layernorm_e4m3", "rowquant_e4m3",
     "layernorm", "attention", "groupnorm_stats", "groupnorm_apply", "stem_gn_relu_maxpool",
     "stem_im2col", "patchify", "upsample2x_add", "write_cls_row", "readout_cls_bias", "pack_conv_weight",
-    "cast_f32_bf16", "head_tail_f32",
+    "cast_f32_bf16", "head_tail_f32", "tile_gather", "tile_overlap_moments", "tile_align_solve", "tile_blend",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -458,3 +458,85 @@ def head_tail_f32(x, w, bias, out, relu: bool, pre=None):
         raise _capi.OdbError("head_tail_f32: x must be contiguous [B,H,W,32]")
     _call("odb_head_tail_f32", {}, lib().odb_head_tail_f32, _same_device(x, w, bias, out, pre), x.data_ptr(),
           w.data_ptr(), bias.data_ptr(), out.data_ptr(), _ptr(pre), b, h, wd, w.shape[0], 1 if relu else 0)
+
+
+# ---------------------------------------------------------------- tiled inference merge (csrc/tiled.cu)
+def _tile_shapes(name, b, h, w, tile, overlap):
+    from .tiled import tile_grid
+    if b < 1 or h < 1 or w < 1 or max(b, h, w) > 65535:
+        raise _capi.OdbError(f"{name}: batch and image size must lie in [1, 65535], got {b}x{h}x{w}")
+    th, tw = tile
+    if th < 32 or tw < 32 or th % 32 or tw % 32 or overlap < 0 or 2 * overlap >= min(th, tw):
+        raise _capi.OdbError(f"{name}: tile {th}x{tw} (multiples of 32) with 0 <= 2 overlap < min(tile), got {overlap}")
+    oy, ox = tile_grid(h, w, tile, overlap)
+    if len(oy) * len(ox) > _capi.TILE_MAX_TILES:
+        raise _capi.OdbError(f"{name}: {len(oy)} x {len(ox)} tiles, at most {_capi.TILE_MAX_TILES} per image")
+    return len(oy), len(ox)
+
+
+def _need_shape(t, shape, dtype, name):
+    _need(t, dtype, name)
+    if tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+        raise _capi.OdbError(f"{name}: expected a contiguous {dtype} tensor {tuple(shape)}, got {tuple(t.shape)}")
+
+
+def tile_gather(x, tiles, tile: Tuple[int, int], overlap: int):
+    """tiles fp32 [B*T, 3, th, tw] = the tiles of x fp32 [B, 3, H, W], edge-replicated where x is smaller."""
+    _need(x, torch.float32, "x")
+    if x.dim() != 4 or x.shape[1] != 3 or not x.is_contiguous():
+        raise _capi.OdbError("tile_gather: x must be a contiguous fp32 [B,3,H,W] tensor")
+    b, _, h, w = x.shape
+    ny, nx = _tile_shapes("tile_gather", b, h, w, tile, overlap)
+    _need_shape(tiles, (b * ny * nx, 3, tile[0], tile[1]), torch.float32, "tiles")
+    if tiles.data_ptr() % 16:
+        raise _capi.OdbError("tile_gather: tiles must be 16-byte aligned")
+    _call("odb_tile_gather", {"bytes": 8 * tiles.numel()}, lib().odb_tile_gather, _same_device(x, tiles), x.data_ptr(),
+          b, h, w, tile[0], tile[1], overlap, tiles.data_ptr())
+
+
+def tile_pairs(ny: int, nx: int) -> int:
+    return ny * (nx - 1) + (ny - 1) * nx
+
+
+def tile_overlap_moments(pred, moments, image_hw: Tuple[int, int], tile: Tuple[int, int], overlap: int):
+    """moments fp64 [B, pairs, 6] = (n, Sa, Sb, Saa, Sbb, Sab) over each neighbour pair's overlap; pred fp32
+    [B*T, th, tw] (a depth model's tile predictions)."""
+    h, w = image_hw
+    b = moments.shape[0] if moments.dim() == 3 else 0
+    ny, nx = _tile_shapes("tile_overlap_moments", b, h, w, tile, overlap)
+    _need_shape(pred, (b * ny * nx, tile[0], tile[1]), torch.float32, "pred")
+    _need_shape(moments, (b, tile_pairs(ny, nx), 6), torch.float64, "moments")
+    _call("odb_tile_overlap_moments", {"bytes": 4 * pred.numel()}, lib().odb_tile_overlap_moments,
+          _same_device(pred, moments), pred.data_ptr(), b, h, w, tile[0], tile[1], overlap, moments.data_ptr())
+
+
+def tile_align_solve(moments, scale_shift, grid: Tuple[int, int]):
+    """scale_shift fp64 [B, T, 2] = per-tile (s, t) of the alignment least squares (csrc/tiled.cu) for a ny x nx grid."""
+    ny, nx = grid
+    b = scale_shift.shape[0] if scale_shift.dim() == 3 else 0
+    if ny < 1 or nx < 1 or ny * nx > _capi.TILE_MAX_TILES or not 1 <= b <= 65535:
+        raise _capi.OdbError(f"tile_align_solve: grid {ny}x{nx} (at most {_capi.TILE_MAX_TILES} tiles), batch {b}")
+    _need_shape(scale_shift, (b, ny * nx, 2), torch.float64, "scale_shift")
+    if moments is not None:
+        _need_shape(moments, (b, tile_pairs(ny, nx), 6), torch.float64, "moments")
+    elif ny * nx > 1:
+        raise _capi.OdbError("tile_align_solve: moments are required for more than one tile")
+    nbytes = int(lib().odb_tile_align_workspace_bytes(b, ny, nx))
+    ws = torch.empty(nbytes, device=scale_shift.device, dtype=torch.uint8) if nbytes > 0 else None
+    _call("odb_tile_align_solve", {}, lib().odb_tile_align_solve, _same_device(moments, scale_shift, ws),
+          _ptr(moments), b, ny, nx, _ptr(ws), scale_shift.data_ptr())
+
+
+def tile_blend(pred, scale_shift, out, tile: Tuple[int, int], overlap: int):
+    """out fp32 [B, C, H, W] = the weighted blend of the tile predictions pred fp32 [B*T, C, th, tw], each mapped by its
+    (s, t) from scale_shift fp64 [B, T, 2] (None: s = 1, t = 0)."""
+    if out.dim() != 4:
+        raise _capi.OdbError("tile_blend: out must be [B,C,H,W]")
+    b, c, h, w = out.shape
+    ny, nx = _tile_shapes("tile_blend", b, h, w, tile, overlap)
+    _need_shape(out, (b, c, h, w), torch.float32, "out")
+    _need_shape(pred, (b * ny * nx, c, tile[0], tile[1]), torch.float32, "pred")
+    if scale_shift is not None:
+        _need_shape(scale_shift, (b, ny * nx, 2), torch.float64, "scale_shift")
+    _call("odb_tile_blend", {}, lib().odb_tile_blend, _same_device(pred, scale_shift, out), pred.data_ptr(),
+          _ptr(scale_shift), b, c, h, w, tile[0], tile[1], overlap, out.data_ptr())

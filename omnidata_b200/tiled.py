@@ -1,0 +1,116 @@
+"""Predict depth and normals on images of any size: tiled inference with on-device alignment and blending.
+
+    from omnidata_b200.tiled import TiledPredictor
+    pred = TiledPredictor(model, tile=(384, 384), overlap=64, max_batch=32)
+    depth = pred(x)          # x: float [B,3,H,W] on the model's device, any H, W >= 1
+
+`model(x)` takes H, W multiples of 32 with at most 4 096 patches.  TiledPredictor cuts the image into overlapping tiles
+of a size the model takes (`tile_grid`), runs them through `model` itself in chunks of at most `max_batch` tiles, and
+merges the predictions at the image's own size (csrc/tiled.cu):
+
+- depth (`num_channels == 1`): the depth model is affine-invariant (trained with the MiDaS scale-and-shift-invariant
+  loss), so each tile's prediction carries its own unknown scale and shift.  One least-squares problem per image finds a
+  scale s_i and shift t_i per tile that make neighbouring tiles agree on their overlaps, with a small ridge towards
+  s = 1, t = 0 that fixes the global affine gauge (include/omnidata_b200.h, odb_tile_align_solve);
+- normals: blended as predicted (s = 1, t = 0).
+
+The blend weights fall off linearly over `overlap` pixels towards tile edges inside the image, and not at the image
+border.  The result has the model's output layout at the input's size: [B,H,W] for one channel, else [B,C,H,W].
+Inference only; the merge is deterministic and does not depend on the batch.
+"""
+from __future__ import annotations
+
+from typing import List, Tuple
+
+import torch
+
+from . import _capi, ops
+from .model import check_input_size
+
+MAX_TILES = _capi.TILE_MAX_TILES          # tiles per image the alignment solve takes (ODB_TILE_MAX_TILES)
+
+
+def _axis(length: int, t: int, overlap: int) -> List[int]:
+    if length <= t:
+        return [0]
+    n = -(-(length - overlap) // (t - overlap))
+    return [(2 * k * (length - t) + n - 1) // (2 * (n - 1)) for k in range(n)]      # round(k (L - t) / (n - 1)), halves up
+
+
+def tile_grid(H: int, W: int, tile: Tuple[int, int], overlap: int) -> Tuple[List[int], List[int]]:
+    """Tile origins (rows, columns) of an H x W image: per axis of length L and tile length t, one tile at 0 when
+    L <= t (the gather replicates the image's edge up to t), else n = ceil((L - overlap) / (t - overlap)) tiles at
+    round(k (L - t) / (n - 1)).  Every tile lies inside the image and neighbours overlap by at least `overlap`.  Tiles
+    are numbered row-major.  (csrc/tiled.cu: tile_count, tile_origin)"""
+    return _axis(H, tile[0], overlap), _axis(W, tile[1], overlap)
+
+
+class TiledPredictor:
+    """Runs `model` on overlapping tiles of any-size images and merges the predictions (module docstring)."""
+
+    def __init__(self, model, tile: Tuple[int, int] = (384, 384), overlap: int = 64, max_batch: int = 32):
+        th, tw = int(tile[0]), int(tile[1])
+        check_input_size(th, tw, model.arch["hybrid"], autograd=False)
+        if not 0 <= overlap < min(th, tw) / 2:
+            raise ValueError(f"overlap must lie in [0, min(tile) / 2), got {overlap} for tile {th}x{tw}")
+        if max_batch < 1:
+            raise ValueError(f"max_batch must be at least 1, got {max_batch}")
+        self.model = model
+        self.tile = (th, tw)
+        self.overlap = int(overlap)
+        self.max_batch = int(max_batch)
+
+    def __call__(self, x: torch.Tensor) -> torch.Tensor:
+        """The merged prediction of x float [B,3,H,W]: [B,H,W] for a one-channel model, else [B,C,H,W]."""
+        pred = self.tile_predictions(x)
+        return self.merge(pred, x.shape[0], x.shape[2], x.shape[3])
+
+    def _grid(self, B: int, H: int, W: int) -> Tuple[int, int]:
+        th, tw = self.tile
+        if min(B, H, W) < 1 or max(B, H, W) > 65535:
+            raise ValueError(f"batch and image size must lie in [1, 65535], got {B}x{H}x{W}")
+        oy, ox = tile_grid(H, W, self.tile, self.overlap)
+        if len(oy) * len(ox) > MAX_TILES:
+            raise ValueError(f"{H}x{W} needs {len(oy)} x {len(ox)} tiles of {th}x{tw}; at most {MAX_TILES} per image")
+        return len(oy), len(ox)
+
+    def tile_predictions(self, x: torch.Tensor) -> torch.Tensor:
+        """`model` on the tiles of x (row-major per image, images in order), as fp32 [B*T, C, th, tw]."""
+        model, (th, tw) = self.model, self.tile
+        if model.training:
+            raise ValueError("TiledPredictor is inference only: call model.eval() first")
+        if x.requires_grad:
+            raise ValueError("TiledPredictor is inference only: x must not require grad")
+        if not x.is_cuda:
+            raise _capi.OdbError("TiledPredictor runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
+        B, _, H, W = x.shape
+        ny, nx = self._grid(B, H, W)
+        n, C = B * ny * nx, model.num_channels
+        with torch.no_grad():
+            x = x.detach().float().contiguous()
+            tiles = torch.empty(n, 3, th, tw, device=x.device)
+            ops.tile_gather(x, tiles, self.tile, self.overlap)
+            pred = torch.empty(n, C, th, tw, device=x.device)
+            for i in range(0, n, self.max_batch):
+                y = model(tiles[i:i + self.max_batch])
+                pred[i:i + y.shape[0]].copy_(y.view(y.shape[0], C, th, tw))
+        return pred
+
+    def merge(self, pred: torch.Tensor, B: int, H: int, W: int) -> torch.Tensor:
+        """Aligns (one channel: depth) and blends tile predictions fp32 [B*T, C, th, tw] into the [B,(C,)H,W] output."""
+        (th, tw), ov = self.tile, self.overlap
+        ny, nx = self._grid(B, H, W)
+        T, C = ny * nx, pred.shape[1]
+        st = None
+        if C == 1:
+            st = torch.empty(B, T, 2, device=pred.device, dtype=torch.float64)
+            moments = None
+            if T > 1:
+                moments = torch.empty(B, ops.tile_pairs(ny, nx), 6, device=pred.device, dtype=torch.float64)
+                ops.tile_overlap_moments(pred.view(B * T, th, tw), moments, (H, W), self.tile, ov)
+            ops.tile_align_solve(moments, st, (ny, nx))
+        out = torch.empty(B, C, H, W, device=pred.device)
+        ops.tile_blend(pred, st, out, self.tile, ov)
+        return out.squeeze(1) if C == 1 else out
