@@ -538,6 +538,54 @@ int odb_tile_align_solve(const double* moments, int32_t b, int32_t tiles_y, int3
 int odb_tile_blend(const float* pred, const double* scale_shift, int32_t b, int32_t c, int32_t h, int32_t w,
                    int32_t tile_h, int32_t tile_w, int32_t overlap, float* out, void* stream);
 
+/* ---- evaluation metrics against ground truth (omnidata_b200/metrics.py DepthMetrics / NormalMetrics) ------------
+ *
+ * No reference counterpart: the reference monitors its training losses only.  Definitions in DESIGN.md §3
+ * "Evaluation metrics"; oracle/metrics_oracle.py restates them in float64.  Inputs are fp32, [b][h][w] per plane;
+ * mask: NULL with ODB_MASK_NONE, or uint8 / fp32 [b][h][w] (nonzero = valid) with ODB_MASK_U8 / ODB_MASK_F32.
+ * b <= 65535, h, w <= 65535.  Per-pixel arithmetic is fp64.  Every image is cut into fixed pixel slabs, combined in a
+ * fixed order and folded into the running state image after image, in image order: the state after a dataset does not
+ * depend on how it was split into batches, and repeat runs give the same bits (no floating-point atomics).  The state
+ * buffers are the caller's, zeroed to start.  workspace: odb_metrics_workspace_bytes(b, h, w) bytes, 8-byte aligned
+ * (negative: refused).  Arguments are checked before any launch.
+ *
+ * odb_depth_metrics_update: pred, gt (depth) fp32 [b][h][w].  Valid set of an image V = {mask != 0, gt finite,
+ * gt > min_depth, gt <= max_depth}; max_depth = +inf means none (required finite in disparity space), 0 <= min_depth <
+ * max_depth.  Per image, (s, t) is the least-squares fit over V of s p + t to y, with the five fp64 moments and the
+ * convention of L/midas_loss.py:10-30 compute_scale_and_shift (s = t = 0 where det <= 0):
+ *   ODB_SPACE_DEPTH:     y = gt,     dh = clamp(s p + t, min_depth, max_depth)
+ *   ODB_SPACE_DISPARITY: y = 1 / gt, dh = clamp(1 / max(s p + t, 1 / max_depth), min_depth, max_depth)
+ * and over V, with e = dh - gt, r = max(dh / gt, gt / dh):  AbsRel = mean |e| / gt, SqRel = mean e^2 / gt,
+ * RMSE = sqrt(mean e^2), RMSE_log = sqrt(mean (ln dh - ln gt)^2), delta_k = #(r < 1.25^k) / |V|.
+ * records fp64 [b][ODB_DEPTH_RECORD] = (|V|, AbsRel, SqRel, RMSE, RMSE_log, #delta1, #delta2, #delta3, s, t, det <= 0,
+ * non-finite predictions on V); a non-finite prediction on V makes the image's metrics NaN.  Images with |V| > 0 add
+ * state_sums fp64 [7] += (AbsRel, SqRel, RMSE, RMSE_log, delta1, delta2, delta3) and state_counts int64 [4] +=
+ * (1, 0, det <= 0, |V|); images with |V| = 0 add (0, 1, 0, 0).  Five launches.
+ *
+ * odb_normal_metrics_update: pred, gt fp32 [b][3][h][w] in the model's output encoding [0, 1].  Per pixel, a = 2 pred - 1,
+ * g = 2 gt - 1, theta = atan2(|a x g|, a . g) in degrees; the pixel takes part where the mask is nonzero and |a|, |g| >
+ * 1e-6.  state_sums fp64 [2] += (S theta, S theta^2), state_counts int64 [5] += (#finite theta, #non-finite theta,
+ * #(theta < 11.25), #(theta < 22.5), #(theta < 30)) over the finite ones, and hist int64 [ODB_NORMAL_HIST_BINS] (bins of
+ * 1 / ODB_NORMAL_HIST_PER_DEGREE degree) += 1 at floor(4096 theta) (integer atomics).  Three launches.
+ * odb_normal_metrics_median: out fp64 [2] = (k, (k + 0.5) / 4096) for the bin k holding the 0-based rank
+ * floor((N - 1) / 2) of the N angles counted in hist (the lower median to 2^-13 degree); (-1, NaN) for N = 0. */
+#define ODB_MASK_NONE 0
+#define ODB_MASK_U8 1
+#define ODB_MASK_F32 2
+#define ODB_SPACE_DEPTH 0
+#define ODB_SPACE_DISPARITY 1
+#define ODB_DEPTH_RECORD 12
+#define ODB_NORMAL_HIST_PER_DEGREE 4096
+#define ODB_NORMAL_HIST_BINS (180 * ODB_NORMAL_HIST_PER_DEGREE + 1)
+int64_t odb_metrics_workspace_bytes(int32_t b, int32_t h, int32_t w);
+int odb_depth_metrics_update(const float* pred, const float* gt, const void* mask, int32_t mask_dtype, int32_t b,
+                             int32_t h, int32_t w, int32_t space, double min_depth, double max_depth, void* workspace,
+                             double* records, double* state_sums, int64_t* state_counts, void* stream);
+int odb_normal_metrics_update(const float* pred, const float* gt, const void* mask, int32_t mask_dtype, int32_t b,
+                              int32_t h, int32_t w, void* workspace, double* state_sums, int64_t* state_counts,
+                              int64_t* hist, void* stream);
+int odb_normal_metrics_median(const int64_t* hist, double* out, void* stream);
+
 /* Introspection (no GPU needed). */
 int odb_abi_version(void);
 const char* odb_last_error(void);

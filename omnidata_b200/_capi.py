@@ -16,6 +16,11 @@ ODB_MAX_TAPS = 9
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 DTYPE_BF16, DTYPE_F32, DTYPE_E4M3 = 0, 1, 2
 TILE_MAX_TILES = 1024  # include/omnidata_b200.h: ODB_TILE_MAX_TILES
+MASK_NONE, MASK_U8, MASK_F32 = 0, 1, 2          # ODB_MASK_*
+SPACE_DEPTH, SPACE_DISPARITY = 0, 1             # ODB_SPACE_*
+DEPTH_RECORD = 12                               # ODB_DEPTH_RECORD
+NORMAL_HIST_PER_DEGREE = 4096                   # ODB_NORMAL_HIST_PER_DEGREE
+NORMAL_HIST_BINS = 180 * NORMAL_HIST_PER_DEGREE + 1
 
 
 class OdbError(RuntimeError):
@@ -194,6 +199,10 @@ _SIGNATURES = {
     "odb_tile_align_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
     "odb_tile_align_solve": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
     "odb_tile_blend": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 7 + [C.c_void_p] * 2),
+    "odb_metrics_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
+    "odb_depth_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 5 + [C.c_double] * 2 + [C.c_void_p] * 5),
+    "odb_normal_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p] * 5),
+    "odb_normal_metrics_median": (C.c_int, [C.c_void_p] * 3),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -1,0 +1,161 @@
+"""Evaluate depth and surface-normal predictions against ground truth on the device (csrc/metrics.cu).
+
+    from omnidata_b200.metrics import DepthMetrics, NormalMetrics
+    metric = DepthMetrics(space="depth", min_depth=1e-3, max_depth=None)
+    for pred, gt, mask in batches:          # fp32 [B,H,W] or [B,1,H,W]; mask optional, uint8 / bool / fp32
+        metric.update(pred, gt, mask)
+    print(metric.compute())                 # {"abs_rel": ..., "delta1": ..., "images": ..., ...}
+
+- DepthMetrics: per image, the prediction is aligned to the ground truth in scale and shift by least squares (in depth
+  or, as the MiDaS zero-shot protocol does, in disparity), then AbsRel, SqRel, RMSE, RMSE_log and delta_1..3 are taken
+  over the image's valid pixels; the dataset value of each is the mean over the images with at least one valid pixel.
+- NormalMetrics: the angle between predicted and true normals, pooled over every valid pixel of the dataset: mean,
+  median (to 2^-13 degree, from a dataset-wide histogram), RMSE and the percentages within 11.25, 22.5 and 30 degrees
+  (the published OASIS surface-normal metrics, without the relative-normal AUC).
+
+Definitions: DESIGN.md §3 "Evaluation metrics" and include/omnidata_b200.h; oracle/metrics_oracle.py restates them in
+float64.  The state lives in fixed device tensors.  `update` neither synchronises the host nor allocates after its first
+call at a shape, so it can be captured in a CUDA graph; only `compute` synchronises.  The state after a dataset does not
+depend on how the dataset was split into batches, and repeat runs give the same bits.
+"""
+from __future__ import annotations
+
+import math
+from typing import Dict, Optional
+
+import torch
+
+from . import _capi, ops
+from .losses import _StepBuffers
+
+DEPTH_KEYS = ("abs_rel", "sq_rel", "rmse", "rmse_log", "delta1", "delta2", "delta3")
+DEPTH_COUNTS = ("images", "excluded", "degenerate", "pixels")
+NORMAL_COUNTS = ("pixels", "nonfinite", "n_11.25", "n_22.5", "n_30")
+
+
+class _Metrics(_StepBuffers):
+    _STATE: Dict[str, tuple] = {}
+
+    def __init__(self):
+        self._bufs = {}
+        self._state: Optional[Dict[str, torch.Tensor]] = None
+
+    def _state_on(self, device: torch.device) -> Dict[str, torch.Tensor]:
+        if self._state is None:
+            self._state = {k: torch.zeros(shape, dtype=dt, device=device) for k, (shape, dt) in self._STATE.items()}
+        elif next(iter(self._state.values())).device != device:
+            raise ValueError(f"{type(self).__name__}: the state lives on {next(iter(self._state.values())).device}, "
+                             f"the inputs on {device}")
+        return self._state
+
+    def _host_state(self) -> Dict[str, torch.Tensor]:
+        if self._state is None:
+            return {k: torch.zeros(shape, dtype=dt) for k, (shape, dt) in self._STATE.items()}
+        return {k: t.cpu() for k, t in self._state.items()}
+
+    def reset(self):
+        """Back to an empty dataset (the state tensors are zeroed in place: a captured update stays valid)."""
+        if self._state is not None:
+            for t in self._state.values():
+                t.zero_()
+
+    def all_reduce(self, group=None):
+        """Replaces every rank's state by the fold of all ranks' states in rank order (torch.distributed all-gather of
+        the fixed-size state).  Counts and the histogram are exact; the sums are deterministic for a given world size
+        and sharding."""
+        import torch.distributed as dist
+        if self._state is None:
+            dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else \
+                torch.device("cpu")
+            self._state_on(dev)
+        world = dist.get_world_size(group)
+        for t in self._state.values():
+            parts = [torch.empty_like(t) for _ in range(world)]
+            dist.all_gather(parts, t, group=group)
+            acc = parts[0].clone()
+            for p in parts[1:]:
+                acc += p
+            t.copy_(acc)
+
+
+class DepthMetrics(_Metrics):
+    """Scale/shift-aligned depth metrics (module docstring).  space "depth" fits s p + t to the depth, "disparity" to its
+    inverse and needs max_depth; valid pixels have mask != 0 and a finite depth in (min_depth, max_depth]."""
+
+    _STATE = {"sums": ((7,), torch.float64), "counts": ((4,), torch.int64)}
+
+    def __init__(self, space: str = "depth", min_depth: float = 1e-3, max_depth: Optional[float] = None):
+        super().__init__()
+        if space not in ("depth", "disparity"):
+            raise ValueError(f"space must be 'depth' or 'disparity', got {space!r}")
+        if space == "disparity" and max_depth is None:
+            raise ValueError("space='disparity' needs max_depth (the predicted disparity is clamped to 1 / max_depth)")
+        min_depth = float(min_depth)
+        max_depth = math.inf if max_depth is None else float(max_depth)
+        if not (math.isfinite(min_depth) and min_depth >= 0.0) or not (max_depth > min_depth):
+            raise ValueError(f"need 0 <= min_depth < max_depth, got min_depth={min_depth}, max_depth={max_depth}")
+        self.space = space
+        self.min_depth, self.max_depth = min_depth, max_depth
+
+    @_capi.on_tensor_device
+    @torch.no_grad()
+    def update(self, pred: torch.Tensor, gt: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Adds a batch: pred, gt fp32 [B,H,W] or [B,1,H,W]; mask None or uint8 / bool / fp32, nonzero = valid.
+        Returns the batch's per-image records fp64 [B, 12] (include/omnidata_b200.h odb_depth_metrics_update), valid
+        until the next update at this shape."""
+        b, h, w, _, _ = ops.check_metric_inputs("DepthMetrics.update", pred, gt, mask, 1)
+        st = self._state_on(pred.device)
+        ws = self._buf("workspace", (ops.metrics_workspace_bytes(b, h, w) // 8,), torch.float64, pred.device)
+        rec = self._buf("records", (b, _capi.DEPTH_RECORD), torch.float64, pred.device)
+        space = _capi.SPACE_DISPARITY if self.space == "disparity" else _capi.SPACE_DEPTH
+        ops.depth_metrics_update(pred, gt, mask, space, self.min_depth, self.max_depth, ws, rec, st["sums"],
+                                 st["counts"])
+        return rec
+
+    def compute(self) -> dict:
+        """Dataset values: the mean over images with valid pixels of each per-image metric (NaN before any such image),
+        and the counts: images (with valid pixels), excluded (none valid), degenerate (det <= 0, aligned to 0),
+        pixels (valid pixels)."""
+        st = self._host_state()
+        counts = [int(c) for c in st["counts"].tolist()]
+        n = counts[0]
+        out = {k: (s / n if n else math.nan) for k, s in zip(DEPTH_KEYS, st["sums"].tolist())}
+        out.update(zip(DEPTH_COUNTS, counts))
+        return out
+
+
+class NormalMetrics(_Metrics):
+    """Angular-error metrics of surface normals, pooled over all valid pixels (module docstring)."""
+
+    _STATE = {"sums": ((2,), torch.float64), "counts": ((5,), torch.int64),
+              "hist": ((_capi.NORMAL_HIST_BINS,), torch.int64)}
+
+    @_capi.on_tensor_device
+    @torch.no_grad()
+    def update(self, pred: torch.Tensor, gt: torch.Tensor, mask: Optional[torch.Tensor] = None) -> None:
+        """Adds a batch: pred, gt fp32 [B,3,H,W] in the model's output encoding [0, 1]; mask None or [B,(1,)H,W]
+        uint8 / bool / fp32, nonzero = valid."""
+        b, h, w, _, _ = ops.check_metric_inputs("NormalMetrics.update", pred, gt, mask, 3)
+        st = self._state_on(pred.device)
+        ws = self._buf("workspace", (ops.metrics_workspace_bytes(b, h, w) // 8,), torch.float64, pred.device)
+        ops.normal_metrics_update(pred, gt, mask, ws, st["sums"], st["counts"], st["hist"])
+
+    def compute(self) -> dict:
+        """mean, median, rmse (degrees), pct_11.25 / pct_22.5 / pct_30 (percent of pixels), median_bin (the histogram
+        bin of the lower median, -1 if none), and the counts: pixels (finite angles), nonfinite (excluded),
+        n_11.25 / n_22.5 / n_30."""
+        med = (-1.0, math.nan)
+        if self._state is not None:
+            buf = self._buf("median", (2,), torch.float64, self._state["hist"].device)
+            ops.normal_metrics_median(self._state["hist"], buf)
+            med = tuple(buf.tolist())
+        st = self._host_state()
+        counts = [int(c) for c in st["counts"].tolist()]
+        n = counts[0]
+        s, s2 = st["sums"].tolist()
+        out = {"mean": s / n if n else math.nan, "median": med[1], "rmse": math.sqrt(s2 / n) if n else math.nan}
+        for k, c in zip(("pct_11.25", "pct_22.5", "pct_30"), counts[2:]):
+            out[k] = 100.0 * c / n if n else math.nan
+        out["median_bin"] = int(med[0])
+        out.update(zip(NORMAL_COUNTS, counts))
+        return out

@@ -7,6 +7,7 @@ sliced / strided views (parity planes, token windows) are passed without copies.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Sequence, Tuple
 
 import torch
@@ -20,6 +21,7 @@ __all__ = [
     "layernorm", "attention", "groupnorm_stats", "groupnorm_apply", "stem_gn_relu_maxpool",
     "stem_im2col", "patchify", "upsample2x_add", "write_cls_row", "readout_cls_bias", "pack_conv_weight",
     "cast_f32_bf16", "head_tail_f32", "tile_gather", "tile_overlap_moments", "tile_align_solve", "tile_blend",
+    "metrics_workspace_bytes", "depth_metrics_update", "normal_metrics_update", "normal_metrics_median",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -540,3 +542,96 @@ def tile_blend(pred, scale_shift, out, tile: Tuple[int, int], overlap: int):
         _need_shape(scale_shift, (b, ny * nx, 2), torch.float64, "scale_shift")
     _call("odb_tile_blend", {}, lib().odb_tile_blend, _same_device(pred, scale_shift, out), pred.data_ptr(),
           _ptr(scale_shift), b, c, h, w, tile[0], tile[1], overlap, out.data_ptr())
+
+
+# ---------------------------------------------------------------- evaluation metrics (csrc/metrics.cu)
+_MASK_KINDS = {torch.uint8: _capi.MASK_U8, torch.bool: _capi.MASK_U8, torch.float32: _capi.MASK_F32}
+
+
+def metrics_plane_shape(pred: torch.Tensor, channels: int, name: str = "pred") -> Tuple[int, int, int]:
+    """(B, H, W) of a metrics input: [B,H,W] or [B,1,H,W] for one channel, [B,C,H,W] otherwise."""
+    if channels == 1 and pred.dim() == 3:
+        return tuple(pred.shape)
+    if pred.dim() == 4 and pred.shape[1] == channels:
+        return pred.shape[0], pred.shape[2], pred.shape[3]
+    want = "[B,H,W] or [B,1,H,W]" if channels == 1 else f"[B,{channels},H,W]"
+    raise _capi.OdbError(f"{name}: expected {want}, got {tuple(pred.shape)}")
+
+
+def check_metric_inputs(name, pred, gt, mask, channels):
+    """Checks pred / gt (fp32, contiguous, one shape) and the optional mask (uint8 / bool / fp32, contiguous,
+    [B,H,W] or [B,1,H,W]); returns (b, h, w, mask pointer, ODB_MASK_*).  Nothing is copied."""
+    b, h, w = metrics_plane_shape(pred, channels)
+    if min(b, h, w) < 1 or b > 65535 or max(h, w) > 65535:
+        raise _capi.OdbError(f"{name}: batch and image size must lie in [1, 65535], got {b}x{h}x{w}")
+    for t, n in ((pred, "pred"), (gt, "gt")):
+        _need(t, torch.float32, n)
+        if metrics_plane_shape(t, channels, n) != (b, h, w) or not t.is_contiguous():
+            raise _capi.OdbError(f"{name}: {n} must be a contiguous fp32 tensor of {b}x{h}x{w} planes, "
+                                 f"got {tuple(t.shape)}")
+    if mask is None:
+        return b, h, w, None, _capi.MASK_NONE
+    if not mask.is_cuda:
+        raise _capi.OdbError(f"{name}: mask must live on a CUDA device (no CPU path exists)")
+    if mask.dtype not in _MASK_KINDS:
+        raise _capi.OdbError(f"{name}: mask must be uint8, bool or float32, got {mask.dtype}")
+    if tuple(mask.shape) not in ((b, h, w), (b, 1, h, w)) or not mask.is_contiguous():
+        raise _capi.OdbError(f"{name}: mask must be a contiguous [B,H,W] or [B,1,H,W] tensor for {b}x{h}x{w}, "
+                             f"got {tuple(mask.shape)}")
+    return b, h, w, mask.data_ptr(), _MASK_KINDS[mask.dtype]
+
+
+def metrics_workspace_bytes(b: int, h: int, w: int) -> int:
+    n = int(lib().odb_metrics_workspace_bytes(b, h, w))
+    if n < 0:
+        raise _capi.OdbError(f"metrics workspace: batch and image size must lie in [1, 65535], got {b}x{h}x{w}")
+    return n
+
+
+def _metric_workspace(name, ws, b, h, w):
+    _need(ws, torch.float64, "workspace")
+    if ws.numel() * 8 < metrics_workspace_bytes(b, h, w) or not ws.is_contiguous():
+        raise _capi.OdbError(f"{name}: workspace needs {metrics_workspace_bytes(b, h, w)} contiguous bytes")
+
+
+def depth_metrics_update(pred, gt, mask, space: int, min_depth: float, max_depth: float, workspace, records, sums,
+                         counts):
+    """Adds the depth metrics of pred / gt fp32 [B,(1,)H,W] (mask: None or [B,(1,)H,W] uint8 / bool / fp32, nonzero =
+    valid) to the state sums fp64 [7], counts int64 [4]; records fp64 [B, 12] receives the per-image results
+    (include/omnidata_b200.h odb_depth_metrics_update).  max_depth = inf: none."""
+    b, h, w, mptr, mkind = check_metric_inputs("depth_metrics_update", pred, gt, mask, 1)
+    if space not in (_capi.SPACE_DEPTH, _capi.SPACE_DISPARITY):
+        raise _capi.OdbError(f"depth_metrics_update: unknown space {space}")
+    if not (math.isfinite(min_depth) and 0 <= min_depth < max_depth) or \
+            (space == _capi.SPACE_DISPARITY and not math.isfinite(max_depth)):
+        raise _capi.OdbError(f"depth_metrics_update: need 0 <= min_depth < max_depth (finite in disparity space), got "
+                             f"{min_depth}, {max_depth}")
+    _metric_workspace("depth_metrics_update", workspace, b, h, w)
+    _need_shape(records, (b, _capi.DEPTH_RECORD), torch.float64, "records")
+    _need_shape(sums, (7,), torch.float64, "sums")
+    _need_shape(counts, (4,), torch.int64, "counts")
+    _call("odb_depth_metrics_update", {"bytes": 2 * 2 * 4 * b * h * w}, lib().odb_depth_metrics_update,
+          _same_device(pred, gt, mask, workspace, records, sums, counts), pred.data_ptr(), gt.data_ptr(), mptr, mkind,
+          b, h, w, space, float(min_depth), float(max_depth), workspace.data_ptr(), records.data_ptr(), sums.data_ptr(),
+          counts.data_ptr())
+
+
+def normal_metrics_update(pred, gt, mask, workspace, sums, counts, hist):
+    """Adds the angular errors of pred / gt fp32 [B,3,H,W] (model encoding [0, 1]; mask as for depth) to the state
+    sums fp64 [2], counts int64 [5] and hist int64 [NORMAL_HIST_BINS] (odb_normal_metrics_update)."""
+    b, h, w, mptr, mkind = check_metric_inputs("normal_metrics_update", pred, gt, mask, 3)
+    _metric_workspace("normal_metrics_update", workspace, b, h, w)
+    _need_shape(sums, (2,), torch.float64, "sums")
+    _need_shape(counts, (5,), torch.int64, "counts")
+    _need_shape(hist, (_capi.NORMAL_HIST_BINS,), torch.int64, "hist")
+    _call("odb_normal_metrics_update", {"bytes": 2 * 3 * 4 * b * h * w}, lib().odb_normal_metrics_update,
+          _same_device(pred, gt, mask, workspace, sums, counts, hist), pred.data_ptr(), gt.data_ptr(), mptr, mkind, b,
+          h, w, workspace.data_ptr(), sums.data_ptr(), counts.data_ptr(), hist.data_ptr())
+
+
+def normal_metrics_median(hist, out):
+    """out fp64 [2] = (bin, its centre in degrees) of the lower median of the angles counted in hist; (-1, NaN) if none."""
+    _need_shape(hist, (_capi.NORMAL_HIST_BINS,), torch.int64, "hist")
+    _need_shape(out, (2,), torch.float64, "out")
+    _call("odb_normal_metrics_median", {}, lib().odb_normal_metrics_median, _same_device(hist, out), hist.data_ptr(),
+          out.data_ptr())
