@@ -3,13 +3,14 @@
 
     python evaluate.py --task {depth,normal} --img_path DIR --gt_path DIR [--mask_path DIR]
                        [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
-                       [--mode {tiled,direct}] [--tile 384 --overlap 64]
+                       [--mode {tiled,direct}] [--tile 384 --overlap 64] [--anchor HxW]
                        [--space {depth,disparity}] [--min_depth] [--max_depth] [--depth_scale] [--depth_invalid]
 
 Images (PNG / JPEG) are matched to ground truth, and to masks, by file stem.  Preprocessing is that of
 `demo.py --full_res` (RGB in [0, 1]; depth normalised to [-1, 1]).  `--mode tiled` predicts at the image's own size with
 `TiledPredictor`; `--mode direct` runs `model(x)` at the image's own size and refuses, naming the file, a size the forward
-does not take.  Predictions are clamped to [0, 1] (demo.py, the training step) and evaluated at the ground truth's
+does not take.  `--anchor HxW` (depth, `--mode tiled` only) fits the tiles to a whole-image forward at H x W
+(`TiledPredictor(anchor=...)`).  Predictions are clamped to [0, 1] (demo.py, the training step) and evaluated at the ground truth's
 resolution, which must equal the image's: nothing is resampled.
 
 Ground truth: `.npy` float (depth in metres [H,W]; normals in [0, 1], [3,H,W] or [H,W,3]); depth as a 16-bit PNG,
@@ -89,13 +90,13 @@ def image_tensor(path: Path, task: str) -> torch.Tensor:
     return t.unsqueeze(0)
 
 
-def predict(model, x: torch.Tensor, mode: str, tile, overlap: int, name: str) -> torch.Tensor:
+def predict(model, x: torch.Tensor, mode: str, tile, overlap: int, name: str, anchor=None) -> torch.Tensor:
     """The clamped fp32 prediction at x's size: [1,H,W] (depth) or [1,3,H,W] (normals)."""
     from omnidata_b200.model import check_input_size
     from omnidata_b200.tiled import TiledPredictor
     with torch.no_grad():
         if mode == "tiled":
-            y = TiledPredictor(model, tile=tile, overlap=overlap)(x)
+            y = TiledPredictor(model, tile=tile, overlap=overlap, anchor=anchor)(x)
         else:
             try:
                 check_input_size(x.shape[2], x.shape[3], model.arch["hybrid"], autograd=False)
@@ -126,15 +127,24 @@ def evaluate(args) -> dict:
         mask = None
         if args.mask_path:
             mask = torch.from_numpy(load_mask(_find(args.mask_path, p.stem, "mask"))).unsqueeze(0).to(device)
-        pred = predict(model, x.to(device), args.mode, tile, args.overlap, p.name)
+        pred = predict(model, x.to(device), args.mode, tile, args.overlap, p.name, args.anchor)
         metric.update(pred, torch.from_numpy(np.ascontiguousarray(gt)).unsqueeze(0).to(device), mask)
     result = {"task": args.task, "backbone": args.backbone, "mode": args.mode, "precision": args.precision,
               "tile": list(tile) if args.mode == "tiled" else None,
-              "overlap": args.overlap if args.mode == "tiled" else None, "images": len(images)}
+              "overlap": args.overlap if args.mode == "tiled" else None,
+              "anchor": list(args.anchor) if args.anchor else None, "images": len(images)}
     if args.task == "depth":
         result.update(space=args.space, min_depth=args.min_depth, max_depth=args.max_depth)
     result["metrics"] = metric.compute()
     return result
+
+
+def _size(text: str):
+    try:
+        h, w = (int(v) for v in text.lower().split("x"))
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected HxW, e.g. 768x1024, got {text!r}") from None
+    return h, w
 
 
 def parse_args(argv=None):
@@ -151,12 +161,17 @@ def parse_args(argv=None):
     ap.add_argument("--mode", default="tiled", choices=("tiled", "direct"))
     ap.add_argument("--tile", type=int, default=384)
     ap.add_argument("--overlap", type=int, default=64)
+    ap.add_argument("--anchor", type=_size, default=None, metavar="HxW",
+                    help="depth, --mode tiled: fit the tiles to the model's prediction of the image resized to HxW")
     ap.add_argument("--space", default="depth", choices=("depth", "disparity"))
     ap.add_argument("--min_depth", type=float, default=1e-3)
     ap.add_argument("--max_depth", type=float, default=None)
     ap.add_argument("--depth_scale", type=float, default=512.0, help="16-bit PNG units per metre")
     ap.add_argument("--depth_invalid", type=int, default=65535, help="16-bit PNG value marking no depth")
-    return ap.parse_args(argv)
+    args = ap.parse_args(argv)
+    if args.anchor is not None and (args.mode != "tiled" or args.task != "depth"):
+        ap.error("--anchor applies to --task depth with --mode tiled only")
+    return args
 
 
 def main(argv=None) -> dict:

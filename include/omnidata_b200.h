@@ -498,6 +498,16 @@ int odb_pil_resize_crop_to_tensor(const void* src, int32_t src_h, int32_t src_w,
 int odb_bicubic_resize_f32(const float* in, int32_t planes, int32_t in_h, int32_t in_w, int32_t out_h,
                            int32_t out_w, int32_t flags, float* out, void* stream);
 
+/* F.interpolate(x, (out_h, out_w), mode='bilinear', align_corners=False, antialias=True) on fp32 planes
+ * [planes][in_h][in_w] -> out [planes][out_h][out_w]: a separable triangle filter whose support scales with the
+ * downsampling factor (plain bilinear when upsampling), horizontal pass into tmp fp32 [planes][in_h][out_w], then
+ * vertical.  Per axis the host passes bounds int32 [out][2] = (first input index, tap count) and weights fp32
+ * [out][ksize] normalised to sum 1 (omnidata_b200/imageproc.py bilinear_aa_weights: Pillow's coefficients before the
+ * 8-bit step).  fp32 fused multiply-adds in tap order; deterministic.  planes, in_h, out_h <= 65535. */
+int odb_resize_bilinear_f32(const float* in, int32_t planes, int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w,
+                            const int32_t* bounds_h, const float* weights_h, int32_t ksize_h, const int32_t* bounds_v,
+                            const float* weights_v, int32_t ksize_v, float* tmp, float* out, void* stream);
+
 /* transforms.ToPILImage() on a float CHW tensor (demo.py:150): out uint8 [h][w][c] = trunc(x * 255);
  * clamp01 != 0 applies the reference's .clamp(0, 1) first (demo.py:140). */
 int odb_f32_chw_to_u8_hwc(const float* in, int32_t c, int32_t h, int32_t w, int32_t clamp01, void* out,
@@ -526,7 +536,17 @@ int odb_f32_chw_to_u8_hwc(const float* in, int32_t c, int32_t h, int32_t w, int3
  * odb_tile_blend: out fp32 [b][c][h][w] (the forward's output layout) = sum_i w_i (s_i d_i + t_i) / sum_i w_i over the
  * tiles covering each pixel, row-major, fp32; pred fp32 [b * T][c][tile_h][tile_w]; scale_shift NULL: s = 1, t = 0.
  * w_i = rho(dy) rho(dx), rho(d) = min(1, (d + 1) / (overlap + 1)), d = the distance to the tile's nearest edge that is
- * not on the image border.  All four are deterministic and batch-independent. */
+ * not on the image border.
+ * odb_tile_anchor_moments (depth, anchored): moments fp64 [b][T][5] = (n, Sa, Saa, Sg, Sag) over each tile's pixels
+ * inside the image (n = min(tile_h, h) min(tile_w, w)), a from pred fp32 [b * T][tile_h][tile_w], g from anchor fp32
+ * [b][h][w] (a whole-image prediction resampled to h x w).
+ * odb_tile_align_solve_anchored (depth): scale_shift as odb_tile_align_solve, minimising
+ *   sum_pairs sum_overlap (s_i a + t_i - s_j b - t_j)^2 + 1e-3 Nbar sum_i (1 / n_i) sum_tile (s_i a + t_i - g)^2
+ *   + 1e-6 1e-3 Nbar sum_i ((s_i - 1)^2 + t_i^2)
+ * — each tile anchored to g with the weight the ridge carries in odb_tile_align_solve, the ridge kept at 1e-6 of it so
+ * that a flat tile stays well-posed.  Same band, workspace and tile cap; anchor_moments (from odb_tile_anchor_moments)
+ * is required, moments may be NULL for a single tile, which then gets compute_scale_and_shift of the tile against g.
+ * All are deterministic and batch-independent. */
 #define ODB_TILE_MAX_TILES 1024
 int odb_tile_gather(const float* image, int32_t b, int32_t h, int32_t w, int32_t tile_h, int32_t tile_w,
                     int32_t overlap, float* tiles, void* stream);
@@ -537,6 +557,10 @@ int odb_tile_align_solve(const double* moments, int32_t b, int32_t tiles_y, int3
                          double* scale_shift, void* stream);
 int odb_tile_blend(const float* pred, const double* scale_shift, int32_t b, int32_t c, int32_t h, int32_t w,
                    int32_t tile_h, int32_t tile_w, int32_t overlap, float* out, void* stream);
+int odb_tile_anchor_moments(const float* pred, const float* anchor, int32_t b, int32_t h, int32_t w, int32_t tile_h,
+                            int32_t tile_w, int32_t overlap, double* moments, void* stream);
+int odb_tile_align_solve_anchored(const double* moments, const double* anchor_moments, int32_t b, int32_t tiles_y,
+                                  int32_t tiles_x, void* workspace, double* scale_shift, void* stream);
 
 /* ---- evaluation metrics against ground truth (omnidata_b200/metrics.py DepthMetrics / NormalMetrics) ------------
  *

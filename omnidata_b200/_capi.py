@@ -193,12 +193,16 @@ _SIGNATURES = {
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "odb_bicubic_resize_f32": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          C.c_void_p, C.c_void_p]),
+    "odb_resize_bilinear_f32": (C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 2 + [C.c_int32] +
+                                [C.c_void_p] * 2 + [C.c_int32] + [C.c_void_p] * 3),
     "odb_f32_chw_to_u8_hwc": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "odb_tile_gather": (C.c_int, [C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p]),
     "odb_tile_overlap_moments": (C.c_int, [C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p, C.c_void_p]),
     "odb_tile_align_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
     "odb_tile_align_solve": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
     "odb_tile_blend": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 7 + [C.c_void_p] * 2),
+    "odb_tile_anchor_moments": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 6 + [C.c_void_p] * 2),
+    "odb_tile_align_solve_anchored": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p] * 3),
     "odb_metrics_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
     "odb_depth_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 5 + [C.c_double] * 2 + [C.c_void_p] * 5),
     "odb_normal_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p] * 5),

@@ -137,6 +137,40 @@ __global__ void __launch_bounds__(256) bicubic_resize_f32_kernel(const float* __
   out[(static_cast<long long>(pl) * oh + y) * ow + x] = acc;
 }
 
+// Antialiased bilinear resampling of fp32 planes (F.interpolate(mode="bilinear", align_corners=False, antialias=True)):
+// the same triangle filter as Pillow's, its per-axis (xmin, count) bounds and normalised fp32 weights from the host
+// (omnidata_b200/imageproc.py bilinear_aa_weights).  Horizontal pass in -> tmp [planes][ih][ow], then vertical pass
+// tmp -> out [planes][oh][ow]; fp32 fused multiply-adds in tap order.
+__global__ void __launch_bounds__(256) resample_h_f32_kernel(const float* __restrict__ in, int ih, int iw, int ow,
+                                                             const int32_t* __restrict__ bounds,
+                                                             const float* __restrict__ wts, int ksize,
+                                                             float* __restrict__ tmp) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= ow) return;
+  const long long row = (long long)blockIdx.z * ih + blockIdx.y;
+  const int xmin = __ldg(bounds + 2 * x), cnt = __ldg(bounds + 2 * x + 1);
+  const float* src = in + row * iw + xmin;
+  const float* k = wts + (long long)x * ksize;
+  float acc = 0.f;
+  for (int t = 0; t < cnt; ++t) acc = __fmaf_rn(__ldg(k + t), __ldg(src + t), acc);
+  tmp[row * ow + x] = acc;
+}
+
+__global__ void __launch_bounds__(256) resample_v_f32_kernel(const float* __restrict__ tmp, int ih, int oh, int ow,
+                                                             const int32_t* __restrict__ bounds,
+                                                             const float* __restrict__ wts, int ksize,
+                                                             float* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= ow) return;
+  const int y = blockIdx.y, pl = blockIdx.z;
+  const int ymin = __ldg(bounds + 2 * y), cnt = __ldg(bounds + 2 * y + 1);
+  const float* src = tmp + ((long long)pl * ih + ymin) * ow + x;
+  const float* k = wts + (long long)y * ksize;
+  float acc = 0.f;
+  for (int t = 0; t < cnt; ++t) acc = __fmaf_rn(__ldg(k + t), __ldg(src + (long long)t * ow), acc);
+  out[((long long)pl * oh + y) * ow + x] = acc;
+}
+
 // ToPILImage for a float CHW tensor: (x * 255) truncated to uint8, HWC (torchvision to_pil_image)
 __global__ void __launch_bounds__(256) f32_chw_to_u8_hwc_kernel(const float* __restrict__ in, int c, int h, int w,
                                                                 int clamp01, uint8_t* __restrict__ out) {
@@ -195,6 +229,23 @@ extern "C" int odb_bicubic_resize_f32(const float* in, int32_t planes, int32_t i
   bicubic_resize_f32_kernel<<<grid, 256, 0, stream>>>(in, planes, in_h, in_w, out_h, out_w, flags, out);
   count_launch();
   return check_launch("bicubic_resize_f32");
+}
+
+extern "C" int odb_resize_bilinear_f32(const float* in, int32_t planes, int32_t in_h, int32_t in_w, int32_t out_h,
+                                       int32_t out_w, const int32_t* bounds_h, const float* weights_h, int32_t ksize_h,
+                                       const int32_t* bounds_v, const float* weights_v, int32_t ksize_v, float* tmp,
+                                       float* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!in || !out || !tmp || !bounds_h || !weights_h || !bounds_v || !weights_v || planes < 1 || planes > 65535 ||
+      in_h < 1 || in_w < 1 || out_h < 1 || out_w < 1 || in_h > 65535 || out_h > 65535 || ksize_h < 1 || ksize_v < 1)
+    return fail(ODB_ERR_INVALID, "resize_bilinear_f32: bad argument");
+  resample_h_f32_kernel<<<dim3((out_w + 255) / 256, in_h, planes), 256, 0, stream>>>(in, in_h, in_w, out_w, bounds_h,
+                                                                                    weights_h, ksize_h, tmp);
+  count_launch();
+  resample_v_f32_kernel<<<dim3((out_w + 255) / 256, out_h, planes), 256, 0, stream>>>(tmp, in_h, out_h, out_w,
+                                                                                     bounds_v, weights_v, ksize_v, out);
+  count_launch();
+  return check_launch("resize_bilinear_f32");
 }
 
 extern "C" int odb_f32_chw_to_u8_hwc(const float* in, int32_t c, int32_t h, int32_t w, int32_t clamp01, void* out,

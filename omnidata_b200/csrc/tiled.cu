@@ -16,7 +16,7 @@
 //   tile_align_solve_kernel   depth: per image the per-tile scale / shift minimising
 //                               E(s,t) = sum_pairs sum_overlap (s_i a + t_i - s_j b - t_j)^2
 //                                        + lambda Nbar sum_i ((s_i - 1)^2 + t_i^2)
-//                             (banded fp64 Cholesky of the 2T x 2T normal equations)
+//                             (banded fp64 Cholesky of the 2T x 2T normal equations; anchored form at the end)
 //   tile_blend_kernel         each output pixel: sum_i w_i (s_i d_i + t_i) / sum_i w_i over its covering tiles
 //
 // The alignment follows the MiDaS scale-and-shift alignment of losses/midas_loss.py:10-30 (compute_scale_and_shift: a
@@ -30,7 +30,7 @@
 
 namespace odb {
 
-constexpr double kAlignLambda = 1e-3;
+constexpr double kAlignLambda = 1e-3, kAnchorKappa = 1e-6;     // kappa: the ridge's share in the anchored solve
 constexpr int kSolveThreads = 256;
 constexpr size_t kSolveSmemMax = 200 * 1024;     // band + right-hand side in shared memory up to this size
 
@@ -133,7 +133,8 @@ __global__ void __launch_bounds__(256) tile_moments_kernel(const float* __restri
 // One CTA per image.  Unknowns interleaved (s_0, t_0, s_1, t_1, ...): the normal equations are SPD and banded with
 // half-bandwidth w - 1 (2 nx + 1; 3 for a single row of tiles).  The lower band is stored row-wise,
 // band[r * w + q] = A[r][r - q], in shared memory when it fits, else in the image's slice of `workspace`.
-__global__ void __launch_bounds__(kSolveThreads) tile_align_solve_kernel(const double* __restrict__ moments, int ny,
+__global__ void __launch_bounds__(kSolveThreads) tile_align_solve_kernel(const double* __restrict__ moments,
+                                                                         const double* __restrict__ anchor, int ny,
                                                                          int nx, int band_in_smem, double* workspace,
                                                                          double* __restrict__ scale_shift) {
   extern __shared__ double sm[];
@@ -150,7 +151,7 @@ __global__ void __launch_bounds__(kSolveThreads) tile_align_solve_kernel(const d
     s_ridge = kAlignLambda * (P > 0 ? fmax(s / P, 1.0) : 1.0);
   }
   __syncthreads();
-  const double ridge = s_ridge;
+  const double ridge = s_ridge, r0 = anchor != nullptr ? kAnchorKappa * ridge : ridge;     // anchored: kappa ridge
   // assembly: tile i writes rows 2i (s_i) and 2i + 1 (t_i): its diagonal 2 x 2 block, and the blocks coupling it to its
   // left and upper neighbour j < i (where i is the pair's second tile, b)
   for (int i = threadIdx.x; i < T; i += blockDim.x) {
@@ -158,7 +159,13 @@ __global__ void __launch_bounds__(kSolveThreads) tile_align_solve_kernel(const d
     double* rt = rs + w;
     for (int q = 0; q < w; ++q) rs[q] = rt[q] = 0.0;
     const int ty = i / nx, tx = i - ty * nx;
-    double ass = ridge, ast = 0.0, att = ridge;
+    double ass = r0, ast = 0.0, att = r0, bs = r0, bt = 0.0;
+    if (anchor != nullptr) {                          // mu_i (Saa, Sa; Sa, n), rhs mu_i (Sag, Sg), mu_i = ridge / n_i
+      const double* g = anchor + ((long long)b * T + i) * 5;
+      const double mu = ridge / g[0];
+      ass = fma(mu, g[2], ass); ast = mu * g[1]; att = fma(mu, g[0], att);
+      bs = fma(mu, g[4], bs); bt = mu * g[3];
+    }
     if (tx < nx - 1) {                                // i is "a" of its right pair
       const double* m = mom + (ty * (nx - 1) + tx) * 6;
       ass += m[3]; ast += m[1]; att += m[0];
@@ -180,8 +187,8 @@ __global__ void __launch_bounds__(kSolveThreads) tile_align_solve_kernel(const d
     rs[0] = ass;
     rt[1] = ast;
     rt[0] = att;
-    rhs[2 * i] = ridge;
-    rhs[2 * i + 1] = 0.0;
+    rhs[2 * i] = bs;
+    rhs[2 * i + 1] = bt;
   }
   __syncthreads();
   // banded Cholesky A = L L^T, in place, column by column; each trailing element is updated by one thread
@@ -271,6 +278,63 @@ __global__ void __launch_bounds__(256) tile_blend_kernel(const float* __restrict
   }
 }
 
+// Anchored alignment (TiledPredictor(anchor=...)): g, a whole-image prediction resampled to the image's size, replaces
+// the ridge.  tile_align_solve_kernel with anchor moments (its nullable `anchor`, [b][T][5]) minimises
+//   E(s,t) = sum_pairs sum_overlap (s_i a + t_i - s_j b - t_j)^2
+//            + lambda Nbar sum_i (1/n_i) sum_tile (s_i a + t_i - g)^2 + kappa lambda Nbar sum_i ((s_i - 1)^2 + t_i^2).
+// tile_anchor_moments_kernel, one CTA per (tile, image): moments[b][i] = (n, Sa, Saa, Sg, Sag) over the tile's pixels
+// inside the image, a the tile's prediction, g the anchor [b][H][W].  Fixed strided shares per thread, combined by
+// ordered_sum8.  A grid has few tiles (9 at 1024^2), so each thread loads kAnchorBatch pixels before summing them, to
+// keep loads in flight; the zeros past the end add nothing.  In the solve, each tile's anchor term adds
+// mu_i = lambda Nbar / n_i times its moments to the tile's diagonal 2 x 2 block and right-hand side only, so the band,
+// the workspace and the tile cap are those of the ridge solve.  oracle/tiled_anchor_oracle.py restates it in float64.
+constexpr int kAnchorBatch = 8;
+__global__ void __launch_bounds__(256) tile_anchor_moments_kernel(const float* __restrict__ pred,
+                                                                  const float* __restrict__ anchor, int H, int W,
+                                                                  int th, int tw, int ny, int nx,
+                                                                  double* __restrict__ moments) {
+  __shared__ double part[4][256];
+  const int i = blockIdx.x, b = blockIdx.y;
+  const int T = ny * nx;
+  const int oy = tile_origin(i / nx, ny, H, th), ox = tile_origin(i % nx, nx, W, tw);
+  const int rh = min(th, H), rw = min(tw, W);
+  const float* A = pred + ((long long)b * T + i) * th * tw;
+  const float* G = anchor + ((long long)b * H + oy) * W + ox;
+  double sa = 0.0, saa = 0.0, sg = 0.0, sag = 0.0;
+  const int n = rh * rw;
+  for (int e0 = threadIdx.x; e0 < n; e0 += kAnchorBatch * blockDim.x) {
+    float av[kAnchorBatch], gv[kAnchorBatch];
+#pragma unroll
+    for (int k = 0; k < kAnchorBatch; ++k) {
+      const int e = e0 + k * blockDim.x;
+      av[k] = gv[k] = 0.0f;
+      if (e < n) {
+        const int y = e / rw, x = e - y * rw;
+        av[k] = __ldg(A + y * tw + x);
+        gv[k] = __ldg(G + (long long)y * W + x);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < kAnchorBatch; ++k) {
+      const double a = av[k], g = gv[k];
+      sa += a;
+      saa = fma(a, a, saa);
+      sg += g;
+      sag = fma(a, g, sag);
+    }
+  }
+  part[0][threadIdx.x] = sa;
+  part[1][threadIdx.x] = saa;
+  part[2][threadIdx.x] = sg;
+  part[3][threadIdx.x] = sag;
+  __syncthreads();
+  const int col = threadIdx.x & 31;
+  const double s = ordered_sum8(256, col < 4, [&](int q) { return part[col][q]; });
+  double* m = moments + ((long long)b * T + i) * 5;
+  if (threadIdx.x < 4) m[1 + col] = s;
+  if (threadIdx.x == 0) m[0] = (double)n;
+}
+
 static bool tile_geometry_ok(int32_t b, int32_t h, int32_t w, int32_t th, int32_t tw, int32_t overlap) {
   if (b < 1 || b > 65535 || h < 1 || w < 1 || h > 65535 || w > 65535 || th < 32 || tw < 32 || th % 32 || tw % 32 ||
       overlap < 0 || 2 * overlap >= min(th, tw))
@@ -319,13 +383,26 @@ extern "C" int64_t odb_tile_align_workspace_bytes(int32_t b, int32_t tiles_y, in
   return (int64_t)b * 2 * tiles_y * tiles_x * band_width(tiles_y, tiles_x) * (int64_t)sizeof(double);
 }
 
-extern "C" int odb_tile_align_solve(const double* moments, int32_t b, int32_t tiles_y, int32_t tiles_x,
-                                    void* workspace, double* scale_shift, void* stream_) {
+extern "C" int odb_tile_anchor_moments(const float* pred, const float* anchor, int32_t b, int32_t h, int32_t w,
+                                       int32_t tile_h, int32_t tile_w, int32_t overlap, double* moments,
+                                       void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!pred || !anchor || !moments || !tile_geometry_ok(b, h, w, tile_h, tile_w, overlap))
+    return fail(ODB_ERR_INVALID, "tile_anchor_moments: bad argument");
+  const int ny = tile_count(h, tile_h, overlap), nx = tile_count(w, tile_w, overlap);
+  tile_anchor_moments_kernel<<<dim3(ny * nx, b), 256, 0, stream>>>(pred, anchor, h, w, tile_h, tile_w, ny, nx,
+                                                                   moments);
+  count_launch();
+  return check_launch("tile_anchor_moments");
+}
+
+static int align_solve(const char* name, const char* bad_argument, const double* moments, const double* anchor,
+                       int32_t b, int32_t tiles_y, int32_t tiles_x, void* workspace, double* scale_shift,
+                       cudaStream_t stream) {
   const int64_t ws = odb_tile_align_workspace_bytes(b, tiles_y, tiles_x);
   const bool single = tiles_y == 1 && tiles_x == 1;
   if (ws < 0 || !scale_shift || (!moments && !single) || (ws > 0 && !workspace) || b > 65535)
-    return fail(ODB_ERR_INVALID, "tile_align_solve: bad argument");
+    return fail(ODB_ERR_INVALID, bad_argument);
   const bool in_smem = ws == 0;
   const size_t n = 2 * (size_t)tiles_y * tiles_x;
   const size_t smem = in_smem ? solve_smem_bytes(tiles_y, tiles_x) : n * sizeof(double);
@@ -337,10 +414,24 @@ extern "C" int odb_tile_align_solve(const double* moments, int32_t b, int32_t ti
     if (e != cudaSuccess) return fail_cuda(e, "tile_align_solve: cudaFuncSetAttribute");
     configured[dev] = true;
   }
-  tile_align_solve_kernel<<<b, kSolveThreads, smem, stream>>>(moments, tiles_y, tiles_x, in_smem ? 1 : 0,
+  tile_align_solve_kernel<<<b, kSolveThreads, smem, stream>>>(moments, anchor, tiles_y, tiles_x, in_smem ? 1 : 0,
                                                               static_cast<double*>(workspace), scale_shift);
   count_launch();
-  return check_launch("tile_align_solve");
+  return check_launch(name);
+}
+
+extern "C" int odb_tile_align_solve(const double* moments, int32_t b, int32_t tiles_y, int32_t tiles_x,
+                                    void* workspace, double* scale_shift, void* stream_) {
+  return align_solve("tile_align_solve", "tile_align_solve: bad argument", moments, nullptr, b, tiles_y, tiles_x,
+                     workspace, scale_shift, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int odb_tile_align_solve_anchored(const double* moments, const double* anchor_moments, int32_t b,
+                                             int32_t tiles_y, int32_t tiles_x, void* workspace, double* scale_shift,
+                                             void* stream_) {
+  if (!anchor_moments) return fail(ODB_ERR_INVALID, "tile_align_solve_anchored: anchor_moments is required");
+  return align_solve("tile_align_solve_anchored", "tile_align_solve_anchored: bad argument", moments, anchor_moments,
+                     b, tiles_y, tiles_x, workspace, scale_shift, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int odb_tile_blend(const float* pred, const double* scale_shift, int32_t b, int32_t c, int32_t h, int32_t w,

@@ -42,16 +42,18 @@ def center_crop_offset(full: int, crop: int) -> int:
 
 
 @lru_cache(maxsize=256)
-def pil_bilinear_coeffs(in_size: int, out_size: int):
-    """Pillow precompute_coeffs + normalize_coeffs_8bpc for the BILINEAR filter over the full axis.
-    Returns (bounds int32 [out_size, 2] = (xmin, count), kk int32 [out_size, ksize], ksize)."""
+def bilinear_aa_weights(in_size: int, out_size: int):
+    """Pillow precompute_coeffs for the BILINEAR filter over the full axis, before the 8-bit step: a triangle filter
+    whose support scales with the downsampling factor, each output's taps normalised to sum 1 in double precision.
+    It is also torch's F.interpolate(mode="bilinear", align_corners=False, antialias=True) coefficient rule.
+    Returns (bounds int32 [out_size, 2] = (xmin, count), weights float64 [out_size, ksize], ksize)."""
     in0, in1 = 0.0, float(in_size)
     scale = (in1 - in0) / out_size
     filterscale = scale if scale >= 1.0 else 1.0
     support = 1.0 * filterscale                      # bilinear: filter support 1.0
     ksize = int(math.ceil(support)) * 2 + 1
     bounds = np.zeros((out_size, 2), dtype=np.int32)
-    kk = np.zeros((out_size, ksize), dtype=np.int32)
+    weights = np.zeros((out_size, ksize), dtype=np.float64)
     ss = 1.0 / filterscale
     for xx in range(out_size):
         center = in0 + (xx + 0.5) * scale
@@ -75,11 +77,32 @@ def pil_bilinear_coeffs(in_size: int, out_size: int):
             w = ws[x]
             if ww != 0.0:
                 w /= ww
-            v = w * (1 << PRECISION_BITS)
-            kk[xx, x] = int(-0.5 + v) if w < 0 else int(0.5 + v)
+            weights[xx, x] = w
         bounds[xx, 0] = xmin
         bounds[xx, 1] = xmax
+    return bounds, weights, ksize
+
+
+@lru_cache(maxsize=256)
+def pil_bilinear_coeffs(in_size: int, out_size: int):
+    """Pillow precompute_coeffs + normalize_coeffs_8bpc for the BILINEAR filter over the full axis.
+    Returns (bounds int32 [out_size, 2] = (xmin, count), kk int32 [out_size, ksize], ksize)."""
+    bounds, weights, ksize = bilinear_aa_weights(in_size, out_size)
+    kk = np.zeros((out_size, ksize), dtype=np.int32)
+    for xx in range(out_size):
+        for x in range(int(bounds[xx, 1])):
+            w = float(weights[xx, x])
+            v = w * (1 << PRECISION_BITS)
+            kk[xx, x] = int(-0.5 + v) if w < 0 else int(0.5 + v)
     return bounds, kk, ksize
+
+
+@lru_cache(maxsize=64)
+def resample_tables(in_size: int, out_size: int, device: torch.device):
+    """bilinear_aa_weights resident on `device`: (bounds int32 [out_size, 2], weights fp32 [out_size, ksize], ksize),
+    cached per (size, device) as the preprocessing plans are."""
+    bounds, weights, ksize = bilinear_aa_weights(in_size, out_size)
+    return (torch.from_numpy(bounds).to(device), torch.from_numpy(weights.astype(np.float32)).to(device), ksize)
 
 
 class _Plan:

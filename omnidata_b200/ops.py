@@ -21,6 +21,7 @@ __all__ = [
     "layernorm", "attention", "groupnorm_stats", "groupnorm_apply", "stem_gn_relu_maxpool",
     "stem_im2col", "patchify", "upsample2x_add", "write_cls_row", "readout_cls_bias", "pack_conv_weight",
     "cast_f32_bf16", "head_tail_f32", "tile_gather", "tile_overlap_moments", "tile_align_solve", "tile_blend",
+    "resize_bilinear", "tile_anchor_moments", "tile_align_solve_anchored",
     "metrics_workspace_bytes", "depth_metrics_update", "normal_metrics_update", "normal_metrics_median",
 ]
 
@@ -512,21 +513,76 @@ def tile_overlap_moments(pred, moments, image_hw: Tuple[int, int], tile: Tuple[i
           _same_device(pred, moments), pred.data_ptr(), b, h, w, tile[0], tile[1], overlap, moments.data_ptr())
 
 
-def tile_align_solve(moments, scale_shift, grid: Tuple[int, int]):
-    """scale_shift fp64 [B, T, 2] = per-tile (s, t) of the alignment least squares (csrc/tiled.cu) for a ny x nx grid."""
+def _align_solve_args(name, moments, scale_shift, grid: Tuple[int, int]):
     ny, nx = grid
     b = scale_shift.shape[0] if scale_shift.dim() == 3 else 0
     if ny < 1 or nx < 1 or ny * nx > _capi.TILE_MAX_TILES or not 1 <= b <= 65535:
-        raise _capi.OdbError(f"tile_align_solve: grid {ny}x{nx} (at most {_capi.TILE_MAX_TILES} tiles), batch {b}")
+        raise _capi.OdbError(f"{name}: grid {ny}x{nx} (at most {_capi.TILE_MAX_TILES} tiles), batch {b}")
     _need_shape(scale_shift, (b, ny * nx, 2), torch.float64, "scale_shift")
     if moments is not None:
         _need_shape(moments, (b, tile_pairs(ny, nx), 6), torch.float64, "moments")
     elif ny * nx > 1:
-        raise _capi.OdbError("tile_align_solve: moments are required for more than one tile")
+        raise _capi.OdbError(f"{name}: moments are required for more than one tile")
     nbytes = int(lib().odb_tile_align_workspace_bytes(b, ny, nx))
     ws = torch.empty(nbytes, device=scale_shift.device, dtype=torch.uint8) if nbytes > 0 else None
+    return b, ws
+
+
+def tile_align_solve(moments, scale_shift, grid: Tuple[int, int]):
+    """scale_shift fp64 [B, T, 2] = per-tile (s, t) of the alignment least squares (csrc/tiled.cu) for a ny x nx grid."""
+    b, ws = _align_solve_args("tile_align_solve", moments, scale_shift, grid)
     _call("odb_tile_align_solve", {}, lib().odb_tile_align_solve, _same_device(moments, scale_shift, ws),
-          _ptr(moments), b, ny, nx, _ptr(ws), scale_shift.data_ptr())
+          _ptr(moments), b, grid[0], grid[1], _ptr(ws), scale_shift.data_ptr())
+
+
+def tile_anchor_moments(pred, anchor, moments, tile: Tuple[int, int], overlap: int):
+    """moments fp64 [B, T, 5] = (n, Sa, Saa, Sg, Sag) over each tile's pixels inside the image; pred fp32 [B*T, th, tw]
+    (a depth model's tile predictions), anchor fp32 [B, H, W] (the whole-image prediction at the image's size)."""
+    _need(anchor, torch.float32, "anchor")
+    if anchor.dim() != 3 or not anchor.is_contiguous():
+        raise _capi.OdbError("tile_anchor_moments: anchor must be a contiguous fp32 [B,H,W] tensor")
+    b, h, w = anchor.shape
+    ny, nx = _tile_shapes("tile_anchor_moments", b, h, w, tile, overlap)
+    _need_shape(pred, (b * ny * nx, tile[0], tile[1]), torch.float32, "pred")
+    _need_shape(moments, (b, ny * nx, 5), torch.float64, "moments")
+    _call("odb_tile_anchor_moments", {"bytes": 4 * (pred.numel() + anchor.numel())}, lib().odb_tile_anchor_moments,
+          _same_device(pred, anchor, moments), pred.data_ptr(), anchor.data_ptr(), b, h, w, tile[0], tile[1], overlap,
+          moments.data_ptr())
+
+
+def tile_align_solve_anchored(moments, anchor_moments, scale_shift, grid: Tuple[int, int]):
+    """scale_shift fp64 [B, T, 2] = per-tile (s, t) of the alignment least squares with every tile anchored to a
+    whole-image prediction (anchor_moments fp64 [B, T, 5] from tile_anchor_moments) instead of the ridge to (1, 0)."""
+    b, ws = _align_solve_args("tile_align_solve_anchored", moments, scale_shift, grid)
+    _need_shape(anchor_moments, (b, grid[0] * grid[1], 5), torch.float64, "anchor_moments")
+    _call("odb_tile_align_solve_anchored", {}, lib().odb_tile_align_solve_anchored,
+          _same_device(moments, anchor_moments, scale_shift, ws), _ptr(moments), anchor_moments.data_ptr(), b,
+          grid[0], grid[1], _ptr(ws), scale_shift.data_ptr())
+
+
+def resize_bilinear(x, out):
+    """out fp32 [..., oh, ow] = F.interpolate(x, (oh, ow), mode="bilinear", align_corners=False, antialias=True) of x
+    fp32 [..., ih, iw] (the same leading dimensions), two passes with cached per-axis tables
+    (imageproc.resample_tables)."""
+    from .imageproc import resample_tables
+    _need(x, torch.float32, "x")
+    _need(out, torch.float32, "out")
+    if x.dim() < 2 or out.dim() != x.dim() or x.shape[:-2] != out.shape[:-2] or not x.is_contiguous() \
+            or not out.is_contiguous():
+        raise _capi.OdbError(f"resize_bilinear: contiguous fp32 [..., h, w] tensors with the same leading dimensions "
+                             f"expected, got {tuple(x.shape)} -> {tuple(out.shape)}")
+    (ih, iw), (oh, ow) = x.shape[-2:], out.shape[-2:]
+    planes = x.numel() // (ih * iw) if x.numel() else 0
+    if not 1 <= planes <= 65535 or min(ih, iw, oh, ow) < 1 or max(ih, iw, oh, ow) > 65535:
+        raise _capi.OdbError(f"resize_bilinear: planes and sizes must lie in [1, 65535], got {planes} planes "
+                             f"{ih}x{iw} -> {oh}x{ow}")
+    dev = _same_device(x, out)
+    bh, wh, kh = resample_tables(iw, ow, dev)
+    bv, wv, kv = resample_tables(ih, oh, dev)
+    tmp = torch.empty(planes * ih * ow, device=dev, dtype=torch.float32)
+    _call("odb_resize_bilinear_f32", {"bytes": 4 * (x.numel() + 2 * tmp.numel() + out.numel())},
+          lib().odb_resize_bilinear_f32, dev, x.data_ptr(), planes, ih, iw, oh, ow, bh.data_ptr(), wh.data_ptr(), kh,
+          bv.data_ptr(), wv.data_ptr(), kv, tmp.data_ptr(), out.data_ptr())
 
 
 def tile_blend(pred, scale_shift, out, tile: Tuple[int, int], overlap: int):

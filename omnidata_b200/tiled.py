@@ -3,6 +3,7 @@
     from omnidata_b200.tiled import TiledPredictor
     pred = TiledPredictor(model, tile=(384, 384), overlap=64, max_batch=32)
     depth = pred(x)          # x: float [B,3,H,W] on the model's device, any H, W >= 1
+    anchored = TiledPredictor(model, anchor=(768, 1024))     # depth: tiles fitted to a whole-image forward
 
 `model(x)` takes H, W multiples of 32 with at most 4 096 patches.  TiledPredictor cuts the image into overlapping tiles
 of a size the model takes (`tile_grid`), runs them through `model` itself in chunks of at most `max_batch` tiles, and
@@ -12,6 +13,10 @@ merges the predictions at the image's own size (csrc/tiled.cu):
   loss), so each tile's prediction carries its own unknown scale and shift.  One least-squares problem per image finds a
   scale s_i and shift t_i per tile that make neighbouring tiles agree on their overlaps, with a small ridge towards
   s = 1, t = 0 that fixes the global affine gauge (include/omnidata_b200.h, odb_tile_align_solve);
+- depth with `anchor=(h, w)`: the image is also resized to h x w (antialiased bilinear) and run through `model` whole;
+  that prediction, resampled to the image's size, replaces the ridge: each tile's (s_i, t_i) is pulled towards fitting
+  it, so the merge lands in the whole-image prediction's affine frame (odb_tile_align_solve_anchored).  One extra
+  forward per image;
 - normals: blended as predicted (s = 1, t = 0).
 
 The blend weights fall off linearly over `overlap` pixels towards tile edges inside the image, and not at the image
@@ -20,7 +25,7 @@ Inference only; the merge is deterministic and does not depend on the batch.
 """
 from __future__ import annotations
 
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 
@@ -48,22 +53,30 @@ def tile_grid(H: int, W: int, tile: Tuple[int, int], overlap: int) -> Tuple[List
 class TiledPredictor:
     """Runs `model` on overlapping tiles of any-size images and merges the predictions (module docstring)."""
 
-    def __init__(self, model, tile: Tuple[int, int] = (384, 384), overlap: int = 64, max_batch: int = 32):
+    def __init__(self, model, tile: Tuple[int, int] = (384, 384), overlap: int = 64, max_batch: int = 32,
+                 anchor: Optional[Tuple[int, int]] = None):
         th, tw = int(tile[0]), int(tile[1])
         check_input_size(th, tw, model.arch["hybrid"], autograd=False)
         if not 0 <= overlap < min(th, tw) / 2:
             raise ValueError(f"overlap must lie in [0, min(tile) / 2), got {overlap} for tile {th}x{tw}")
         if max_batch < 1:
             raise ValueError(f"max_batch must be at least 1, got {max_batch}")
+        if anchor is not None:
+            if model.num_channels != 1:
+                raise ValueError(f"anchor applies to depth models only, got a model with {model.num_channels} channels")
+            anchor = (int(anchor[0]), int(anchor[1]))
+            check_input_size(anchor[0], anchor[1], model.arch["hybrid"], autograd=False)
         self.model = model
         self.tile = (th, tw)
         self.overlap = int(overlap)
         self.max_batch = int(max_batch)
+        self.anchor = anchor
 
     def __call__(self, x: torch.Tensor) -> torch.Tensor:
         """The merged prediction of x float [B,3,H,W]: [B,H,W] for a one-channel model, else [B,C,H,W]."""
         pred = self.tile_predictions(x)
-        return self.merge(pred, x.shape[0], x.shape[2], x.shape[3])
+        g = self.anchor_prediction(x) if self.anchor is not None else None
+        return self.merge(pred, x.shape[0], x.shape[2], x.shape[3], anchor=g)
 
     def _grid(self, B: int, H: int, W: int) -> Tuple[int, int]:
         th, tw = self.tile
@@ -98,19 +111,46 @@ class TiledPredictor:
                 pred[i:i + y.shape[0]].copy_(y.view(y.shape[0], C, th, tw))
         return pred
 
-    def merge(self, pred: torch.Tensor, B: int, H: int, W: int) -> torch.Tensor:
-        """Aligns (one channel: depth) and blends tile predictions fp32 [B*T, C, th, tw] into the [B,(C,)H,W] output."""
+    def anchor_prediction(self, x: torch.Tensor) -> torch.Tensor:
+        """The anchor of x float [B,3,H,W]: x resized to the anchor size, run through `model` in chunks of at most
+        `max_batch` images, the prediction resized back to H x W; fp32 [B,H,W]."""
+        if self.anchor is None:
+            raise ValueError("this TiledPredictor has no anchor size")
+        model, (ah, aw) = self.model, self.anchor
+        B, _, H, W = x.shape
+        with torch.no_grad():
+            x = x.detach().float().contiguous()
+            small = torch.empty(B, 3, ah, aw, device=x.device)
+            ops.resize_bilinear(x, small)
+            g_small = torch.empty(B, ah, aw, device=x.device)
+            for i in range(0, B, self.max_batch):
+                y = model(small[i:i + self.max_batch])
+                g_small[i:i + y.shape[0]].copy_(y.view(y.shape[0], ah, aw))
+            g = torch.empty(B, H, W, device=x.device)
+            ops.resize_bilinear(g_small, g)
+        return g
+
+    def merge(self, pred: torch.Tensor, B: int, H: int, W: int, anchor: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Aligns (one channel: depth) and blends tile predictions fp32 [B*T, C, th, tw] into the [B,(C,)H,W] output.
+        With `anchor` (fp32 [B,H,W], `anchor_prediction`) the alignment fits the tiles to it instead of the ridge."""
         (th, tw), ov = self.tile, self.overlap
         ny, nx = self._grid(B, H, W)
         T, C = ny * nx, pred.shape[1]
         st = None
+        if anchor is not None and C != 1:
+            raise ValueError("an anchor applies to one-channel (depth) predictions only")
         if C == 1:
             st = torch.empty(B, T, 2, device=pred.device, dtype=torch.float64)
             moments = None
             if T > 1:
                 moments = torch.empty(B, ops.tile_pairs(ny, nx), 6, device=pred.device, dtype=torch.float64)
                 ops.tile_overlap_moments(pred.view(B * T, th, tw), moments, (H, W), self.tile, ov)
-            ops.tile_align_solve(moments, st, (ny, nx))
+            if anchor is None:
+                ops.tile_align_solve(moments, st, (ny, nx))
+            else:
+                am = torch.empty(B, T, 5, device=pred.device, dtype=torch.float64)
+                ops.tile_anchor_moments(pred.view(B * T, th, tw), anchor, am, self.tile, ov)
+                ops.tile_align_solve_anchored(moments, am, st, (ny, nx))
         out = torch.empty(B, C, H, W, device=pred.device)
         ops.tile_blend(pred, st, out, self.tile, ov)
         return out.squeeze(1) if C == 1 else out
