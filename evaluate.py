@@ -4,13 +4,16 @@
     python evaluate.py --task {depth,normal} --img_path DIR --gt_path DIR [--mask_path DIR]
                        [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
                        [--mode {tiled,direct}] [--tile 384 --overlap 64] [--anchor HxW]
+                       [--ensemble_sizes HxW,... --flip]
                        [--space {depth,disparity}] [--min_depth] [--max_depth] [--depth_scale] [--depth_invalid]
 
 Images (PNG / JPEG) are matched to ground truth, and to masks, by file stem.  Preprocessing is that of
 `demo.py --full_res` (RGB in [0, 1]; depth normalised to [-1, 1]).  `--mode tiled` predicts at the image's own size with
 `TiledPredictor`; `--mode direct` runs `model(x)` at the image's own size and refuses, naming the file, a size the forward
 does not take.  `--anchor HxW` (depth, `--mode tiled` only) fits the tiles to a whole-image forward at H x W
-(`TiledPredictor(anchor=...)`).  Predictions are clamped to [0, 1] (demo.py, the training step) and evaluated at the ground truth's
+(`TiledPredictor(anchor=...)`).  `--ensemble_sizes` and `--flip` wrap the direct or tiled predictor in an
+`EnsemblePredictor`: one member per listed size (`native`: the image's own) and, with `--flip`, its mirror; `--flip`
+alone ensembles the image with its mirror at its own size.  Predictions are clamped to [0, 1] (demo.py, the training step) and evaluated at the ground truth's
 resolution, which must equal the image's: nothing is resampled.
 
 Ground truth: `.npy` float (depth in metres [H,W]; normals in [0, 1], [3,H,W] or [H,W,3]); depth as a 16-bit PNG,
@@ -90,12 +93,21 @@ def image_tensor(path: Path, task: str) -> torch.Tensor:
     return t.unsqueeze(0)
 
 
-def predict(model, x: torch.Tensor, mode: str, tile, overlap: int, name: str, anchor=None) -> torch.Tensor:
-    """The clamped fp32 prediction at x's size: [1,H,W] (depth) or [1,3,H,W] (normals)."""
+def predict(model, x: torch.Tensor, mode: str, tile, overlap: int, name: str, anchor=None, ensemble=None,
+            flip: bool = False) -> torch.Tensor:
+    """The clamped fp32 prediction at x's size: [1,H,W] (depth) or [1,3,H,W] (normals).  `ensemble` (a list of sizes,
+    None: the image's own) or `flip`: an EnsemblePredictor around the tiled or direct predictor."""
+    from omnidata_b200.ensemble import EnsemblePredictor
     from omnidata_b200.model import check_input_size
     from omnidata_b200.tiled import TiledPredictor
     with torch.no_grad():
-        if mode == "tiled":
+        if ensemble is not None or flip:
+            base = TiledPredictor(model, tile=tile, overlap=overlap, anchor=anchor) if mode == "tiled" else model
+            try:
+                y = EnsemblePredictor(base, sizes=ensemble, flip=flip)(x)
+            except ValueError as e:
+                raise ValueError(f"{name}: the ensemble cannot take this image: {e}") from None
+        elif mode == "tiled":
             y = TiledPredictor(model, tile=tile, overlap=overlap, anchor=anchor)(x)
         else:
             try:
@@ -127,12 +139,16 @@ def evaluate(args) -> dict:
         mask = None
         if args.mask_path:
             mask = torch.from_numpy(load_mask(_find(args.mask_path, p.stem, "mask"))).unsqueeze(0).to(device)
-        pred = predict(model, x.to(device), args.mode, tile, args.overlap, p.name, args.anchor)
+        pred = predict(model, x.to(device), args.mode, tile, args.overlap, p.name, args.anchor, args.ensemble_sizes,
+                       args.flip)
         metric.update(pred, torch.from_numpy(np.ascontiguousarray(gt)).unsqueeze(0).to(device), mask)
     result = {"task": args.task, "backbone": args.backbone, "mode": args.mode, "precision": args.precision,
               "tile": list(tile) if args.mode == "tiled" else None,
               "overlap": args.overlap if args.mode == "tiled" else None,
               "anchor": list(args.anchor) if args.anchor else None, "images": len(images)}
+    if args.ensemble_sizes is not None or args.flip:
+        result["ensemble"] = {"sizes": [list(s) if s else None for s in args.ensemble_sizes or [None]],
+                              "flip": args.flip}
     if args.task == "depth":
         result.update(space=args.space, min_depth=args.min_depth, max_depth=args.max_depth)
     result["metrics"] = metric.compute()
@@ -145,6 +161,11 @@ def _size(text: str):
     except ValueError:
         raise argparse.ArgumentTypeError(f"expected HxW, e.g. 768x1024, got {text!r}") from None
     return h, w
+
+
+def _sizes(text: str):
+    """HxW,... -> [(H, W) or None]; `native` stands for the image's own size."""
+    return [None if part.strip().lower() == "native" else _size(part) for part in text.split(",")]
 
 
 def parse_args(argv=None):
@@ -163,6 +184,11 @@ def parse_args(argv=None):
     ap.add_argument("--overlap", type=int, default=64)
     ap.add_argument("--anchor", type=_size, default=None, metavar="HxW",
                     help="depth, --mode tiled: fit the tiles to the model's prediction of the image resized to HxW")
+    ap.add_argument("--ensemble_sizes", type=_sizes, default=None, metavar="HxW,...",
+                    help="ensemble the predictions at these input sizes (`native`: the image's own), merged on the "
+                         "device (EnsemblePredictor)")
+    ap.add_argument("--flip", action="store_true",
+                    help="ensemble each size with its horizontal mirror (alone: the image and its mirror)")
     ap.add_argument("--space", default="depth", choices=("depth", "disparity"))
     ap.add_argument("--min_depth", type=float, default=1e-3)
     ap.add_argument("--max_depth", type=float, default=None)

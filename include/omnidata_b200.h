@@ -610,6 +610,42 @@ int odb_normal_metrics_update(const float* pred, const float* gt, const void* ma
                               int64_t* hist, void* stream);
 int odb_normal_metrics_median(const int64_t* hist, double* out, void* stream);
 
+/* ---- test-time ensembles of depth and normal predictions (omnidata_b200/ensemble.py EnsemblePredictor) -----------
+ *
+ * No reference counterpart: the reference predicts once per image.  Definitions in DESIGN.md §3 "Test-time
+ * ensembles"; oracle/ensemble_oracle.py restates them in float64.  members fp32 [k][b][c][h][w]: k predictions of the
+ * same b images at h x w, member j stored mirrored (columns reversed) where bit j of `flips` is set; the kernels read
+ * them un-mirrored (column w - 1 - x for x).  Member 0 is the reference frame and is never mirrored (bit 0 clear).
+ * 1 <= k <= ODB_ENSEMBLE_MAX_MEMBERS, b, h, w <= 65535.  No floating-point atomics: results are independent of the
+ * batch and bit-reproducible.  Arguments are checked before any launch.
+ *
+ * odb_ensemble_gram (depth, c = 1): gram fp64 [b][(k + 1)(k + 2) / 2] = the packed upper triangle (row-major, i <= j)
+ * of the Gram matrix of v = (a_0, ..., a_{k-1}, 1) summed over V, the pixels where all k members are finite: entry
+ * (j, k) is S a_j, entry (k, k) is n = |V|.  Fixed 4 096-pixel slabs (the partition depends on h x w only), fp64 sums
+ * of exact fp32 products, slabs combined in a fixed order.  workspace: odb_ensemble_gram_workspace_bytes(k, b, h, w)
+ * bytes, 8-byte aligned (negative: refused).  Two launches.
+ * odb_ensemble_align_solve (depth): scale_shift fp64 [b][k][2] = (s_j, t_j) minimising, with s_0 = 1, t_0 = 0,
+ *   E = sum_{i<j} sum_{p in V} (s_i a_ip + t_i - s_j a_jp - t_j)^2 + 1e-6 n sum_{j>=1} ((s_j - 1)^2 + t_j^2)
+ * from gram: the 2 (k - 1) normal equations by a dense fp64 Cholesky, one warp per image; k = 1 writes (1, 0).
+ * odb_ensemble_merge_depth: per pixel where all members are finite, d_j = fp32(s_j a_j + t_j) (fp64 multiply and add,
+ * each rounded to nearest, one rounding to fp32); out fp32 [b][h][w] = the median of the d_j (the middle value for odd
+ * k, the fp32 mean (lo + hi) * 0.5 of the two middle values for even k); spread fp32 [b][h][w] (NULL: not written) =
+ * the same median of |d_j - out| (fp32).  Elsewhere out = member 0 and spread = NaN.  Not clamped.
+ * odb_ensemble_merge_normal (c = 3, the model's encoding [0, 1]): n_j = 2 clamp(a_j, 0, 1) - 1 (a NaN component clamps
+ * to 0), the x component (channel 0) negated for a mirrored member; m = (S_j n_j) / k; out fp32 [b][3][h][w] =
+ * (m / |m| + 1) / 2, fp64 with round-to-nearest operations and one rounding to fp32, or member 0's clamped value where
+ * |m| <= 1e-6; spread fp32 [b][h][w] (NULL: not written) = the mean over j of atan2(|n_j x o|, n_j . o) in degrees,
+ * o = 2 out - 1.  The merges read and write 16 bytes per access where w % 4 == 0 and the buffers are 16-byte aligned. */
+#define ODB_ENSEMBLE_MAX_MEMBERS 16
+int64_t odb_ensemble_gram_workspace_bytes(int32_t k, int32_t b, int32_t h, int32_t w);
+int odb_ensemble_gram(const float* members, int32_t k, int32_t flips, int32_t b, int32_t h, int32_t w,
+                      void* workspace, double* gram, void* stream);
+int odb_ensemble_align_solve(const double* gram, int32_t k, int32_t b, double* scale_shift, void* stream);
+int odb_ensemble_merge_depth(const float* members, const double* scale_shift, int32_t k, int32_t flips, int32_t b,
+                             int32_t h, int32_t w, float* out, float* spread, void* stream);
+int odb_ensemble_merge_normal(const float* members, int32_t k, int32_t flips, int32_t b, int32_t h, int32_t w,
+                              float* out, float* spread, void* stream);
+
 /* Introspection (no GPU needed). */
 int odb_abi_version(void);
 const char* odb_last_error(void);

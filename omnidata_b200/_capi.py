@@ -21,6 +21,7 @@ SPACE_DEPTH, SPACE_DISPARITY = 0, 1             # ODB_SPACE_*
 DEPTH_RECORD = 12                               # ODB_DEPTH_RECORD
 NORMAL_HIST_PER_DEGREE = 4096                   # ODB_NORMAL_HIST_PER_DEGREE
 NORMAL_HIST_BINS = 180 * NORMAL_HIST_PER_DEGREE + 1
+ENSEMBLE_MAX_MEMBERS = 16                       # ODB_ENSEMBLE_MAX_MEMBERS
 
 
 class OdbError(RuntimeError):
@@ -207,6 +208,11 @@ _SIGNATURES = {
     "odb_depth_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 5 + [C.c_double] * 2 + [C.c_void_p] * 5),
     "odb_normal_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p] * 5),
     "odb_normal_metrics_median": (C.c_int, [C.c_void_p] * 3),
+    "odb_ensemble_gram_workspace_bytes": (C.c_int64, [C.c_int32] * 4),
+    "odb_ensemble_gram": (C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3),
+    "odb_ensemble_align_solve": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "odb_ensemble_merge_depth": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 5 + [C.c_void_p] * 3),
+    "odb_ensemble_merge_normal": (C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

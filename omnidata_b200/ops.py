@@ -23,6 +23,8 @@ __all__ = [
     "cast_f32_bf16", "head_tail_f32", "tile_gather", "tile_overlap_moments", "tile_align_solve", "tile_blend",
     "resize_bilinear", "tile_anchor_moments", "tile_align_solve_anchored",
     "metrics_workspace_bytes", "depth_metrics_update", "normal_metrics_update", "normal_metrics_median",
+    "ensemble_gram_workspace_bytes", "ensemble_gram", "ensemble_align_solve", "ensemble_merge_depth",
+    "ensemble_merge_normal",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -691,3 +693,83 @@ def normal_metrics_median(hist, out):
     _need_shape(out, (2,), torch.float64, "out")
     _call("odb_normal_metrics_median", {}, lib().odb_normal_metrics_median, _same_device(hist, out), hist.data_ptr(),
           out.data_ptr())
+
+
+# ---------------------------------------------------------------- test-time ensembles (csrc/ensemble.cu)
+def _ensemble_members(name, members, flips: int, channels: int):
+    """Checks members fp32 [K, B, C, H, W] (contiguous; C = channels) and the mirror bits; returns (K, B, H, W)."""
+    _need(members, torch.float32, "members")
+    if members.dim() != 5 or members.shape[2] != channels or not members.is_contiguous():
+        raise _capi.OdbError(f"{name}: members must be a contiguous fp32 [K,B,{channels},H,W] tensor, got "
+                             f"{tuple(members.shape)}")
+    k, b, _, h, w = members.shape
+    if not 1 <= k <= _capi.ENSEMBLE_MAX_MEMBERS or not 1 <= b <= 65535 or min(h, w) < 1 or max(h, w) > 65535:
+        raise _capi.OdbError(f"{name}: need 1 <= K <= {_capi.ENSEMBLE_MAX_MEMBERS} members, batch and image size in "
+                             f"[1, 65535], got {k}x{b}x{h}x{w}")
+    if not 0 <= flips < (1 << k) or flips & 1:
+        raise _capi.OdbError(f"{name}: flips must be a bit mask of the K members with member 0 unmirrored, got {flips}")
+    return k, b, h, w
+
+
+def _ensemble_spread(spread, b, h, w):
+    if spread is not None:
+        _need_shape(spread, (b, h, w), torch.float32, "spread")
+
+
+def ensemble_gram_workspace_bytes(k: int, b: int, h: int, w: int) -> int:
+    n = int(lib().odb_ensemble_gram_workspace_bytes(k, b, h, w))
+    if n < 0:
+        raise _capi.OdbError(f"ensemble gram workspace: refused {k} members, {b}x{h}x{w}")
+    return n
+
+
+def ensemble_gram(members, flips: int, gram, workspace):
+    """gram fp64 [B, (K+1)(K+2)/2] = the packed upper triangle of the Gram matrix of (a_0, .., a_{K-1}, 1) over the
+    pixels where all members are finite; members fp32 [K, B, 1, H, W], member k mirrored where bit k of flips is set
+    (include/omnidata_b200.h odb_ensemble_gram).  workspace: fp64, ensemble_gram_workspace_bytes of them."""
+    k, b, h, w = _ensemble_members("ensemble_gram", members, flips, 1)
+    _need_shape(gram, (b, (k + 1) * (k + 2) // 2), torch.float64, "gram")
+    _need(workspace, torch.float64, "workspace")
+    if workspace.numel() * 8 < ensemble_gram_workspace_bytes(k, b, h, w) or not workspace.is_contiguous():
+        raise _capi.OdbError(f"ensemble_gram: workspace needs {ensemble_gram_workspace_bytes(k, b, h, w)} contiguous bytes")
+    _call("odb_ensemble_gram", {"bytes": 4 * members.numel()}, lib().odb_ensemble_gram,
+          _same_device(members, gram, workspace), members.data_ptr(), k, flips, b, h, w, workspace.data_ptr(),
+          gram.data_ptr())
+
+
+def ensemble_align_solve(gram, scale_shift):
+    """scale_shift fp64 [B, K, 2] = the (s_k, t_k) that put every member in member 0's frame, from gram fp64
+    [B, (K+1)(K+2)/2] (odb_ensemble_align_solve)."""
+    b = scale_shift.shape[0] if scale_shift.dim() == 3 else 0
+    k = scale_shift.shape[1] if scale_shift.dim() == 3 else 0
+    if not 1 <= k <= _capi.ENSEMBLE_MAX_MEMBERS or not 1 <= b <= 65535:
+        raise _capi.OdbError(f"ensemble_align_solve: scale_shift must be [B, K, 2] with 1 <= K <= "
+                             f"{_capi.ENSEMBLE_MAX_MEMBERS}, got {tuple(scale_shift.shape)}")
+    _need_shape(scale_shift, (b, k, 2), torch.float64, "scale_shift")
+    _need_shape(gram, (b, (k + 1) * (k + 2) // 2), torch.float64, "gram")
+    _call("odb_ensemble_align_solve", {}, lib().odb_ensemble_align_solve, _same_device(gram, scale_shift),
+          gram.data_ptr(), k, b, scale_shift.data_ptr())
+
+
+def ensemble_merge_depth(members, flips: int, scale_shift, out, spread=None):
+    """out fp32 [B, H, W] = the per-pixel median of s_k a_k + t_k over the members fp32 [K, B, 1, H, W]; spread fp32
+    [B, H, W] (optional) = the median absolute deviation from it (odb_ensemble_merge_depth)."""
+    k, b, h, w = _ensemble_members("ensemble_merge_depth", members, flips, 1)
+    _need_shape(scale_shift, (b, k, 2), torch.float64, "scale_shift")
+    _need_shape(out, (b, h, w), torch.float32, "out")
+    _ensemble_spread(spread, b, h, w)
+    _call("odb_ensemble_merge_depth", {"bytes": 4 * (members.numel() + out.numel() * (1 + (spread is not None)))},
+          lib().odb_ensemble_merge_depth, _same_device(members, scale_shift, out, spread), members.data_ptr(),
+          scale_shift.data_ptr(), k, flips, b, h, w, out.data_ptr(), _ptr(spread))
+
+
+def ensemble_merge_normal(members, flips: int, out, spread=None):
+    """out fp32 [B, 3, H, W] = the re-encoded normalised mean of the decoded, un-mirrored members fp32 [K, B, 3, H, W];
+    spread fp32 [B, H, W] (optional) = the members' mean angle to it in degrees (odb_ensemble_merge_normal)."""
+    k, b, h, w = _ensemble_members("ensemble_merge_normal", members, flips, 3)
+    _need_shape(out, (b, 3, h, w), torch.float32, "out")
+    _ensemble_spread(spread, b, h, w)
+    _call("odb_ensemble_merge_normal", {"bytes": 4 * (members.numel() + out.numel() + (0 if spread is None else
+                                                                                      members.numel() + spread.numel()))},
+          lib().odb_ensemble_merge_normal, _same_device(members, out, spread), members.data_ptr(), k, flips, b, h, w,
+          out.data_ptr(), _ptr(spread))
