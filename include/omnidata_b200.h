@@ -626,7 +626,7 @@ int odb_normal_metrics_median(const int64_t* hist, double* out, void* stream);
  * bytes, 8-byte aligned (negative: refused).  Two launches.
  * odb_ensemble_align_solve (depth): scale_shift fp64 [b][k][2] = (s_j, t_j) minimising, with s_0 = 1, t_0 = 0,
  *   E = sum_{i<j} sum_{p in V} (s_i a_ip + t_i - s_j a_jp - t_j)^2 + 1e-6 n sum_{j>=1} ((s_j - 1)^2 + t_j^2)
- * from gram: the 2 (k - 1) normal equations by a dense fp64 Cholesky, one warp per image; k = 1 writes (1, 0).
+ * from gram: the 2 (k - 1) normal equations by a dense fp64 Cholesky, one CTA per image; k = 1 writes (1, 0).
  * odb_ensemble_merge_depth: per pixel where all members are finite, d_j = fp32(s_j a_j + t_j) (fp64 multiply and add,
  * each rounded to nearest, one rounding to fp32); out fp32 [b][h][w] = the median of the d_j (the middle value for odd
  * k, the fp32 mean (lo + hi) * 0.5 of the two middle values for even k); spread fp32 [b][h][w] (NULL: not written) =

@@ -7,33 +7,32 @@
 // on un-mirroring.  Member 0 is the reference frame.
 //
 //   depth:  ensemble_gram_kernel (fixed 4 096-pixel slabs) -> ensemble_gram_reduce_kernel (per image, fixed order)
-//           -> ensemble_align_solve_kernel (one warp per image: dense fp64 Cholesky of the 2 (K - 1) normal equations)
+//           -> ensemble_align_solve_kernel (one CTA per image: fp64 Cholesky of the 2 (K - 1) normal equations,
+//              band_cholesky_solve at full band width)
 //           -> ensemble_merge_depth_kernel<N> (per pixel: d_k = s_k a_k + t_k, median and MAD by a sorting network)
 //   normal: ensemble_merge_normal_kernel (per pixel: normalised mean of the decoded, un-mirrored members)
 //
 // No floating-point atomics; the slab partition depends on H x W only, so every result is independent of the batch and
-// repeat runs give the same bits.  Built without fast-math: the merges are written with explicit round-to-nearest fp64
-// operations so that the float64 oracle reproduces them operation by operation.
+// repeat runs give the same bits.  Built without fast-math: the merges (and angle_deg, fp64.cuh) are written with
+// explicit round-to-nearest fp64 operations so that the float64 oracle reproduces them operation by operation.
 #include <cmath>
 
 #include "common.cuh"
+#include "fp64.cuh"
 #include "host_util.h"
 #include "../../include/omnidata_b200.h"
 
 namespace odb {
 
 constexpr int kEnsThreads = 256;
-constexpr int kEnsSlabIters = 16;
-constexpr long long kEnsSlab = (long long)kEnsThreads * kEnsSlabIters;   // pixels per slab
+constexpr int kEnsSlabIters = kSlab / kEnsThreads;
 constexpr int kEnsMaxK = ODB_ENSEMBLE_MAX_MEMBERS;
 constexpr double kEnsKappa = 1e-6;
-constexpr double kEnsRadToDeg = 180.0 / 3.141592653589793;
 
 // Gram sums of the augmented member vector v = (a_0, ..., a_{K-1}, 1) over the pixels where all members are finite:
 // the packed upper triangle of v^T v, (i, j) with i <= j <= K at tri(i, j); G(K, K) = n, G(k, K) = S a_k.
 __host__ __device__ inline int gram_size(int k) { return (k + 1) * (k + 2) / 2; }
 __host__ __device__ inline int tri(int i, int j, int k) { return i * (k + 1) - i * (i - 1) / 2 + (j - i); }
-static int ens_slabs(int h, int w) { return (int)(((long long)h * w + kEnsSlab - 1) / kEnsSlab); }
 
 ODB_DEVINL long long member_index(long long plane, int y, int x, int W, bool flipped) {
   return plane + (long long)y * W + (flipped ? W - 1 - x : x);
@@ -56,7 +55,7 @@ __global__ void __launch_bounds__(kEnsThreads) ensemble_gram_kernel(const float*
       if (e == q) qi = i, qj = j;
   double acc0 = 0.0, acc1 = 0.0;                            // two chains, added at the end in a fixed order
   for (int it = 0; it < kEnsSlabIters; ++it) {
-    const long long i = blockIdx.x * kEnsSlab + it * kEnsThreads + threadIdx.x;
+    const long long i = blockIdx.x * kSlab + it * kEnsThreads + threadIdx.x;
     bool valid = i < hw;
     const int y = valid ? (int)(i / W) : 0, x = valid ? (int)(i - (long long)y * W) : 0;
 #pragma unroll 4
@@ -97,54 +96,34 @@ __global__ void __launch_bounds__(256) ensemble_gram_reduce_kernel(const double*
   if (threadIdx.x < 32 && q < nq) gram[(long long)b * nq + q] = s;
 }
 
-// One warp per image.  Unknowns x = (s_1, t_1, ..., s_{K-1}, t_{K-1}), s_0 = 1, t_0 = 0.  With c_km = K [k = m] - 1,
+// One CTA per image.  Unknowns x = (s_1, t_1, ..., s_{K-1}, t_{K-1}), s_0 = 1, t_0 = 0.  With c_km = K [k = m] - 1,
 // G_km = S a_k a_m, S_k = S a_k, n = |V| and kn = kappa n, the gradient of E set to zero reads, for m >= 1:
 //   s_m: sum_{k>=1} c_km (G_km s_k + S_m t_k) + kn s_m = kn + G_0m
 //   t_m: sum_{k>=1} c_km (S_k s_k + n t_k)   + kn t_m = S_0
-// (E = K sum_k |d_k|^2 - |sum_k d_k|^2 + kappa n sum_{k>=1} ((s_k - 1)^2 + t_k^2), d_k = s_k a_k + t_k).  Dense
-// Cholesky, one row per lane, then forward and back substitution by lane 0.  scale_shift[b][k] = (s_k, t_k).
-__global__ void __launch_bounds__(32) ensemble_align_solve_kernel(const double* __restrict__ gram, int K,
-                                                                  double* __restrict__ scale_shift) {
+// (E = K sum_k |d_k|^2 - |sum_k d_k|^2 + kappa n sum_{k>=1} ((s_k - 1)^2 + t_k^2), d_k = s_k a_k + t_k).  The lower
+// triangle is assembled as a band of full width M (band_cholesky_solve, fp64.cuh).  scale_shift[b][k] = (s_k, t_k).
+__global__ void __launch_bounds__(kEnsThreads) ensemble_align_solve_kernel(const double* __restrict__ gram, int K,
+                                                                           double* __restrict__ scale_shift) {
   constexpr int kM = 2 * (kEnsMaxK - 1);
-  __shared__ double A[kM][kM + 1];
+  __shared__ double band[kM * kM];
   __shared__ double rhs[kM];
-  const int b = blockIdx.x, lane = threadIdx.x, M = 2 * (K - 1), nq = gram_size(K);
+  const int b = blockIdx.x, M = 2 * (K - 1), nq = gram_size(K);
   const double* G = gram + (long long)b * nq;
   const double n = G[tri(K, K, K)], kn = kEnsKappa * n;
-  for (int e = lane; e < M * M; e += 32) {
+  for (int e = threadIdx.x; e < M * M; e += blockDim.x) {
     const int row = e / M, col = e - row * M, m = row / 2 + 1, k = col / 2 + 1;
+    if (col > row) continue;
     const double c = (k == m ? (double)K : 0.0) - 1.0, ridge = (k == m && (row & 1) == (col & 1)) ? kn : 0.0;
     double g;
     if ((row & 1) == 0) g = (col & 1) == 0 ? G[tri(min(k, m), max(k, m), K)] : G[tri(m, K, K)];
     else g = (col & 1) == 0 ? G[tri(k, K, K)] : n;
-    A[row][col] = c * g + ridge;
+    band[row * M + (row - col)] = c * g + ridge;
   }
-  for (int row = lane; row < M; row += 32) rhs[row] = (row & 1) == 0 ? kn + G[tri(0, row / 2 + 1, K)] : G[tri(0, K, K)];
-  __syncwarp();
-  for (int j = 0; j < M; ++j) {                              // A = L L^T, lower triangle in place
-    const double d = sqrt(A[j][j]);
-    __syncwarp();
-    for (int row = j + 1 + lane; row < M; row += 32) A[row][j] /= d;
-    __syncwarp();
-    for (int row = j + 1 + lane; row < M; row += 32)
-      for (int col = j + 1; col <= row; ++col) A[row][col] -= A[row][j] * A[col][j];
-    if (lane == 0) A[j][j] = d;
-    __syncwarp();
-  }
-  if (lane == 0) {
-    for (int i = 0; i < M; ++i) {
-      double s = rhs[i];
-      for (int c = 0; c < i; ++c) s -= A[i][c] * rhs[c];
-      rhs[i] = s / A[i][i];
-    }
-    for (int i = M - 1; i >= 0; --i) {
-      double s = rhs[i];
-      for (int r = i + 1; r < M; ++r) s -= A[r][i] * rhs[r];
-      rhs[i] = s / A[i][i];
-    }
-  }
-  __syncwarp();
-  for (int k = lane; k < K; k += 32) {
+  for (int row = threadIdx.x; row < M; row += blockDim.x)
+    rhs[row] = (row & 1) == 0 ? kn + G[tri(0, row / 2 + 1, K)] : G[tri(0, K, K)];
+  __syncthreads();
+  band_cholesky_solve(band, rhs, M, M);
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
     double* st = scale_shift + ((long long)b * K + k) * 2;
     st[0] = k == 0 ? 1.0 : rhs[2 * (k - 1)];
     st[1] = k == 0 ? 0.0 : rhs[2 * (k - 1) + 1];
@@ -336,16 +315,7 @@ __global__ void __launch_bounds__(kEnsThreads) ensemble_merge_normal_kernel(cons
       }
     }
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const double* p = n[u];
-      const double* q = o[u];
-      const double cx = __dsub_rn(__dmul_rn(p[1], q[2]), __dmul_rn(p[2], q[1]));
-      const double cy = __dsub_rn(__dmul_rn(p[2], q[0]), __dmul_rn(p[0], q[2]));
-      const double cz = __dsub_rn(__dmul_rn(p[0], q[1]), __dmul_rn(p[1], q[0]));
-      const double cr = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(cx, cx), __dmul_rn(cy, cy)), __dmul_rn(cz, cz)));
-      const double dot = __dadd_rn(__dadd_rn(__dmul_rn(p[0], q[0]), __dmul_rn(p[1], q[1])), __dmul_rn(p[2], q[2]));
-      th[u] = __dadd_rn(th[u], __dmul_rn(atan2(cr, dot), kEnsRadToDeg));
-    }
+    for (int u = 0; u < 4; ++u) th[u] = __dadd_rn(th[u], angle_deg(n[u], o[u]));
   }
   float4 sp;
 #pragma unroll
@@ -354,13 +324,12 @@ __global__ void __launch_bounds__(kEnsThreads) ensemble_merge_normal_kernel(cons
 }
 
 static bool ens_geometry_ok(int32_t k, int32_t b, int32_t h, int32_t w) {
-  return k >= 1 && k <= kEnsMaxK && b >= 1 && b <= 65535 && h >= 1 && w >= 1 && h <= 65535 && w <= 65535;
+  return k >= 1 && k <= kEnsMaxK && planes_ok(b, h, w);
 }
 static bool ens_flips_ok(int32_t k, int32_t flips) { return flips >= 0 && (flips >> k) == 0 && (flips & 1) == 0; }
-static bool ens_aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 // 16-byte accesses: rows of a multiple of 4 floats and 16-byte aligned buffers
 static bool ens_vec(int32_t w, const void* members, const void* out, const void* spread) {
-  return w % 4 == 0 && ens_aligned(members, 16) && ens_aligned(out, 16) && (!spread || ens_aligned(spread, 16));
+  return w % 4 == 0 && aligned(members, 16) && aligned(out, 16) && (!spread || aligned(spread, 16));
 }
 static dim3 merge_grid(int32_t b, int32_t h, int32_t w) {
   const long long quads = (long long)h * ((w + 3) / 4);
@@ -380,16 +349,16 @@ using namespace odb;
 
 extern "C" int64_t odb_ensemble_gram_workspace_bytes(int32_t k, int32_t b, int32_t h, int32_t w) {
   if (!ens_geometry_ok(k, b, h, w)) return -1;
-  return (int64_t)b * ens_slabs(h, w) * gram_size(k) * (int64_t)sizeof(double);
+  return (int64_t)b * slab_count(h, w) * gram_size(k) * (int64_t)sizeof(double);
 }
 
 extern "C" int odb_ensemble_gram(const float* members, int32_t k, int32_t flips, int32_t b, int32_t h, int32_t w,
                                  void* workspace, double* gram, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!members || !workspace || !gram || !ens_geometry_ok(k, b, h, w) || !ens_flips_ok(k, flips) ||
-      !ens_aligned(members, 4) || !ens_aligned(workspace, 8) || !ens_aligned(gram, 8))
+      !aligned(members, 4) || !aligned(workspace, 8) || !aligned(gram, 8))
     return fail(ODB_ERR_INVALID, "ensemble_gram: bad argument");
-  const int slabs = ens_slabs(h, w), nq = gram_size(k);
+  const int slabs = slab_count(h, w), nq = gram_size(k);
   double* part = static_cast<double*>(workspace);
   ensemble_gram_kernel<<<dim3(slabs, b), kEnsThreads, 0, stream>>>(members, k, flips, b, h, w, part);
   count_launch();
@@ -400,9 +369,9 @@ extern "C" int odb_ensemble_gram(const float* members, int32_t k, int32_t flips,
 
 extern "C" int odb_ensemble_align_solve(const double* gram, int32_t k, int32_t b, double* scale_shift, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!gram || !scale_shift || !ens_geometry_ok(k, b, 1, 1) || !ens_aligned(gram, 8) || !ens_aligned(scale_shift, 8))
+  if (!gram || !scale_shift || !ens_geometry_ok(k, b, 1, 1) || !aligned(gram, 8) || !aligned(scale_shift, 8))
     return fail(ODB_ERR_INVALID, "ensemble_align_solve: bad argument");
-  ensemble_align_solve_kernel<<<b, 32, 0, stream>>>(gram, k, scale_shift);
+  ensemble_align_solve_kernel<<<b, kEnsThreads, 0, stream>>>(gram, k, scale_shift);
   count_launch();
   return check_launch("ensemble_align_solve");
 }
@@ -411,7 +380,7 @@ extern "C" int odb_ensemble_merge_depth(const float* members, const double* scal
                                         int32_t b, int32_t h, int32_t w, float* out, float* spread, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!members || !scale_shift || !out || !ens_geometry_ok(k, b, h, w) || !ens_flips_ok(k, flips) ||
-      !ens_aligned(members, 4) || !ens_aligned(out, 4) || !ens_aligned(spread, 4) || !ens_aligned(scale_shift, 8))
+      !aligned(members, 4) || !aligned(out, 4) || !aligned(spread, 4) || !aligned(scale_shift, 8))
     return fail(ODB_ERR_INVALID, "ensemble_merge_depth: bad argument");
   const int vec = ens_vec(w, members, out, spread) ? 1 : 0;
   if (k <= 2) launch_merge_depth<2>(members, scale_shift, k, flips, b, h, w, vec, out, spread, stream);
@@ -425,8 +394,8 @@ extern "C" int odb_ensemble_merge_depth(const float* members, const double* scal
 extern "C" int odb_ensemble_merge_normal(const float* members, int32_t k, int32_t flips, int32_t b, int32_t h, int32_t w,
                                          float* out, float* spread, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!members || !out || !ens_geometry_ok(k, b, h, w) || !ens_flips_ok(k, flips) || !ens_aligned(members, 4) ||
-      !ens_aligned(out, 4) || !ens_aligned(spread, 4))
+  if (!members || !out || !ens_geometry_ok(k, b, h, w) || !ens_flips_ok(k, flips) || !aligned(members, 4) ||
+      !aligned(out, 4) || !aligned(spread, 4))
     return fail(ODB_ERR_INVALID, "ensemble_merge_normal: bad argument");
   const int vec = ens_vec(w, members, out, spread) ? 1 : 0;
   ensemble_merge_normal_kernel<<<merge_grid(b, h, w), kEnsThreads, 0, stream>>>(members, k, flips, b, h, w, vec, out,

@@ -24,6 +24,17 @@ int encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, int rank, void* ba
 
 bool pdl_enabled();
 
+// argument checks of the entry points
+inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+// b images (a grid dimension) of h x w planes
+inline bool planes_ok(int32_t b, int32_t h, int32_t w) {
+  return b >= 1 && b <= 65535 && h >= 1 && h <= 65535 && w >= 1 && w <= 65535;
+}
+// The per-pixel reductions (metrics.cu, ensemble.cu) cut every image into fixed slabs of kSlab pixels, so the partition
+// depends on h x w only, never on the batch.
+constexpr long long kSlab = 4096;
+inline int slab_count(int32_t h, int32_t w) { return (int)(((long long)h * w + kSlab - 1) / kSlab); }
+
 // fp32 correctness mode of odb_conv_gemm (fp32_path.cu)
 
 

@@ -14,11 +14,13 @@
 //   normal: normal_angle_kernel (slabs, histogram) -> slab_reduce_kernel -> normal_fold_kernel (one thread)
 //           normal_median_kernel: block prefix scan over the histogram
 //
-// Built without fast-math: the metrics promise IEEE fp64 arithmetic, and d-hat and the angle are written with explicit
-// round-to-nearest operations (no fma contraction) so that the float64 oracle reproduces them operation by operation.
+// Built without fast-math: the metrics promise IEEE fp64 arithmetic, and d-hat and the angle (angle_deg, fp64.cuh) are
+// written with explicit round-to-nearest operations (no fma contraction) so that the float64 oracle reproduces them
+// operation by operation.
 #include <cmath>
 
 #include "common.cuh"
+#include "fp64.cuh"
 #include "host_util.h"
 #include "select.cuh"
 #include "../../include/omnidata_b200.h"
@@ -26,10 +28,8 @@
 namespace odb {
 
 constexpr int kMetricThreads = 256;
-constexpr int kSlabIters = 16;
-constexpr long long kSlab = (long long)kMetricThreads * kSlabIters;   // pixels per slab
+constexpr int kSlabIters = kSlab / kMetricThreads;
 constexpr int kPartStride = 8;                                          // doubles per slab partial / image record
-constexpr double kRadToDeg = 180.0 / 3.141592653589793;
 constexpr int kMedianThreads = 1024;
 
 ODB_DEVINL bool mask_valid(const void* mask, int kind, long long i) {
@@ -208,12 +208,7 @@ __global__ void __launch_bounds__(kMetricThreads) normal_angle_kernel(const floa
       const double na = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(a[0], a[0]), __dmul_rn(a[1], a[1])), __dmul_rn(a[2], a[2])));
       const double nc = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(c[0], c[0]), __dmul_rn(c[1], c[1])), __dmul_rn(c[2], c[2])));
       if (!(na <= 1e-6) && !(nc <= 1e-6)) {                           // NaN norms take part (and count as non-finite)
-        const double x = __dsub_rn(__dmul_rn(a[1], c[2]), __dmul_rn(a[2], c[1]));
-        const double y = __dsub_rn(__dmul_rn(a[2], c[0]), __dmul_rn(a[0], c[2]));
-        const double z = __dsub_rn(__dmul_rn(a[0], c[1]), __dmul_rn(a[1], c[0]));
-        const double cr = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
-        const double dot = __dadd_rn(__dadd_rn(__dmul_rn(a[0], c[0]), __dmul_rn(a[1], c[1])), __dmul_rn(a[2], c[2]));
-        const double th = __dmul_rn(atan2(cr, dot), kRadToDeg);
+        const double th = angle_deg(a, c);
         if (isfinite(th)) {
           acc[0] += 1.0;
           acc[1] += th;
@@ -297,11 +292,6 @@ __global__ void __launch_bounds__(kMedianThreads) normal_median_kernel(const uns
   }
 }
 
-static bool metric_geometry_ok(int32_t b, int32_t h, int32_t w) {
-  return b >= 1 && b <= 65535 && h >= 1 && w >= 1 && h <= 65535 && w <= 65535;
-}
-static int slab_count(int32_t h, int32_t w) { return (int)(((long long)h * w + kSlab - 1) / kSlab); }
-static bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 static bool mask_ok(const void* mask, int32_t kind) {
   if (kind == ODB_MASK_NONE) return mask == nullptr;
   if (kind == ODB_MASK_U8) return mask != nullptr;
@@ -313,7 +303,7 @@ static bool mask_ok(const void* mask, int32_t kind) {
 using namespace odb;
 
 extern "C" int64_t odb_metrics_workspace_bytes(int32_t b, int32_t h, int32_t w) {
-  if (!metric_geometry_ok(b, h, w)) return -1;
+  if (!planes_ok(b, h, w)) return -1;
   return ((int64_t)b * slab_count(h, w) + 2 * (int64_t)b) * kPartStride * (int64_t)sizeof(double);
 }
 
@@ -323,7 +313,7 @@ extern "C" int odb_depth_metrics_update(const float* pred, const float* gt, cons
                                         int64_t* state_counts, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool disparity = space == ODB_SPACE_DISPARITY;
-  if (!pred || !gt || !workspace || !records || !state_sums || !state_counts || !metric_geometry_ok(b, h, w) ||
+  if (!pred || !gt || !workspace || !records || !state_sums || !state_counts || !planes_ok(b, h, w) ||
       !mask_ok(mask, mask_dtype) || !aligned(pred, 4) || !aligned(gt, 4) || !aligned(workspace, 8) ||
       !aligned(records, 8) || !aligned(state_sums, 8) || !aligned(state_counts, 8) ||
       (space != ODB_SPACE_DEPTH && !disparity) || !std::isfinite(min_depth) || min_depth < 0.0 ||
@@ -355,7 +345,7 @@ extern "C" int odb_normal_metrics_update(const float* pred, const float* gt, con
                                          int32_t b, int32_t h, int32_t w, void* workspace, double* state_sums,
                                          int64_t* state_counts, int64_t* hist, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!pred || !gt || !workspace || !state_sums || !state_counts || !hist || !metric_geometry_ok(b, h, w) ||
+  if (!pred || !gt || !workspace || !state_sums || !state_counts || !hist || !planes_ok(b, h, w) ||
       !mask_ok(mask, mask_dtype) || !aligned(pred, 4) || !aligned(gt, 4) || !aligned(workspace, 8) ||
       !aligned(state_sums, 8) || !aligned(state_counts, 8) || !aligned(hist, 8))
     return fail(ODB_ERR_INVALID, "normal_metrics_update: bad argument");

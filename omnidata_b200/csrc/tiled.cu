@@ -12,11 +12,12 @@
 //
 // Kernels (no floating-point atomics; every result is bit-reproducible and independent of the batch):
 //   tile_gather_kernel        image fp32 NCHW -> tiles [B*T][3][th][tw], 16-byte stores (HBM-bound)
-//   tile_moments_kernel       depth: per (pair, image) n, Sa, Sb, Saa, Sbb, Sab over the overlap, fp64
+//   tile_moments_kernel       depth: per (pair, image) n, Sa, Sb, Saa, Sbb, Sab over the overlap, fp64 (rect_moments)
 //   tile_align_solve_kernel   depth: per image the per-tile scale / shift minimising
 //                               E(s,t) = sum_pairs sum_overlap (s_i a + t_i - s_j b - t_j)^2
 //                                        + lambda Nbar sum_i ((s_i - 1)^2 + t_i^2)
-//                             (banded fp64 Cholesky of the 2T x 2T normal equations; anchored form at the end)
+//                             (fp64 band_cholesky_solve, fp64.cuh, of the 2T x 2T normal equations; anchored form at
+//                             the end)
 //   tile_blend_kernel         each output pixel: sum_i w_i (s_i d_i + t_i) / sum_i w_i over its covering tiles
 //
 // The alignment follows the MiDaS scale-and-shift alignment of losses/midas_loss.py:10-30 (compute_scale_and_shift: a
@@ -25,6 +26,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "fp64.cuh"
 #include "host_util.h"
 #include "../../include/omnidata_b200.h"
 
@@ -67,11 +69,56 @@ __global__ void __launch_bounds__(256) tile_gather_kernel(const float* __restric
   tiles[((((long long)b * T + ti) * 3 + c) * th * tw >> 2) + e] = v;
 }
 
-// One CTA per (pair, image): moments[b][p] = (n, Sa, Sb, Saa, Sbb, Sab) over the pair's overlap inside the image.  Every
-// thread sums a fixed, strided share of the overlap in fp64; the 256 per-thread partials are combined by ordered_sum8.
+// Moments of two fp32 planes over an rh x rw rectangle, a at A[y * lda + x] and b at B[y * ldb + x]: returns
+// S(a, b, a^2, b^2, a b)[q] in fp64 to thread q < 5 of the (256-thread) CTA.  Pixel e = y rw + x is summed by thread
+// e % 256, each thread's pixels in increasing order; the 256 per-thread partials are combined by ordered_sum8.  The
+// walk steps (y, x) by 256 pixels without divisions, and each thread loads kMomentBatch pixels before summing them, to
+// keep loads in flight (a grid has few pairs and tiles: 12 and 9 at 1024^2); the zeros past the end add nothing.
+constexpr int kMomentBatch = 8;
+ODB_DEVINL double rect_moments(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb, int rh,
+                               int rw) {
+  __shared__ double part[5][256];
+  double s[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  if (rw > 0) {
+    const int dy = blockDim.x / rw, dx = blockDim.x - dy * rw;
+    int y = threadIdx.x / rw, x = threadIdx.x - y * rw;
+    while (y < rh) {
+      float av[kMomentBatch], bv[kMomentBatch];
+#pragma unroll
+      for (int k = 0; k < kMomentBatch; ++k) {
+        av[k] = bv[k] = 0.0f;
+        if (y < rh) {
+          av[k] = __ldg(A + (long long)y * lda + x);
+          bv[k] = __ldg(B + (long long)y * ldb + x);
+        }
+        x += dx;
+        y += dy;
+        if (x >= rw) {
+          x -= rw;
+          ++y;
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < kMomentBatch; ++k) {
+        const double a = av[k], b = bv[k];
+        s[0] += a;
+        s[1] += b;
+        s[2] = fma(a, a, s[2]);
+        s[3] = fma(b, b, s[3]);
+        s[4] = fma(a, b, s[4]);
+      }
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < 5; ++q) part[q][threadIdx.x] = s[q];
+  __syncthreads();
+  const int col = threadIdx.x & 31;
+  return ordered_sum8(256, col < 5, [&](int q) { return part[col][q]; });
+}
+
+// One CTA per (pair, image): moments[b][p] = (n, Sa, Sb, Saa, Sbb, Sab) over the pair's overlap inside the image.
 __global__ void __launch_bounds__(256) tile_moments_kernel(const float* __restrict__ pred, int H, int W, int th, int tw,
                                                            int ny, int nx, double* __restrict__ moments) {
-  __shared__ double part[5][256];
   const int p = blockIdx.x, b = blockIdx.y;
   const int T = ny * nx, nh = ny * (nx - 1), P = nh + (ny - 1) * nx;
   int i, j, y0, y1, x0, x1;                          // tiles and the overlap rectangle, image coordinates
@@ -95,38 +142,11 @@ __global__ void __launch_bounds__(256) tile_moments_kernel(const float* __restri
   const int rw = max(x1 - x0, 0), rh = max(y1 - y0, 0);
   const int oyi = tile_origin(i / nx, ny, H, th), oxi = tile_origin(i % nx, nx, W, tw);
   const int oyj = tile_origin(j / nx, ny, H, th), oxj = tile_origin(j % nx, nx, W, tw);
-  const float* A = pred + ((long long)b * T + i) * th * tw;
-  const float* B = pred + ((long long)b * T + j) * th * tw;
-  double sa = 0.0, sb = 0.0, saa = 0.0, sbb = 0.0, sab = 0.0;
-  if (rw > 0) {
-    const int dy = blockDim.x / rw, dx = blockDim.x - dy * rw;
-    int y = threadIdx.x / rw, x = threadIdx.x - y * rw;   // walk the rectangle with stride blockDim.x, no divisions
-    while (y < rh) {
-      const double a = A[(y0 + y - oyi) * tw + (x0 + x - oxi)];
-      const double bb = B[(y0 + y - oyj) * tw + (x0 + x - oxj)];
-      sa += a;
-      sb += bb;
-      saa = fma(a, a, saa);
-      sbb = fma(bb, bb, sbb);
-      sab = fma(a, bb, sab);
-      x += dx;
-      y += dy;
-      if (x >= rw) {
-        x -= rw;
-        ++y;
-      }
-    }
-  }
-  part[0][threadIdx.x] = sa;
-  part[1][threadIdx.x] = sb;
-  part[2][threadIdx.x] = saa;
-  part[3][threadIdx.x] = sbb;
-  part[4][threadIdx.x] = sab;
-  __syncthreads();
-  const int col = threadIdx.x & 31;
-  const double s = ordered_sum8(256, col < 5, [&](int q) { return part[col][q]; });
+  const float* A = pred + ((long long)b * T + i) * th * tw + (y0 - oyi) * tw + (x0 - oxi);
+  const float* B = pred + ((long long)b * T + j) * th * tw + (y0 - oyj) * tw + (x0 - oxj);
+  const double s = rect_moments(A, tw, B, tw, rh, rw);
   double* m = moments + ((long long)b * P + p) * 6;
-  if (threadIdx.x < 5) m[1 + col] = s;
+  if (threadIdx.x < 5) m[1 + threadIdx.x] = s;
   if (threadIdx.x == 0) m[0] = (double)rw * (double)rh;
 }
 
@@ -191,38 +211,7 @@ __global__ void __launch_bounds__(kSolveThreads) tile_align_solve_kernel(const d
     rhs[2 * i + 1] = bt;
   }
   __syncthreads();
-  // banded Cholesky A = L L^T, in place, column by column; each trailing element is updated by one thread
-  for (int k = 0; k < n; ++k) {
-    const int m = min(w - 1, n - 1 - k);
-    const double d = sqrt(band[(long long)k * w]);
-    for (int r = 1 + threadIdx.x; r <= m; r += blockDim.x) band[(long long)(k + r) * w + r] /= d;
-    __syncthreads();
-    if (threadIdx.x == 0) band[(long long)k * w] = d;
-    for (int e = threadIdx.x; e < m * m; e += blockDim.x) {
-      const int r = e / m + 1, c = e - (r - 1) * m + 1;
-      if (c <= r)
-        band[(long long)(k + r) * w + (r - c)] -= band[(long long)(k + r) * w + r] * band[(long long)(k + c) * w + c];
-    }
-    __syncthreads();
-  }
-  // L y = rhs, then L^T x = y (column-oriented; rhs is overwritten by y, then by x).  Step k reads rhs[k] and updates
-  // the entries after (before) it, so thread 0's store of rhs[k] needs no barrier of its own
-  for (int k = 0; k < n; ++k) {
-    const int m = min(w - 1, n - 1 - k);
-    const double yk = rhs[k] / band[(long long)k * w];
-    for (int r = 1 + threadIdx.x; r <= m; r += blockDim.x) rhs[k + r] -= band[(long long)(k + r) * w + r] * yk;
-    __syncthreads();
-    if (threadIdx.x == 0) rhs[k] = yk;
-  }
-  __syncthreads();
-  for (int k = n - 1; k >= 0; --k) {
-    const int m = min(w - 1, k);
-    const double xk = rhs[k] / band[(long long)k * w];
-    for (int q = 1 + threadIdx.x; q <= m; q += blockDim.x) rhs[k - q] -= band[(long long)k * w + q] * xk;
-    __syncthreads();
-    if (threadIdx.x == 0) rhs[k] = xk;
-  }
-  __syncthreads();
+  band_cholesky_solve(band, rhs, n, w);
   for (int e = threadIdx.x; e < n; e += blockDim.x) scale_shift[(long long)b * n + e] = rhs[e];
 }
 
@@ -283,61 +272,28 @@ __global__ void __launch_bounds__(256) tile_blend_kernel(const float* __restrict
 //   E(s,t) = sum_pairs sum_overlap (s_i a + t_i - s_j b - t_j)^2
 //            + lambda Nbar sum_i (1/n_i) sum_tile (s_i a + t_i - g)^2 + kappa lambda Nbar sum_i ((s_i - 1)^2 + t_i^2).
 // tile_anchor_moments_kernel, one CTA per (tile, image): moments[b][i] = (n, Sa, Saa, Sg, Sag) over the tile's pixels
-// inside the image, a the tile's prediction, g the anchor [b][H][W].  Fixed strided shares per thread, combined by
-// ordered_sum8.  A grid has few tiles (9 at 1024^2), so each thread loads kAnchorBatch pixels before summing them, to
-// keep loads in flight; the zeros past the end add nothing.  In the solve, each tile's anchor term adds
+// inside the image, a the tile's prediction, g the anchor [b][H][W].  In the solve, each tile's anchor term adds
 // mu_i = lambda Nbar / n_i times its moments to the tile's diagonal 2 x 2 block and right-hand side only, so the band,
 // the workspace and the tile cap are those of the ridge solve.  oracle/tiled_anchor_oracle.py restates it in float64.
-constexpr int kAnchorBatch = 8;
 __global__ void __launch_bounds__(256) tile_anchor_moments_kernel(const float* __restrict__ pred,
                                                                   const float* __restrict__ anchor, int H, int W,
                                                                   int th, int tw, int ny, int nx,
                                                                   double* __restrict__ moments) {
-  __shared__ double part[4][256];
   const int i = blockIdx.x, b = blockIdx.y;
   const int T = ny * nx;
   const int oy = tile_origin(i / nx, ny, H, th), ox = tile_origin(i % nx, nx, W, tw);
   const int rh = min(th, H), rw = min(tw, W);
   const float* A = pred + ((long long)b * T + i) * th * tw;
   const float* G = anchor + ((long long)b * H + oy) * W + ox;
-  double sa = 0.0, saa = 0.0, sg = 0.0, sag = 0.0;
-  const int n = rh * rw;
-  for (int e0 = threadIdx.x; e0 < n; e0 += kAnchorBatch * blockDim.x) {
-    float av[kAnchorBatch], gv[kAnchorBatch];
-#pragma unroll
-    for (int k = 0; k < kAnchorBatch; ++k) {
-      const int e = e0 + k * blockDim.x;
-      av[k] = gv[k] = 0.0f;
-      if (e < n) {
-        const int y = e / rw, x = e - y * rw;
-        av[k] = __ldg(A + y * tw + x);
-        gv[k] = __ldg(G + (long long)y * W + x);
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < kAnchorBatch; ++k) {
-      const double a = av[k], g = gv[k];
-      sa += a;
-      saa = fma(a, a, saa);
-      sg += g;
-      sag = fma(a, g, sag);
-    }
-  }
-  part[0][threadIdx.x] = sa;
-  part[1][threadIdx.x] = saa;
-  part[2][threadIdx.x] = sg;
-  part[3][threadIdx.x] = sag;
-  __syncthreads();
-  const int col = threadIdx.x & 31;
-  const double s = ordered_sum8(256, col < 4, [&](int q) { return part[col][q]; });
+  const double s = rect_moments(A, tw, G, W, rh, rw);          // thread q: (Sa, Sg, Saa, Sgg, Sag)[q]
   double* m = moments + ((long long)b * T + i) * 5;
-  if (threadIdx.x < 4) m[1 + col] = s;
-  if (threadIdx.x == 0) m[0] = (double)n;
+  const int q = threadIdx.x;
+  if (q < 5 && q != 3) m[q == 0 ? 1 : q == 1 ? 3 : q] = s;
+  if (q == 0) m[0] = (double)(rh * rw);
 }
 
 static bool tile_geometry_ok(int32_t b, int32_t h, int32_t w, int32_t th, int32_t tw, int32_t overlap) {
-  if (b < 1 || b > 65535 || h < 1 || w < 1 || h > 65535 || w > 65535 || th < 32 || tw < 32 || th % 32 || tw % 32 ||
-      overlap < 0 || 2 * overlap >= min(th, tw))
+  if (!planes_ok(b, h, w) || th < 32 || tw < 32 || th % 32 || tw % 32 || overlap < 0 || 2 * overlap >= min(th, tw))
     return false;
   return (long long)tile_count(h, th, overlap) * tile_count(w, tw, overlap) <= ODB_TILE_MAX_TILES;
 }
@@ -354,8 +310,7 @@ using namespace odb;
 extern "C" int odb_tile_gather(const float* image, int32_t b, int32_t h, int32_t w, int32_t tile_h, int32_t tile_w,
                                int32_t overlap, float* tiles, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!image || !tiles || !tile_geometry_ok(b, h, w, tile_h, tile_w, overlap) ||
-      (reinterpret_cast<uintptr_t>(tiles) & 15))
+  if (!image || !tiles || !tile_geometry_ok(b, h, w, tile_h, tile_w, overlap) || !aligned(tiles, 16))
     return fail(ODB_ERR_INVALID, "tile_gather: bad argument");
   const int ny = tile_count(h, tile_h, overlap), nx = tile_count(w, tile_w, overlap);
   const dim3 grid((tile_h * (tile_w / 4) + 255) / 256, 3 * ny * nx, b);

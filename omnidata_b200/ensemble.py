@@ -33,7 +33,7 @@ import torch
 
 from . import _capi, ops
 from .model import DPTDepthModel, check_input_size
-from .tiled import MAX_TILES, TiledPredictor, tile_grid
+from .tiled import TiledPredictor, check_inference_input, chunked_forward
 
 MAX_MEMBERS = _capi.ENSEMBLE_MAX_MEMBERS
 
@@ -71,24 +71,14 @@ class EnsemblePredictor:
         """ValueError for a member size `predictor` refuses, before anything is launched."""
         if isinstance(predictor, DPTDepthModel):
             check_input_size(h, w, predictor.arch["hybrid"], autograd=False)
+        elif isinstance(predictor, TiledPredictor):
+            predictor._grid(1, h, w)
         elif not (1 <= h <= 65535 and 1 <= w <= 65535):
             raise ValueError(f"member sizes must lie in [1, 65535], got {h}x{w}")
-        elif isinstance(predictor, TiledPredictor):
-            oy, ox = tile_grid(h, w, predictor.tile, predictor.overlap)
-            if len(oy) * len(ox) > MAX_TILES:
-                raise ValueError(f"{h}x{w} needs {len(oy) * len(ox)} tiles of {predictor.tile}; at most {MAX_TILES}")
 
     def _check_input(self, x: torch.Tensor):
         p = self.predictor
-        model = p.model if isinstance(p, TiledPredictor) else p
-        if getattr(model, "training", False):
-            raise ValueError("EnsemblePredictor is inference only: call model.eval() first")
-        if x.requires_grad:
-            raise ValueError("EnsemblePredictor is inference only: x must not require grad")
-        if not x.is_cuda:
-            raise _capi.OdbError("EnsemblePredictor runs on a CUDA (sm_90a) device only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
+        check_inference_input("EnsemblePredictor", p.model if isinstance(p, TiledPredictor) else p, x)
         B, _, H, W = x.shape
         if not 1 <= B <= 65535:
             raise ValueError(f"batch must lie in [1, 65535], got {B}")
@@ -130,7 +120,6 @@ class EnsemblePredictor:
         buffer is kept for the next call at this shape, which overwrites it."""
         self._check_input(x)
         B, _, H, W = x.shape
-        C = self.num_channels
         with torch.no_grad():
             x = x.detach().float().contiguous()
             members = self._buffer(B, H, W, x.device)["members"]
@@ -143,14 +132,7 @@ class EnsemblePredictor:
                     ops.resize_bilinear(x, xs)
                 for flipped in ((False, True) if self.flip else (False,)):
                     xin = torch.flip(xs, dims=(3,)) if flipped else xs
-                    for i in range(0, B, self.max_batch):
-                        y = self.predictor(xin[i:i + self.max_batch])
-                        n = y.shape[0]
-                        y = y.float().reshape(n, C, h, w).contiguous()
-                        if (h, w) == (H, W):
-                            members[k, i:i + n].copy_(y)
-                        else:
-                            ops.resize_bilinear(y, members[k, i:i + n])
+                    chunked_forward(self.predictor, xin, self.max_batch, members[k])
                     k += 1
         return members
 

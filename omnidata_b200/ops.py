@@ -465,11 +465,22 @@ def head_tail_f32(x, w, bias, out, relu: bool, pre=None):
           w.data_ptr(), bias.data_ptr(), out.data_ptr(), _ptr(pre), b, h, wd, w.shape[0], 1 if relu else 0)
 
 
+def _check_planes(name: str, *sizes: int, what: str = "batch and image size"):
+    """OdbError unless every size (images as a grid dimension, plane height and width) lies in [1, 65535]."""
+    if not all(1 <= s <= 65535 for s in sizes):
+        raise _capi.OdbError(f"{name}: {what} must lie in [1, 65535], got {'x'.join(str(s) for s in sizes)}")
+
+
+def _check_workspace(name: str, ws: torch.Tensor, nbytes: int):
+    _need(ws, torch.float64, "workspace")
+    if ws.numel() * 8 < nbytes or not ws.is_contiguous():
+        raise _capi.OdbError(f"{name}: workspace needs {nbytes} contiguous bytes")
+
+
 # ---------------------------------------------------------------- tiled inference merge (csrc/tiled.cu)
 def _tile_shapes(name, b, h, w, tile, overlap):
     from .tiled import tile_grid
-    if b < 1 or h < 1 or w < 1 or max(b, h, w) > 65535:
-        raise _capi.OdbError(f"{name}: batch and image size must lie in [1, 65535], got {b}x{h}x{w}")
+    _check_planes(name, b, h, w)
     th, tw = tile
     if th < 32 or tw < 32 or th % 32 or tw % 32 or overlap < 0 or 2 * overlap >= min(th, tw):
         raise _capi.OdbError(f"{name}: tile {th}x{tw} (multiples of 32) with 0 <= 2 overlap < min(tile), got {overlap}")
@@ -518,8 +529,9 @@ def tile_overlap_moments(pred, moments, image_hw: Tuple[int, int], tile: Tuple[i
 def _align_solve_args(name, moments, scale_shift, grid: Tuple[int, int]):
     ny, nx = grid
     b = scale_shift.shape[0] if scale_shift.dim() == 3 else 0
-    if ny < 1 or nx < 1 or ny * nx > _capi.TILE_MAX_TILES or not 1 <= b <= 65535:
-        raise _capi.OdbError(f"{name}: grid {ny}x{nx} (at most {_capi.TILE_MAX_TILES} tiles), batch {b}")
+    if ny < 1 or nx < 1 or ny * nx > _capi.TILE_MAX_TILES:
+        raise _capi.OdbError(f"{name}: grid {ny}x{nx}, at most {_capi.TILE_MAX_TILES} tiles")
+    _check_planes(name, b, what="batch")
     _need_shape(scale_shift, (b, ny * nx, 2), torch.float64, "scale_shift")
     if moments is not None:
         _need_shape(moments, (b, tile_pairs(ny, nx), 6), torch.float64, "moments")
@@ -620,8 +632,7 @@ def check_metric_inputs(name, pred, gt, mask, channels):
     """Checks pred / gt (fp32, contiguous, one shape) and the optional mask (uint8 / bool / fp32, contiguous,
     [B,H,W] or [B,1,H,W]); returns (b, h, w, mask pointer, ODB_MASK_*).  Nothing is copied."""
     b, h, w = metrics_plane_shape(pred, channels)
-    if min(b, h, w) < 1 or b > 65535 or max(h, w) > 65535:
-        raise _capi.OdbError(f"{name}: batch and image size must lie in [1, 65535], got {b}x{h}x{w}")
+    _check_planes(name, b, h, w)
     for t, n in ((pred, "pred"), (gt, "gt")):
         _need(t, torch.float32, n)
         if metrics_plane_shape(t, channels, n) != (b, h, w) or not t.is_contiguous():
@@ -646,12 +657,6 @@ def metrics_workspace_bytes(b: int, h: int, w: int) -> int:
     return n
 
 
-def _metric_workspace(name, ws, b, h, w):
-    _need(ws, torch.float64, "workspace")
-    if ws.numel() * 8 < metrics_workspace_bytes(b, h, w) or not ws.is_contiguous():
-        raise _capi.OdbError(f"{name}: workspace needs {metrics_workspace_bytes(b, h, w)} contiguous bytes")
-
-
 def depth_metrics_update(pred, gt, mask, space: int, min_depth: float, max_depth: float, workspace, records, sums,
                          counts):
     """Adds the depth metrics of pred / gt fp32 [B,(1,)H,W] (mask: None or [B,(1,)H,W] uint8 / bool / fp32, nonzero =
@@ -664,7 +669,7 @@ def depth_metrics_update(pred, gt, mask, space: int, min_depth: float, max_depth
             (space == _capi.SPACE_DISPARITY and not math.isfinite(max_depth)):
         raise _capi.OdbError(f"depth_metrics_update: need 0 <= min_depth < max_depth (finite in disparity space), got "
                              f"{min_depth}, {max_depth}")
-    _metric_workspace("depth_metrics_update", workspace, b, h, w)
+    _check_workspace("depth_metrics_update", workspace, metrics_workspace_bytes(b, h, w))
     _need_shape(records, (b, _capi.DEPTH_RECORD), torch.float64, "records")
     _need_shape(sums, (7,), torch.float64, "sums")
     _need_shape(counts, (4,), torch.int64, "counts")
@@ -678,7 +683,7 @@ def normal_metrics_update(pred, gt, mask, workspace, sums, counts, hist):
     """Adds the angular errors of pred / gt fp32 [B,3,H,W] (model encoding [0, 1]; mask as for depth) to the state
     sums fp64 [2], counts int64 [5] and hist int64 [NORMAL_HIST_BINS] (odb_normal_metrics_update)."""
     b, h, w, mptr, mkind = check_metric_inputs("normal_metrics_update", pred, gt, mask, 3)
-    _metric_workspace("normal_metrics_update", workspace, b, h, w)
+    _check_workspace("normal_metrics_update", workspace, metrics_workspace_bytes(b, h, w))
     _need_shape(sums, (2,), torch.float64, "sums")
     _need_shape(counts, (5,), torch.int64, "counts")
     _need_shape(hist, (_capi.NORMAL_HIST_BINS,), torch.int64, "hist")
@@ -703,9 +708,9 @@ def _ensemble_members(name, members, flips: int, channels: int):
         raise _capi.OdbError(f"{name}: members must be a contiguous fp32 [K,B,{channels},H,W] tensor, got "
                              f"{tuple(members.shape)}")
     k, b, _, h, w = members.shape
-    if not 1 <= k <= _capi.ENSEMBLE_MAX_MEMBERS or not 1 <= b <= 65535 or min(h, w) < 1 or max(h, w) > 65535:
-        raise _capi.OdbError(f"{name}: need 1 <= K <= {_capi.ENSEMBLE_MAX_MEMBERS} members, batch and image size in "
-                             f"[1, 65535], got {k}x{b}x{h}x{w}")
+    if not 1 <= k <= _capi.ENSEMBLE_MAX_MEMBERS:
+        raise _capi.OdbError(f"{name}: need 1 <= K <= {_capi.ENSEMBLE_MAX_MEMBERS} members, got {k}")
+    _check_planes(name, b, h, w)
     if not 0 <= flips < (1 << k) or flips & 1:
         raise _capi.OdbError(f"{name}: flips must be a bit mask of the K members with member 0 unmirrored, got {flips}")
     return k, b, h, w
@@ -729,9 +734,7 @@ def ensemble_gram(members, flips: int, gram, workspace):
     (include/omnidata_b200.h odb_ensemble_gram).  workspace: fp64, ensemble_gram_workspace_bytes of them."""
     k, b, h, w = _ensemble_members("ensemble_gram", members, flips, 1)
     _need_shape(gram, (b, (k + 1) * (k + 2) // 2), torch.float64, "gram")
-    _need(workspace, torch.float64, "workspace")
-    if workspace.numel() * 8 < ensemble_gram_workspace_bytes(k, b, h, w) or not workspace.is_contiguous():
-        raise _capi.OdbError(f"ensemble_gram: workspace needs {ensemble_gram_workspace_bytes(k, b, h, w)} contiguous bytes")
+    _check_workspace("ensemble_gram", workspace, ensemble_gram_workspace_bytes(k, b, h, w))
     _call("odb_ensemble_gram", {"bytes": 4 * members.numel()}, lib().odb_ensemble_gram,
           _same_device(members, gram, workspace), members.data_ptr(), k, flips, b, h, w, workspace.data_ptr(),
           gram.data_ptr())
@@ -742,9 +745,10 @@ def ensemble_align_solve(gram, scale_shift):
     [B, (K+1)(K+2)/2] (odb_ensemble_align_solve)."""
     b = scale_shift.shape[0] if scale_shift.dim() == 3 else 0
     k = scale_shift.shape[1] if scale_shift.dim() == 3 else 0
-    if not 1 <= k <= _capi.ENSEMBLE_MAX_MEMBERS or not 1 <= b <= 65535:
+    if not 1 <= k <= _capi.ENSEMBLE_MAX_MEMBERS:
         raise _capi.OdbError(f"ensemble_align_solve: scale_shift must be [B, K, 2] with 1 <= K <= "
                              f"{_capi.ENSEMBLE_MAX_MEMBERS}, got {tuple(scale_shift.shape)}")
+    _check_planes("ensemble_align_solve", b, what="batch")
     _need_shape(scale_shift, (b, k, 2), torch.float64, "scale_shift")
     _need_shape(gram, (b, (k + 1) * (k + 2) // 2), torch.float64, "gram")
     _call("odb_ensemble_align_solve", {}, lib().odb_ensemble_align_solve, _same_device(gram, scale_shift),

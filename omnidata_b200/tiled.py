@@ -50,6 +50,34 @@ def tile_grid(H: int, W: int, tile: Tuple[int, int], overlap: int) -> Tuple[List
     return _axis(H, tile[0], overlap), _axis(W, tile[1], overlap)
 
 
+def check_inference_input(name: str, model, x: torch.Tensor):
+    """Refuses, before anything is launched, an input the predictor `name` does not take: `model` in training mode, x
+    requiring grad, x not on a CUDA device, or x not [B,3,H,W]."""
+    if getattr(model, "training", False):
+        raise ValueError(f"{name} is inference only: call model.eval() first")
+    if x.requires_grad:
+        raise ValueError(f"{name} is inference only: x must not require grad")
+    if not x.is_cuda:
+        raise _capi.OdbError(f"{name} runs on a CUDA (sm_90a) device only; there is no CPU fallback")
+    if x.dim() != 4 or x.shape[1] != 3:
+        raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
+
+
+def chunked_forward(model, x: torch.Tensor, max_batch: int, out: torch.Tensor):
+    """Runs `model` over x [B,3,h,w] in chunks of at most `max_batch` images into the preallocated fp32 out [B,C,H,W]:
+    each chunk's prediction is copied, or resized (ops.resize_bilinear) where h x w differs from H x W."""
+    C, H, W = out.shape[1:]
+    h, w = x.shape[2:]
+    for i in range(0, x.shape[0], max_batch):
+        y = model(x[i:i + max_batch])
+        n = y.shape[0]
+        y = y.reshape(n, C, h, w)
+        if (h, w) == (H, W):
+            out[i:i + n].copy_(y)
+        else:
+            ops.resize_bilinear(y.float().contiguous(), out[i:i + n])
+
+
 class TiledPredictor:
     """Runs `model` on overlapping tiles of any-size images and merges the predictions (module docstring)."""
 
@@ -90,14 +118,7 @@ class TiledPredictor:
     def tile_predictions(self, x: torch.Tensor) -> torch.Tensor:
         """`model` on the tiles of x (row-major per image, images in order), as fp32 [B*T, C, th, tw]."""
         model, (th, tw) = self.model, self.tile
-        if model.training:
-            raise ValueError("TiledPredictor is inference only: call model.eval() first")
-        if x.requires_grad:
-            raise ValueError("TiledPredictor is inference only: x must not require grad")
-        if not x.is_cuda:
-            raise _capi.OdbError("TiledPredictor runs on a CUDA (sm_90a) device only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
+        check_inference_input("TiledPredictor", model, x)
         B, _, H, W = x.shape
         ny, nx = self._grid(B, H, W)
         n, C = B * ny * nx, model.num_channels
@@ -106,9 +127,7 @@ class TiledPredictor:
             tiles = torch.empty(n, 3, th, tw, device=x.device)
             ops.tile_gather(x, tiles, self.tile, self.overlap)
             pred = torch.empty(n, C, th, tw, device=x.device)
-            for i in range(0, n, self.max_batch):
-                y = model(tiles[i:i + self.max_batch])
-                pred[i:i + y.shape[0]].copy_(y.view(y.shape[0], C, th, tw))
+            chunked_forward(model, tiles, self.max_batch, pred)
         return pred
 
     def anchor_prediction(self, x: torch.Tensor) -> torch.Tensor:
@@ -122,12 +141,10 @@ class TiledPredictor:
             x = x.detach().float().contiguous()
             small = torch.empty(B, 3, ah, aw, device=x.device)
             ops.resize_bilinear(x, small)
-            g_small = torch.empty(B, ah, aw, device=x.device)
-            for i in range(0, B, self.max_batch):
-                y = model(small[i:i + self.max_batch])
-                g_small[i:i + y.shape[0]].copy_(y.view(y.shape[0], ah, aw))
+            g_small = torch.empty(B, 1, ah, aw, device=x.device)
+            chunked_forward(model, small, self.max_batch, g_small)
             g = torch.empty(B, H, W, device=x.device)
-            ops.resize_bilinear(g_small, g)
+            ops.resize_bilinear(g_small.view(B, ah, aw), g)
         return g
 
     def merge(self, pred: torch.Tensor, B: int, H: int, W: int, anchor: Optional[torch.Tensor] = None) -> torch.Tensor:
