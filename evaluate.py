@@ -3,15 +3,17 @@
 
     python evaluate.py --task {depth,normal} --img_path DIR --gt_path DIR [--mask_path DIR]
                        [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
-                       [--mode {tiled,direct}] [--tile 384 --overlap 64] [--anchor HxW]
-                       [--ensemble_sizes HxW,... --flip]
+                       [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--anchor HxW]
+                       [--guided_size HxW [--radius R] [--eps E]] [--ensemble_sizes HxW,... --flip]
                        [--space {depth,disparity}] [--min_depth] [--max_depth] [--depth_scale] [--depth_invalid]
 
 Images (PNG / JPEG) are matched to ground truth, and to masks, by file stem.  Preprocessing is that of
 `demo.py --full_res` (RGB in [0, 1]; depth normalised to [-1, 1]).  `--mode tiled` predicts at the image's own size with
 `TiledPredictor`; `--mode direct` runs `model(x)` at the image's own size and refuses, naming the file, a size the forward
 does not take.  `--anchor HxW` (depth, `--mode tiled` only) fits the tiles to a whole-image forward at H x W
-(`TiledPredictor(anchor=...)`).  `--ensemble_sizes` and `--flip` wrap the direct or tiled predictor in an
+(`TiledPredictor(anchor=...)`).  `--mode guided --guided_size HxW` runs one forward at H x W and upsamples it with the
+image as the guide (`GuidedPredictor`, radius `--radius`, ridge `--eps`).  `--ensemble_sizes` and `--flip` wrap the
+direct, tiled or guided predictor in an
 `EnsemblePredictor`: one member per listed size (`native`: the image's own) and, with `--flip`, its mirror; `--flip`
 alone ensembles the image with its mirror at its own size.  Predictions are clamped to [0, 1] (demo.py, the training step) and evaluated at the ground truth's
 resolution, which must equal the image's: nothing is resampled.
@@ -94,14 +96,23 @@ def image_tensor(path: Path, task: str) -> torch.Tensor:
 
 
 def predict(model, x: torch.Tensor, mode: str, tile, overlap: int, name: str, anchor=None, ensemble=None,
-            flip: bool = False) -> torch.Tensor:
+            flip: bool = False, guided=None) -> torch.Tensor:
     """The clamped fp32 prediction at x's size: [1,H,W] (depth) or [1,3,H,W] (normals).  `ensemble` (a list of sizes,
-    None: the image's own) or `flip`: an EnsemblePredictor around the tiled or direct predictor."""
+    None: the image's own) or `flip`: an EnsemblePredictor around the tiled, direct or guided predictor.  `guided`
+    (mode "guided"): (size, radius, eps) of the GuidedPredictor."""
     from omnidata_b200.ensemble import EnsemblePredictor
+    from omnidata_b200.guided import GuidedPredictor
     from omnidata_b200.model import check_input_size
     from omnidata_b200.tiled import TiledPredictor
     with torch.no_grad():
-        if ensemble is not None or flip:
+        if mode == "guided":
+            size, radius, eps = guided
+            base = GuidedPredictor(model, size=size, radius=radius, eps=eps)
+            try:
+                y = EnsemblePredictor(base, sizes=ensemble, flip=flip)(x) if ensemble is not None or flip else base(x)
+            except ValueError as e:
+                raise ValueError(f"{name}: the guided predictor cannot take this image: {e}") from None
+        elif ensemble is not None or flip:
             base = TiledPredictor(model, tile=tile, overlap=overlap, anchor=anchor) if mode == "tiled" else model
             try:
                 y = EnsemblePredictor(base, sizes=ensemble, flip=flip)(x)
@@ -130,6 +141,10 @@ def evaluate(args) -> dict:
     else:
         metric = NormalMetrics()
     tile = (args.tile, args.tile)
+    guided = (args.guided_size, args.radius, args.eps) if args.mode == "guided" else None
+    if guided is not None:                          # a refused size or setting fails here, before the first image
+        from omnidata_b200.guided import GuidedPredictor
+        GuidedPredictor(model, size=args.guided_size, radius=args.radius, eps=args.eps)
     for p in images:
         gt = load_gt(_find(args.gt_path, p.stem, "ground truth"), args.task, args.depth_scale, args.depth_invalid)
         x = image_tensor(p, args.task)
@@ -140,12 +155,13 @@ def evaluate(args) -> dict:
         if args.mask_path:
             mask = torch.from_numpy(load_mask(_find(args.mask_path, p.stem, "mask"))).unsqueeze(0).to(device)
         pred = predict(model, x.to(device), args.mode, tile, args.overlap, p.name, args.anchor, args.ensemble_sizes,
-                       args.flip)
+                       args.flip, guided)
         metric.update(pred, torch.from_numpy(np.ascontiguousarray(gt)).unsqueeze(0).to(device), mask)
     result = {"task": args.task, "backbone": args.backbone, "mode": args.mode, "precision": args.precision,
               "tile": list(tile) if args.mode == "tiled" else None,
               "overlap": args.overlap if args.mode == "tiled" else None,
-              "anchor": list(args.anchor) if args.anchor else None, "images": len(images)}
+              "anchor": list(args.anchor) if args.anchor else None, "images": len(images),
+              "guided": {"size": list(args.guided_size), "radius": args.radius, "eps": args.eps} if guided else None}
     if args.ensemble_sizes is not None or args.flip:
         result["ensemble"] = {"sizes": [list(s) if s else None for s in args.ensemble_sizes or [None]],
                               "flip": args.flip}
@@ -179,11 +195,17 @@ def parse_args(argv=None):
     w.add_argument("--synthetic_weights", action="store_true", help="seeded random weights (no checkpoint)")
     ap.add_argument("--backbone", default="vitb_rn50_384", choices=("vitb_rn50_384", "vitl16_384", "vitb16_384"))
     ap.add_argument("--precision", default="bf16", choices=("fp32", "bf16", "fp8"))
-    ap.add_argument("--mode", default="tiled", choices=("tiled", "direct"))
+    ap.add_argument("--mode", default="tiled", choices=("tiled", "direct", "guided"))
     ap.add_argument("--tile", type=int, default=384)
     ap.add_argument("--overlap", type=int, default=64)
     ap.add_argument("--anchor", type=_size, default=None, metavar="HxW",
                     help="depth, --mode tiled: fit the tiles to the model's prediction of the image resized to HxW")
+    ap.add_argument("--guided_size", type=_size, default=None, metavar="HxW",
+                    help="--mode guided: the input size of the one forward, upsampled with the image as the guide")
+    ap.add_argument("--radius", type=int, default=None,
+                    help="--mode guided: window radius in low-resolution pixels (default 4, untuned)")
+    ap.add_argument("--eps", type=float, default=None,
+                    help="--mode guided: ridge, in squared units of the model's input (default 1e-3, untuned)")
     ap.add_argument("--ensemble_sizes", type=_sizes, default=None, metavar="HxW,...",
                     help="ensemble the predictions at these input sizes (`native`: the image's own), merged on the "
                          "device (EnsemblePredictor)")
@@ -197,6 +219,13 @@ def parse_args(argv=None):
     args = ap.parse_args(argv)
     if args.anchor is not None and (args.mode != "tiled" or args.task != "depth"):
         ap.error("--anchor applies to --task depth with --mode tiled only")
+    if args.mode == "guided":
+        if args.guided_size is None:
+            ap.error("--mode guided needs --guided_size HxW")
+        args.radius = 4 if args.radius is None else args.radius
+        args.eps = 1e-3 if args.eps is None else args.eps
+    elif args.guided_size is not None or args.radius is not None or args.eps is not None:
+        ap.error("--guided_size, --radius and --eps apply to --mode guided only")
     return args
 
 

@@ -646,6 +646,34 @@ int odb_ensemble_merge_depth(const float* members, const double* scale_shift, in
 int odb_ensemble_merge_normal(const float* members, int32_t k, int32_t flips, int32_t b, int32_t h, int32_t w,
                               float* out, float* spread, void* stream);
 
+/* ---- guided upsampling of a low-resolution prediction (omnidata_b200/guided.py GuidedPredictor) ---------------------
+ *
+ * No reference counterpart.  The fast guided filter (He & Sun, "Fast Guided Image Filtering", 2015): a local linear
+ * model q = a^T I + b of the prediction against the RGB guide, fitted at low resolution and applied to the
+ * full-resolution image.  Definitions in DESIGN.md §3 "Guided upsampling"; oracle/guided_oracle.py restates them in
+ * float64.  c = 1 (depth) or 3 (normals); b, h, w, H, W <= 65535.  No floating-point atomics: results are independent
+ * of the batch and bit-reproducible.  NaN and inf reach every output whose windows or taps touch them.  Arguments are
+ * checked before any launch.
+ *
+ * odb_guided_coefficients: guide fp32 [b][3][h][w], pred fp32 [b][c][h][w].  Window W_i = the pixels within Chebyshev
+ * distance radius of i, clipped at the border (1 <= radius <= ODB_GUIDED_MAX_RADIUS); mean_W(f)_i = (S_{W_i} f) / |W_i|,
+ * summed down each column, then along the row, in fp64.  mu = mean_W(g), Sigma = mean_W(g g^T) - mu mu^T, m_c =
+ * mean_W(p_c), v_c = mean_W(g p_c) - mu m_c; a_c = (Sigma + eps I)^-1 v_c (3x3 Cholesky, eps finite > 0), b_c = m_c -
+ * a_c^T mu; coef fp32 [b][4c][h][w]: plane 4 j + k = mean_W(a_jk) (k < 3) and mean_W(b_j) (k = 3), each rounded to fp32
+ * once.  workspace: odb_guided_workspace_bytes(b, c, h, w) bytes, 8-byte aligned (negative: refused).  Four launches.
+ * odb_guided_apply: out fp32 [b][c][H][W] = B_j + A_j0 x_0 + A_j1 x_1 + A_j2 x_2 (fp32 FMAs in channel order, starting
+ * from B_j), image x fp32 [b][3][H][W], where A, B are coef resampled to H x W exactly as odb_resize_bilinear_f32 does
+ * with the same tables (bounds_h / weights_h / ksize_h over w -> W, bounds_v / weights_v / ksize_v over h -> H, from
+ * omnidata_b200/imageproc.py bilinear_aa_weights).  The resampled coefficients are not written to memory.  16-byte
+ * accesses of image and out where W % 4 == 0 and both are 16-byte aligned.  One launch. */
+#define ODB_GUIDED_MAX_RADIUS 32
+int64_t odb_guided_workspace_bytes(int32_t b, int32_t c, int32_t h, int32_t w);
+int odb_guided_coefficients(const float* guide, const float* pred, int32_t b, int32_t c, int32_t h, int32_t w,
+                            int32_t radius, double eps, void* workspace, float* coef, void* stream);
+int odb_guided_apply(const float* image, const float* coef, int32_t b, int32_t c, int32_t h, int32_t w, int32_t H,
+                     int32_t W, const int32_t* bounds_h, const float* weights_h, int32_t ksize_h,
+                     const int32_t* bounds_v, const float* weights_v, int32_t ksize_v, float* out, void* stream);
+
 /* Introspection (no GPU needed). */
 int odb_abi_version(void);
 const char* odb_last_error(void);

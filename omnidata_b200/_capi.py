@@ -22,6 +22,7 @@ DEPTH_RECORD = 12                               # ODB_DEPTH_RECORD
 NORMAL_HIST_PER_DEGREE = 4096                   # ODB_NORMAL_HIST_PER_DEGREE
 NORMAL_HIST_BINS = 180 * NORMAL_HIST_PER_DEGREE + 1
 ENSEMBLE_MAX_MEMBERS = 16                       # ODB_ENSEMBLE_MAX_MEMBERS
+GUIDED_MAX_RADIUS = 32                          # ODB_GUIDED_MAX_RADIUS
 
 
 class OdbError(RuntimeError):
@@ -213,6 +214,10 @@ _SIGNATURES = {
     "odb_ensemble_align_solve": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "odb_ensemble_merge_depth": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 5 + [C.c_void_p] * 3),
     "odb_ensemble_merge_normal": (C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3),
+    "odb_guided_workspace_bytes": (C.c_int64, [C.c_int32] * 4),
+    "odb_guided_coefficients": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 5 + [C.c_double] + [C.c_void_p] * 3),
+    "odb_guided_apply": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 6 + [C.c_void_p] * 2 + [C.c_int32] +
+                         [C.c_void_p] * 2 + [C.c_int32] + [C.c_void_p] * 2),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -32,8 +32,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import _capi, ops
-from .model import DPTDepthModel, check_input_size
-from .tiled import TiledPredictor, check_inference_input, chunked_forward
+from .tiled import TiledPredictor, check_inference_input, check_predictor_size, chunked_forward
 
 MAX_MEMBERS = _capi.ENSEMBLE_MAX_MEMBERS
 
@@ -56,7 +55,7 @@ class EnsemblePredictor:
             raise ValueError(f"ensembles merge depth (1 channel) or normals (3 channels), got {channels} channels")
         for s in sizes:
             if s is not None:
-                self._check_size(predictor, *s)
+                check_predictor_size(predictor, *s)
         self.predictor = predictor
         self.sizes: List[Optional[Tuple[int, int]]] = sizes
         self.flip = bool(flip)
@@ -66,16 +65,6 @@ class EnsemblePredictor:
         self.flips = sum(1 << i for i, (_, f) in enumerate(self.members) if f)      # member i mirrored: bit i
         self._buffers: Dict[tuple, dict] = {}
 
-    @staticmethod
-    def _check_size(predictor, h: int, w: int):
-        """ValueError for a member size `predictor` refuses, before anything is launched."""
-        if isinstance(predictor, DPTDepthModel):
-            check_input_size(h, w, predictor.arch["hybrid"], autograd=False)
-        elif isinstance(predictor, TiledPredictor):
-            predictor._grid(1, h, w)
-        elif not (1 <= h <= 65535 and 1 <= w <= 65535):
-            raise ValueError(f"member sizes must lie in [1, 65535], got {h}x{w}")
-
     def _check_input(self, x: torch.Tensor):
         p = self.predictor
         check_inference_input("EnsemblePredictor", p.model if isinstance(p, TiledPredictor) else p, x)
@@ -83,7 +72,7 @@ class EnsemblePredictor:
         if not 1 <= B <= 65535:
             raise ValueError(f"batch must lie in [1, 65535], got {B}")
         for s in self.sizes:
-            self._check_size(p, *(s or (H, W)))
+            check_predictor_size(p, *(s or (H, W)))
 
     def __call__(self, x: torch.Tensor, return_spread: bool = False):
         """The merged prediction of x float [B,3,H,W]: [B,H,W] for depth, [B,3,H,W] for normals; with

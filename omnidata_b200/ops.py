@@ -24,7 +24,7 @@ __all__ = [
     "resize_bilinear", "tile_anchor_moments", "tile_align_solve_anchored",
     "metrics_workspace_bytes", "depth_metrics_update", "normal_metrics_update", "normal_metrics_median",
     "ensemble_gram_workspace_bytes", "ensemble_gram", "ensemble_align_solve", "ensemble_merge_depth",
-    "ensemble_merge_normal",
+    "ensemble_merge_normal", "guided_workspace_bytes", "guided_coefficients", "guided_apply",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -777,3 +777,66 @@ def ensemble_merge_normal(members, flips: int, out, spread=None):
                                                                                       members.numel() + spread.numel()))},
           lib().odb_ensemble_merge_normal, _same_device(members, out, spread), members.data_ptr(), k, flips, b, h, w,
           out.data_ptr(), _ptr(spread))
+
+
+# ---------------------------------------------------------------- guided upsampling (csrc/guided.cu)
+def _guided_planes(name, t, channels, tname):
+    """Checks t fp32 [B, channels, h, w] (contiguous); returns (B, h, w)."""
+    _need(t, torch.float32, tname)
+    if t.dim() != 4 or t.shape[1] != channels or not t.is_contiguous():
+        raise _capi.OdbError(f"{name}: {tname} must be a contiguous fp32 [B,{channels},h,w] tensor, got "
+                             f"{tuple(t.shape)}")
+    b, _, h, w = t.shape
+    _check_planes(name, b, h, w)
+    return b, h, w
+
+
+def _guided_channels(name, c):
+    if c not in (1, 3):
+        raise _capi.OdbError(f"{name}: 1 (depth) or 3 (normal) prediction channels, got {c}")
+
+
+def guided_workspace_bytes(b: int, c: int, h: int, w: int) -> int:
+    n = int(lib().odb_guided_workspace_bytes(b, c, h, w))
+    if n < 0:
+        raise _capi.OdbError(f"guided workspace: refused {b}x{c}x{h}x{w}")
+    return n
+
+
+def guided_coefficients(guide, pred, radius: int, eps: float, workspace, coef):
+    """coef fp32 [B, 4C, h, w] = the box-averaged local linear coefficients (plane 4c + k: a_ck for k < 3, b_c for
+    k = 3) of pred fp32 [B, C, h, w] against guide fp32 [B, 3, h, w] over (2 radius + 1)^2 windows, ridge eps
+    (include/omnidata_b200.h odb_guided_coefficients).  workspace: fp64, guided_workspace_bytes of them."""
+    b, h, w = _guided_planes("guided_coefficients", guide, 3, "guide")
+    c = pred.shape[1] if pred.dim() == 4 else 0
+    _guided_channels("guided_coefficients", c)
+    if _guided_planes("guided_coefficients", pred, c, "pred") != (b, h, w):
+        raise _capi.OdbError(f"guided_coefficients: pred {tuple(pred.shape)} does not match guide {tuple(guide.shape)}")
+    if not 1 <= radius <= _capi.GUIDED_MAX_RADIUS:
+        raise _capi.OdbError(f"guided_coefficients: radius must lie in [1, {_capi.GUIDED_MAX_RADIUS}], got {radius}")
+    if not (math.isfinite(eps) and eps > 0):
+        raise _capi.OdbError(f"guided_coefficients: eps must be finite and > 0, got {eps}")
+    _need_shape(coef, (b, 4 * c, h, w), torch.float32, "coef")
+    _check_workspace("guided_coefficients", workspace, guided_workspace_bytes(b, c, h, w))
+    _call("odb_guided_coefficients", {"bytes": 4 * (guide.numel() + pred.numel() + coef.numel())},
+          lib().odb_guided_coefficients, _same_device(guide, pred, workspace, coef), guide.data_ptr(), pred.data_ptr(),
+          b, c, h, w, int(radius), float(eps), workspace.data_ptr(), coef.data_ptr())
+
+
+def guided_apply(image, coef, out):
+    """out fp32 [B, C, H, W] = B_c + A_c . x per pixel, x = image fp32 [B, 3, H, W] and (A_c, B_c) = coef fp32
+    [B, 4C, h, w] resampled to H x W as resize_bilinear resamples (odb_guided_apply)."""
+    b, H, W = _guided_planes("guided_apply", image, 3, "image")
+    c4 = coef.shape[1] if coef.dim() == 4 else 0
+    _guided_channels("guided_apply", c4 // 4 if c4 % 4 == 0 else 0)
+    bc, h, w = _guided_planes("guided_apply", coef, c4, "coef")
+    if bc != b:
+        raise _capi.OdbError(f"guided_apply: coef {tuple(coef.shape)} and image {tuple(image.shape)} differ in batch")
+    _need_shape(out, (b, c4 // 4, H, W), torch.float32, "out")
+    from .imageproc import resample_tables
+    dev = _same_device(image, coef, out)
+    bh, wh, kh = resample_tables(w, W, dev)
+    bv, wv, kv = resample_tables(h, H, dev)
+    _call("odb_guided_apply", {"bytes": 4 * (image.numel() + out.numel())}, lib().odb_guided_apply, dev,
+          image.data_ptr(), coef.data_ptr(), b, c4 // 4, h, w, H, W, bh.data_ptr(), wh.data_ptr(), kh, bv.data_ptr(),
+          wv.data_ptr(), kv, out.data_ptr())

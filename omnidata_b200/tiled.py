@@ -30,7 +30,7 @@ from typing import List, Optional, Tuple
 import torch
 
 from . import _capi, ops
-from .model import check_input_size
+from .model import DPTDepthModel, check_input_size
 
 MAX_TILES = _capi.TILE_MAX_TILES          # tiles per image the alignment solve takes (ODB_TILE_MAX_TILES)
 
@@ -61,6 +61,17 @@ def check_inference_input(name: str, model, x: torch.Tensor):
         raise _capi.OdbError(f"{name} runs on a CUDA (sm_90a) device only; there is no CPU fallback")
     if x.dim() != 4 or x.shape[1] != 3:
         raise ValueError(f"expected input [B,3,H,W], got {tuple(x.shape)}")
+
+
+def check_predictor_size(predictor, h: int, w: int):
+    """ValueError for an input size `predictor` refuses, before anything is launched: the forward's size rule for a
+    `DPTDepthModel`, the tile cap for a `TiledPredictor`, [1, 65535] for anything else."""
+    if isinstance(predictor, DPTDepthModel):
+        check_input_size(h, w, predictor.arch["hybrid"], autograd=False)
+    elif isinstance(predictor, TiledPredictor):
+        predictor._grid(1, h, w)
+    elif not (1 <= h <= 65535 and 1 <= w <= 65535):
+        raise ValueError(f"member sizes must lie in [1, 65535], got {h}x{w}")
 
 
 def chunked_forward(model, x: torch.Tensor, max_batch: int, out: torch.Tensor):
