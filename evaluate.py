@@ -6,6 +6,7 @@
                        [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--anchor HxW]
                        [--guided_size HxW [--radius R] [--eps E]] [--ensemble_sizes HxW,... --flip]
                        [--space {depth,disparity}] [--min_depth] [--max_depth] [--depth_scale] [--depth_invalid]
+                       [--boundary [--edge_path DIR]]
 
 Images (PNG / JPEG) are matched to ground truth, and to masks, by file stem.  Preprocessing is that of
 `demo.py --full_res` (RGB in [0, 1]; depth normalised to [-1, 1]).  `--mode tiled` predicts at the image's own size with
@@ -21,7 +22,9 @@ resolution, which must equal the image's: nothing is resampled.
 Ground truth: `.npy` float (depth in metres [H,W]; normals in [0, 1], [3,H,W] or [H,W,3]); depth as a 16-bit PNG,
 depth = value / --depth_scale with --depth_invalid marking no depth (defaults 512 and 65535: our reading of the Omnidata
 starter dataset's depth_zbuffer files; check them against a real file before relying on them); normals as an 8-bit RGB
-PNG / 255.  Masks: 8-bit PNG or `.npy`, nonzero = valid.  Prints one JSON line: the metrics (omnidata_b200.metrics),
+PNG / 255.  Masks: 8-bit PNG or `.npy`, nonzero = valid.  `--boundary` (depth) adds the depth-boundary errors
+(`BoundaryMetrics`, under the `boundary` key) against ground-truth edge maps from `--edge_path` (8-bit PNG or `.npy`,
+nonzero = edge, matched by file stem) or, without it, edges detected in the ground-truth depth.  Prints one JSON line: the metrics (omnidata_b200.metrics),
 the mode, precision, tile settings and the number of images.  Runs on cuda:0; there is no CPU path.
 """
 from __future__ import annotations
@@ -67,6 +70,11 @@ def load_mask(path: Path) -> np.ndarray:
     if a.ndim == 3:
         a = a[..., 0] if a.shape[-1] in (3, 4) else a[0]
     return (a != 0).astype(np.uint8)
+
+
+def load_edges(path: Path) -> np.ndarray:
+    """uint8 [H,W], 1 = edge, from an 8-bit PNG or a `.npy` (nonzero = edge)."""
+    return load_mask(path)
 
 
 def build_model(task: str, backbone: str, checkpoint, synthetic: bool, precision: str, device):
@@ -130,7 +138,7 @@ def predict(model, x: torch.Tensor, mode: str, tile, overlap: int, name: str, an
 
 
 def evaluate(args) -> dict:
-    from omnidata_b200.metrics import DepthMetrics, NormalMetrics
+    from omnidata_b200.metrics import BoundaryMetrics, DepthMetrics, NormalMetrics
     device = torch.device("cuda:0")
     images = sorted(p for p in Path(args.img_path).iterdir() if p.suffix.lower() in IMAGE_EXT)
     if not images:
@@ -140,6 +148,7 @@ def evaluate(args) -> dict:
         metric = DepthMetrics(space=args.space, min_depth=args.min_depth, max_depth=args.max_depth)
     else:
         metric = NormalMetrics()
+    boundary = BoundaryMetrics(min_depth=args.min_depth, max_depth=args.max_depth) if args.boundary else None
     tile = (args.tile, args.tile)
     guided = (args.guided_size, args.radius, args.eps) if args.mode == "guided" else None
     if guided is not None:                          # a refused size or setting fails here, before the first image
@@ -156,7 +165,16 @@ def evaluate(args) -> dict:
             mask = torch.from_numpy(load_mask(_find(args.mask_path, p.stem, "mask"))).unsqueeze(0).to(device)
         pred = predict(model, x.to(device), args.mode, tile, args.overlap, p.name, args.anchor, args.ensemble_sizes,
                        args.flip, guided)
-        metric.update(pred, torch.from_numpy(np.ascontiguousarray(gt)).unsqueeze(0).to(device), mask)
+        gt_t = torch.from_numpy(np.ascontiguousarray(gt)).unsqueeze(0).to(device)
+        metric.update(pred, gt_t, mask)
+        if boundary is not None:
+            edges = None
+            if args.edge_path:
+                edges = torch.from_numpy(load_edges(_find(args.edge_path, p.stem, "edge map"))).unsqueeze(0).to(device)
+                if tuple(edges.shape[-2:]) != tuple(gt.shape[-2:]):
+                    raise ValueError(f"{p.name}: the edge map is {edges.shape[-2]}x{edges.shape[-1]}, the ground "
+                                     f"truth {gt.shape[-2]}x{gt.shape[-1]}")
+            boundary.update(pred, gt_t, mask, edges)
     result = {"task": args.task, "backbone": args.backbone, "mode": args.mode, "precision": args.precision,
               "tile": list(tile) if args.mode == "tiled" else None,
               "overlap": args.overlap if args.mode == "tiled" else None,
@@ -168,6 +186,8 @@ def evaluate(args) -> dict:
     if args.task == "depth":
         result.update(space=args.space, min_depth=args.min_depth, max_depth=args.max_depth)
     result["metrics"] = metric.compute()
+    if boundary is not None:
+        result["boundary"] = dict(boundary.compute(), edges="given" if args.edge_path else "detected")
     return result
 
 
@@ -216,7 +236,16 @@ def parse_args(argv=None):
     ap.add_argument("--max_depth", type=float, default=None)
     ap.add_argument("--depth_scale", type=float, default=512.0, help="16-bit PNG units per metre")
     ap.add_argument("--depth_invalid", type=int, default=65535, help="16-bit PNG value marking no depth")
+    ap.add_argument("--boundary", action="store_true",
+                    help="depth: also report the depth-boundary errors (BoundaryMetrics) under the `boundary` key")
+    ap.add_argument("--edge_path", default=None, metavar="DIR",
+                    help="--boundary: ground-truth edge maps (8-bit PNG or .npy, nonzero = edge) matched by file "
+                         "stem; without it, edges are detected in the ground-truth depth")
     args = ap.parse_args(argv)
+    if args.boundary and args.task != "depth":
+        ap.error("--boundary applies to --task depth only")
+    if args.edge_path is not None and not args.boundary:
+        ap.error("--edge_path applies with --boundary only")
     if args.anchor is not None and (args.mode != "tiled" or args.task != "depth"):
         ap.error("--anchor applies to --task depth with --mode tiled only")
     if args.mode == "guided":

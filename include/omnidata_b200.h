@@ -610,6 +610,60 @@ int odb_normal_metrics_update(const float* pred, const float* gt, const void* ma
                               int64_t* hist, void* stream);
 int odb_normal_metrics_median(const int64_t* hist, double* out, void* stream);
 
+/* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
+ *
+ * The depth-boundary error (DBE) of iBims-1 (Koch et al., ECCV Workshops 2018): how far predicted depth edges lie from
+ * the true ones.  Definitions in DESIGN.md §3 "Depth-boundary metrics"; oracle/boundary_oracle.py restates them in
+ * float64.  Inputs fp32 [b][h][w]; mask as for the metrics above; b, h, w <= 65535.  Every value is fp64 with explicit
+ * round-to-nearest operations; no floating-point atomics, so results are independent of the batch and
+ * bit-reproducible.  workspace: odb_boundary_workspace_bytes(b, h, w) bytes, 8-byte aligned (negative: refused): 31
+ * bytes per pixel and 8 * 8 * (slabs + 3) bytes per image, slabs = ceil(h w / 4096).  Arguments are checked before any
+ * launch.
+ *
+ * Edge detector E(f, V), modelled on skimage.feature.canny.  V = {mask != 0, g finite, min_depth < g <= max_depth}
+ * (g: the ground truth, or the depth itself for odb_depth_edges); 0 < sigma <= 4, 0 <= low <= high (finite),
+ * 0 <= min_depth < max_depth (+inf: none).
+ *  1. lo, hi = min, max of f over V.  No edges if |V| = 0, hi = lo or f is not finite somewhere on V; otherwise
+ *     fhat = (f - lo) / (hi - lo) on V, 0 elsewhere.
+ *  2. Taps w_k = exp(-k^2 / (2 sigma^2)) / S_j exp(-j^2 / (2 sigma^2)), |k| <= R = floor(4 sigma + 0.5), fp64 on the
+ *     host.  num = G * (fhat 1_V), den = G * 1_V, separable: along rows, then columns, each a sum over k = -R .. R in
+ *     order of w_k v (zeros outside the image); s = num / den where den > 0, else 0.
+ *  3. gx = (dx_-1 + 2 dx_0) + dx_1 with dx_j = s[y+j][x+1] - s[y+j][x-1]; gy = (dy_-1 + 2 dy_0) + dy_1 with
+ *     dy_j = s[y+1][x+j] - s[y-1][x+j]; m = sqrt(gx^2 + gy^2); m = 0 on the image's one-pixel border.
+ *  4. Candidates: the 3x3 neighbourhood lies in the image and in V, m > 0.  With sx, sy = sign(gx), sign(gy) (+1 for
+ *     0): if |gx| >= |gy|, w = |gy| / |gx| and the two points interpolate m(x +- sx, y) (1 - w) + m(x +- sx, y +- sy) w;
+ *     otherwise w = |gx| / |gy| and m(x, y +- sy) (1 - w) + m(x +- sx, y +- sy) w.  Kept if m >= both.
+ *  5. Weak: kept and m >= low; strong: weak and m >= high.  E = the weak pixels whose 8-connected component of weak
+ *     pixels holds a strong pixel.
+ *
+ * odb_depth_edges: edges uint8 [b][h][w] = E(depth, V) (1 = edge).  Eight launches.
+ * odb_edge_hysteresis: step 5 alone on weak_strong uint8 [b][h][w] (bit 0 weak, bit 1 strong; a strong pixel counts as
+ * weak): edges uint8 [b][h][w].  Four launches.
+ * odb_edge_distance2: dist2 uint64 [b][h][w] = the exact squared Euclidean distance in pixels to the nearest edge
+ * pixel (nonzero byte) of the image, 0 on one; UINT64_MAX everywhere in an image without edges.  Two launches.
+ * odb_boundary_metrics_update: E_p = E(pred, V); E_g = gt_edges (uint8 [b][h][w], nonzero = edge) or, when NULL,
+ * E(gt, V).  D_g, D_p = the Euclidean distance transforms of E_g, E_p (sqrt, correctly rounded, of the exact squared
+ * distance).  An image with |E_g| = 0 is excluded.  Otherwise A = {p in E_p : D_g(p) < max_dist} (max_dist finite > 0);
+ * accuracy = S_A D_g / |A| and completeness = S_{E_g} D_p / |E_g|, both = max_dist when A is empty.  A non-finite pred
+ * on V makes them NaN.  records fp64 [b][ODB_BOUNDARY_RECORD] = (accuracy, completeness, |E_p|, |E_g|, |A|, non-finite
+ * predictions on V, |E_g| = 0, A empty), NaN errors for an excluded image; state_sums fp64 [2] += (accuracy,
+ * completeness) of the images not excluded and state_counts int64 [5] += (1, |E_g| = 0, A empty, |E_p|, |E_g|), image
+ * after image in image order.  21 launches (13 with gt_edges).  After a call, the first 8 b h w bytes of the workspace
+ * hold D_g^2 as odb_edge_distance2 writes it. */
+#define ODB_BOUNDARY_RECORD 8
+int64_t odb_boundary_workspace_bytes(int32_t b, int32_t h, int32_t w);
+int odb_depth_edges(const float* depth, const void* mask, int32_t mask_dtype, int32_t b, int32_t h, int32_t w,
+                    double sigma, double low, double high, double min_depth, double max_depth, void* workspace,
+                    uint8_t* edges, void* stream);
+int odb_edge_hysteresis(const uint8_t* weak_strong, int32_t b, int32_t h, int32_t w, void* workspace, uint8_t* edges,
+                        void* stream);
+int odb_edge_distance2(const uint8_t* edges, int32_t b, int32_t h, int32_t w, void* workspace, uint64_t* dist2,
+                       void* stream);
+int odb_boundary_metrics_update(const float* pred, const float* gt, const void* mask, int32_t mask_dtype,
+                                const uint8_t* gt_edges, int32_t b, int32_t h, int32_t w, double sigma, double low,
+                                double high, double max_dist, double min_depth, double max_depth, void* workspace,
+                                double* records, double* state_sums, int64_t* state_counts, void* stream);
+
 /* ---- test-time ensembles of depth and normal predictions (omnidata_b200/ensemble.py EnsemblePredictor) -----------
  *
  * No reference counterpart: the reference predicts once per image.  Definitions in DESIGN.md §3 "Test-time

@@ -23,6 +23,7 @@ NORMAL_HIST_PER_DEGREE = 4096                   # ODB_NORMAL_HIST_PER_DEGREE
 NORMAL_HIST_BINS = 180 * NORMAL_HIST_PER_DEGREE + 1
 ENSEMBLE_MAX_MEMBERS = 16                       # ODB_ENSEMBLE_MAX_MEMBERS
 GUIDED_MAX_RADIUS = 32                          # ODB_GUIDED_MAX_RADIUS
+BOUNDARY_RECORD = 8                             # ODB_BOUNDARY_RECORD
 
 
 class OdbError(RuntimeError):
@@ -218,6 +219,12 @@ _SIGNATURES = {
     "odb_guided_coefficients": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 5 + [C.c_double] + [C.c_void_p] * 3),
     "odb_guided_apply": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 6 + [C.c_void_p] * 2 + [C.c_int32] +
                          [C.c_void_p] * 2 + [C.c_int32] + [C.c_void_p] * 2),
+    "odb_boundary_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
+    "odb_depth_edges": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_double] * 5 + [C.c_void_p] * 3),
+    "odb_edge_hysteresis": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
+    "odb_edge_distance2": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
+    "odb_boundary_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] + [C.c_int32] * 3 +
+                                    [C.c_double] * 6 + [C.c_void_p] * 5),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -34,6 +34,11 @@ inline bool planes_ok(int32_t b, int32_t h, int32_t w) {
 // depends on h x w only, never on the batch.
 constexpr long long kSlab = 4096;
 inline int slab_count(int32_t h, int32_t w) { return (int)(((long long)h * w + kSlab - 1) / kSlab); }
+constexpr int kPartStride = 8;            // doubles per slab partial / image record of those reductions
+// metrics.cu: out[i][q] (stride kPartStride) = the fixed-order reduction of part[i][slab][q] over the slabs of each of
+// `images` images, q < nq: the sum, or the minimum / maximum where bit q of min_mask / max_mask is set.  One launch.
+void launch_slab_reduce(const double* part, int images, int slabs, int nq, unsigned min_mask, unsigned max_mask,
+                        double* out, cudaStream_t stream);
 
 // fp32 correctness mode of odb_conv_gemm (fp32_path.cu)
 

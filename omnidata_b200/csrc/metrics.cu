@@ -29,7 +29,6 @@ namespace odb {
 
 constexpr int kMetricThreads = 256;
 constexpr int kSlabIters = kSlab / kMetricThreads;
-constexpr int kPartStride = 8;                                          // doubles per slab partial / image record
 constexpr int kMedianThreads = 1024;
 
 ODB_DEVINL bool mask_valid(const void* mask, int kind, long long i) {
@@ -74,16 +73,29 @@ __global__ void __launch_bounds__(kMetricThreads) depth_moments_kernel(const flo
   }
 }
 
-// out[b][q] = sum over the image's slabs of part[b][slab][q], q < nq, in a fixed order.  grid (b)
+// out[b][q] = sum over the image's slabs of part[b][slab][q], q < nq, in a fixed order; the minimum or the maximum
+// instead where bit q of min_mask or max_mask is set.  grid (b)
 __global__ void __launch_bounds__(kMetricThreads) slab_reduce_kernel(const double* __restrict__ part, int slabs, int nq,
+                                                                     unsigned min_mask, unsigned max_mask,
                                                                      double* __restrict__ out) {
   __shared__ double scratch[32];
   const int b = blockIdx.x;
   const double* p = part + (long long)b * slabs * kPartStride;
   for (int q = 0; q < nq; ++q) {
-    double acc = 0.0;
-    for (int s = threadIdx.x; s < slabs; s += kMetricThreads) acc += p[(long long)s * kPartStride + q];
-    const double r = block_sum_d(acc, scratch);
+    double r;
+    if ((min_mask | max_mask) >> q & 1u) {
+      const bool lo = min_mask >> q & 1u;
+      double acc = lo ? INFINITY : -INFINITY;
+      for (int s = threadIdx.x; s < slabs; s += kMetricThreads) {
+        const double v = p[(long long)s * kPartStride + q];
+        acc = lo ? fmin(acc, v) : fmax(acc, v);
+      }
+      r = lo ? block_min_d(acc, scratch) : block_max_d(acc, scratch);
+    } else {
+      double acc = 0.0;
+      for (int s = threadIdx.x; s < slabs; s += kMetricThreads) acc += p[(long long)s * kPartStride + q];
+      r = block_sum_d(acc, scratch);
+    }
     if (threadIdx.x == 0) out[(long long)b * kPartStride + q] = r;
   }
 }
@@ -298,6 +310,12 @@ static bool mask_ok(const void* mask, int32_t kind) {
   return kind == ODB_MASK_F32 && mask != nullptr && aligned(mask, 4);
 }
 
+void launch_slab_reduce(const double* part, int images, int slabs, int nq, unsigned min_mask, unsigned max_mask,
+                        double* out, cudaStream_t stream) {
+  slab_reduce_kernel<<<images, kMetricThreads, 0, stream>>>(part, slabs, nq, min_mask, max_mask, out);
+  count_launch();
+}
+
 }  // namespace odb
 
 using namespace odb;
@@ -328,12 +346,12 @@ extern "C" int odb_depth_metrics_update(const float* pred, const float* gt, cons
   depth_moments_kernel<<<dim3(slabs, b), kMetricThreads, 0, stream>>>(pred, gt, mask, mask_dtype, hw, disp, min_depth,
                                                                       max_depth, part);
   count_launch();
-  slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 6, mom);
+  slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 6, 0u, 0u, mom);
   count_launch();
   depth_error_kernel<<<dim3(slabs, b), kMetricThreads, 0, stream>>>(pred, gt, mask, mask_dtype, hw, disp, min_depth,
                                                                     max_depth, mom, part);
   count_launch();
-  slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 7, err);
+  slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 7, 0u, 0u, err);
   count_launch();
   depth_fold_kernel<<<1, 32, 0, stream>>>(mom, err, b, records, state_sums,
                                           reinterpret_cast<long long*>(state_counts));
@@ -355,7 +373,7 @@ extern "C" int odb_normal_metrics_update(const float* pred, const float* gt, con
   normal_angle_kernel<<<dim3(slabs, b), kMetricThreads, 0, stream>>>(pred, gt, mask, mask_dtype, (long long)h * w,
                                                                      part, reinterpret_cast<unsigned long long*>(hist));
   count_launch();
-  slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 7, img);
+  slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 7, 0u, 0u, img);
   count_launch();
   normal_fold_kernel<<<1, 32, 0, stream>>>(img, b, state_sums, reinterpret_cast<long long*>(state_counts));
   count_launch();

@@ -26,6 +26,31 @@ ODB_DEVINL double block_sum_d(double v, double* scratch /* [32] shared */) {
   }
   return r;
 }
+// block minimum / maximum (result valid in thread 0); exact, so the order does not matter
+template <bool kMin>
+ODB_DEVINL double block_extreme_d(double v, double* scratch /* [32] shared */) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double u = __shfl_down_sync(0xffffffffu, v, o);
+    v = kMin ? fmin(v, u) : fmax(v, u);
+  }
+  __syncthreads();
+  if (lane == 0) scratch[warp] = v;
+  __syncthreads();
+  double r = v;
+  if (warp == 0) {
+    r = lane < (int)(blockDim.x >> 5) ? scratch[lane] : (kMin ? INFINITY : -INFINITY);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const double u = __shfl_down_sync(0xffffffffu, r, o);
+      r = kMin ? fmin(r, u) : fmax(r, u);
+    }
+  }
+  return r;
+}
+ODB_DEVINL double block_min_d(double v, double* scratch) { return block_extreme_d<true>(v, scratch); }
+ODB_DEVINL double block_max_d(double v, double* scratch) { return block_extreme_d<false>(v, scratch); }
 ODB_DEVINL uint32_t sortable_key(float x) {
   const uint32_t u = __float_as_uint(x);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);

@@ -12,6 +12,10 @@
 - NormalMetrics: the angle between predicted and true normals, pooled over every valid pixel of the dataset: mean,
   median (to 2^-13 degree, from a dataset-wide histogram), RMSE and the percentages within 11.25, 22.5 and 30 degrees
   (the published OASIS surface-normal metrics, without the relative-normal AUC).
+- BoundaryMetrics: the depth-boundary errors (DBE) of iBims-1: edges are detected in the prediction (and, unless given,
+  in the ground truth) with a masked Canny detector; accuracy is the mean distance in pixels from predicted edges to
+  true ones (those within max_dist), completeness the mean distance from true edges to predicted ones.  Csrc:
+  boundary.cu.
 
 Definitions: DESIGN.md §3 "Evaluation metrics" and include/omnidata_b200.h; oracle/metrics_oracle.py restates them in
 float64.  The state lives in fixed device tensors.  `update` neither synchronises the host nor allocates after its first
@@ -31,6 +35,7 @@ from .losses import _StepBuffers
 DEPTH_KEYS = ("abs_rel", "sq_rel", "rmse", "rmse_log", "delta1", "delta2", "delta3")
 DEPTH_COUNTS = ("images", "excluded", "degenerate", "pixels")
 NORMAL_COUNTS = ("pixels", "nonfinite", "n_11.25", "n_22.5", "n_30")
+BOUNDARY_COUNTS = ("images", "no_gt_edges", "no_pred_edges", "pred_edge_pixels", "gt_edge_pixels")
 
 
 class _Metrics(_StepBuffers):
@@ -158,4 +163,74 @@ class NormalMetrics(_Metrics):
             out[k] = 100.0 * c / n if n else math.nan
         out["median_bin"] = int(med[0])
         out.update(zip(NORMAL_COUNTS, counts))
+        return out
+
+
+class BoundaryMetrics(_Metrics):
+    """Depth-boundary errors (module docstring; DESIGN.md §3 "Depth-boundary metrics").  sigma, low and high configure
+    the edge detector (Gaussian width in pixels, hysteresis thresholds on the Sobel magnitude of the depth normalised
+    to [0, 1] over the valid pixels); predicted edges at max_dist pixels or more from every true edge are left out of
+    the accuracy.  Valid pixels as in DepthMetrics: mask != 0 and a finite depth in (min_depth, max_depth]."""
+
+    _STATE = {"sums": ((2,), torch.float64), "counts": ((5,), torch.int64)}
+
+    def __init__(self, sigma: float = math.sqrt(2.0), low: float = 0.1, high: float = 0.2, max_dist: float = 10.0,
+                 min_depth: float = 1e-3, max_depth: Optional[float] = None):
+        super().__init__()
+        sigma, low, high, max_dist = float(sigma), float(low), float(high), float(max_dist)
+        min_depth = float(min_depth)
+        max_depth = math.inf if max_depth is None else float(max_depth)
+        if not (0.0 < sigma <= 4.0):
+            raise ValueError(f"sigma must lie in (0, 4], got {sigma}")
+        if not (math.isfinite(low) and math.isfinite(high) and 0.0 <= low <= high):
+            raise ValueError(f"need finite 0 <= low <= high, got low={low}, high={high}")
+        if not (math.isfinite(max_dist) and max_dist > 0.0):
+            raise ValueError(f"max_dist must be finite and > 0, got {max_dist}")
+        if not (math.isfinite(min_depth) and min_depth >= 0.0) or not (max_depth > min_depth):
+            raise ValueError(f"need 0 <= min_depth < max_depth, got min_depth={min_depth}, max_depth={max_depth}")
+        self.sigma, self.low, self.high, self.max_dist = sigma, low, high, max_dist
+        self.min_depth, self.max_depth = min_depth, max_depth
+
+    def _workspace(self, b, h, w, device):
+        return self._buf("workspace", (-(-ops.boundary_workspace_bytes(b, h, w) // 8),), torch.float64, device)
+
+    @_capi.on_tensor_device
+    @torch.no_grad()
+    def update(self, pred: torch.Tensor, gt: torch.Tensor, mask: Optional[torch.Tensor] = None,
+               gt_edges: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Adds a batch: pred, gt fp32 [B,H,W] or [B,1,H,W]; mask None or uint8 / bool / fp32, nonzero = valid;
+        gt_edges None (detected in gt) or uint8 / bool [B,(1,)H,W], nonzero = edge.  Returns the batch's per-image
+        records fp64 [B, 8] (include/omnidata_b200.h odb_boundary_metrics_update), valid until the next update at this
+        shape."""
+        b, h, w, _, _ = ops.check_metric_inputs("BoundaryMetrics.update", pred, gt, mask, 1)
+        if gt_edges is not None:
+            ops._edge_map("BoundaryMetrics.update", gt_edges, b, h, w, "gt_edges")
+        st = self._state_on(pred.device)
+        ws = self._workspace(b, h, w, pred.device)
+        rec = self._buf("records", (b, _capi.BOUNDARY_RECORD), torch.float64, pred.device)
+        ops.boundary_metrics_update(pred, gt, mask, gt_edges, self.sigma, self.low, self.high, self.max_dist,
+                                    self.min_depth, self.max_depth, ws, rec, st["sums"], st["counts"])
+        return rec
+
+    @_capi.on_tensor_device
+    @torch.no_grad()
+    def edges(self, depth: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The detector's edge map uint8 [B,H,W] (1 = edge) of depth fp32 [B,(1,)H,W], valid pixels taken from depth
+        itself and the mask, for visualisation and tests.  A new tensor."""
+        b, h, w, _, _ = ops.check_metric_inputs("BoundaryMetrics.edges", depth, depth, mask, 1)
+        out = torch.empty(b, h, w, dtype=torch.uint8, device=depth.device)
+        ops.depth_edges(depth, mask, self.sigma, self.low, self.high, self.min_depth, self.max_depth,
+                        self._workspace(b, h, w, depth.device), out)
+        return out
+
+    def compute(self) -> dict:
+        """dbe_acc, dbe_comp: the means over the images with ground-truth edges of the per-image accuracy and
+        completeness in pixels (NaN before any such image), and the counts: images (all), no_gt_edges (excluded),
+        no_pred_edges (no predicted edge within max_dist: both errors max_dist), pred_edge_pixels, gt_edge_pixels."""
+        st = self._host_state()
+        counts = [int(c) for c in st["counts"].tolist()]
+        n = counts[0] - counts[1]
+        acc, comp = st["sums"].tolist()
+        out = {"dbe_acc": acc / n if n else math.nan, "dbe_comp": comp / n if n else math.nan}
+        out.update(zip(BOUNDARY_COUNTS, counts))
         return out

@@ -25,6 +25,7 @@ __all__ = [
     "metrics_workspace_bytes", "depth_metrics_update", "normal_metrics_update", "normal_metrics_median",
     "ensemble_gram_workspace_bytes", "ensemble_gram", "ensemble_align_solve", "ensemble_merge_depth",
     "ensemble_merge_normal", "guided_workspace_bytes", "guided_coefficients", "guided_apply",
+    "boundary_workspace_bytes", "depth_edges", "edge_hysteresis", "edge_distance2", "boundary_metrics_update",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -698,6 +699,101 @@ def normal_metrics_median(hist, out):
     _need_shape(out, (2,), torch.float64, "out")
     _call("odb_normal_metrics_median", {}, lib().odb_normal_metrics_median, _same_device(hist, out), hist.data_ptr(),
           out.data_ptr())
+
+
+# ---------------------------------------------------------------- depth-boundary errors (csrc/boundary.cu)
+def boundary_workspace_bytes(b: int, h: int, w: int) -> int:
+    n = int(lib().odb_boundary_workspace_bytes(b, h, w))
+    if n < 0:
+        raise _capi.OdbError(f"boundary workspace: batch and image size must lie in [1, 65535], got {b}x{h}x{w}")
+    return n
+
+
+def check_edge_params(name: str, sigma: float, low: float, high: float, min_depth: float, max_depth: float):
+    """OdbError unless 0 < sigma <= 4, low and high are finite with 0 <= low <= high, and 0 <= min_depth < max_depth
+    (max_depth = inf: none)."""
+    if not (0.0 < sigma <= 4.0):
+        raise _capi.OdbError(f"{name}: sigma must lie in (0, 4], got {sigma}")
+    if not (math.isfinite(low) and math.isfinite(high) and 0.0 <= low <= high):
+        raise _capi.OdbError(f"{name}: need finite 0 <= low <= high, got low={low}, high={high}")
+    if not (math.isfinite(min_depth) and 0.0 <= min_depth < max_depth):
+        raise _capi.OdbError(f"{name}: need 0 <= min_depth < max_depth, got {min_depth}, {max_depth}")
+
+
+def _edge_map(name: str, t: torch.Tensor, b: int, h: int, w: int, what: str):
+    """Checks a uint8 / bool [B,H,W] or [B,1,H,W] map for b x h x w planes."""
+    if not t.is_cuda:
+        raise _capi.OdbError(f"{name}: {what} must live on a CUDA device (no CPU path exists)")
+    if t.dtype not in (torch.uint8, torch.bool):
+        raise _capi.OdbError(f"{name}: {what} must be uint8 or bool, got {t.dtype}")
+    if tuple(t.shape) not in ((b, h, w), (b, 1, h, w)) or not t.is_contiguous():
+        raise _capi.OdbError(f"{name}: {what} must be a contiguous [B,H,W] or [B,1,H,W] tensor for {b}x{h}x{w}, "
+                             f"got {tuple(t.shape)}")
+
+
+def depth_edges(depth, mask, sigma: float, low: float, high: float, min_depth: float, max_depth: float, workspace,
+                edges):
+    """edges uint8 [B,H,W] = the edge map E(depth, V) of depth fp32 [B,(1,)H,W], V from depth itself and the mask
+    (include/omnidata_b200.h odb_depth_edges).  workspace: fp64, boundary_workspace_bytes of them."""
+    b, h, w, mptr, mkind = check_metric_inputs("depth_edges", depth, depth, mask, 1)
+    check_edge_params("depth_edges", sigma, low, high, min_depth, max_depth)
+    _check_workspace("depth_edges", workspace, boundary_workspace_bytes(b, h, w))
+    _need_shape(edges, (b, h, w), torch.uint8, "edges")
+    _call("odb_depth_edges", {"bytes": 4 * b * h * w}, lib().odb_depth_edges,
+          _same_device(depth, mask, workspace, edges), depth.data_ptr(), mptr, mkind, b, h, w, float(sigma),
+          float(low), float(high), float(min_depth), float(max_depth), workspace.data_ptr(), edges.data_ptr())
+
+
+def edge_hysteresis(weak_strong, workspace, edges):
+    """edges uint8 [B,H,W] = the weak pixels of weak_strong uint8 [B,H,W] (bit 0 weak, bit 1 strong) whose 8-connected
+    weak component holds a strong pixel (odb_edge_hysteresis)."""
+    _need(weak_strong, torch.uint8, "weak_strong")
+    if weak_strong.dim() != 3:
+        raise _capi.OdbError(f"edge_hysteresis: weak_strong must be [B,H,W], got {tuple(weak_strong.shape)}")
+    b, h, w = weak_strong.shape
+    _check_planes("edge_hysteresis", b, h, w)
+    _edge_map("edge_hysteresis", weak_strong, b, h, w, "weak_strong")
+    _check_workspace("edge_hysteresis", workspace, boundary_workspace_bytes(b, h, w))
+    _need_shape(edges, (b, h, w), torch.uint8, "edges")
+    _call("odb_edge_hysteresis", {"bytes": 2 * b * h * w}, lib().odb_edge_hysteresis,
+          _same_device(weak_strong, workspace, edges), weak_strong.data_ptr(), b, h, w, workspace.data_ptr(),
+          edges.data_ptr())
+
+
+def edge_distance2(edges, workspace, dist2):
+    """dist2 int64 [B,H,W] = the exact squared Euclidean distance to the nearest nonzero pixel of edges uint8 / bool
+    [B,H,W]; -1 (all bits set) throughout an image without one (odb_edge_distance2)."""
+    if edges.dim() != 3:
+        raise _capi.OdbError(f"edge_distance2: edges must be [B,H,W], got {tuple(edges.shape)}")
+    b, h, w = edges.shape
+    _check_planes("edge_distance2", b, h, w)
+    _edge_map("edge_distance2", edges, b, h, w, "edges")
+    _check_workspace("edge_distance2", workspace, boundary_workspace_bytes(b, h, w))
+    _need_shape(dist2, (b, h, w), torch.int64, "dist2")
+    _call("odb_edge_distance2", {"bytes": 9 * b * h * w}, lib().odb_edge_distance2,
+          _same_device(edges, workspace, dist2), edges.data_ptr(), b, h, w, workspace.data_ptr(), dist2.data_ptr())
+
+
+def boundary_metrics_update(pred, gt, mask, gt_edges, sigma: float, low: float, high: float, max_dist: float,
+                            min_depth: float, max_depth: float, workspace, records, sums, counts):
+    """Adds the depth-boundary errors of pred / gt fp32 [B,(1,)H,W] (mask as for depth_metrics_update; gt_edges None
+    or uint8 / bool [B,(1,)H,W], nonzero = edge) to the state sums fp64 [2], counts int64 [5]; records fp64
+    [B, BOUNDARY_RECORD] receives the per-image results (include/omnidata_b200.h odb_boundary_metrics_update)."""
+    b, h, w, mptr, mkind = check_metric_inputs("boundary_metrics_update", pred, gt, mask, 1)
+    if gt_edges is not None:
+        _edge_map("boundary_metrics_update", gt_edges, b, h, w, "gt_edges")
+    check_edge_params("boundary_metrics_update", sigma, low, high, min_depth, max_depth)
+    if not (math.isfinite(max_dist) and max_dist > 0.0):
+        raise _capi.OdbError(f"boundary_metrics_update: max_dist must be finite and > 0, got {max_dist}")
+    _check_workspace("boundary_metrics_update", workspace, boundary_workspace_bytes(b, h, w))
+    _need_shape(records, (b, _capi.BOUNDARY_RECORD), torch.float64, "records")
+    _need_shape(sums, (2,), torch.float64, "sums")
+    _need_shape(counts, (5,), torch.int64, "counts")
+    _call("odb_boundary_metrics_update", {"bytes": 2 * 4 * b * h * w}, lib().odb_boundary_metrics_update,
+          _same_device(pred, gt, mask, gt_edges, workspace, records, sums, counts), pred.data_ptr(), gt.data_ptr(),
+          mptr, mkind, _ptr(gt_edges), b, h, w, float(sigma), float(low), float(high), float(max_dist),
+          float(min_depth), float(max_depth), workspace.data_ptr(), records.data_ptr(), sums.data_ptr(),
+          counts.data_ptr())
 
 
 # ---------------------------------------------------------------- test-time ensembles (csrc/ensemble.cu)
