@@ -7,6 +7,8 @@
                        [--guided_size HxW [--radius R] [--eps E]] [--ensemble_sizes HxW,... --flip]
                        [--space {depth,disparity}] [--min_depth] [--max_depth] [--depth_scale] [--depth_invalid]
                        [--boundary [--edge_path DIR]]
+                       [--sparse_points N [--sparse_seed S] | --sparse_path DIR] [--sparse_grid GYxGX]
+                       [--sparse_smooth L] [--huber D [--huber_iterations K]]
 
 Images (PNG / JPEG) are matched to ground truth, and to masks, by file stem.  Preprocessing is that of
 `demo.py --full_res` (RGB in [0, 1]; depth normalised to [-1, 1]).  `--mode tiled` predicts at the image's own size with
@@ -24,14 +26,24 @@ depth = value / --depth_scale with --depth_invalid marking no depth (defaults 51
 starter dataset's depth_zbuffer files; check them against a real file before relying on them); normals as an 8-bit RGB
 PNG / 255.  Masks: 8-bit PNG or `.npy`, nonzero = valid.  `--boundary` (depth) adds the depth-boundary errors
 (`BoundaryMetrics`, under the `boundary` key) against ground-truth edge maps from `--edge_path` (8-bit PNG or `.npy`,
-nonzero = edge, matched by file stem) or, without it, edges detected in the ground-truth depth.  Prints one JSON line: the metrics (omnidata_b200.metrics),
-the mode, precision, tile settings and the number of images.  Runs on cuda:0; there is no CPU path.
+nonzero = edge, matched by file stem) or, without it, edges detected in the ground-truth depth.  `--sparse_points N` or
+`--sparse_path DIR` (depth) also scores metric depth: the evaluated prediction is aligned in `--space` to sparse
+depths (`SparseDepthAligner`, grid `--sparse_grid`, smoothing `--sparse_smooth`, Huber IRLS with `--huber`) and scored
+without a further fit (`DepthMetrics(align=False)`), under the `sparse` key.  The sparse depths are N valid
+ground-truth pixels per image, drawn without replacement by numpy `default_rng([--sparse_seed, crc32(stem)])` (all of
+them when fewer are valid; 200 is the sparse-to-dense protocol of Ma & Karaman on NYUv2), or read from DIR by file
+stem: a 16-bit PNG under --depth_scale / --depth_invalid (0 is also no measurement) or a float `.npy` in metres (0 /
+NaN: none).  Prints one JSON
+line: the metrics (omnidata_b200.metrics), the mode, precision, tile settings and the number of images.  Runs on cuda:0;
+there is no CPU path.
 """
 from __future__ import annotations
 
 import argparse
 import json
+import math
 import sys
+import zlib
 from pathlib import Path
 
 import numpy as np
@@ -75,6 +87,33 @@ def load_mask(path: Path) -> np.ndarray:
 def load_edges(path: Path) -> np.ndarray:
     """uint8 [H,W], 1 = edge, from an 8-bit PNG or a `.npy` (nonzero = edge)."""
     return load_mask(path)
+
+
+def load_sparse(path: Path, depth_scale: float, depth_invalid: int) -> np.ndarray:
+    """float32 [H,W] sparse depth in metres, 0 where there is no measurement."""
+    if path.suffix == ".npy":
+        a = np.load(path).astype(np.float32)
+        a = a.reshape(a.shape[-2:]) if a.ndim == 3 and a.shape[0] == 1 else a
+        return np.where(np.isfinite(a), a, 0.0).astype(np.float32)
+    v = np.asarray(Image.open(path)).astype(np.int64)
+    return np.where((v == depth_invalid) | (v == 0), 0.0, v / depth_scale).astype(np.float32)
+
+
+def sample_sparse(gt: np.ndarray, n: int, seed: int, stem: str, min_depth: float, max_depth: float,
+                  mask: np.ndarray = None) -> np.ndarray:
+    """float32 [H,W]: n of gt's valid pixels (DepthMetrics' rule: mask != 0, finite, in (min_depth, max_depth]), drawn
+    without replacement by default_rng([seed, crc32(stem)]) from the valid pixels in row-major order (all of them when
+    fewer are valid); 0 elsewhere."""
+    with np.errstate(invalid="ignore"):
+        valid = np.isfinite(gt) & (gt > min_depth) & (gt <= max_depth)
+    if mask is not None:
+        valid &= mask != 0
+    idx = np.flatnonzero(valid)
+    if idx.size > n:
+        idx = np.sort(np.random.default_rng([seed, zlib.crc32(stem.encode())]).choice(idx, n, replace=False))
+    out = np.zeros(gt.size, np.float32)
+    out[idx] = gt.reshape(-1)[idx]
+    return out.reshape(gt.shape)
 
 
 def build_model(task: str, backbone: str, checkpoint, synthetic: bool, precision: str, device):
@@ -149,6 +188,14 @@ def evaluate(args) -> dict:
     else:
         metric = NormalMetrics()
     boundary = BoundaryMetrics(min_depth=args.min_depth, max_depth=args.max_depth) if args.boundary else None
+    sparse_on = args.sparse_points is not None or args.sparse_path is not None
+    if sparse_on:
+        from omnidata_b200.sparse import SparseDepthAligner
+        aligner = SparseDepthAligner(space=args.space, grid=args.sparse_grid, smooth=args.sparse_smooth,
+                                     robust=args.huber, iterations=args.huber_iterations, min_depth=args.min_depth,
+                                     max_depth=args.max_depth)
+        sparse_metric = DepthMetrics(min_depth=args.min_depth, max_depth=args.max_depth, align=False)
+        sparse_records = []
     tile = (args.tile, args.tile)
     guided = (args.guided_size, args.radius, args.eps) if args.mode == "guided" else None
     if guided is not None:                          # a refused size or setting fails here, before the first image
@@ -175,6 +222,19 @@ def evaluate(args) -> dict:
                     raise ValueError(f"{p.name}: the edge map is {edges.shape[-2]}x{edges.shape[-1]}, the ground "
                                      f"truth {gt.shape[-2]}x{gt.shape[-1]}")
             boundary.update(pred, gt_t, mask, edges)
+        if sparse_on:
+            if args.sparse_path:
+                sp = load_sparse(_find(args.sparse_path, p.stem, "sparse depth"), args.depth_scale, args.depth_invalid)
+                if tuple(sp.shape) != tuple(gt.shape):
+                    raise ValueError(f"{p.name}: the sparse depth is {sp.shape[0]}x{sp.shape[1]}, the ground truth "
+                                     f"{gt.shape[0]}x{gt.shape[1]}")
+            else:
+                sp = sample_sparse(gt, args.sparse_points, args.sparse_seed, p.stem, args.min_depth,
+                                   math.inf if args.max_depth is None else args.max_depth,
+                                   None if mask is None else mask[0].cpu().numpy())
+            nodes, rec = aligner.fit(pred, torch.from_numpy(sp).unsqueeze(0).to(device))
+            sparse_records.append(rec.clone())
+            sparse_metric.update(aligner.apply(pred, nodes), gt_t, mask)
     result = {"task": args.task, "backbone": args.backbone, "mode": args.mode, "precision": args.precision,
               "tile": list(tile) if args.mode == "tiled" else None,
               "overlap": args.overlap if args.mode == "tiled" else None,
@@ -188,6 +248,18 @@ def evaluate(args) -> dict:
     result["metrics"] = metric.compute()
     if boundary is not None:
         result["boundary"] = dict(boundary.compute(), edges="given" if args.edge_path else "detected")
+    if sparse_on:
+        rec = torch.cat(sparse_records).cpu()
+        status = rec[:, 1].long()
+        result["sparse"] = {
+            "source": "path" if args.sparse_path else "points", "points": args.sparse_points,
+            "seed": args.sparse_seed if args.sparse_points is not None else None, "grid": list(args.sparse_grid),
+            "smooth": args.sparse_smooth, "huber": args.huber,
+            "huber_iterations": aligner.iterations if args.huber is not None else None,
+            "metrics": sparse_metric.compute(),
+            "records": {"ok": int((status == 0).sum()), "no_points": int((status == 1).sum()),
+                        "degenerate": int((status == 2).sum()), "nonfinite": int((status == 3).sum()),
+                        "mean_points": float(rec[:, 0].mean())}}
     return result
 
 
@@ -241,7 +313,48 @@ def parse_args(argv=None):
     ap.add_argument("--edge_path", default=None, metavar="DIR",
                     help="--boundary: ground-truth edge maps (8-bit PNG or .npy, nonzero = edge) matched by file "
                          "stem; without it, edges are detected in the ground-truth depth")
+    ap.add_argument("--sparse_points", type=int, default=None, metavar="N",
+                    help="depth: also score metric depth aligned to N ground-truth samples per image (`sparse` key)")
+    ap.add_argument("--sparse_path", default=None, metavar="DIR",
+                    help="depth: also score metric depth aligned to sparse depths read from DIR by file stem "
+                         "(16-bit PNG or .npy in metres)")
+    ap.add_argument("--sparse_seed", type=int, default=None, help="--sparse_points: sampler seed (default 0)")
+    ap.add_argument("--sparse_grid", type=_size, default=None, metavar="GYxGX",
+                    help="sparse alignment: scale / shift node grid (default 1x1: one global fit)")
+    ap.add_argument("--sparse_smooth", type=float, default=None,
+                    help="sparse alignment: smoothness between neighbouring nodes (default 0.1, untuned)")
+    ap.add_argument("--huber", type=float, default=None, metavar="D",
+                    help="sparse alignment: Huber IRLS threshold on the relative residual (default: plain least "
+                         "squares)")
+    ap.add_argument("--huber_iterations", type=int, default=None,
+                    help="--huber: number of reweighted solves in [2, 32] (default 5)")
     args = ap.parse_args(argv)
+    sparse_on = args.sparse_points is not None or args.sparse_path is not None
+    if args.sparse_points is not None and args.sparse_path is not None:
+        ap.error("give one of --sparse_points and --sparse_path")
+    if sparse_on and args.task != "depth":
+        ap.error("--sparse_points / --sparse_path apply to --task depth only")
+    if not sparse_on and any(v is not None for v in (args.sparse_grid, args.sparse_smooth, args.huber,
+                                                     args.huber_iterations, args.sparse_seed)):
+        ap.error("--sparse_grid, --sparse_smooth, --huber, --huber_iterations and --sparse_seed apply with "
+                 "--sparse_points or --sparse_path only")
+    if args.sparse_seed is not None and args.sparse_points is None:
+        ap.error("--sparse_seed applies with --sparse_points only")
+    if args.sparse_points is not None and args.sparse_points < 1:
+        ap.error("--sparse_points must be at least 1")
+    if args.huber_iterations is not None and args.huber is None:
+        ap.error("--huber_iterations applies with --huber only")
+    if sparse_on:
+        args.sparse_grid = (1, 1) if args.sparse_grid is None else args.sparse_grid
+        args.sparse_smooth = 0.1 if args.sparse_smooth is None else args.sparse_smooth
+        if args.sparse_points is not None:
+            args.sparse_seed = 0 if args.sparse_seed is None else args.sparse_seed
+        from omnidata_b200.sparse import SparseDepthAligner
+        try:
+            SparseDepthAligner(space=args.space, grid=args.sparse_grid, smooth=args.sparse_smooth, robust=args.huber,
+                               iterations=args.huber_iterations, min_depth=args.min_depth, max_depth=args.max_depth)
+        except ValueError as e:
+            ap.error(f"sparse alignment: {e}")
     if args.boundary and args.task != "depth":
         ap.error("--boundary applies to --task depth only")
     if args.edge_path is not None and not args.boundary:

@@ -609,6 +609,55 @@ int odb_normal_metrics_update(const float* pred, const float* gt, const void* ma
                               int32_t h, int32_t w, void* workspace, double* state_sums, int64_t* state_counts,
                               int64_t* hist, void* stream);
 int odb_normal_metrics_median(const int64_t* hist, double* out, void* stream);
+/* odb_depth_metrics_update_metric: odb_depth_metrics_update in depth space without the fit, for predictions that are
+ * already metric (a sparse alignment's output): dh = clamp(pred, min_depth, max_depth), and the records hold s = 1,
+ * t = 0, det <= 0 never.  Five launches. */
+int odb_depth_metrics_update_metric(const float* pred, const float* gt, const void* mask, int32_t mask_dtype,
+                                    int32_t b, int32_t h, int32_t w, double min_depth, double max_depth,
+                                    void* workspace, double* records, double* state_sums, int64_t* state_counts,
+                                    void* stream);
+
+/* ---- sparse metric alignment (omnidata_b200/sparse.py SparseDepthAligner) -----------------------------------------
+ *
+ * No reference counterpart.  Maps an affine-invariant depth prediction to metres with scale and shift fields fitted to
+ * sparse measured depths (LiDAR returns, SfM points).  Definitions in DESIGN.md §3 "Sparse metric alignment";
+ * oracle/sparse_oracle.py restates them in float64.  pred, sparse fp32 [b][h][w] (sparse in metres, 0 / NaN = none);
+ * mask as for the metrics above; b, h, w <= 65535.  Points V = {mask != 0, sparse finite, min_depth < sparse <=
+ * max_depth}, y = sparse (ODB_SPACE_DEPTH) or 1 / sparse (ODB_SPACE_DISPARITY, max_depth finite); max_depth = +inf:
+ * none, 0 <= min_depth < max_depth.
+ *
+ * Fields: nodes fp64 [b][grid_y][grid_x][2] = (s_i, t_i), 1 <= grid_y <= h, 1 <= grid_x <= w, grid_y grid_x <=
+ * ODB_SPARSE_MAX_NODES.  S(p), T(p) = the bilinear resize of the node maps to h x w (align_corners=False, no
+ * antialiasing): u = ((x + 0.5) grid_x) / w - 0.5 clamped to [0, grid_x - 1], likewise along y, in fp64 round-to-nearest
+ * operations.  z_p = S(p) a_p + T(p).  The fit minimises
+ *   E = S_V w_p (z_p - y_p)^2 + smooth (n / n_e) S_{i~j} mean_V((s_i - s_j) a_p + (t_i - t_j))^2
+ * over the n_e 4-neighbour node edges (n = |V|; smooth finite >= 0, > 0 when there is more than one node).
+ * robust = 0: one solve with w = 1 (iterations = 1).  robust = delta > 0: `iterations` in [2, 32] solves, the first with
+ * w = 1, each later one with w_p = min(1, delta / |r_p|), r_p = (z_p - y_p) / y_p of the previous solve (Huber IRLS).
+ * The normal equations (half-bandwidth 2 grid_x + 3) are solved in fp64 by a banded Cholesky factorisation.
+ * records fp64 [b][ODB_SPARSE_RECORD] = (n, status, RMS of r over V for the final nodes, fraction of V with w < 1 in
+ * the last solve, 0, 0, 0, 0); status 0 ok, 1 n < 2, 2 degenerate (S w a^2 S w - (S w a)^2 <= 0: all a equal on V),
+ * 3 a non-finite prediction on V; for status != 0 the nodes and the residual are NaN.
+ *
+ * odb_sparse_align_fit: workspace odb_sparse_align_workspace_bytes(b, h, w, grid_y, grid_x) bytes, 8-byte aligned
+ * (negative: refused).  3 (iterations + 1) launches.
+ * odb_sparse_align_apply: out fp32 [b][h][w] = clamp(z, min_depth, max_depth) (depth space) or clamp(1 / max(z,
+ * 1 / max_depth), min_depth, max_depth) (disparity space), computed in fp64 (odb_depth_metrics_update's dh with s = S(p),
+ * t = T(p)) and rounded to fp32 once; NaN where a_p is not finite or the nodes are NaN.  S and T are not written to
+ * memory.  16-byte accesses where w % 4 == 0 and pred, out are 16-byte aligned.  One launch.
+ *
+ * No floating-point atomics and fixed partitions: results are bit-reproducible and independent of the batch.  Arguments
+ * are checked before any launch. */
+#define ODB_SPARSE_MAX_NODES 1024
+#define ODB_SPARSE_RECORD 8
+int64_t odb_sparse_align_workspace_bytes(int32_t b, int32_t h, int32_t w, int32_t grid_y, int32_t grid_x);
+int odb_sparse_align_fit(const float* pred, const float* sparse, const void* mask, int32_t mask_dtype, int32_t b,
+                         int32_t h, int32_t w, int32_t grid_y, int32_t grid_x, int32_t space, double min_depth,
+                         double max_depth, double smooth, double robust, int32_t iterations, void* workspace,
+                         double* nodes, double* records, void* stream);
+int odb_sparse_align_apply(const float* pred, const double* nodes, int32_t b, int32_t h, int32_t w, int32_t grid_y,
+                           int32_t grid_x, int32_t space, double min_depth, double max_depth, float* out,
+                           void* stream);
 
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *

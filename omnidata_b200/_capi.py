@@ -24,6 +24,8 @@ NORMAL_HIST_BINS = 180 * NORMAL_HIST_PER_DEGREE + 1
 ENSEMBLE_MAX_MEMBERS = 16                       # ODB_ENSEMBLE_MAX_MEMBERS
 GUIDED_MAX_RADIUS = 32                          # ODB_GUIDED_MAX_RADIUS
 BOUNDARY_RECORD = 8                             # ODB_BOUNDARY_RECORD
+SPARSE_MAX_NODES = 1024                         # ODB_SPARSE_MAX_NODES
+SPARSE_RECORD = 8                               # ODB_SPARSE_RECORD
 
 
 class OdbError(RuntimeError):
@@ -210,6 +212,8 @@ _SIGNATURES = {
     "odb_depth_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 5 + [C.c_double] * 2 + [C.c_void_p] * 5),
     "odb_normal_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_void_p] * 5),
     "odb_normal_metrics_median": (C.c_int, [C.c_void_p] * 3),
+    "odb_depth_metrics_update_metric": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_double] * 2 +
+                                        [C.c_void_p] * 5),
     "odb_ensemble_gram_workspace_bytes": (C.c_int64, [C.c_int32] * 4),
     "odb_ensemble_gram": (C.c_int, [C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3),
     "odb_ensemble_align_solve": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
@@ -225,6 +229,10 @@ _SIGNATURES = {
     "odb_edge_distance2": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 3),
     "odb_boundary_metrics_update": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] + [C.c_int32] * 3 +
                                     [C.c_double] * 6 + [C.c_void_p] * 5),
+    "odb_sparse_align_workspace_bytes": (C.c_int64, [C.c_int32] * 5),
+    "odb_sparse_align_fit": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 7 + [C.c_double] * 4 + [C.c_int32] +
+                             [C.c_void_p] * 4),
+    "odb_sparse_align_apply": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 6 + [C.c_double] * 2 + [C.c_void_p] * 2),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -1,12 +1,32 @@
-// fp64 routines shared by the post-processing kernels: the SPD band solve of the tiled and ensemble alignments
-// (tiled.cu, ensemble.cu) and the angle between two vectors of the normal metrics and the normal ensemble merge
-// (metrics.cu, ensemble.cu).  Callers are built without fast-math.
+// fp64 routines shared by the post-processing kernels: the SPD band solve of the tiled, ensemble and sparse alignments
+// (tiled.cu, ensemble.cu, sparse.cu), the angle between two vectors of the normal metrics and the normal ensemble merge
+// (metrics.cu, ensemble.cu), and the valid set and clamped depth of the depth metrics and the sparse alignment
+// (metrics.cu, sparse.cu).  Callers are built without fast-math.
 #pragma once
 #include "common.cuh"
+#include "../../include/omnidata_b200.h"
 
 namespace odb {
 
 constexpr double kRadToDeg = 180.0 / 3.141592653589793;
+constexpr size_t kBandSmemMax = 200 * 1024;      // band + right-hand side of a band solve in shared memory up to this
+
+ODB_DEVINL bool mask_valid(const void* mask, int kind, long long i) {
+  if (kind == ODB_MASK_U8) return static_cast<const uint8_t*>(mask)[i] != 0;
+  if (kind == ODB_MASK_F32) return static_cast<const float*>(mask)[i] != 0.0f;
+  return true;
+}
+
+ODB_DEVINL bool depth_valid(double g, double min_depth, double max_depth) {
+  return isfinite(g) && g > min_depth && g <= max_depth;           // max_depth = +inf when not given
+}
+
+// d-hat = clamp(s p + t, min, max) (depth space) or clamp(1 / max(s p + t, 1 / max), min, max) (disparity space)
+ODB_DEVINL double depth_hat(double p, double s, double t, int disparity, double min_depth, double max_depth) {
+  const double a = __dadd_rn(__dmul_rn(s, p), t);
+  const double d = disparity ? __drcp_rn(fmax(a, __drcp_rn(max_depth))) : a;
+  return fmin(fmax(d, min_depth), max_depth);
+}
 
 // Solves A x = rhs in place for A symmetric positive definite of order n with half-bandwidth w - 1 (w = n: dense).
 // The lower band is stored row-wise, band[r * w + q] = A[r][r - q] (entries with q > r are not read); it is

@@ -8,6 +8,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "../../include/omnidata_b200.h"
+
 namespace odb {
 
 int fail(int status, const char* msg);
@@ -29,6 +31,12 @@ inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<u
 // b images (a grid dimension) of h x w planes
 inline bool planes_ok(int32_t b, int32_t h, int32_t w) {
   return b >= 1 && b <= 65535 && h >= 1 && h <= 65535 && w >= 1 && w <= 65535;
+}
+// mask argument of the metrics and the sparse alignment: NULL with ODB_MASK_NONE, else uint8 or (4-byte aligned) fp32
+inline bool metric_mask_ok(const void* mask, int32_t kind) {
+  if (kind == ODB_MASK_NONE) return mask == nullptr;
+  if (kind == ODB_MASK_U8) return mask != nullptr;
+  return kind == ODB_MASK_F32 && mask != nullptr && aligned(mask, 4);
 }
 // The per-pixel reductions (metrics.cu, ensemble.cu) cut every image into fixed slabs of kSlab pixels, so the partition
 // depends on h x w only, never on the batch.

@@ -31,16 +31,6 @@ constexpr int kMetricThreads = 256;
 constexpr int kSlabIters = kSlab / kMetricThreads;
 constexpr int kMedianThreads = 1024;
 
-ODB_DEVINL bool mask_valid(const void* mask, int kind, long long i) {
-  if (kind == ODB_MASK_U8) return static_cast<const uint8_t*>(mask)[i] != 0;
-  if (kind == ODB_MASK_F32) return static_cast<const float*>(mask)[i] != 0.0f;
-  return true;
-}
-
-ODB_DEVINL bool depth_valid(double g, double min_depth, double max_depth) {
-  return isfinite(g) && g > min_depth && g <= max_depth;           // max_depth = +inf when not given
-}
-
 // Slab partials [b][slab][8] over V of the image: (n, Sp, Spp, Sy, Spy, non-finite predictions), y = g (depth space) or
 // 1 / g (disparity space).  grid (slabs, b)
 __global__ void __launch_bounds__(kMetricThreads) depth_moments_kernel(const float* __restrict__ pred,
@@ -111,26 +101,20 @@ ODB_DEVINL void depth_scale_shift(const double* m, double& s, double& t) {
   }
 }
 
-// d-hat = clamp(s p + t, min, max) (depth space) or clamp(1 / max(s p + t, 1 / max), min, max) (disparity space)
-ODB_DEVINL double depth_hat(double p, double s, double t, int disparity, double min_depth, double max_depth) {
-  const double a = __dadd_rn(__dmul_rn(s, p), t);
-  const double d = disparity ? __drcp_rn(fmax(a, __drcp_rn(max_depth))) : a;
-  return fmin(fmax(d, min_depth), max_depth);
-}
-
 // Slab partials [b][slab][8] over V: (S|e|/g, Se^2/g, Se^2, S(ln dh - ln g)^2, #(r < 1.25), #(r < 1.25^2),
-// #(r < 1.25^3)), e = dh - g, r = max(dh / g, g / dh); each CTA solves its image's (s, t) from mom.  grid (slabs, b)
+// #(r < 1.25^3)), e = dh - g, r = max(dh / g, g / dh); each CTA solves its image's (s, t) from mom, or takes (1, 0)
+// without `align` (a metric prediction, depth space).  grid (slabs, b)
 __global__ void __launch_bounds__(kMetricThreads) depth_error_kernel(const float* __restrict__ pred,
                                                                      const float* __restrict__ gt, const void* mask,
                                                                      int mask_kind, long long hw, int disparity,
                                                                      double min_depth, double max_depth,
-                                                                     const double* __restrict__ mom,
+                                                                     const double* __restrict__ mom, int align,
                                                                      double* __restrict__ part) {
   __shared__ double scratch[32];
   const int b = blockIdx.y;
   const long long base = (long long)b * hw;
-  double s, t;
-  depth_scale_shift(mom + (long long)b * kPartStride, s, t);
+  double s = 1.0, t = 0.0;
+  if (align) depth_scale_shift(mom + (long long)b * kPartStride, s, t);
   double acc[7] = {0, 0, 0, 0, 0, 0, 0};
   for (int k = 0; k < kSlabIters; ++k) {
     const long long i = blockIdx.x * kSlab + k * kMetricThreads + threadIdx.x;
@@ -158,10 +142,11 @@ __global__ void __launch_bounds__(kMetricThreads) depth_error_kernel(const float
 }
 
 // One thread, images in order: records[b][12] = (n, AbsRel, SqRel, RMSE, RMSE_log, #delta1, #delta2, #delta3, s, t,
-// det <= 0, non-finite predictions); the state adds each image with n > 0:
+// det <= 0, non-finite predictions) (s = 1, t = 0 and never det <= 0 without `align`); the state adds each image with
+// n > 0:
 // sums[7] += (AbsRel, SqRel, RMSE, RMSE_log, delta1, delta2, delta3), counts[4] += (images, excluded, det <= 0, pixels).
 // A non-finite prediction on a valid pixel makes the image's metrics NaN.
-__global__ void depth_fold_kernel(const double* __restrict__ mom, const double* __restrict__ err, int b_n,
+__global__ void depth_fold_kernel(const double* __restrict__ mom, const double* __restrict__ err, int b_n, int align,
                                   double* __restrict__ records, double* __restrict__ sums,
                                   long long* __restrict__ counts) {
   if (threadIdx.x != 0) return;
@@ -170,9 +155,9 @@ __global__ void depth_fold_kernel(const double* __restrict__ mom, const double* 
     const double* e = err + (long long)b * kPartStride;
     double* r = records + (long long)b * ODB_DEPTH_RECORD;
     const double n = m[0];
-    double s, t;
-    depth_scale_shift(m, s, t);
-    const bool degenerate = n > 0.0 && m[2] * m[0] - m[1] * m[1] <= 0.0;
+    double s = 1.0, t = 0.0;
+    if (align) depth_scale_shift(m, s, t);
+    const bool degenerate = align && n > 0.0 && m[2] * m[0] - m[1] * m[1] <= 0.0;
     const double bad = m[5] > 0.0 ? NAN : 0.0;                      // NaN + x = NaN, 0 + x = x
     const double v[7] = {e[0] / n + bad, e[1] / n + bad, sqrt(e[2] / n) + bad, sqrt(e[3] / n) + bad,
                          e[4] / n + bad, e[5] / n + bad, e[6] / n + bad};
@@ -304,12 +289,6 @@ __global__ void __launch_bounds__(kMedianThreads) normal_median_kernel(const uns
   }
 }
 
-static bool mask_ok(const void* mask, int32_t kind) {
-  if (kind == ODB_MASK_NONE) return mask == nullptr;
-  if (kind == ODB_MASK_U8) return mask != nullptr;
-  return kind == ODB_MASK_F32 && mask != nullptr && aligned(mask, 4);
-}
-
 void launch_slab_reduce(const double* part, int images, int slabs, int nq, unsigned min_mask, unsigned max_mask,
                         double* out, cudaStream_t stream) {
   slab_reduce_kernel<<<images, kMetricThreads, 0, stream>>>(part, slabs, nq, min_mask, max_mask, out);
@@ -325,18 +304,17 @@ extern "C" int64_t odb_metrics_workspace_bytes(int32_t b, int32_t h, int32_t w) 
   return ((int64_t)b * slab_count(h, w) + 2 * (int64_t)b) * kPartStride * (int64_t)sizeof(double);
 }
 
-extern "C" int odb_depth_metrics_update(const float* pred, const float* gt, const void* mask, int32_t mask_dtype,
-                                        int32_t b, int32_t h, int32_t w, int32_t space, double min_depth,
-                                        double max_depth, void* workspace, double* records, double* state_sums,
-                                        int64_t* state_counts, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+static int depth_update(const char* name, const char* bad_argument, const float* pred, const float* gt,
+                        const void* mask, int32_t mask_dtype, int32_t b, int32_t h, int32_t w, int32_t space,
+                        int align, double min_depth, double max_depth, void* workspace, double* records,
+                        double* state_sums, int64_t* state_counts, cudaStream_t stream) {
   const bool disparity = space == ODB_SPACE_DISPARITY;
   if (!pred || !gt || !workspace || !records || !state_sums || !state_counts || !planes_ok(b, h, w) ||
-      !mask_ok(mask, mask_dtype) || !aligned(pred, 4) || !aligned(gt, 4) || !aligned(workspace, 8) ||
+      !metric_mask_ok(mask, mask_dtype) || !aligned(pred, 4) || !aligned(gt, 4) || !aligned(workspace, 8) ||
       !aligned(records, 8) || !aligned(state_sums, 8) || !aligned(state_counts, 8) ||
       (space != ODB_SPACE_DEPTH && !disparity) || !std::isfinite(min_depth) || min_depth < 0.0 ||
       std::isnan(max_depth) || !(max_depth > min_depth) || (disparity && !std::isfinite(max_depth)))
-    return fail(ODB_ERR_INVALID, "depth_metrics_update: bad argument");
+    return fail(ODB_ERR_INVALID, bad_argument);
   const int slabs = slab_count(h, w);
   const long long hw = (long long)h * w;
   double* part = static_cast<double*>(workspace);
@@ -349,14 +327,32 @@ extern "C" int odb_depth_metrics_update(const float* pred, const float* gt, cons
   slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 6, 0u, 0u, mom);
   count_launch();
   depth_error_kernel<<<dim3(slabs, b), kMetricThreads, 0, stream>>>(pred, gt, mask, mask_dtype, hw, disp, min_depth,
-                                                                    max_depth, mom, part);
+                                                                    max_depth, mom, align, part);
   count_launch();
   slab_reduce_kernel<<<b, kMetricThreads, 0, stream>>>(part, slabs, 7, 0u, 0u, err);
   count_launch();
-  depth_fold_kernel<<<1, 32, 0, stream>>>(mom, err, b, records, state_sums,
+  depth_fold_kernel<<<1, 32, 0, stream>>>(mom, err, b, align, records, state_sums,
                                           reinterpret_cast<long long*>(state_counts));
   count_launch();
-  return check_launch("depth_metrics_update");
+  return check_launch(name);
+}
+
+extern "C" int odb_depth_metrics_update(const float* pred, const float* gt, const void* mask, int32_t mask_dtype,
+                                        int32_t b, int32_t h, int32_t w, int32_t space, double min_depth,
+                                        double max_depth, void* workspace, double* records, double* state_sums,
+                                        int64_t* state_counts, void* stream_) {
+  return depth_update("depth_metrics_update", "depth_metrics_update: bad argument", pred, gt, mask, mask_dtype, b, h,
+                      w, space, 1, min_depth, max_depth, workspace, records, state_sums, state_counts,
+                      static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int odb_depth_metrics_update_metric(const float* pred, const float* gt, const void* mask,
+                                               int32_t mask_dtype, int32_t b, int32_t h, int32_t w, double min_depth,
+                                               double max_depth, void* workspace, double* records, double* state_sums,
+                                               int64_t* state_counts, void* stream_) {
+  return depth_update("depth_metrics_update_metric", "depth_metrics_update_metric: bad argument", pred, gt, mask,
+                      mask_dtype, b, h, w, ODB_SPACE_DEPTH, 0, min_depth, max_depth, workspace, records,
+                      state_sums, state_counts, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int odb_normal_metrics_update(const float* pred, const float* gt, const void* mask, int32_t mask_dtype,
@@ -364,7 +360,7 @@ extern "C" int odb_normal_metrics_update(const float* pred, const float* gt, con
                                          int64_t* state_counts, int64_t* hist, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!pred || !gt || !workspace || !state_sums || !state_counts || !hist || !planes_ok(b, h, w) ||
-      !mask_ok(mask, mask_dtype) || !aligned(pred, 4) || !aligned(gt, 4) || !aligned(workspace, 8) ||
+      !metric_mask_ok(mask, mask_dtype) || !aligned(pred, 4) || !aligned(gt, 4) || !aligned(workspace, 8) ||
       !aligned(state_sums, 8) || !aligned(state_counts, 8) || !aligned(hist, 8))
     return fail(ODB_ERR_INVALID, "normal_metrics_update: bad argument");
   const int slabs = slab_count(h, w);

@@ -34,7 +34,7 @@ namespace odb {
 
 constexpr double kAlignLambda = 1e-3, kAnchorKappa = 1e-6;     // kappa: the ridge's share in the anchored solve
 constexpr int kSolveThreads = 256;
-constexpr size_t kSolveSmemMax = 200 * 1024;     // band + right-hand side in shared memory up to this size
+constexpr size_t kSolveSmemMax = kBandSmemMax;
 
 __host__ __device__ inline int tile_count(int L, int t, int v) {
   return L <= t ? 1 : (L - v + (t - v) - 1) / (t - v);

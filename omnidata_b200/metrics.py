@@ -85,14 +85,19 @@ class _Metrics(_StepBuffers):
 
 class DepthMetrics(_Metrics):
     """Scale/shift-aligned depth metrics (module docstring).  space "depth" fits s p + t to the depth, "disparity" to its
-    inverse and needs max_depth; valid pixels have mask != 0 and a finite depth in (min_depth, max_depth]."""
+    inverse and needs max_depth; valid pixels have mask != 0 and a finite depth in (min_depth, max_depth].
+    align=False (depth space only) scores a metric prediction, such as a SparseDepthAligner's output, as it is:
+    d-hat = clamp(p, min_depth, max_depth)."""
 
     _STATE = {"sums": ((7,), torch.float64), "counts": ((4,), torch.int64)}
 
-    def __init__(self, space: str = "depth", min_depth: float = 1e-3, max_depth: Optional[float] = None):
+    def __init__(self, space: str = "depth", min_depth: float = 1e-3, max_depth: Optional[float] = None,
+                 align: bool = True):
         super().__init__()
         if space not in ("depth", "disparity"):
             raise ValueError(f"space must be 'depth' or 'disparity', got {space!r}")
+        if not align and space != "depth":
+            raise ValueError("align=False scores metric depth as predicted and takes space='depth' only")
         if space == "disparity" and max_depth is None:
             raise ValueError("space='disparity' needs max_depth (the predicted disparity is clamped to 1 / max_depth)")
         min_depth = float(min_depth)
@@ -100,6 +105,7 @@ class DepthMetrics(_Metrics):
         if not (math.isfinite(min_depth) and min_depth >= 0.0) or not (max_depth > min_depth):
             raise ValueError(f"need 0 <= min_depth < max_depth, got min_depth={min_depth}, max_depth={max_depth}")
         self.space = space
+        self.align = bool(align)
         self.min_depth, self.max_depth = min_depth, max_depth
 
     @_capi.on_tensor_device
@@ -114,7 +120,7 @@ class DepthMetrics(_Metrics):
         rec = self._buf("records", (b, _capi.DEPTH_RECORD), torch.float64, pred.device)
         space = _capi.SPACE_DISPARITY if self.space == "disparity" else _capi.SPACE_DEPTH
         ops.depth_metrics_update(pred, gt, mask, space, self.min_depth, self.max_depth, ws, rec, st["sums"],
-                                 st["counts"])
+                                 st["counts"], align=self.align)
         return rec
 
     def compute(self) -> dict:

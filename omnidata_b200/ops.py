@@ -26,6 +26,7 @@ __all__ = [
     "ensemble_gram_workspace_bytes", "ensemble_gram", "ensemble_align_solve", "ensemble_merge_depth",
     "ensemble_merge_normal", "guided_workspace_bytes", "guided_coefficients", "guided_apply",
     "boundary_workspace_bytes", "depth_edges", "edge_hysteresis", "edge_distance2", "boundary_metrics_update",
+    "sparse_align_workspace_bytes", "sparse_align_fit", "sparse_align_apply",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -659,13 +660,16 @@ def metrics_workspace_bytes(b: int, h: int, w: int) -> int:
 
 
 def depth_metrics_update(pred, gt, mask, space: int, min_depth: float, max_depth: float, workspace, records, sums,
-                         counts):
+                         counts, align: bool = True):
     """Adds the depth metrics of pred / gt fp32 [B,(1,)H,W] (mask: None or [B,(1,)H,W] uint8 / bool / fp32, nonzero =
     valid) to the state sums fp64 [7], counts int64 [4]; records fp64 [B, 12] receives the per-image results
-    (include/omnidata_b200.h odb_depth_metrics_update).  max_depth = inf: none."""
+    (include/omnidata_b200.h odb_depth_metrics_update).  max_depth = inf: none.  align=False: pred is already metric
+    and is only clamped (odb_depth_metrics_update_metric; depth space only)."""
     b, h, w, mptr, mkind = check_metric_inputs("depth_metrics_update", pred, gt, mask, 1)
     if space not in (_capi.SPACE_DEPTH, _capi.SPACE_DISPARITY):
         raise _capi.OdbError(f"depth_metrics_update: unknown space {space}")
+    if not align and space != _capi.SPACE_DEPTH:
+        raise _capi.OdbError("depth_metrics_update: align=False takes depth space only")
     if not (math.isfinite(min_depth) and 0 <= min_depth < max_depth) or \
             (space == _capi.SPACE_DISPARITY and not math.isfinite(max_depth)):
         raise _capi.OdbError(f"depth_metrics_update: need 0 <= min_depth < max_depth (finite in disparity space), got "
@@ -674,10 +678,15 @@ def depth_metrics_update(pred, gt, mask, space: int, min_depth: float, max_depth
     _need_shape(records, (b, _capi.DEPTH_RECORD), torch.float64, "records")
     _need_shape(sums, (7,), torch.float64, "sums")
     _need_shape(counts, (4,), torch.int64, "counts")
-    _call("odb_depth_metrics_update", {"bytes": 2 * 2 * 4 * b * h * w}, lib().odb_depth_metrics_update,
-          _same_device(pred, gt, mask, workspace, records, sums, counts), pred.data_ptr(), gt.data_ptr(), mptr, mkind,
-          b, h, w, space, float(min_depth), float(max_depth), workspace.data_ptr(), records.data_ptr(), sums.data_ptr(),
-          counts.data_ptr())
+    dev = _same_device(pred, gt, mask, workspace, records, sums, counts)
+    tail = (float(min_depth), float(max_depth), workspace.data_ptr(), records.data_ptr(), sums.data_ptr(),
+            counts.data_ptr())
+    if align:
+        _call("odb_depth_metrics_update", {"bytes": 2 * 2 * 4 * b * h * w}, lib().odb_depth_metrics_update, dev,
+              pred.data_ptr(), gt.data_ptr(), mptr, mkind, b, h, w, space, *tail)
+    else:
+        _call("odb_depth_metrics_update_metric", {"bytes": 2 * 2 * 4 * b * h * w},
+              lib().odb_depth_metrics_update_metric, dev, pred.data_ptr(), gt.data_ptr(), mptr, mkind, b, h, w, *tail)
 
 
 def normal_metrics_update(pred, gt, mask, workspace, sums, counts, hist):
@@ -936,3 +945,74 @@ def guided_apply(image, coef, out):
     _call("odb_guided_apply", {"bytes": 4 * (image.numel() + out.numel())}, lib().odb_guided_apply, dev,
           image.data_ptr(), coef.data_ptr(), b, c4 // 4, h, w, H, W, bh.data_ptr(), wh.data_ptr(), kh, bv.data_ptr(),
           wv.data_ptr(), kv, out.data_ptr())
+
+
+# ---------------------------------------------------------------- sparse metric alignment (csrc/sparse.cu)
+def check_sparse_grid(name: str, grid: Tuple[int, int], h: int, w: int):
+    """OdbError unless 1 <= gy <= h, 1 <= gx <= w and gy gx <= SPARSE_MAX_NODES."""
+    gy, gx = grid
+    if not (1 <= gy <= h and 1 <= gx <= w and gy * gx <= _capi.SPARSE_MAX_NODES):
+        raise _capi.OdbError(f"{name}: grid {gy}x{gx} for {h}x{w} images: need 1 <= gy <= h, 1 <= gx <= w and at "
+                             f"most {_capi.SPARSE_MAX_NODES} nodes")
+
+
+def _check_depth_range(name: str, space: int, min_depth: float, max_depth: float):
+    if space not in (_capi.SPACE_DEPTH, _capi.SPACE_DISPARITY):
+        raise _capi.OdbError(f"{name}: unknown space {space}")
+    if not (math.isfinite(min_depth) and 0 <= min_depth < max_depth) or \
+            (space == _capi.SPACE_DISPARITY and not math.isfinite(max_depth)):
+        raise _capi.OdbError(f"{name}: need 0 <= min_depth < max_depth (finite in disparity space), got "
+                             f"{min_depth}, {max_depth}")
+
+
+def sparse_align_workspace_bytes(b: int, h: int, w: int, grid: Tuple[int, int]) -> int:
+    _check_planes("sparse_align_workspace_bytes", b, h, w)
+    check_sparse_grid("sparse_align_workspace_bytes", grid, h, w)
+    return int(lib().odb_sparse_align_workspace_bytes(b, h, w, grid[0], grid[1]))
+
+
+def sparse_align_fit(pred, sparse, mask, grid: Tuple[int, int], space: int, min_depth: float, max_depth: float,
+                     smooth: float, robust: float, iterations: int, workspace, nodes, records):
+    """nodes fp64 [B, gy, gx, 2] = the scale / shift nodes fitted to the sparse depths sparse fp32 [B,(1,)H,W] (metres;
+    mask: None or [B,(1,)H,W] uint8 / bool / fp32, nonzero = valid) from pred fp32 [B,(1,)H,W]; records fp64
+    [B, SPARSE_RECORD] (include/omnidata_b200.h odb_sparse_align_fit).  robust = 0: one least-squares solve
+    (iterations 1); robust = delta > 0: iterations in [2, 32] Huber IRLS solves.  max_depth = inf: none."""
+    name = "sparse_align_fit"
+    b, h, w, mptr, mkind = check_metric_inputs(name, pred, sparse, mask, 1)
+    check_sparse_grid(name, grid, h, w)
+    _check_depth_range(name, space, min_depth, max_depth)
+    if not (math.isfinite(smooth) and smooth >= 0 and (smooth > 0 or grid[0] * grid[1] == 1)):
+        raise _capi.OdbError(f"{name}: smooth must be finite, >= 0, and > 0 for more than one node, got {smooth}")
+    if not (math.isfinite(robust) and robust >= 0) or \
+            not (2 <= iterations <= 32 if robust > 0 else iterations == 1):
+        raise _capi.OdbError(f"{name}: need robust = 0 with 1 iteration or robust > 0 with 2..32 iterations, got "
+                             f"robust={robust}, iterations={iterations}")
+    _check_workspace(name, workspace, sparse_align_workspace_bytes(b, h, w, grid))
+    _need_shape(nodes, (b, grid[0], grid[1], 2), torch.float64, "nodes")
+    _need_shape(records, (b, _capi.SPARSE_RECORD), torch.float64, "records")
+    _call("odb_sparse_align_fit", {"bytes": 2 * 4 * b * h * w * (iterations + 1)}, lib().odb_sparse_align_fit,
+          _same_device(pred, sparse, mask, workspace, nodes, records), pred.data_ptr(), sparse.data_ptr(), mptr, mkind,
+          b, h, w, grid[0], grid[1], space, float(min_depth), float(max_depth), float(smooth), float(robust),
+          int(iterations), workspace.data_ptr(), nodes.data_ptr(), records.data_ptr())
+
+
+def sparse_align_apply(pred, nodes, out, space: int, min_depth: float, max_depth: float):
+    """out fp32 [B,H,W] = the metric depth of pred fp32 [B,(1,)H,W] under the nodes fp64 [B, gy, gx, 2]
+    (odb_sparse_align_apply)."""
+    name = "sparse_align_apply"
+    b, h, w = metrics_plane_shape(pred, 1)
+    _check_planes(name, b, h, w)
+    _need(pred, torch.float32, "pred")
+    if not pred.is_contiguous():
+        raise _capi.OdbError(f"{name}: pred must be contiguous")
+    _need(nodes, torch.float64, "nodes")
+    if nodes.dim() != 4 or nodes.shape[0] != b or nodes.shape[3] != 2:
+        raise _capi.OdbError(f"{name}: nodes must be fp64 [{b}, gy, gx, 2], got {tuple(nodes.shape)}")
+    grid = (nodes.shape[1], nodes.shape[2])
+    check_sparse_grid(name, grid, h, w)
+    _need_shape(nodes, (b, grid[0], grid[1], 2), torch.float64, "nodes")
+    _check_depth_range(name, space, min_depth, max_depth)
+    _need_shape(out, (b, h, w), torch.float32, "out")
+    _call("odb_sparse_align_apply", {"bytes": 2 * 4 * b * h * w}, lib().odb_sparse_align_apply,
+          _same_device(pred, nodes, out), pred.data_ptr(), nodes.data_ptr(), b, h, w, grid[0], grid[1], space,
+          float(min_depth), float(max_depth), out.data_ptr())
