@@ -9,6 +9,8 @@
                        [--boundary [--edge_path DIR]]
                        [--sparse_points N [--sparse_seed S] | --sparse_path DIR] [--sparse_grid GYxGX]
                        [--sparse_smooth L] [--huber D [--huber_iterations K]]
+                       [--fuse_normals --intrinsics FX,FY,CX,CY [--normal_checkpoint CKPT] [--fusion_weight W]
+                        [--no_shift]]
 
 Images (PNG / JPEG) are matched to ground truth, and to masks, by file stem.  Preprocessing is that of
 `demo.py --full_res` (RGB in [0, 1]; depth normalised to [-1, 1]).  `--mode tiled` predicts at the image's own size with
@@ -33,7 +35,12 @@ without a further fit (`DepthMetrics(align=False)`), under the `sparse` key.  Th
 ground-truth pixels per image, drawn without replacement by numpy `default_rng([--sparse_seed, crc32(stem)])` (all of
 them when fewer are valid; 200 is the sparse-to-dense protocol of Ma & Karaman on NYUv2), or read from DIR by file
 stem: a 16-bit PNG under --depth_scale / --depth_invalid (0 is also no measurement) or a float `.npy` in metres (0 /
-NaN: none).  Prints one JSON
+NaN: none).  `--fuse_normals` (depth) also runs the normal model (`--normal_checkpoint`, or seeded weights with
+`--synthetic_weights`) with the same mode, ensemble and guided settings on the image in [0, 1], fuses the depth
+prediction with its normals (`DepthNormalFusion`, intrinsics in pixels of the image, weight `--fusion_weight`, no shift
+with `--no_shift`) and reports, under the `fusion` key, the depth metrics of the fused depth, the angular agreement of
+the normals implied by the predicted and by the fused depth with the normal prediction (`depth_normals`,
+`NormalMetrics`), and the fusion records.  Prints one JSON
 line: the metrics (omnidata_b200.metrics), the mode, precision, tile settings and the number of images.  Runs on cuda:0;
 there is no CPU path.
 """
@@ -196,6 +203,14 @@ def evaluate(args) -> dict:
                                      max_depth=args.max_depth)
         sparse_metric = DepthMetrics(min_depth=args.min_depth, max_depth=args.max_depth, align=False)
         sparse_records = []
+    if args.fuse_normals:
+        from omnidata_b200.fusion import DepthNormalFusion, depth_normals
+        normal_model = build_model("normal", args.backbone, args.normal_checkpoint, args.synthetic_weights,
+                                   args.precision, device)
+        fusion = DepthNormalFusion(weight=args.fusion_weight, shift=not args.no_shift)
+        fused_metric = DepthMetrics(space=args.space, min_depth=args.min_depth, max_depth=args.max_depth)
+        agree = {"pred": NormalMetrics(), "fused": NormalMetrics()}
+        fusion_records = []
     tile = (args.tile, args.tile)
     guided = (args.guided_size, args.radius, args.eps) if args.mode == "guided" else None
     if guided is not None:                          # a refused size or setting fails here, before the first image
@@ -235,6 +250,14 @@ def evaluate(args) -> dict:
             nodes, rec = aligner.fit(pred, torch.from_numpy(sp).unsqueeze(0).to(device))
             sparse_records.append(rec.clone())
             sparse_metric.update(aligner.apply(pred, nodes), gt_t, mask)
+        if args.fuse_normals:
+            normals = predict(normal_model, image_tensor(p, "normal").to(device), args.mode, tile, args.overlap,
+                              p.name, None, args.ensemble_sizes, args.flip, guided)
+            fused, rec = fusion.fit(pred, normals, args.intrinsics, mask)
+            fusion_records.append(rec.clone())
+            fused_metric.update(fused, gt_t, mask)
+            for key, d in (("pred", pred), ("fused", fused)):
+                agree[key].update(depth_normals(d, args.intrinsics, mask=mask), normals, mask)
     result = {"task": args.task, "backbone": args.backbone, "mode": args.mode, "precision": args.precision,
               "tile": list(tile) if args.mode == "tiled" else None,
               "overlap": args.overlap if args.mode == "tiled" else None,
@@ -260,7 +283,27 @@ def evaluate(args) -> dict:
             "records": {"ok": int((status == 0).sum()), "no_points": int((status == 1).sum()),
                         "degenerate": int((status == 2).sum()), "nonfinite": int((status == 3).sum()),
                         "mean_points": float(rec[:, 0].mean())}}
+    if args.fuse_normals:
+        rec = torch.cat(fusion_records).cpu()
+        status = rec[:, 1].long()
+        result["fusion"] = {
+            "intrinsics": list(args.intrinsics), "weight": args.fusion_weight, "shift": not args.no_shift,
+            "metrics": fused_metric.compute(),
+            "consistency": {"pred": agree["pred"].compute(), "fused": agree["fused"].compute()},
+            "records": {"converged": int((status == 0).sum()), "empty": int((status == 1).sum()),
+                        "flat": int((status == 2).sum()), "not_converged": int((status == 3).sum()),
+                        "mean_iterations": float(rec[:, 3].mean())}}
     return result
+
+
+def _intrinsics(text: str):
+    try:
+        k = tuple(float(v) for v in text.split(","))
+    except ValueError:
+        k = ()
+    if len(k) != 4 or not all(math.isfinite(v) for v in k) or k[0] <= 0 or k[1] <= 0:
+        raise argparse.ArgumentTypeError(f"expected FX,FY,CX,CY (pixels, fx, fy > 0), got {text!r}")
+    return k
 
 
 def _size(text: str):
@@ -328,7 +371,32 @@ def parse_args(argv=None):
                          "squares)")
     ap.add_argument("--huber_iterations", type=int, default=None,
                     help="--huber: number of reweighted solves in [2, 32] (default 5)")
+    ap.add_argument("--fuse_normals", action="store_true",
+                    help="depth: also fuse the depth with the normal model's prediction (`fusion` key)")
+    ap.add_argument("--normal_checkpoint", default=None, help="--fuse_normals: the normal model's checkpoint")
+    ap.add_argument("--intrinsics", type=_intrinsics, default=None, metavar="FX,FY,CX,CY",
+                    help="--fuse_normals: camera intrinsics in pixels of the image")
+    ap.add_argument("--fusion_weight", type=float, default=None,
+                    help="--fuse_normals: weight of the depth prediction (default 0.1, untuned)")
+    ap.add_argument("--no_shift", action="store_true", help="--fuse_normals: do not recover a shift")
     args = ap.parse_args(argv)
+    if args.fuse_normals:
+        if args.task != "depth":
+            ap.error("--fuse_normals applies to --task depth only")
+        if args.intrinsics is None:
+            ap.error("--fuse_normals needs --intrinsics FX,FY,CX,CY")
+        if args.normal_checkpoint is None and not args.synthetic_weights:
+            ap.error("--fuse_normals needs --normal_checkpoint, or --synthetic_weights")
+        if args.normal_checkpoint is not None and args.synthetic_weights:
+            ap.error("--normal_checkpoint and --synthetic_weights exclude each other")
+        args.fusion_weight = 0.1 if args.fusion_weight is None else args.fusion_weight
+        from omnidata_b200.fusion import DepthNormalFusion
+        try:
+            DepthNormalFusion(weight=args.fusion_weight, shift=not args.no_shift)
+        except ValueError as e:
+            ap.error(f"fusion: {e}")
+    elif any(v is not None for v in (args.normal_checkpoint, args.intrinsics, args.fusion_weight)) or args.no_shift:
+        ap.error("--normal_checkpoint, --intrinsics, --fusion_weight and --no_shift apply with --fuse_normals only")
     sparse_on = args.sparse_points is not None or args.sparse_path is not None
     if args.sparse_points is not None and args.sparse_path is not None:
         ap.error("give one of --sparse_points and --sparse_path")

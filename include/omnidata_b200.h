@@ -659,6 +659,55 @@ int odb_sparse_align_apply(const float* pred, const double* nodes, int32_t b, in
                            int32_t grid_x, int32_t space, double min_depth, double max_depth, float* out,
                            void* stream);
 
+/* ---- depth-normal fusion (omnidata_b200/fusion.py DepthNormalFusion, depth_normals) ----------------------------
+ *
+ * No reference counterpart.  Combines a depth prediction with the surface-normal prediction of the same frame.
+ * Definitions in DESIGN.md §3 "Depth-normal fusion"; oracle/fusion_oracle.py restates them in float64.
+ * depth a fp32 [b][h][w] (z-depth: the clamped relative prediction or metres); normals c fp32 [b][3][h][w] in the
+ * normal model's output encoding [0, 1]; mask as for the metrics above; b, h, w <= 65535.  Intrinsics fx, fy > 0, cx,
+ * cy finite, in pixels of this resolution, one set for the call.  Pixel (x, y) has the ray r = ((x - cx) / fx,
+ * (y - cy) / fy, 1) (OpenCV frame, integer pixel centres).  axis_x, axis_y, axis_z = +-1 map the model's encoding to
+ * that frame: n = axes (2 clamp(c, 0, 1) - 1); (1, -1, -1) reads it as x right, y up, z towards the camera.
+ * V = {mask != 0, a finite}.  A normal is usable when its three channels are finite and |n| >= 0.5; it is then
+ * normalised.  A 4-neighbour edge (p, q) is kept when both ends are in V with usable normals, n_p . n_q > 0 and
+ * |a_q - a_p| <= jump (max_V a - min_V a) (jump finite > 0).  Every operation of the coefficients is an fp64
+ * round-to-nearest operation.
+ *
+ * odb_depth_normal_fusion: with m = normalise(n_p + n_q), alpha = m . r_p, beta = m . r_q, e_pq = beta z_q - alpha z_p,
+ *   E(z, t) = weight S_V (z - a - t)^2 + weight kappa |V| t^2 + S_kept e_pq^2,   kappa = 1e-6,
+ * t = 0 when shift = 0.  Eliminating t leaves M z = weight (z - s(z)) + N z = weight (a - s(a)), s(v) = S_V v /
+ * (|V| (1 + kappa)) (s = 0 without shift), solved by Jacobi-preconditioned conjugate gradients in fp64 from z = a.
+ * An image stops when |r| <= tol |b| (tol finite > 0) or after `iterations` in [1, 10000]; a stopped image's state is
+ * not written again, so the result does not depend on the batch.  weight finite > 0, shift 0 or 1.
+ * out fp32 [b][h][w] = z rounded once, NaN off V.  records fp64 [b][ODB_FUSION_RECORD] = (|V|, status, kept edges,
+ * iterations run, final |r| / |b|, t, RMS over V of z - a - t, 0); status 0 converged, 1 V empty, 2 a constant on V
+ * (1 and 2: output, |r| / |b|, t and RMS NaN), 3 not converged (the output is the last iterate).
+ * workspace: odb_fusion_workspace_bytes(b, h, w) bytes (88 per pixel and a small per-image head), 16-byte aligned
+ * (negative: refused).  A memset, then 2 iterations + 6 launches, and no host synchronisation; once every image has
+ * stopped the remaining launches return after reading one flag.  An edge whose two coefficients are both 0 adds nothing
+ * to E and is not counted.
+ *
+ * odb_depth_normals: out fp32 [b][3][h][w] = the normals of the depth map in the model's encoding.  X = a r on V; an
+ * edge is kept when both ends are in V and |a_q - a_p| <= jump (max_V a - min_V a).  t_x = X(x+1) - X(x-1) with both
+ * horizontal edges kept, else the one-sided difference over the kept one; t_y likewise.  n = normalise(t_y x t_x),
+ * negated when n . X > 0 (facing the camera), out = (axes n + 1) / 2; NaN in all three channels off V or where a tangent
+ * is missing.  fp64 round-to-nearest operations, rounded to fp32 once; 16-byte stores where w % 4 == 0 and out is
+ * 16-byte aligned.  workspace: odb_depth_normals_workspace_bytes(b, h, w) bytes, 8-byte aligned.  Three launches.
+ *
+ * No floating-point atomics and fixed partitions: results are bit-reproducible and independent of the batch.  Arguments
+ * are checked before any launch. */
+#define ODB_FUSION_RECORD 8
+int64_t odb_fusion_workspace_bytes(int32_t b, int32_t h, int32_t w);
+int64_t odb_depth_normals_workspace_bytes(int32_t b, int32_t h, int32_t w);
+int odb_depth_normal_fusion(const float* depth, const float* normals, const void* mask, int32_t mask_dtype, int32_t b,
+                            int32_t h, int32_t w, double fx, double fy, double cx, double cy, int32_t axis_x,
+                            int32_t axis_y, int32_t axis_z, double jump, double weight, int32_t shift,
+                            int32_t iterations, double tol, void* workspace, float* out, double* records,
+                            void* stream);
+int odb_depth_normals(const float* depth, const void* mask, int32_t mask_dtype, int32_t b, int32_t h, int32_t w,
+                      double fx, double fy, double cx, double cy, int32_t axis_x, int32_t axis_y, int32_t axis_z,
+                      double jump, void* workspace, float* out, void* stream);
+
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *
  * The depth-boundary error (DBE) of iBims-1 (Koch et al., ECCV Workshops 2018): how far predicted depth edges lie from

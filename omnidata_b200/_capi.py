@@ -26,6 +26,7 @@ GUIDED_MAX_RADIUS = 32                          # ODB_GUIDED_MAX_RADIUS
 BOUNDARY_RECORD = 8                             # ODB_BOUNDARY_RECORD
 SPARSE_MAX_NODES = 1024                         # ODB_SPARSE_MAX_NODES
 SPARSE_RECORD = 8                               # ODB_SPARSE_RECORD
+FUSION_RECORD = 8                               # ODB_FUSION_RECORD
 
 
 class OdbError(RuntimeError):
@@ -233,6 +234,12 @@ _SIGNATURES = {
     "odb_sparse_align_fit": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 7 + [C.c_double] * 4 + [C.c_int32] +
                              [C.c_void_p] * 4),
     "odb_sparse_align_apply": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 6 + [C.c_double] * 2 + [C.c_void_p] * 2),
+    "odb_fusion_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
+    "odb_depth_normals_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
+    "odb_depth_normal_fusion": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 4 + [C.c_double] * 4 + [C.c_int32] * 3 +
+                                [C.c_double] * 2 + [C.c_int32] * 2 + [C.c_double] + [C.c_void_p] * 4),
+    "odb_depth_normals": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_double] * 4 + [C.c_int32] * 3 +
+                          [C.c_double] + [C.c_void_p] * 3),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -27,6 +27,7 @@ __all__ = [
     "ensemble_merge_normal", "guided_workspace_bytes", "guided_coefficients", "guided_apply",
     "boundary_workspace_bytes", "depth_edges", "edge_hysteresis", "edge_distance2", "boundary_metrics_update",
     "sparse_align_workspace_bytes", "sparse_align_fit", "sparse_align_apply",
+    "fusion_workspace_bytes", "depth_normals_workspace_bytes", "depth_normal_fusion", "depth_normals",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -1016,3 +1017,74 @@ def sparse_align_apply(pred, nodes, out, space: int, min_depth: float, max_depth
     _call("odb_sparse_align_apply", {"bytes": 2 * 4 * b * h * w}, lib().odb_sparse_align_apply,
           _same_device(pred, nodes, out), pred.data_ptr(), nodes.data_ptr(), b, h, w, grid[0], grid[1], space,
           float(min_depth), float(max_depth), out.data_ptr())
+
+
+# ---------------------------------------------------------------- depth-normal fusion (csrc/fusion.cu)
+def check_intrinsics(name: str, intrinsics) -> Tuple[float, float, float, float]:
+    """(fx, fy, cx, cy) as floats; OdbError unless fx, fy > 0 and all four are finite."""
+    try:
+        fx, fy, cx, cy = (float(v) for v in intrinsics)
+    except (TypeError, ValueError):
+        raise _capi.OdbError(f"{name}: intrinsics must be (fx, fy, cx, cy), got {intrinsics!r}") from None
+    if not all(math.isfinite(v) for v in (fx, fy, cx, cy)) or fx <= 0 or fy <= 0:
+        raise _capi.OdbError(f"{name}: intrinsics need finite fx, fy > 0 and finite cx, cy, got {intrinsics!r}")
+    return fx, fy, cx, cy
+
+
+def _check_axes_jump(name: str, axes, jump: float):
+    if len(tuple(axes)) != 3 or any(v not in (1, -1) for v in axes):
+        raise _capi.OdbError(f"{name}: axes must be three signs +-1, got {axes!r}")
+    if not (math.isfinite(jump) and jump > 0):
+        raise _capi.OdbError(f"{name}: jump must be finite and > 0, got {jump}")
+
+
+def fusion_workspace_bytes(b: int, h: int, w: int) -> int:
+    _check_planes("fusion_workspace_bytes", b, h, w)
+    return int(lib().odb_fusion_workspace_bytes(b, h, w))
+
+
+def depth_normals_workspace_bytes(b: int, h: int, w: int) -> int:
+    _check_planes("depth_normals_workspace_bytes", b, h, w)
+    return int(lib().odb_depth_normals_workspace_bytes(b, h, w))
+
+
+def depth_normal_fusion(depth, normals, mask, intrinsics, axes, jump: float, weight: float, shift: bool,
+                        iterations: int, tol: float, workspace, out, records):
+    """out fp32 [B,H,W] = depth fp32 [B,(1,)H,W] fused with normals fp32 [B,3,H,W] (the normal model's [0, 1] encoding;
+    mask: None or [B,(1,)H,W] uint8 / bool / fp32, nonzero = valid); records fp64 [B, FUSION_RECORD]
+    (include/omnidata_b200.h odb_depth_normal_fusion)."""
+    name = "depth_normal_fusion"
+    b, h, w, mptr, mkind = check_metric_inputs(name, depth, depth, mask, 1)
+    _need(normals, torch.float32, "normals")
+    if tuple(normals.shape) != (b, 3, h, w) or not normals.is_contiguous():
+        raise _capi.OdbError(f"{name}: normals must be a contiguous fp32 [{b}, 3, {h}, {w}] tensor, got "
+                             f"{tuple(normals.shape)}")
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    _check_axes_jump(name, axes, jump)
+    if not (math.isfinite(weight) and weight > 0) or not (math.isfinite(tol) and tol > 0) or \
+            not 1 <= iterations <= 10000:
+        raise _capi.OdbError(f"{name}: need weight > 0, tol > 0 (finite) and iterations in [1, 10000], got "
+                             f"{weight}, {tol}, {iterations}")
+    _check_workspace(name, workspace, fusion_workspace_bytes(b, h, w))
+    if workspace.data_ptr() % 16:
+        raise _capi.OdbError(f"{name}: workspace must be 16-byte aligned")
+    _need_shape(out, (b, h, w), torch.float32, "out")
+    _need_shape(records, (b, _capi.FUSION_RECORD), torch.float64, "records")
+    _call("odb_depth_normal_fusion", {"bytes": 128 * b * h * w * iterations}, lib().odb_depth_normal_fusion,
+          _same_device(depth, normals, mask, workspace, out, records), depth.data_ptr(), normals.data_ptr(), mptr,
+          mkind, b, h, w, fx, fy, cx, cy, int(axes[0]), int(axes[1]), int(axes[2]), float(jump), float(weight),
+          1 if shift else 0, int(iterations), float(tol), workspace.data_ptr(), out.data_ptr(), records.data_ptr())
+
+
+def depth_normals(depth, mask, intrinsics, axes, jump: float, workspace, out):
+    """out fp32 [B,3,H,W] = the normals of depth fp32 [B,(1,)H,W] in the normal model's encoding, NaN where undefined
+    (include/omnidata_b200.h odb_depth_normals)."""
+    name = "depth_normals"
+    b, h, w, mptr, mkind = check_metric_inputs(name, depth, depth, mask, 1)
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    _check_axes_jump(name, axes, jump)
+    _check_workspace(name, workspace, depth_normals_workspace_bytes(b, h, w))
+    _need_shape(out, (b, 3, h, w), torch.float32, "out")
+    _call("odb_depth_normals", {"bytes": 16 * b * h * w}, lib().odb_depth_normals,
+          _same_device(depth, mask, workspace, out), depth.data_ptr(), mptr, mkind, b, h, w, fx, fy, cx, cy,
+          int(axes[0]), int(axes[1]), int(axes[2]), float(jump), workspace.data_ptr(), out.data_ptr())
