@@ -708,6 +708,59 @@ int odb_depth_normals(const float* depth, const void* mask, int32_t mask_dtype, 
                       double fx, double fy, double cx, double cy, int32_t axis_x, int32_t axis_y, int32_t axis_z,
                       double jump, void* workspace, float* out, void* stream);
 
+/* ---- TSDF volumes (omnidata_b200/volume.py TSDFVolume) ------------------------------------------------------------
+ *
+ * No reference counterpart.  Fuses posed depth frames into one dense truncated signed-distance grid, renders depth
+ * back from it and extracts a triangle mesh.  Definitions in DESIGN.md §3 "TSDF volumes"; oracle/volume_oracle.py
+ * restates them in float64.  Camera frame: OpenCV (x right, y down, z forward, integer pixel centres); intrinsics fx,
+ * fy > 0, cx, cy finite, in pixels of the depth map.  A pose cam_to_world is a HOST array of 16 doubles, the row-major
+ * 4 x 4 camera-to-world matrix [R t; 0 0 0 1] (finite, last row exactly 0 0 0 1, |R^T R - I| <= 1e-6 entrywise); the
+ * entry points read it during the call and pass it to the kernels by value, so the caller copies nothing to the device.
+ * Grid: nx, ny, nz in [2, ODB_TSDF_MAX_DIM], nx ny nz <= ODB_TSDF_MAX_POINTS, points X(i, j, k) = origin + voxel (i, j,
+ * k) (origin finite, voxel finite > 0).  tsdf, weight fp32 [nz][ny][nx] (i fastest); color NULL or fp32 [3][nz][ny][nx].
+ *
+ * odb_tsdf_integrate: depth fp32 [b][h][w] in metres with b poses (cam_to_world [b][16]); rgb fp32 [b][3][h][w] exactly
+ * when color is given.  Each grid point loops over the b frames in order, in fp64 round-to-nearest operations: Xc =
+ * R^T (X - t); no observation when z <= 0; u = fx x / z + cx, v = fy y / z + cy; the pixel (floor(u + 0.5),
+ * floor(v + 0.5)) must lie in the image; its depth d must be finite and > 0; eta = d - z, no observation when
+ * eta < -trunc (trunc finite > 0); f = min(1, eta / trunc) rounded to fp32.  An observation updates, in fp32 operations,
+ * F = (F W + f) / (W + 1), the colour means likewise, then W = W + 1.  One launch per 16 frames; no workspace.
+ *
+ * odb_tsdf_raycast: out fp32 [h][w] = the z-depth of the first surface along each pixel's ray, 0 where none is hit.  The
+ * unit ray R r / |r|, r = ((x - cx) / fx, (y - cy) / fy, 1), from t is clipped to the grid's box [origin, origin + voxel
+ * (n - 1)]; samples at t_k = t_enter + k step (step finite in [voxel / 64, voxel]) while t_k <= t_exit are trilinear
+ * interpolations of F, valid when all 8 corners have W > 0.  The hit is the first pair of valid samples k, k + 1 with
+ * F_k > 0 >= F_k+1 at t_k + step F_k / (F_k - F_k+1); out = that t / |r|.  fp64 round-to-nearest over the fp32 loads.
+ *
+ * odb_tsdf_mesh_count + odb_tsdf_mesh_emit: marching tetrahedra on the Kuhn split of each cell into 6 tetrahedra (one
+ * per permutation of the axes).  Each point p owns the 7 lattice edges (p, p + d), d in {0,1}^3 \ {0}, direction index
+ * dx + 2 dy + 4 dz - 1; an edge carries a vertex when both ends have W > 0 and exactly one has F < 0, at world position
+ * origin + voxel (p + d F_p / (F_p - F_q)) (fp64, stored fp32; colour interpolated likewise).  Vertex ids follow
+ * (k, j, i, direction).  A tetrahedron whose 4 corners have W > 0 and 1-3 corners with F < 0 emits 1 or 2 triangles,
+ * ordered by (cell, tetrahedron, triangle) and wound by a fixed table so that normals point from F < 0 to F > 0.
+ * count: writes counts int64 [2] = (vertices, faces) on the device and the per-point tables to workspace
+ * (odb_tsdf_mesh_workspace_bytes(nx, ny, nz) bytes, 8-byte aligned, negative: refused); three launches.  emit: after
+ * count on the same workspace, writes vertices fp32 [V][3], faces int32 [F][3] and colors fp32 [V][3] (exactly when
+ * color is given); the caller reads the counts and sizes the outputs.  One launch.
+ *
+ * Integer scans and no atomics: every output is bit-reproducible, and integrating frames in one call or several gives
+ * the same bits.  Arguments are checked before any launch. */
+#define ODB_TSDF_MAX_DIM 2048
+#define ODB_TSDF_MAX_POINTS 268435456
+int64_t odb_tsdf_mesh_workspace_bytes(int32_t nx, int32_t ny, int32_t nz);
+int odb_tsdf_integrate(float* tsdf, float* weight, float* color, int32_t nx, int32_t ny, int32_t nz, double ox,
+                       double oy, double oz, double voxel, double trunc, const float* depth, const float* rgb, int32_t b,
+                       int32_t h, int32_t w, double fx, double fy, double cx, double cy, const double* cam_to_world,
+                       void* stream);
+int odb_tsdf_raycast(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz, double ox, double oy,
+                     double oz, double voxel, const double* cam_to_world, int32_t h, int32_t w, double fx, double fy,
+                     double cx, double cy, double step, float* out, void* stream);
+int odb_tsdf_mesh_count(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz, void* workspace,
+                        int64_t* counts, void* stream);
+int odb_tsdf_mesh_emit(const float* tsdf, const float* weight, const float* color, int32_t nx, int32_t ny, int32_t nz,
+                       double ox, double oy, double oz, double voxel, const void* workspace, float* vertices,
+                       int32_t* faces, float* colors, void* stream);
+
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *
  * The depth-boundary error (DBE) of iBims-1 (Koch et al., ECCV Workshops 2018): how far predicted depth edges lie from

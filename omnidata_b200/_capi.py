@@ -27,6 +27,8 @@ BOUNDARY_RECORD = 8                             # ODB_BOUNDARY_RECORD
 SPARSE_MAX_NODES = 1024                         # ODB_SPARSE_MAX_NODES
 SPARSE_RECORD = 8                               # ODB_SPARSE_RECORD
 FUSION_RECORD = 8                               # ODB_FUSION_RECORD
+TSDF_MAX_DIM = 2048                             # ODB_TSDF_MAX_DIM
+TSDF_MAX_POINTS = 1 << 28                       # ODB_TSDF_MAX_POINTS
 
 
 class OdbError(RuntimeError):
@@ -240,6 +242,13 @@ _SIGNATURES = {
                                 [C.c_double] * 2 + [C.c_int32] * 2 + [C.c_double] + [C.c_void_p] * 4),
     "odb_depth_normals": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_double] * 4 + [C.c_int32] * 3 +
                           [C.c_double] + [C.c_void_p] * 3),
+    "odb_tsdf_mesh_workspace_bytes": (C.c_int64, [C.c_int32] * 3),
+    "odb_tsdf_integrate": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_double] * 5 + [C.c_void_p] * 2 +
+                           [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] * 2),
+    "odb_tsdf_raycast": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] +
+                         [C.c_int32] * 2 + [C.c_double] * 5 + [C.c_void_p] * 2),
+    "odb_tsdf_mesh_count": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p] * 3),
+    "odb_tsdf_mesh_emit": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] * 5),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -10,6 +10,7 @@ import ctypes as C
 import math
 from typing import Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _capi
@@ -28,6 +29,7 @@ __all__ = [
     "boundary_workspace_bytes", "depth_edges", "edge_hysteresis", "edge_distance2", "boundary_metrics_update",
     "sparse_align_workspace_bytes", "sparse_align_fit", "sparse_align_apply",
     "fusion_workspace_bytes", "depth_normals_workspace_bytes", "depth_normal_fusion", "depth_normals",
+    "tsdf_mesh_workspace_bytes", "tsdf_integrate", "tsdf_raycast", "tsdf_mesh_count", "tsdf_mesh_emit",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -1088,3 +1090,144 @@ def depth_normals(depth, mask, intrinsics, axes, jump: float, workspace, out):
     _call("odb_depth_normals", {"bytes": 16 * b * h * w}, lib().odb_depth_normals,
           _same_device(depth, mask, workspace, out), depth.data_ptr(), mptr, mkind, b, h, w, fx, fy, cx, cy,
           int(axes[0]), int(axes[1]), int(axes[2]), float(jump), workspace.data_ptr(), out.data_ptr())
+
+
+# ---------------------------------------------------------------- TSDF volumes (csrc/volume.cu)
+def check_volume_grid(name: str, dims, origin, voxel: float) -> Tuple[Tuple[int, int, int], Tuple[float, float, float]]:
+    """((nx, ny, nz), origin) as ints / floats; OdbError unless each dimension lies in [2, TSDF_MAX_DIM], nx ny nz <=
+    TSDF_MAX_POINTS, the origin is finite and voxel is finite and > 0."""
+    try:
+        nx, ny, nz = (int(v) for v in dims)
+        ox, oy, oz = (float(v) for v in origin)
+    except (TypeError, ValueError):
+        raise _capi.OdbError(f"{name}: dims must be (nx, ny, nz) and origin (x, y, z), got {dims!r}, {origin!r}") \
+            from None
+    if tuple(dims) != (nx, ny, nz) or not all(2 <= d <= _capi.TSDF_MAX_DIM for d in (nx, ny, nz)) or \
+            nx * ny * nz > _capi.TSDF_MAX_POINTS:
+        raise _capi.OdbError(f"{name}: dims must lie in [2, {_capi.TSDF_MAX_DIM}] with nx ny nz <= "
+                             f"{_capi.TSDF_MAX_POINTS}, got {dims!r}")
+    if not all(math.isfinite(v) for v in (ox, oy, oz)) or not (math.isfinite(voxel) and voxel > 0):
+        raise _capi.OdbError(f"{name}: need a finite origin and a finite voxel > 0, got {origin!r}, {voxel}")
+    return (nx, ny, nz), (ox, oy, oz)
+
+
+def check_poses(name: str, cam_to_world) -> np.ndarray:
+    """Host float64 [B, 16] (row-major 4 x 4 camera-to-world matrices) from numpy or a CPU tensor, [B,4,4] or [4,4];
+    OdbError unless every pose is finite with last row 0 0 0 1 and |R^T R - I| <= 1e-6 entrywise."""
+    if isinstance(cam_to_world, torch.Tensor):
+        if cam_to_world.device.type != "cpu":
+            raise _capi.OdbError(f"{name}: poses are host data (numpy or a CPU tensor), got a {cam_to_world.device} "
+                                 "tensor")
+        cam_to_world = cam_to_world.numpy()
+    T = np.asarray(cam_to_world, dtype=np.float64)
+    if T.shape == (4, 4):
+        T = T[None]
+    if T.ndim != 3 or T.shape[1:] != (4, 4) or T.shape[0] < 1:
+        raise _capi.OdbError(f"{name}: poses must be [B,4,4] or [4,4], got {T.shape}")
+    if not np.isfinite(T).all():
+        raise _capi.OdbError(f"{name}: poses must be finite")
+    if not (T[:, 3] == np.array([0.0, 0.0, 0.0, 1.0])).all():
+        raise _capi.OdbError(f"{name}: the last row of a pose must be 0 0 0 1")
+    R = T[:, :3, :3]
+    if np.abs(np.einsum("bki,bkj->bij", R, R) - np.eye(3)).max() > 1e-6:
+        raise _capi.OdbError(f"{name}: the rotation of a pose is not orthonormal (|R^T R - I| > 1e-6)")
+    return np.ascontiguousarray(T.reshape(-1, 16))
+
+
+def _volume_planes(name: str, tsdf, weight, color, dims):
+    nx, ny, nz = dims
+    _need_shape(tsdf, (nz, ny, nx), torch.float32, "tsdf")
+    _need_shape(weight, (nz, ny, nx), torch.float32, "weight")
+    if color is not None:
+        _need_shape(color, (3, nz, ny, nx), torch.float32, "color")
+
+
+def tsdf_mesh_workspace_bytes(dims) -> int:
+    nx, ny, nz = check_volume_grid("tsdf_mesh_workspace_bytes", dims, (0, 0, 0), 1.0)[0]
+    return int(lib().odb_tsdf_mesh_workspace_bytes(nx, ny, nz))
+
+
+def tsdf_integrate(tsdf, weight, color, dims, origin, voxel: float, trunc: float, depth, rgb, intrinsics,
+                   cam_to_world):
+    """Integrates depth fp32 [B,H,W] (metres; rgb fp32 [B,3,H,W] exactly when color is given) seen from cam_to_world
+    (host, see check_poses) into tsdf, weight fp32 [nz,ny,nx] and color fp32 [3,nz,ny,nx] in place
+    (include/omnidata_b200.h odb_tsdf_integrate)."""
+    name = "tsdf_integrate"
+    dims, origin = check_volume_grid(name, dims, origin, voxel)
+    if not (math.isfinite(trunc) and trunc > 0):
+        raise _capi.OdbError(f"{name}: trunc must be finite and > 0, got {trunc}")
+    _volume_planes(name, tsdf, weight, color, dims)
+    _need(depth, torch.float32, "depth")
+    if depth.dim() != 3 or not depth.is_contiguous():
+        raise _capi.OdbError(f"{name}: depth must be a contiguous fp32 [B,H,W] tensor, got {tuple(depth.shape)}")
+    b, h, w = depth.shape
+    _check_planes(name, b, h, w)
+    if (color is None) != (rgb is None):
+        raise _capi.OdbError(f"{name}: rgb is required exactly when the volume stores colour")
+    if rgb is not None:
+        _need_shape(rgb, (b, 3, h, w), torch.float32, "rgb")
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    T = check_poses(name, cam_to_world)
+    if T.shape[0] != b:
+        raise _capi.OdbError(f"{name}: {b} depth frames but {T.shape[0]} poses")
+    n = dims[0] * dims[1] * dims[2]
+    _call(name, {"bytes": 8 * n + 4 * b * h * w}, lib().odb_tsdf_integrate,
+          _same_device(tsdf, weight, color, depth, rgb), tsdf.data_ptr(), weight.data_ptr(), _ptr(color), *dims,
+          *origin, float(voxel), float(trunc), depth.data_ptr(), _ptr(rgb), b, h, w, fx, fy, cx, cy, T.ctypes.data)
+
+
+def tsdf_raycast(tsdf, weight, dims, origin, voxel: float, intrinsics, cam_to_world, step: float, out):
+    """out fp32 [H,W] = the z-depth of the first surface seen from cam_to_world (host [4,4]), 0 where none
+    (include/omnidata_b200.h odb_tsdf_raycast)."""
+    name = "tsdf_raycast"
+    dims, origin = check_volume_grid(name, dims, origin, voxel)
+    _volume_planes(name, tsdf, weight, None, dims)
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    T = check_poses(name, cam_to_world)
+    if T.shape[0] != 1:
+        raise _capi.OdbError(f"{name}: one pose, got {T.shape[0]}")
+    if not (math.isfinite(step) and voxel / 64 <= step <= voxel):
+        raise _capi.OdbError(f"{name}: step must lie in [voxel / 64, voxel], got {step}")
+    _need(out, torch.float32, "out")
+    if out.dim() != 2 or not out.is_contiguous():
+        raise _capi.OdbError(f"{name}: out must be a contiguous fp32 [H,W] tensor, got {tuple(out.shape)}")
+    h, w = out.shape
+    _check_planes(name, 1, h, w)
+    _call(name, {"bytes": 4 * h * w}, lib().odb_tsdf_raycast, _same_device(tsdf, weight, out), tsdf.data_ptr(),
+          weight.data_ptr(), *dims, *origin, float(voxel), T.ctypes.data, h, w, fx, fy, cx, cy, float(step),
+          out.data_ptr())
+
+
+def tsdf_mesh_count(tsdf, weight, dims, workspace, counts):
+    """counts int64 [2] = (vertices, faces) of the mesh of tsdf / weight; fills workspace for tsdf_mesh_emit
+    (include/omnidata_b200.h odb_tsdf_mesh_count)."""
+    name = "tsdf_mesh_count"
+    dims = check_volume_grid(name, dims, (0, 0, 0), 1.0)[0]
+    _volume_planes(name, tsdf, weight, None, dims)
+    _check_workspace(name, workspace, tsdf_mesh_workspace_bytes(dims))
+    _need_shape(counts, (2,), torch.int64, "counts")
+    n = dims[0] * dims[1] * dims[2]
+    _call(name, {"bytes": 14 * n}, lib().odb_tsdf_mesh_count, _same_device(tsdf, weight, workspace, counts),
+          tsdf.data_ptr(), weight.data_ptr(), *dims, workspace.data_ptr(), counts.data_ptr())
+
+
+def tsdf_mesh_emit(tsdf, weight, color, dims, origin, voxel: float, workspace, vertices, faces, colors):
+    """vertices fp32 [V,3], faces int32 [F,3] and colors fp32 [V,3] (exactly when color is given), sized from the counts
+    of tsdf_mesh_count on the same workspace (include/omnidata_b200.h odb_tsdf_mesh_emit)."""
+    name = "tsdf_mesh_emit"
+    dims, origin = check_volume_grid(name, dims, origin, voxel)
+    _volume_planes(name, tsdf, weight, color, dims)
+    _check_workspace(name, workspace, tsdf_mesh_workspace_bytes(dims))
+    for t, dt, n in ((vertices, torch.float32, "vertices"), (faces, torch.int32, "faces")):
+        _need(t, dt, n)
+        if t.dim() != 2 or t.shape[1] != 3 or not t.is_contiguous():
+            raise _capi.OdbError(f"{name}: {n} must be a contiguous [N, 3] tensor, got {tuple(t.shape)}")
+    if (color is None) != (colors is None):
+        raise _capi.OdbError(f"{name}: colors is required exactly when the volume stores colour")
+    if colors is not None:
+        _need_shape(colors, tuple(vertices.shape), torch.float32, "colors")
+    n = dims[0] * dims[1] * dims[2]
+    _call(name, {"bytes": 14 * n}, lib().odb_tsdf_mesh_emit,
+          _same_device(tsdf, weight, color, workspace, vertices, faces, colors), tsdf.data_ptr(), weight.data_ptr(),
+          _ptr(color), *dims, *origin, float(voxel), workspace.data_ptr(), vertices.data_ptr(), faces.data_ptr(),
+          _ptr(colors))

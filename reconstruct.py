@@ -1,0 +1,183 @@
+#!/usr/bin/env python
+"""Reconstruct a scene from posed images: predict each frame's depth, align it to metres and to what is already fused,
+integrate it into a TSDF volume on the device, and write the extracted mesh as a PLY:
+
+    python reconstruct.py --img_path DIR --pose_path DIR --intrinsics FX,FY,CX,CY --voxel V
+                          --bounds X0,Y0,Z0,X1,Y1,Z1 --out mesh.ply
+                          [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
+                          [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--guided_size HxW]
+                          [--sparse_path DIR [--depth_scale 1000]] [--trunc T]
+
+Frames are the images of --img_path (PNG / JPEG) in file-name order.  Each has a pose, the 4 x 4 camera-to-world matrix
+as text (ScanNet's pose/<stem>.txt), in --pose_path by file stem.  The intrinsics are in pixels of the images.  The grid
+covers --bounds with points every --voxel metres (write `--bounds=-1,...` when X0 is negative).
+
+Per frame: the depth model predicts at the image's size (evaluate.py's predictor and preprocessing; `--mode`, `--tile`,
+`--overlap`, `--guided_size`).  `SparseDepthAligner(grid=(1, 1), robust=0.05)` then fits one scale and shift (Huber IRLS, so that
+rays that pass through not-yet-observed space and hit a surface behind it do not pull the fit).  The target is the
+frame's sparse depths when --sparse_path has a file for it (16-bit PNG / --depth_scale units per metre, or a `.npy` in
+metres; 0 is no measurement).  Otherwise it is the volume's own raycast at the frame's pose, so each frame is aligned
+to what is already fused.  Frame 0 must have sparse depths: they fix the scene's metric scale.  The aligned depth is
+integrated (`TSDFVolume`).  A frame whose fit fails (fewer than two target pixels, a flat prediction) is skipped and
+named in the summary.
+
+Prints one JSON line: frames used and skipped, vertices, faces and seconds.  Runs on cuda:0; there is no CPU path.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import math
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+import torch
+
+import evaluate
+
+# Huber threshold on the relative residual of the per-frame fit.  A raycast ray can pass through space no frame has
+# observed yet (the pair of valid samples breaks) and hit a fused surface behind it; those pixels are outliers that a
+# plain least-squares fit follows.  5 IRLS solves, 0.05 not tuned.
+ROBUST = 0.05
+
+
+def _floats(n: int, what: str):
+    def parse(text: str):
+        try:
+            v = tuple(float(x) for x in text.split(","))
+        except ValueError:
+            v = ()
+        if len(v) != n or not all(math.isfinite(x) for x in v):
+            raise argparse.ArgumentTypeError(f"expected {what} ({n} finite numbers), got {text!r}")
+        return v
+    return parse
+
+
+def load_pose(path: Path) -> np.ndarray:
+    """float64 [4,4] camera-to-world from a whitespace-separated text file."""
+    T = np.loadtxt(path, dtype=np.float64)
+    if T.shape != (4, 4):
+        raise ValueError(f"{path}: a pose is a 4 x 4 matrix, got {T.shape}")
+    return T
+
+
+def parse_args(argv=None):
+    from omnidata_b200.volume import MAX_DIM, MAX_POINTS
+    ap = argparse.ArgumentParser(description="Fuse depth predictions of posed images into a TSDF volume and a mesh")
+    ap.add_argument("--img_path", required=True, help="directory of RGB frames")
+    ap.add_argument("--pose_path", required=True, help="directory of <stem>.txt camera-to-world 4 x 4 poses")
+    ap.add_argument("--intrinsics", required=True, type=evaluate._intrinsics, metavar="FX,FY,CX,CY",
+                    help="camera intrinsics in pixels of the frames")
+    ap.add_argument("--voxel", required=True, type=float, help="grid spacing in metres")
+    ap.add_argument("--bounds", required=True, type=_floats(6, "X0,Y0,Z0,X1,Y1,Z1"), metavar="X0,Y0,Z0,X1,Y1,Z1",
+                    help="world-space box the grid covers")
+    ap.add_argument("--out", required=True, help="output mesh (binary PLY)")
+    w = ap.add_mutually_exclusive_group(required=True)
+    w.add_argument("--checkpoint", default=None)
+    w.add_argument("--synthetic_weights", action="store_true", help="seeded random weights (no checkpoint)")
+    ap.add_argument("--backbone", default="vitb_rn50_384", choices=("vitb_rn50_384", "vitl16_384", "vitb16_384"))
+    ap.add_argument("--precision", default="bf16", choices=("fp32", "bf16", "fp8"))
+    ap.add_argument("--mode", default="tiled", choices=("tiled", "direct", "guided"))
+    ap.add_argument("--tile", type=int, default=384)
+    ap.add_argument("--overlap", type=int, default=64)
+    ap.add_argument("--guided_size", type=evaluate._size, default=None, metavar="HxW",
+                    help="--mode guided: the input size of the one forward")
+    ap.add_argument("--sparse_path", default=None, metavar="DIR",
+                    help="sparse depths by file stem (16-bit PNG or .npy in metres); frame 0 must have one")
+    ap.add_argument("--depth_scale", type=float, default=1000.0, help="16-bit PNG units per metre (default mm)")
+    ap.add_argument("--trunc", type=float, default=None, help="truncation distance in metres (default 3 voxels)")
+    args = ap.parse_args(argv)
+    if not (math.isfinite(args.voxel) and args.voxel > 0):
+        ap.error(f"--voxel must be finite and > 0, got {args.voxel}")
+    lo, hi = args.bounds[:3], args.bounds[3:]
+    if not all(h > l for l, h in zip(lo, hi)):
+        ap.error(f"--bounds must have X1 > X0, Y1 > Y0 and Z1 > Z0, got {args.bounds}")
+    args.origin = tuple(lo)
+    args.dims = tuple(int(math.floor((h - l) / args.voxel + 1e-9)) + 1 for l, h in zip(lo, hi))
+    if not all(2 <= d <= MAX_DIM for d in args.dims) or math.prod(args.dims) > MAX_POINTS:
+        ap.error(f"--bounds / --voxel give a {args.dims} grid; each dimension must lie in [2, {MAX_DIM}] and the "
+                 f"grid hold at most {MAX_POINTS} points")
+    if args.sparse_path is None:
+        ap.error("--sparse_path is required: frame 0's sparse depths fix the scene's metric scale")
+    if not (math.isfinite(args.depth_scale) and args.depth_scale > 0):
+        ap.error(f"--depth_scale must be finite and > 0, got {args.depth_scale}")
+    if args.trunc is not None and not (math.isfinite(args.trunc) and args.trunc > 0):
+        ap.error(f"--trunc must be finite and > 0, got {args.trunc}")
+    if args.mode == "guided":
+        if args.guided_size is None:
+            ap.error("--mode guided needs --guided_size HxW")
+    elif args.guided_size is not None:
+        ap.error("--guided_size applies to --mode guided only")
+    return args
+
+
+def align_and_integrate(volume, aligner, pred: torch.Tensor, intrinsics, pose: np.ndarray, sparse=None):
+    """One frame of the loop: fit pred fp32 [1,H,W] to sparse [1,H,W] (metres, 0 = none) or, without it, to the
+    volume's raycast at pose; integrate the aligned depth when the fit is ok.  Returns the aligner's record (fp64 [8],
+    on the host) and the nodes (scale, shift)."""
+    h, w = pred.shape[-2:]
+    target = sparse if sparse is not None else volume.raycast(intrinsics, pose, (h, w)).unsqueeze(0)
+    nodes, rec = aligner.fit(pred, target)
+    rec, st = rec[0].cpu(), nodes.reshape(2).cpu()
+    if int(rec[1]) == 0:
+        volume.integrate(aligner.apply(pred, nodes), intrinsics, pose)
+    return rec, (float(st[0]), float(st[1]))
+
+
+def reconstruct(args) -> dict:
+    from omnidata_b200.sparse import STATUS, SparseDepthAligner
+    from omnidata_b200.volume import TSDFVolume, write_ply
+    t0 = time.perf_counter()
+    device = torch.device("cuda:0")
+    images = sorted(p for p in Path(args.img_path).iterdir() if p.suffix.lower() in evaluate.IMAGE_EXT)
+    if not images:
+        raise FileNotFoundError(f"no images in {args.img_path}")
+    poses = [load_pose(Path(args.pose_path) / (p.stem + ".txt")) for p in images]
+    evaluate._find(args.sparse_path, images[0].stem, "sparse depth for frame 0")
+    model = evaluate.build_model("depth", args.backbone, args.checkpoint, args.synthetic_weights, args.precision,
+                                 device)
+    guided = (args.guided_size, 4, 1e-3) if args.mode == "guided" else None
+    volume = TSDFVolume(args.origin, args.voxel, args.dims, trunc=args.trunc, device=device)
+    aligner = SparseDepthAligner(grid=(1, 1), robust=ROBUST)
+    used, skipped = [], []
+    for q, (p, pose) in enumerate(zip(images, poses)):
+        x = evaluate.image_tensor(p, "depth").to(device)
+        pred = evaluate.predict(model, x, args.mode, (args.tile, args.tile), args.overlap, p.name, guided=guided)
+        sparse = None
+        try:
+            sp = evaluate.load_sparse(evaluate._find(args.sparse_path, p.stem, "sparse depth"), args.depth_scale,
+                                      65535)
+        except FileNotFoundError:
+            sp = None
+        if sp is not None:
+            if tuple(sp.shape) != tuple(pred.shape[-2:]):
+                raise ValueError(f"{p.name}: the sparse depth is {sp.shape[0]}x{sp.shape[1]}, the image "
+                                 f"{pred.shape[-2]}x{pred.shape[-1]}")
+            sparse = torch.from_numpy(sp).unsqueeze(0).to(device)
+        rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse)
+        status = int(rec[1])
+        if status == 0:
+            used.append(p.name)
+        else:
+            skipped.append({"frame": p.name, "status": STATUS[status]})
+    vertices, faces, _ = volume.extract_mesh()
+    write_ply(args.out, vertices, faces)
+    return {"frames": len(images), "frames_used": len(used), "frames_skipped": skipped,
+            "vertices": int(vertices.shape[0]), "faces": int(faces.shape[0]), "dims": list(args.dims),
+            "voxel": args.voxel, "out": str(args.out), "seconds": round(time.perf_counter() - t0, 3)}
+
+
+def main(argv=None) -> dict:
+    args = parse_args(argv)
+    if not torch.cuda.is_available():
+        print("reconstruct.py: a CUDA (sm_90a) device is required; this implementation has no CPU path")
+        sys.exit(1)
+    result = reconstruct(args)
+    print(json.dumps(result))
+    return result
+
+
+if __name__ == "__main__":
+    main()
