@@ -761,6 +761,42 @@ int odb_tsdf_mesh_emit(const float* tsdf, const float* weight, const float* colo
                        double ox, double oy, double oz, double voxel, const void* workspace, float* vertices,
                        int32_t* faces, float* colors, void* stream);
 
+/* ---- camera tracking (omnidata_b200/track.py FrameTracker) ---------------------------------------------------------
+ *
+ * No reference counterpart.  Solves one frame's camera pose (and, with affine, the scale and shift of its depth) against
+ * a model depth map rendered at a reference pose: point-to-plane ICP with projective association (KinectFusion), one
+ * Gauss-Newton step per launch.  Definition in DESIGN.md §3 "Camera tracking"; oracle/track_oracle.py restates it in
+ * float64.  Frames, intrinsics and poses as for the TSDF volumes above; ref_pose and init_pose are HOST arrays of 16
+ * doubles passed to the kernels by value.
+ *
+ * pred fp32 [h][w] (the frame's depth a), ref_depth fp32 [h][w] (the model's z-depth at ref_pose, no surface unless
+ * finite and > 0), ref_normals fp32 [3][h][w] (depth_normals of ref_depth with axes (1, 1, 1): n = 2 c - 1 in the
+ * reference camera frame, unusable unless all three are finite).  init_nodes fp64 [2] on the device, the initial (s, t),
+ * exactly when affine = 1; with affine = 0, s = 1 and t = 0 are fixed.  With M = ref_pose^-1 T = [Rm tm], a frame pixel
+ * with finite a and z = s a + t > 0 has P = z r; Q = Rm P + tm must have Q.z > 0 and its nearest reference pixel q
+ * (floor(u + 0.5), floor(v + 0.5)) must lie in the image with a surface and a usable normal n; with V = ref_depth_q r_q,
+ * the pair is a correspondence when |Q - V| <= max_dist.  Residual e = n.(Q - V), Huber weight w = min(1, robust / |e|),
+ * Jacobian row (m, P x m, m.(a r), m.r) with m = Rm^T n for the step T <- T exp(xi) in the camera frame (the last two
+ * entries with affine only).  The normal matrix is scaled to a unit diagonal and solved by Cholesky in fp64.
+ * At most `iterations` (1..100) launches; a frame stops when |omega|, |v|, |ds|, |dt| <= tol.  Status (record[1]): 0 ok;
+ * 1 no_overlap (fewer than min_overlap, in (0, 1], of the valid pixels have a correspondence); 2 degenerate (a scaled
+ * Cholesky pivot below 1e-6, or a zero diagonal); 3 nonfinite (NaN in init_nodes, the sums or the update).  A failed
+ * frame returns init_pose and init_nodes (bit for bit).
+ *
+ * Outputs on the device: pose fp64 [16] (row-major camera-to-world), nodes fp64 [2] (s, t; SparseDepthAligner's
+ * grid (1, 1) layout), record fp64 [ODB_TRACK_RECORD] = (correspondences of the last iteration, status, weighted RMS of
+ * e in metres, fraction with w < 1, iterations run, s, t, valid frame pixels).  workspace: odb_track_workspace_bytes(h,
+ * w) bytes, 8-byte aligned (negative: refused).  A call is a memset of the ticket and iterations + 2 launches, with no
+ * host synchronisation, so it can be captured in a CUDA graph.  Fixed pixel chunks and fixed-order sums, no
+ * floating-point atomics: results are bit-reproducible.  Arguments are checked before any launch. */
+#define ODB_TRACK_RECORD 8
+int64_t odb_track_workspace_bytes(int32_t h, int32_t w);
+int odb_track_frame(const float* pred, const float* ref_depth, const float* ref_normals, int32_t h, int32_t w,
+                    double fx, double fy, double cx, double cy, const double* ref_pose, const double* init_pose,
+                    const double* init_nodes, int32_t affine, int32_t iterations, double tol, double robust,
+                    double max_dist, double min_overlap, void* workspace, double* pose, double* nodes, double* record,
+                    void* stream);
+
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *
  * The depth-boundary error (DBE) of iBims-1 (Koch et al., ECCV Workshops 2018): how far predicted depth edges lie from

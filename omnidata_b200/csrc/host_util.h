@@ -3,6 +3,8 @@
 // the library links against libcudart only).
 #pragma once
 
+#include <cmath>
+
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,6 +49,24 @@ constexpr int kPartStride = 8;            // doubles per slab partial / image re
 // `images` images, q < nq: the sum, or the minimum / maximum where bit q of min_mask / max_mask is set.  One launch.
 void launch_slab_reduce(const double* part, int images, int slabs, int nq, unsigned min_mask, unsigned max_mask,
                         double* out, cudaStream_t stream);
+
+// a 4 x 4 row-major camera-to-world matrix: finite, last row 0 0 0 1, |R^T R - I| <= 1e-6 entrywise
+inline bool pose_ok(const double* T, double out[12]) {
+  for (int e = 0; e < 16; ++e)
+    if (!std::isfinite(T[e])) return false;
+  if (T[12] != 0.0 || T[13] != 0.0 || T[14] != 0.0 || T[15] != 1.0) return false;
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) {
+      double s = 0.0;
+      for (int r = 0; r < 3; ++r) s += T[4 * r + a] * T[4 * r + b];
+      if (std::fabs(s - (a == b ? 1.0 : 0.0)) > 1e-6) return false;
+    }
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) out[3 * r + c] = T[4 * r + c];
+    out[9 + r] = T[4 * r + 3];
+  }
+  return true;
+}
 
 // fp32 correctness mode of odb_conv_gemm (fp32_path.cu)
 

@@ -1,0 +1,405 @@
+// Camera tracking (omnidata_b200/track.py FrameTracker): one frame's pose, and with `affine` the scale and shift of its
+// depth, solved against a model depth map rendered at a reference pose (normally TSDFVolume.raycast) by point-to-plane
+// ICP with projective association (KinectFusion, Newcombe et al. 2011).  Definition in DESIGN.md §3 "Camera tracking"
+// and include/omnidata_b200.h; oracle/track_oracle.py restates it in float64.
+//
+//   track_setup_kernel   one thread: the state from init_pose (by value) and init_nodes (device)
+//   track_step_kernel    one Gauss-Newton iteration per launch.  Per fixed chunk of kChunk pixels: association, residual,
+//                        Huber weight and Jacobian row of each pixel, and the chunk's fp64 partial sums (warp butterfly,
+//                        then the warps in order).  The CTA takes an integer ticket; the last one folds the partials in
+//                        chunk order (ordered_sum8), solves the scaled 8 x 8 (6 x 6) normal equations by Cholesky, writes
+//                        the next state and re-arms the ticket
+//   track_output_kernel  one thread: pose, nodes and record (init_pose / init_nodes for a failed frame)
+//
+// The state (pose, M = ref^-1 T, s, t, done flag, status, counters) lives in the workspace.  Every CTA copies it to
+// shared memory before it does anything else, so strictly before it takes the ticket; the last CTA, which rewrites it,
+// takes the ticket after every other CTA of the launch has read it.  One buffer is therefore enough.  A stopped frame's
+// later launches return after reading the done flag, so the launch sequence is fixed and a call can be captured in a
+// CUDA graph.  The association, the Jacobian and the exponential are explicit round-to-nearest fp64 operations (no
+// contraction into FMAs), so that the oracle reproduces every association decision.  No floating-point atomics; built
+// without fast-math.
+#include <cmath>
+
+#include "common.cuh"
+#include "fp64.cuh"
+#include "host_util.h"
+#include "../../include/omnidata_b200.h"
+
+namespace odb {
+
+constexpr int kTrkThreads = 256;
+constexpr int kChunk = 8 * kTrkThreads;           // pixels per CTA: depends on nothing but this constant
+constexpr int kUnknowns = 8;
+constexpr int kTri = kUnknowns * (kUnknowns + 1) / 2;
+// partial sums: 0..35 the upper triangle of sum w J J^T (row-major, i <= j), 36..43 sum w J e, then these
+constexpr int kG = kTri, kCount = kG + kUnknowns, kWE2 = kCount + 1, kWSum = kCount + 2, kDown = kCount + 3,
+              kValid = kCount + 4, kSums = kCount + 5;
+constexpr int kPart = 64;                         // doubles per chunk partial (two ordered_sum8 column blocks)
+constexpr double kPivotMin = 1e-6;                // smallest Cholesky pivot of the unit-diagonal matrix (not tuned)
+constexpr double kSeriesTheta = 1e-2;             // |omega| below this: series for the exponential's coefficients
+constexpr double kPi = 3.141592653589793;
+// state [kState] doubles
+constexpr int kT = 0, kM = 12, kS = 24, kSh = 25, kDone = 26, kStatus = 27, kIters = 28, kCorr = 29, kRms = 30,
+              kFrac = 31, kNValid = 32, kState = 34;
+constexpr int kStatusOk = 0, kNoOverlap = 1, kDegenerate = 2, kNonfinite = 3;
+
+struct TrkParams {
+  int h, w, affine, unknowns;
+  double fx, fy, cx, cy, tol, robust, max_dist, min_overlap;
+  double ref[12], init[12];                       // R row-major (9), then t (3), of camera-to-world
+};
+
+static int trk_chunks(int h, int w) { return (int)(((long long)h * w + kChunk - 1) / kChunk); }
+
+ODB_DEVINL double dot3_rn(const double u[3], const double v[3]) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(u[0], v[0]), __dmul_rn(u[1], v[1])), __dmul_rn(u[2], v[2]));
+}
+
+// M = ref^-1 T: Rm = Rref^T R, tm = Rref^T (t - tref)
+ODB_DEVINL void relative_pose(const double* ref, const double* T, double* M) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+      M[3 * i + j] = __dadd_rn(__dadd_rn(__dmul_rn(ref[i], T[j]), __dmul_rn(ref[3 + i], T[3 + j])),
+                               __dmul_rn(ref[6 + i], T[6 + j]));
+    M[9 + i] = __dadd_rn(__dadd_rn(__dmul_rn(ref[i], __dsub_rn(T[9], ref[9])),
+                                   __dmul_rn(ref[3 + i], __dsub_rn(T[10], ref[10]))),
+                         __dmul_rn(ref[6 + i], __dsub_rn(T[11], ref[11])));
+  }
+}
+
+// exp of the twist (v, omega): R = I + A W + B W^2, u = (I + B W + C W^2) v with W = [omega]x, W^2 = omega omega^T -
+// theta^2 I, A = sin(theta) / theta, B = (1 - cos(theta)) / theta^2, C = (theta - sin(theta)) / theta^3; below
+// kSeriesTheta the Taylor series to theta^4
+ODB_DEVINL void se3_exp(const double xi[6], double R[9], double u[3]) {
+  const double om[3] = {xi[3], xi[4], xi[5]};
+  const double th2 = dot3_rn(om, om), th = __dsqrt_rn(th2);
+  double A, B, C;
+  if (th < kSeriesTheta) {
+    const double th4 = __dmul_rn(th2, th2);
+    A = __dadd_rn(__dsub_rn(1.0, __ddiv_rn(th2, 6.0)), __ddiv_rn(th4, 120.0));
+    B = __dadd_rn(__dsub_rn(0.5, __ddiv_rn(th2, 24.0)), __ddiv_rn(th4, 720.0));
+    C = __dadd_rn(__dsub_rn(1.0 / 6.0, __ddiv_rn(th2, 120.0)), __ddiv_rn(th4, 5040.0));
+  } else {
+    double sn, cs;                                  // sin(theta), cos(theta); no Payne-Hanek path (no stack frame)
+    sincospi(__ddiv_rn(th, kPi), &sn, &cs);
+    A = __ddiv_rn(sn, th);
+    B = __ddiv_rn(__dsub_rn(1.0, cs), th2);
+    C = __ddiv_rn(__dsub_rn(th, sn), __dmul_rn(th2, th));
+  }
+  const double W[9] = {0.0, -om[2], om[1], om[2], 0.0, -om[0], -om[1], om[0], 0.0};
+  double V[9];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      const double w2 = i == j ? __dsub_rn(__dmul_rn(om[i], om[j]), th2) : __dmul_rn(om[i], om[j]);
+      const double id = i == j ? 1.0 : 0.0;
+      R[3 * i + j] = __dadd_rn(__dadd_rn(id, __dmul_rn(A, W[3 * i + j])), __dmul_rn(B, w2));
+      V[3 * i + j] = __dadd_rn(__dadd_rn(id, __dmul_rn(B, W[3 * i + j])), __dmul_rn(C, w2));
+    }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) u[i] = dot3_rn(V + 3 * i, xi);
+}
+
+__global__ void track_setup_kernel(TrkParams P, const double* __restrict__ init_nodes, double* __restrict__ st) {
+  if (threadIdx.x != 0) return;
+  const double s = P.affine ? init_nodes[0] : 1.0, t = P.affine ? init_nodes[1] : 0.0;
+  for (int k = 0; k < 12; ++k) st[kT + k] = P.init[k];
+  relative_pose(P.ref, P.init, st + kM);
+  st[kS] = s;
+  st[kSh] = t;
+  const bool bad = !(isfinite(s) && isfinite(t));
+  st[kDone] = bad ? 1.0 : 0.0;
+  st[kStatus] = bad ? kNonfinite : kStatusOk;
+  for (int k = kIters; k < kState; ++k) st[k] = 0.0;
+}
+
+// One pixel's terms added to acc (nothing when it has no correspondence)
+ODB_DEVINL void pixel_terms(const float* __restrict__ pred, const float* __restrict__ ref,
+                            const float* __restrict__ nrm, const TrkParams& P, const double* M, double s, double t,
+                            long long i, double (&acc)[kSums]) {
+  const long long hw = (long long)P.h * P.w;
+  const float af = pred[i];
+  if (!isfinite(af)) return;
+  const double a = af, z = __dadd_rn(__dmul_rn(s, a), t);
+  if (!(z > 0.0)) return;
+  acc[kValid] += 1.0;
+  const int y = (int)(i / P.w), x = (int)(i - (long long)y * P.w);
+  const double r[3] = {__ddiv_rn(__dsub_rn((double)x, P.cx), P.fx), __ddiv_rn(__dsub_rn((double)y, P.cy), P.fy), 1.0};
+  const double Pp[3] = {__dmul_rn(z, r[0]), __dmul_rn(z, r[1]), z};
+  double Q[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) Q[k] = __dadd_rn(dot3_rn(M + 3 * k, Pp), M[9 + k]);
+  if (!(Q[2] > 0.0)) return;
+  const double u = floor(__dadd_rn(__dadd_rn(__ddiv_rn(__dmul_rn(P.fx, Q[0]), Q[2]), P.cx), 0.5));
+  const double v = floor(__dadd_rn(__dadd_rn(__ddiv_rn(__dmul_rn(P.fy, Q[1]), Q[2]), P.cy), 0.5));
+  if (!(u >= 0.0 && u <= (double)(P.w - 1) && v >= 0.0 && v <= (double)(P.h - 1))) return;
+  const long long q = (long long)v * P.w + (long long)u;
+  const float dq = ref[q], c0 = nrm[q], c1 = nrm[hw + q], c2 = nrm[2 * hw + q];
+  if (!(isfinite(dq) && dq > 0.f && isfinite(c0) && isfinite(c1) && isfinite(c2))) return;
+  const double n[3] = {__dsub_rn(__dmul_rn(2.0, (double)c0), 1.0), __dsub_rn(__dmul_rn(2.0, (double)c1), 1.0),
+                       __dsub_rn(__dmul_rn(2.0, (double)c2), 1.0)};
+  const double d = dq;
+  const double Vq[3] = {__dmul_rn(d, __ddiv_rn(__dsub_rn(u, P.cx), P.fx)),
+                        __dmul_rn(d, __ddiv_rn(__dsub_rn(v, P.cy), P.fy)), d};
+  const double df[3] = {__dsub_rn(Q[0], Vq[0]), __dsub_rn(Q[1], Vq[1]), __dsub_rn(Q[2], Vq[2])};
+  if (!(__dsqrt_rn(dot3_rn(df, df)) <= P.max_dist)) return;
+  const double e = dot3_rn(n, df), ae = fabs(e);
+  const double wt = ae <= P.robust ? 1.0 : __ddiv_rn(P.robust, ae);
+  double m[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j)
+    m[j] = __dadd_rn(__dadd_rn(__dmul_rn(M[j], n[0]), __dmul_rn(M[3 + j], n[1])), __dmul_rn(M[6 + j], n[2]));
+  const double ar[3] = {__dmul_rn(a, r[0]), __dmul_rn(a, r[1]), a};
+  const double J[kUnknowns] = {m[0], m[1], m[2],
+                               __dsub_rn(__dmul_rn(Pp[1], m[2]), __dmul_rn(Pp[2], m[1])),
+                               __dsub_rn(__dmul_rn(Pp[2], m[0]), __dmul_rn(Pp[0], m[2])),
+                               __dsub_rn(__dmul_rn(Pp[0], m[1]), __dmul_rn(Pp[1], m[0])),
+                               dot3_rn(m, ar), dot3_rn(m, r)};
+  int k = 0;
+#pragma unroll
+  for (int p = 0; p < kUnknowns; ++p) {
+    const double wj = wt * J[p];
+#pragma unroll
+    for (int c = p; c < kUnknowns; ++c) acc[k++] += wj * J[c];
+    acc[kG + p] += wj * e;
+  }
+  acc[kCount] += 1.0;
+  acc[kWE2] += wt * e * e;
+  acc[kWSum] += wt;
+  acc[kDown] += ae > P.robust ? 1.0 : 0.0;
+}
+
+ODB_DEVINL int tri_index(int i, int j) {          // i <= j
+  return i * kUnknowns - i * (i - 1) / 2 + (j - i);
+}
+
+// The last CTA, thread 0: status, solve result and the next state from the folded sums tot and the factor in band / rhs
+ODB_DEVINL void track_update(const TrkParams& P, const double* tot, const double* band, const double* rhs,
+                             const double* scale, int code, double* st) {
+  const int n = P.unknowns;
+  st[kIters] += 1.0;
+  st[kCorr] = tot[kCount];
+  st[kNValid] = tot[kValid];
+  st[kRms] = tot[kWSum] > 0.0 ? sqrt(tot[kWE2] / tot[kWSum]) : 0.0;
+  st[kFrac] = tot[kCount] > 0.0 ? tot[kDown] / tot[kCount] : 0.0;
+  double x[kUnknowns] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  if (code == kStatusOk) {
+    for (int k = 0; k < n; ++k) {
+      const double l = band[k * n];                 // the factor's diagonal: sqrt of the k-th pivot
+      if (!(__dmul_rn(l, l) >= kPivotMin)) code = kDegenerate;
+    }
+  }
+  if (code == kStatusOk) {
+#pragma unroll
+    for (int k = 0; k < kUnknowns; ++k) {
+      if (k < n) x[k] = __ddiv_rn(rhs[k], scale[k]);
+      if (!isfinite(x[k])) code = kNonfinite;
+    }
+  }
+  double Tn[12];
+  if (code == kStatusOk) {
+    double Re[9], u[3];
+    se3_exp(x, Re, u);
+    const double* T = st + kT;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+#pragma unroll
+      for (int j = 0; j < 3; ++j)
+        Tn[3 * i + j] = __dadd_rn(__dadd_rn(__dmul_rn(T[3 * i], Re[j]), __dmul_rn(T[3 * i + 1], Re[3 + j])),
+                                  __dmul_rn(T[3 * i + 2], Re[6 + j]));
+      Tn[9 + i] = __dadd_rn(dot3_rn(T + 3 * i, u), T[9 + i]);
+    }
+#pragma unroll
+    for (int k = 0; k < 12; ++k)
+      if (!isfinite(Tn[k])) code = kNonfinite;
+  }
+  if (code != kStatusOk) {
+    st[kStatus] = code;
+    st[kDone] = 1.0;
+    return;
+  }
+#pragma unroll
+  for (int k = 0; k < 12; ++k) st[kT + k] = Tn[k];
+  relative_pose(P.ref, Tn, st + kM);
+  st[kS] = __dadd_rn(st[kS], x[6]);
+  st[kSh] = __dadd_rn(st[kSh], x[7]);
+  const double vv[3] = {x[0], x[1], x[2]}, om[3] = {x[3], x[4], x[5]};
+  if (__dsqrt_rn(dot3_rn(om, om)) <= P.tol && __dsqrt_rn(dot3_rn(vv, vv)) <= P.tol && fabs(x[6]) <= P.tol &&
+      fabs(x[7]) <= P.tol)
+    st[kDone] = 1.0;
+}
+
+__global__ void __launch_bounds__(kTrkThreads) track_step_kernel(const float* __restrict__ pred,
+                                                                 const float* __restrict__ ref,
+                                                                 const float* __restrict__ nrm, TrkParams P,
+                                                                 double* __restrict__ st, double* __restrict__ part,
+                                                                 unsigned int* __restrict__ ticket) {
+  __shared__ double S[kDone + 1];
+  __shared__ double red[kTrkThreads / 32][kSums];
+  __shared__ bool last;
+  if (threadIdx.x <= kDone) S[threadIdx.x] = st[threadIdx.x];
+  __syncthreads();
+  if (S[kDone] != 0.0) return;
+  double acc[kSums];
+#pragma unroll
+  for (int k = 0; k < kSums; ++k) acc[k] = 0.0;
+  const long long hw = (long long)P.h * P.w;
+#pragma unroll 1
+  for (int k = 0; k < kChunk / kTrkThreads; ++k) {
+    const long long i = (long long)blockIdx.x * kChunk + k * kTrkThreads + threadIdx.x;
+    if (i < hw) pixel_terms(pred, ref, nrm, P, S + kM, S[kS], S[kSh], i, acc);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < kSums; ++k) {
+    double v = acc[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) red[warp][k] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < kSums) {
+    double v = 0.0;
+#pragma unroll
+    for (int q = 0; q < kTrkThreads / 32; ++q) v += red[q][threadIdx.x];
+    part[(long long)blockIdx.x * kPart + threadIdx.x] = v;
+    __threadfence();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  // fold the partials in chunk order: columns 0..31, then 32..kSums-1
+  __shared__ double tot[kPart];
+  const int col = threadIdx.x & 31;
+  const double lo = ordered_sum8(gridDim.x, true, [&](int c) { return __ldcg(part + (long long)c * kPart + col); });
+  if (threadIdx.x < 32) tot[col] = lo;
+  __syncthreads();
+  const double hi = ordered_sum8(gridDim.x, 32 + col < kSums,
+                                 [&](int c) { return __ldcg(part + (long long)c * kPart + 32 + col); });
+  if (threadIdx.x < 32) tot[32 + col] = hi;
+  __syncthreads();
+  // unit-diagonal scaling D^-1 H D^-1 y = -D^-1 g, x = D^-1 y; the lower band of band_cholesky_solve with w = n
+  __shared__ double band[kUnknowns * kUnknowns], rhs[kUnknowns], scale[kUnknowns];
+  __shared__ int code;
+  const int n = P.unknowns;
+  if (threadIdx.x == 0) {
+    int c = kStatusOk;
+    for (int k = 0; k < kSums; ++k)
+      if (!isfinite(tot[k])) c = kNonfinite;
+    if (c == kStatusOk && !(tot[kValid] > 0.0 && tot[kCount] >= __dmul_rn(P.min_overlap, tot[kValid]) &&
+                            tot[kCount] > 0.0))
+      c = kNoOverlap;
+    if (c == kStatusOk)
+      for (int k = 0; k < n; ++k) {
+        const double hkk = tot[tri_index(k, k)];
+        if (!(hkk > 0.0)) c = kDegenerate;
+        scale[k] = __dsqrt_rn(hkk);
+      }
+    if (c == kStatusOk)
+      for (int r = 0; r < n; ++r) {
+        for (int q = 0; q <= r; ++q) {
+          const int cc = r - q;
+          band[r * n + q] = __ddiv_rn(tot[tri_index(cc, r)], __dmul_rn(scale[r], scale[cc]));
+        }
+        rhs[r] = -__ddiv_rn(tot[kG + r], scale[r]);
+      }
+    code = c;
+  }
+  __syncthreads();
+  if (code == kStatusOk) band_cholesky_solve(band, rhs, n, n);
+  if (threadIdx.x == 0) {
+    track_update(P, tot, band, rhs, scale, code, st);
+    *ticket = 0u;                                   // re-armed for the next launch
+  }
+}
+
+__global__ void track_output_kernel(TrkParams P, const double* __restrict__ init_nodes, const double* __restrict__ st,
+                                    double* __restrict__ pose, double* __restrict__ nodes,
+                                    double* __restrict__ record) {
+  if (threadIdx.x != 0) return;
+  const bool ok = st[kStatus] == (double)kStatusOk;
+  const double* T = ok ? st + kT : P.init;
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) pose[4 * r + c] = T[3 * r + c];
+    pose[4 * r + 3] = T[9 + r];
+  }
+  pose[12] = pose[13] = pose[14] = 0.0;
+  pose[15] = 1.0;
+  double s = 1.0, t = 0.0;
+  if (ok) {
+    s = st[kS];
+    t = st[kSh];
+  } else if (P.affine) {
+    s = init_nodes[0];
+    t = init_nodes[1];
+  }
+  nodes[0] = s;
+  nodes[1] = t;
+  record[0] = st[kCorr];
+  record[1] = st[kStatus];
+  record[2] = st[kRms];
+  record[3] = st[kFrac];
+  record[4] = st[kIters];
+  record[5] = s;
+  record[6] = t;
+  record[7] = st[kNValid];
+}
+
+}  // namespace odb
+
+using namespace odb;
+
+extern "C" int64_t odb_track_workspace_bytes(int32_t h, int32_t w) {
+  if (!planes_ok(1, h, w)) return -1;
+  return (1 + kState + (int64_t)trk_chunks(h, w) * kPart) * (int64_t)sizeof(double);
+}
+
+extern "C" int odb_track_frame(const float* pred, const float* ref_depth, const float* ref_normals, int32_t h,
+                               int32_t w, double fx, double fy, double cx, double cy, const double* ref_pose,
+                               const double* init_pose, const double* init_nodes, int32_t affine, int32_t iterations,
+                               double tol, double robust, double max_dist, double min_overlap, void* workspace,
+                               double* pose, double* nodes, double* record, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!pred || !ref_depth || !ref_normals || !ref_pose || !init_pose || !workspace || !pose || !nodes || !record ||
+      (affine != 0 && affine != 1) || (init_nodes == nullptr) != (affine == 0) || !planes_ok(1, h, w) ||
+      !(std::isfinite(fx) && fx > 0.0 && std::isfinite(fy) && fy > 0.0 && std::isfinite(cx) && std::isfinite(cy)) ||
+      iterations < 1 || iterations > 100 || !(std::isfinite(tol) && tol > 0.0) ||
+      !(std::isfinite(robust) && robust > 0.0) || !(std::isfinite(max_dist) && max_dist > 0.0) ||
+      !(min_overlap > 0.0 && min_overlap <= 1.0) || !aligned(pred, 4) || !aligned(ref_depth, 4) ||
+      !aligned(ref_normals, 4) || !aligned(init_nodes, 8) || !aligned(workspace, 8) || !aligned(pose, 8) ||
+      !aligned(nodes, 8) || !aligned(record, 8))
+    return fail(ODB_ERR_INVALID, "track_frame: bad argument");
+  TrkParams P;
+  if (!pose_ok(ref_pose, P.ref) || !pose_ok(init_pose, P.init))
+    return fail(ODB_ERR_INVALID, "track_frame: a pose is not a finite rigid camera-to-world matrix");
+  P.h = h;
+  P.w = w;
+  P.affine = affine;
+  P.unknowns = affine ? 8 : 6;
+  P.fx = fx; P.fy = fy; P.cx = cx; P.cy = cy;
+  P.tol = tol;
+  P.robust = robust;
+  P.max_dist = max_dist;
+  P.min_overlap = min_overlap;
+  double* ws = static_cast<double*>(workspace);
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(ws);
+  double* st = ws + 1;
+  double* part = st + kState;
+  cudaError_t e = cudaMemsetAsync(ticket, 0, sizeof(double), stream);
+  if (e != cudaSuccess) return fail_cuda(e, "track_frame: cudaMemsetAsync");
+  track_setup_kernel<<<1, 32, 0, stream>>>(P, init_nodes, st);
+  count_launch();
+  const int chunks = trk_chunks(h, w);
+  for (int it = 0; it < iterations; ++it) {
+    track_step_kernel<<<chunks, kTrkThreads, 0, stream>>>(pred, ref_depth, ref_normals, P, st, part, ticket);
+    count_launch();
+  }
+  track_output_kernel<<<1, 32, 0, stream>>>(P, init_nodes, st, pose, nodes, record);
+  count_launch();
+  return check_launch("track_frame");
+}

@@ -443,24 +443,6 @@ static bool cam_ok(double fx, double fy, double cx, double cy, VolCam& K) {
   return true;
 }
 
-// a 4 x 4 row-major camera-to-world matrix: finite, last row 0 0 0 1, |R^T R - I| <= 1e-6 entrywise
-static bool pose_ok(const double* T, double out[12]) {
-  for (int e = 0; e < 16; ++e)
-    if (!std::isfinite(T[e])) return false;
-  if (T[12] != 0.0 || T[13] != 0.0 || T[14] != 0.0 || T[15] != 1.0) return false;
-  for (int a = 0; a < 3; ++a)
-    for (int b = 0; b < 3; ++b) {
-      double s = 0.0;
-      for (int r = 0; r < 3; ++r) s += T[4 * r + a] * T[4 * r + b];
-      if (std::fabs(s - (a == b ? 1.0 : 0.0)) > 1e-6) return false;
-    }
-  for (int r = 0; r < 3; ++r) {
-    for (int c = 0; c < 3; ++c) out[3 * r + c] = T[4 * r + c];
-    out[9 + r] = T[4 * r + 3];
-  }
-  return true;
-}
-
 }  // namespace odb
 
 using namespace odb;

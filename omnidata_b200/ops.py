@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 from typing import Optional, Sequence, Tuple
 
 import numpy as np
@@ -1231,3 +1232,73 @@ def tsdf_mesh_emit(tsdf, weight, color, dims, origin, voxel: float, workspace, v
           _same_device(tsdf, weight, color, workspace, vertices, faces, colors), tsdf.data_ptr(), weight.data_ptr(),
           _ptr(color), *dims, *origin, float(voxel), workspace.data_ptr(), vertices.data_ptr(), faces.data_ptr(),
           _ptr(colors))
+
+
+# ---------------------------------------------------------------- camera tracking (csrc/track.cu)
+TRACK_MAX_ITERATIONS = 100
+
+
+def track_workspace_bytes(h: int, w: int) -> int:
+    _check_planes("track_workspace_bytes", 1, h, w)
+    return int(lib().odb_track_workspace_bytes(h, w))
+
+
+def check_track_params(name: str, affine, iterations, tol: float, robust: float, max_dist: float, min_overlap: float):
+    """OdbError unless affine is a bool, iterations an integer in [1, 100], tol, robust and max_dist finite and > 0, and
+    min_overlap in (0, 1]."""
+    if not isinstance(affine, bool):
+        raise _capi.OdbError(f"{name}: affine must be a bool, got {affine!r}")
+    if isinstance(iterations, bool) or not isinstance(iterations, (int, np.integer)) or \
+            not 1 <= iterations <= TRACK_MAX_ITERATIONS:
+        raise _capi.OdbError(f"{name}: iterations must be an integer in [1, {TRACK_MAX_ITERATIONS}], got "
+                             f"{iterations!r}")
+    for what, v in (("tol", tol), ("robust", robust), ("max_dist", max_dist)):
+        if isinstance(v, bool) or not (isinstance(v, numbers.Real) and math.isfinite(v) and v > 0):
+            raise _capi.OdbError(f"{name}: {what} must be finite and > 0, got {v!r}")
+    if isinstance(min_overlap, bool) or not (isinstance(min_overlap, numbers.Real) and 0 < min_overlap <= 1):
+        raise _capi.OdbError(f"{name}: min_overlap must lie in (0, 1], got {min_overlap!r}")
+
+
+def track_frame(pred, ref_depth, ref_normals, intrinsics, ref_pose, init_pose, init_nodes, affine: bool,
+                iterations: int, tol: float, robust: float, max_dist: float, min_overlap: float, workspace, pose,
+                nodes, record):
+    """pose fp64 [4,4], nodes fp64 [1,1,1,2] and record fp64 [TRACK_RECORD] of pred fp32 [(1,)H,W] tracked against
+    ref_depth fp32 [H,W] and its normals ref_normals fp32 [(1,)3,H,W] (depth_normals with axes (1, 1, 1)) rendered at
+    ref_pose, from init_pose (both host [4,4]) and init_nodes fp64 [1,1,1,2] (exactly when affine)
+    (include/omnidata_b200.h odb_track_frame)."""
+    name = "track_frame"
+    _need(pred, torch.float32, "pred")
+    if pred.dim() == 3 and pred.shape[0] == 1:
+        pred = pred[0]
+    if pred.dim() != 2 or not pred.is_contiguous():
+        raise _capi.OdbError(f"{name}: pred must be a contiguous fp32 [H,W] or [1,H,W] tensor, got "
+                             f"{tuple(pred.shape)}")
+    h, w = pred.shape
+    _check_planes(name, 1, h, w)
+    _need_shape(ref_depth, (h, w), torch.float32, "ref_depth")
+    _need(ref_normals, torch.float32, "ref_normals")
+    if tuple(ref_normals.shape) not in ((3, h, w), (1, 3, h, w)) or not ref_normals.is_contiguous():
+        raise _capi.OdbError(f"{name}: ref_normals must be a contiguous fp32 [3, {h}, {w}] tensor, got "
+                             f"{tuple(ref_normals.shape)}")
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    poses = []
+    for what, T in (("ref_pose", ref_pose), ("init_pose", init_pose)):
+        T = check_poses(f"{name} {what}", T)
+        if T.shape[0] != 1:
+            raise _capi.OdbError(f"{name}: {what} must be one [4,4] pose, got {T.shape[0]}")
+        poses.append(T)
+    check_track_params(name, affine, iterations, tol, robust, max_dist, min_overlap)
+    if affine != (init_nodes is not None):
+        raise _capi.OdbError(f"{name}: init_nodes is required exactly when affine (the initial scale and shift)")
+    if init_nodes is not None:
+        _need_shape(init_nodes, (1, 1, 1, 2), torch.float64, "init_nodes")
+    _check_workspace(name, workspace, track_workspace_bytes(h, w))
+    _need_shape(pose, (4, 4), torch.float64, "pose")
+    _need_shape(nodes, (1, 1, 1, 2), torch.float64, "nodes")
+    _need_shape(record, (_capi.TRACK_RECORD,), torch.float64, "record")
+    _call(name, {"bytes": 20 * h * w * iterations}, lib().odb_track_frame,
+          _same_device(pred, ref_depth, ref_normals, init_nodes, workspace, pose, nodes, record), pred.data_ptr(),
+          ref_depth.data_ptr(), ref_normals.data_ptr(), h, w, fx, fy, cx, cy, poses[0].ctypes.data,
+          poses[1].ctypes.data, _ptr(init_nodes), 1 if affine else 0, int(iterations), float(tol), float(robust),
+          float(max_dist), float(min_overlap), workspace.data_ptr(), pose.data_ptr(), nodes.data_ptr(),
+          record.data_ptr())

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Reconstruct a scene from posed images: predict each frame's depth, align it to metres and to what is already fused,
-integrate it into a TSDF volume on the device, and write the extracted mesh as a PLY:
+"""Reconstruct a scene from images, posed or not: predict each frame's depth, align it to metres and to what is
+already fused, track its camera when it has no pose, integrate it into a TSDF volume on the device, and write the
+extracted mesh as a PLY:
 
-    python reconstruct.py --img_path DIR --pose_path DIR --intrinsics FX,FY,CX,CY --voxel V
-                          --bounds X0,Y0,Z0,X1,Y1,Z1 --out mesh.ply
+    python reconstruct.py --img_path DIR [--pose_path DIR [--track]] --intrinsics FX,FY,CX,CY --voxel V
+                          --bounds X0,Y0,Z0,X1,Y1,Z1 --out mesh.ply [--pose_out DIR]
                           [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
                           [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--guided_size HxW]
                           [--sparse_path DIR [--depth_scale 1000]] [--trunc T]
@@ -20,6 +21,17 @@ metres; 0 is no measurement).  Otherwise it is the volume's own raycast at the f
 to what is already fused.  Frame 0 must have sparse depths: they fix the scene's metric scale.  The aligned depth is
 integrated (`TSDFVolume`).  A frame whose fit fails (fewer than two target pixels, a flat prediction) is skipped and
 named in the summary.
+
+Without --pose_path the cameras are tracked (`FrameTracker`, point-to-plane ICP against the volume).  This mode and
+--track are experimental: tracking against the fused model drifts (on the analytic test scene at 12.5 mm voxels, 13.5
+mm over 48 frames, and refined poses end a mean 6.8 mm from the truth when given 20 mm off; DESIGN.md §6).  Frame 0's pose is
+the identity, so --bounds are in frame 0's camera coordinates (x right, y down, z forward); frame 0 still needs sparse
+depths.  Every later frame starts from the last tracked pose: the volume is raycast there, one scale and shift is fitted
+as above (to the frame's sparse depths when it has them, then the aligned metres are tracked with the pose alone;
+otherwise to that raycast, then the scale and shift are tracked with the pose), and the frame is integrated at the
+tracked pose.  A frame whose fit or tracking fails is skipped and named with its status; the next frame starts from the
+last good pose.  With --pose_path and --track the given poses are the initial guesses (pose refinement).  --pose_out
+DIR writes each used frame's pose as <stem>.txt, in the format --pose_path reads.
 
 Prints one JSON line: frames used and skipped, vertices, faces and seconds.  Runs on cuda:0; there is no CPU path.
 """
@@ -67,7 +79,12 @@ def parse_args(argv=None):
     from omnidata_b200.volume import MAX_DIM, MAX_POINTS
     ap = argparse.ArgumentParser(description="Fuse depth predictions of posed images into a TSDF volume and a mesh")
     ap.add_argument("--img_path", required=True, help="directory of RGB frames")
-    ap.add_argument("--pose_path", required=True, help="directory of <stem>.txt camera-to-world 4 x 4 poses")
+    ap.add_argument("--pose_path", default=None,
+                    help="directory of <stem>.txt camera-to-world 4 x 4 poses (without it the cameras are tracked, "
+                         "experimental)")
+    ap.add_argument("--track", action="store_true",
+                    help="experimental: with --pose_path, refine the given poses by tracking against the volume")
+    ap.add_argument("--pose_out", default=None, metavar="DIR", help="write each used frame's pose as <stem>.txt")
     ap.add_argument("--intrinsics", required=True, type=evaluate._intrinsics, metavar="FX,FY,CX,CY",
                     help="camera intrinsics in pixels of the frames")
     ap.add_argument("--voxel", required=True, type=float, help="grid spacing in metres")
@@ -105,6 +122,10 @@ def parse_args(argv=None):
         ap.error(f"--depth_scale must be finite and > 0, got {args.depth_scale}")
     if args.trunc is not None and not (math.isfinite(args.trunc) and args.trunc > 0):
         ap.error(f"--trunc must be finite and > 0, got {args.trunc}")
+    if args.track and args.pose_path is None:
+        ap.error("--track refines the poses of --pose_path; without --pose_path every frame is tracked already")
+    if args.pose_out is not None and Path(args.pose_out).exists() and not Path(args.pose_out).is_dir():
+        ap.error(f"--pose_out must be a directory, got the file {args.pose_out}")
     if args.mode == "guided":
         if args.guided_size is None:
             ap.error("--mode guided needs --guided_size HxW")
@@ -126,21 +147,58 @@ def align_and_integrate(volume, aligner, pred: torch.Tensor, intrinsics, pose: n
     return rec, (float(st[0]), float(st[1]))
 
 
+def track_and_integrate(volume, aligner, trackers, pred: torch.Tensor, intrinsics, init_pose: np.ndarray,
+                        sparse=None):
+    """One frame of the tracking loop: raycast the volume at init_pose, fit pred fp32 [1,H,W] with the aligner to
+    sparse [1,H,W] (metres, 0 = none) or, without it, to that raycast, track it (trackers[False] on the aligned metres
+    with sparse, else trackers[True] on pred with the fitted (s, t) as initial nodes), and integrate the aligned depth at
+    the tracked pose.  Returns (failure, pose, (s, t)): failure None when the frame was integrated, else
+    "fit: <status>" or "track: <status>"; pose the tracked host float64 [4,4] (None on failure)."""
+    from omnidata_b200.sparse import STATUS as FIT_STATUS
+    from omnidata_b200.track import STATUS as TRACK_STATUS
+    h, w = pred.shape[-2:]
+    ref = volume.raycast(intrinsics, init_pose, (h, w))
+    nodes, rec = aligner.fit(pred, sparse if sparse is not None else ref.unsqueeze(0))
+    status = int(rec[0, 1].item())
+    if status != 0:
+        return f"fit: {FIT_STATUS[status]}", None, None
+    if sparse is not None:
+        metres = aligner.apply(pred, nodes)
+        pose, _, trec = trackers[False].track(metres, ref, intrinsics, init_pose)
+    else:
+        pose, nodes, trec = trackers[True].track(pred, ref, intrinsics, init_pose, init_nodes=nodes)
+        metres = aligner.apply(pred, nodes)
+    status = int(trec[1].item())
+    if status != 0:
+        return f"track: {TRACK_STATUS[status]}", None, None
+    pose = pose.cpu().numpy()
+    volume.integrate(metres, intrinsics, pose)
+    st = nodes.reshape(2).cpu()
+    return None, pose, (float(st[0]), float(st[1]))
+
+
 def reconstruct(args) -> dict:
     from omnidata_b200.sparse import STATUS, SparseDepthAligner
+    from omnidata_b200.track import FrameTracker
     from omnidata_b200.volume import TSDFVolume, write_ply
     t0 = time.perf_counter()
     device = torch.device("cuda:0")
     images = sorted(p for p in Path(args.img_path).iterdir() if p.suffix.lower() in evaluate.IMAGE_EXT)
     if not images:
         raise FileNotFoundError(f"no images in {args.img_path}")
-    poses = [load_pose(Path(args.pose_path) / (p.stem + ".txt")) for p in images]
+    posed = args.pose_path is not None
+    poses = [load_pose(Path(args.pose_path) / (p.stem + ".txt")) for p in images] if posed else [None] * len(images)
     evaluate._find(args.sparse_path, images[0].stem, "sparse depth for frame 0")
     model = evaluate.build_model("depth", args.backbone, args.checkpoint, args.synthetic_weights, args.precision,
                                  device)
     guided = (args.guided_size, 4, 1e-3) if args.mode == "guided" else None
     volume = TSDFVolume(args.origin, args.voxel, args.dims, trunc=args.trunc, device=device)
     aligner = SparseDepthAligner(grid=(1, 1), robust=ROBUST)
+    tracking = args.track or not posed
+    trackers = {a: FrameTracker(affine=a) for a in (False, True)} if tracking else None
+    if args.pose_out is not None:
+        Path(args.pose_out).mkdir(parents=True, exist_ok=True)
+    last = np.eye(4)                                  # the last good pose: frame 0's without --pose_path
     used, skipped = [], []
     for q, (p, pose) in enumerate(zip(images, poses)):
         x = evaluate.image_tensor(p, "depth").to(device)
@@ -156,12 +214,20 @@ def reconstruct(args) -> dict:
                 raise ValueError(f"{p.name}: the sparse depth is {sp.shape[0]}x{sp.shape[1]}, the image "
                                  f"{pred.shape[-2]}x{pred.shape[-1]}")
             sparse = torch.from_numpy(sp).unsqueeze(0).to(device)
-        rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse)
-        status = int(rec[1])
-        if status == 0:
-            used.append(p.name)
+        if tracking and used:
+            failure, pose, _ = track_and_integrate(volume, aligner, trackers, pred, args.intrinsics,
+                                                   pose if posed else last, sparse)
         else:
-            skipped.append({"frame": p.name, "status": STATUS[status]})
+            pose = last if pose is None else pose
+            rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse)
+            failure = None if int(rec[1]) == 0 else STATUS[int(rec[1])]
+        if failure is None:
+            used.append(p.name)
+            last = pose
+            if args.pose_out is not None:
+                np.savetxt(Path(args.pose_out) / (p.stem + ".txt"), pose)
+        else:
+            skipped.append({"frame": p.name, "status": failure})
     vertices, faces, _ = volume.extract_mesh()
     write_ply(args.out, vertices, faces)
     return {"frames": len(images), "frames_used": len(used), "frames_skipped": skipped,
