@@ -731,6 +731,9 @@ int odb_depth_normals(const float* depth, const void* mask, int32_t mask_dtype, 
  * (n - 1)]; samples at t_k = t_enter + k step (step finite in [voxel / 64, voxel]) while t_k <= t_exit are trilinear
  * interpolations of F, valid when all 8 corners have W > 0.  The hit is the first pair of valid samples k, k + 1 with
  * F_k > 0 >= F_k+1 at t_k + step F_k / (F_k - F_k+1); out = that t / |r|.  fp64 round-to-nearest over the fp32 loads.
+ * odb_tsdf_raycast_color: the same out, bit for bit, and rgb fp32 [3][h][w] = the colour at the hit, NaN where out = 0:
+ * the colour trilinearly interpolated (the same corners and x, y, z order as F) at t_k and at t_k+1, blended as
+ * c_k + f (c_k+1 - c_k) with f = F_k / (F_k - F_k+1).  The colour is read only at the hit.
  *
  * odb_tsdf_mesh_count + odb_tsdf_mesh_emit: marching tetrahedra on the Kuhn split of each cell into 6 tetrahedra (one
  * per permutation of the axes).  Each point p owns the 7 lattice edges (p, p + d), d in {0,1}^3 \ {0}, direction index
@@ -755,6 +758,10 @@ int odb_tsdf_integrate(float* tsdf, float* weight, float* color, int32_t nx, int
 int odb_tsdf_raycast(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz, double ox, double oy,
                      double oz, double voxel, const double* cam_to_world, int32_t h, int32_t w, double fx, double fy,
                      double cx, double cy, double step, float* out, void* stream);
+int odb_tsdf_raycast_color(const float* tsdf, const float* weight, const float* color, int32_t nx, int32_t ny,
+                           int32_t nz, double ox, double oy, double oz, double voxel, const double* cam_to_world,
+                           int32_t h, int32_t w, double fx, double fy, double cx, double cy, double step, float* out,
+                           float* rgb, void* stream);
 int odb_tsdf_mesh_count(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz, void* workspace,
                         int64_t* counts, void* stream);
 int odb_tsdf_mesh_emit(const float* tsdf, const float* weight, const float* color, int32_t nx, int32_t ny, int32_t nz,
@@ -796,6 +803,29 @@ int odb_track_frame(const float* pred, const float* ref_depth, const float* ref_
                     const double* init_nodes, int32_t affine, int32_t iterations, double tol, double robust,
                     double max_dist, double min_overlap, void* workspace, double* pose, double* nodes, double* record,
                     void* stream);
+
+/* odb_track_frame_rgbd: odb_track_frame with a photometric term (DESIGN.md §3 "Camera tracking", photometric term;
+ * oracle/photometric_oracle.py restates it in float64).
+ * rgb fp32 [3][h][w] is the frame's image and ref_rgb fp32 [3][h][w] the model's colour at ref_pose (NaN: none), both
+ * in [0, 1]; ref_intensity fp32 [3][h][w] is scratch the call overwrites with the reference's (Y, g_u, g_v).
+ * photometric = lambda finite > 0 (m^2 per squared intensity step), photometric_robust = delta_c finite > 0.
+ * Luminance Y = (0.299 R + 0.587 G) + 0.114 B.  A reference pixel is usable with a surface, a finite colour and a usable
+ * normal; its gradient (g_u, g_v) is the 3 x 3 Sobel kernel / 8, defined when all 9 window pixels lie in the image, are
+ * usable and differ in depth from the centre by at most 5 % of the centre's depth.  Each correspondence of the
+ * geometric term whose unrounded projection (u, v) has its bilinear base (floor u, floor v) in [0, w - 2] x [0, h - 2],
+ * with finite Y and gradient at the four corners and a finite frame luminance, adds a term: Y, g_u, g_v interpolated x
+ * first, e_c = Y_ref(u, v) - Y_frame(p), w_c = min(1, delta_c / |e_c|), the row (m_c, P x m_c, m_c.(a r), m_c.r) with
+ * m_c = Rm^T g3, g3 = (g_u fx / Q.z, g_v fy / Q.z, -(g_u fx Q.x + g_v fy Q.y) / Q.z^2), weighted by lambda w_c.  Stopping,
+ * statuses and min_overlap (geometric correspondences) are odb_track_frame's.  record fp64 [ODB_TRACK_RGBD_RECORD]:
+ * columns 0..7 as odb_track_frame's, then (photometric terms of the last iteration, weighted RMS of e_c, fraction with
+ * w_c < 1).  One launch more than odb_track_frame (the reference gradient), same workspace. */
+#define ODB_TRACK_RGBD_RECORD 11
+int odb_track_frame_rgbd(const float* pred, const float* rgb, const float* ref_depth, const float* ref_rgb,
+                         const float* ref_normals, float* ref_intensity, int32_t h, int32_t w, double fx, double fy,
+                         double cx, double cy, const double* ref_pose, const double* init_pose,
+                         const double* init_nodes, int32_t affine, int32_t iterations, double tol, double robust,
+                         double max_dist, double min_overlap, double photometric, double photometric_robust,
+                         void* workspace, double* pose, double* nodes, double* record, void* stream);
 
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *

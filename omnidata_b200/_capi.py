@@ -30,6 +30,7 @@ FUSION_RECORD = 8                               # ODB_FUSION_RECORD
 TSDF_MAX_DIM = 2048                             # ODB_TSDF_MAX_DIM
 TSDF_MAX_POINTS = 1 << 28                       # ODB_TSDF_MAX_POINTS
 TRACK_RECORD = 8                                # ODB_TRACK_RECORD
+TRACK_RGBD_RECORD = 11                          # ODB_TRACK_RGBD_RECORD
 
 
 class OdbError(RuntimeError):
@@ -248,11 +249,15 @@ _SIGNATURES = {
                            [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] * 2),
     "odb_tsdf_raycast": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] +
                          [C.c_int32] * 2 + [C.c_double] * 5 + [C.c_void_p] * 2),
+    "odb_tsdf_raycast_color": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] +
+                               [C.c_int32] * 2 + [C.c_double] * 5 + [C.c_void_p] * 3),
     "odb_tsdf_mesh_count": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p] * 3),
     "odb_tsdf_mesh_emit": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] * 5),
     "odb_track_workspace_bytes": (C.c_int64, [C.c_int32] * 2),
     "odb_track_frame": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 3 +
                         [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 5),
+    "odb_track_frame_rgbd": (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 3 +
+                             [C.c_int32] * 2 + [C.c_double] * 6 + [C.c_void_p] * 5),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

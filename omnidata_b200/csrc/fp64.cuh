@@ -1,7 +1,8 @@
 // fp64 routines shared by the post-processing kernels: the SPD band solve of the tiled, ensemble and sparse alignments
 // (tiled.cu, ensemble.cu, sparse.cu), the angle between two vectors of the normal metrics and the normal ensemble merge
 // (metrics.cu, ensemble.cu), and the valid set and clamped depth of the depth metrics and the sparse alignment
-// (metrics.cu, sparse.cu).  Callers are built without fast-math.
+// (metrics.cu, sparse.cu), and the round-to-nearest linear interpolation of the TSDF raycast and the tracker's bilinear
+// lookups (volume.cu, track.cu).  Callers are built without fast-math.
 #pragma once
 #include "common.cuh"
 #include "../../include/omnidata_b200.h"
@@ -16,6 +17,9 @@ ODB_DEVINL bool mask_valid(const void* mask, int kind, long long i) {
   if (kind == ODB_MASK_F32) return static_cast<const float*>(mask)[i] != 0.0f;
   return true;
 }
+
+// a + t (b - a), each operation rounded to nearest
+ODB_DEVINL double lerp_rn(double a, double b, double t) { return __dadd_rn(a, __dmul_rn(t, __dsub_rn(b, a))); }
 
 ODB_DEVINL bool depth_valid(double g, double min_depth, double max_depth) {
   return isfinite(g) && g > min_depth && g <= max_depth;           // max_depth = +inf when not given

@@ -1,14 +1,19 @@
 // Camera tracking (omnidata_b200/track.py FrameTracker): one frame's pose, and with `affine` the scale and shift of its
 // depth, solved against a model depth map rendered at a reference pose (normally TSDFVolume.raycast) by point-to-plane
 // ICP with projective association (KinectFusion, Newcombe et al. 2011).  Definition in DESIGN.md §3 "Camera tracking"
-// and include/omnidata_b200.h; oracle/track_oracle.py restates it in float64.
+// and include/omnidata_b200.h; oracle/track_oracle.py restates it in float64, oracle/photometric_oracle.py the
+// photometric term.
 //
+//   track_intensity_kernel  (photometric only) one thread per reference pixel: luminance and Sobel gradient of
+//                        ref_rgb into the fp32 planes the tracker keeps
 //   track_setup_kernel   one thread: the state from init_pose (by value) and init_nodes (device)
 //   track_step_kernel    one Gauss-Newton iteration per launch.  Per fixed chunk of kChunk pixels: association, residual,
 //                        Huber weight and Jacobian row of each pixel, and the chunk's fp64 partial sums (warp butterfly,
 //                        then the warps in order).  The CTA takes an integer ticket; the last one folds the partials in
 //                        chunk order (ordered_sum8), solves the scaled 8 x 8 (6 x 6) normal equations by Cholesky, writes
-//                        the next state and re-arms the ticket
+//                        the next state and re-arms the ticket.  Templated on kPhoto: the photometric instantiation
+//                        adds each correspondence's colour term to the same sums, so the geometric arithmetic exists
+//                        once
 //   track_output_kernel  one thread: pose, nodes and record (init_pose / init_nodes for a failed frame)
 //
 // The state (pose, M = ref^-1 T, s, t, done flag, status, counters) lives in the workspace.  Every CTA copies it to
@@ -19,6 +24,7 @@
 // contraction into FMAs), so that the oracle reproduces every association decision.  No floating-point atomics; built
 // without fast-math.
 #include <cmath>
+#include <string>
 
 #include "common.cuh"
 #include "fp64.cuh"
@@ -34,6 +40,8 @@ constexpr int kTri = kUnknowns * (kUnknowns + 1) / 2;
 // partial sums: 0..35 the upper triangle of sum w J J^T (row-major, i <= j), 36..43 sum w J e, then these
 constexpr int kG = kTri, kCount = kG + kUnknowns, kWE2 = kCount + 1, kWSum = kCount + 2, kDown = kCount + 3,
               kValid = kCount + 4, kSums = kCount + 5;
+// the photometric instantiation's four more: count, sum w_c e_c^2, sum w_c and the count with w_c < 1
+constexpr int kPCount = kSums, kPWE2 = kSums + 1, kPWSum = kSums + 2, kPDown = kSums + 3, kSumsRgbd = kSums + 4;
 constexpr int kPart = 64;                         // doubles per chunk partial (two ordered_sum8 column blocks)
 constexpr double kPivotMin = 1e-6;                // smallest Cholesky pivot of the unit-diagonal matrix (not tuned)
 constexpr double kSeriesTheta = 1e-2;             // |omega| below this: series for the exponential's coefficients
@@ -42,10 +50,13 @@ constexpr double kPi = 3.141592653589793;
 constexpr int kT = 0, kM = 12, kS = 24, kSh = 25, kDone = 26, kStatus = 27, kIters = 28, kCorr = 29, kRms = 30,
               kFrac = 31, kNValid = 32, kState = 34;
 constexpr int kStatusOk = 0, kNoOverlap = 1, kDegenerate = 2, kNonfinite = 3;
+// luminance weights (ITU-R BT.601) and the largest depth step inside a gradient window, relative to its centre
+constexpr double kLumR = 0.299, kLumG = 0.587, kLumB = 0.114, kStepRel = 0.05;
 
 struct TrkParams {
   int h, w, affine, unknowns;
   double fx, fy, cx, cy, tol, robust, max_dist, min_overlap;
+  double photometric, photometric_robust;         // lambda and delta_c (the photometric instantiation only)
   double ref[12], init[12];                       // R row-major (9), then t (3), of camera-to-world
 };
 
@@ -53,6 +64,11 @@ static int trk_chunks(int h, int w) { return (int)(((long long)h * w + kChunk - 
 
 ODB_DEVINL double dot3_rn(const double u[3], const double v[3]) {
   return __dadd_rn(__dadd_rn(__dmul_rn(u[0], v[0]), __dmul_rn(u[1], v[1])), __dmul_rn(u[2], v[2]));
+}
+
+// Y = (0.299 R + 0.587 G) + 0.114 B
+ODB_DEVINL double luminance(float r, float g, float b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(kLumR, (double)r), __dmul_rn(kLumG, (double)g)), __dmul_rn(kLumB, (double)b));
 }
 
 // M = ref^-1 T: Rm = Rref^T R, tm = Rref^T (t - tref)
@@ -103,8 +119,62 @@ ODB_DEVINL void se3_exp(const double xi[6], double R[9], double u[3]) {
   for (int i = 0; i < 3; ++i) u[i] = dot3_rn(V + 3 * i, xi);
 }
 
-__global__ void track_setup_kernel(TrkParams P, const double* __restrict__ init_nodes, double* __restrict__ st) {
+// A reference pixel is usable with a surface, a finite colour and a usable normal; its luminance Y in fp64
+ODB_DEVINL bool usable_pixel(const float* __restrict__ ref, const float* __restrict__ rgb,
+                             const float* __restrict__ nrm, long long hw, long long q, double& d, double& Y) {
+  const float dq = ref[q], r = rgb[q], g = rgb[hw + q], b = rgb[2 * hw + q];
+  if (!(isfinite(dq) && dq > 0.f && isfinite(r) && isfinite(g) && isfinite(b) && isfinite(nrm[q]) &&
+        isfinite(nrm[hw + q]) && isfinite(nrm[2 * hw + q])))
+    return false;
+  d = dq;
+  Y = luminance(r, g, b);
+  return true;
+}
+
+// ig [3][h][w] = (Y, g_u, g_v) rounded to fp32: Y NaN unless the pixel is usable; the 3 x 3 Sobel gradient / 8 NaN
+// unless the window lies in the image, all 9 pixels are usable and none lies further in depth from the centre than
+// kStepRel of the centre's depth (depth_normals keeps one-sided normals at a depth step, so the normals alone do not
+// keep occlusion edges out)
+__global__ void __launch_bounds__(kTrkThreads) track_intensity_kernel(const float* __restrict__ ref,
+                                                                      const float* __restrict__ rgb,
+                                                                      const float* __restrict__ nrm, int h, int w,
+                                                                      float* __restrict__ ig) {
+  const long long hw = (long long)h * w;
+  const long long i = (long long)blockIdx.x * kTrkThreads + threadIdx.x;
+  if (i >= hw) return;
+  const int y = (int)(i / w), x = (int)(i - (long long)y * w);
+  double dc = 0.0, Yc = 0.0;
+  const bool uc = usable_pixel(ref, rgb, nrm, hw, i, dc, Yc);
+  float gu = NAN, gv = NAN;
+  if (uc && x >= 1 && x <= w - 2 && y >= 1 && y <= h - 2) {
+    const double lim = __dmul_rn(kStepRel, dc);
+    double Yw[9];
+    bool ok = true;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+      double dk = 0.0;
+      Yw[k] = 0.0;
+      if (!usable_pixel(ref, rgb, nrm, hw, i + (long long)(k / 3 - 1) * w + (k % 3 - 1), dk, Yw[k]) ||
+          !(fabs(__dsub_rn(dk, dc)) <= lim))
+        ok = false;
+    }
+    if (ok) {                                     // Yw[3 j + k]: row y + j - 1, column x + k - 1
+      const double dx0 = __dsub_rn(Yw[2], Yw[0]), dx1 = __dsub_rn(Yw[5], Yw[3]), dx2 = __dsub_rn(Yw[8], Yw[6]);
+      const double dy0 = __dsub_rn(Yw[6], Yw[0]), dy1 = __dsub_rn(Yw[7], Yw[1]), dy2 = __dsub_rn(Yw[8], Yw[2]);
+      gu = (float)__ddiv_rn(__dadd_rn(__dadd_rn(dx0, __dmul_rn(2.0, dx1)), dx2), 8.0);
+      gv = (float)__ddiv_rn(__dadd_rn(__dadd_rn(dy0, __dmul_rn(2.0, dy1)), dy2), 8.0);
+    }
+  }
+  ig[i] = uc ? (float)Yc : NAN;
+  ig[hw + i] = gu;
+  ig[2 * hw + i] = gv;
+}
+
+// prec: the photometric record columns 8..10 (NULL without the photometric term), zero until a step writes them
+__global__ void track_setup_kernel(TrkParams P, const double* __restrict__ init_nodes, double* __restrict__ st,
+                                   double* __restrict__ prec) {
   if (threadIdx.x != 0) return;
+  if (prec) prec[0] = prec[1] = prec[2] = 0.0;
   const double s = P.affine ? init_nodes[0] : 1.0, t = P.affine ? init_nodes[1] : 0.0;
   for (int k = 0; k < 12; ++k) st[kT + k] = P.init[k];
   relative_pose(P.ref, P.init, st + kM);
@@ -116,10 +186,48 @@ __global__ void track_setup_kernel(TrkParams P, const double* __restrict__ init_
   for (int k = kIters; k < kState; ++k) st[k] = 0.0;
 }
 
-// One pixel's terms added to acc (nothing when it has no correspondence)
+// w J J^T and w J e added to the sums (upper triangle row-major, then the gradient)
+template <int N>
+ODB_DEVINL void add_row(double (&acc)[N], const double (&J)[kUnknowns], double wt, double e) {
+  int k = 0;
+#pragma unroll
+  for (int p = 0; p < kUnknowns; ++p) {
+    const double wj = wt * J[p];
+#pragma unroll
+    for (int c = p; c < kUnknowns; ++c) acc[k++] += wj * J[c];
+    acc[kG + p] += wj * e;
+  }
+}
+
+// the Jacobian row (m, P x m, m.(a r), m.r) with m = Rm^T g for a residual whose gradient with respect to Q is g
+ODB_DEVINL void jacobian_row(const double* M, const double g[3], const double Pp[3], const double r[3], double a,
+                             double (&J)[kUnknowns]) {
+  double m[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j)
+    m[j] = __dadd_rn(__dadd_rn(__dmul_rn(M[j], g[0]), __dmul_rn(M[3 + j], g[1])), __dmul_rn(M[6 + j], g[2]));
+  const double ar[3] = {__dmul_rn(a, r[0]), __dmul_rn(a, r[1]), a};
+  J[0] = m[0];
+  J[1] = m[1];
+  J[2] = m[2];
+  J[3] = __dsub_rn(__dmul_rn(Pp[1], m[2]), __dmul_rn(Pp[2], m[1]));
+  J[4] = __dsub_rn(__dmul_rn(Pp[2], m[0]), __dmul_rn(Pp[0], m[2]));
+  J[5] = __dsub_rn(__dmul_rn(Pp[0], m[1]), __dmul_rn(Pp[1], m[0]));
+  J[6] = dot3_rn(m, ar);
+  J[7] = dot3_rn(m, r);
+}
+
+// The photometric inputs of one pixel's term (kPhoto): the frame's rgb [3][h][w] and the reference's (Y, g_u, g_v)
+struct PhotoIn {
+  const float* rgb;
+  const float* ig;
+};
+
+// One pixel's terms added to acc (nothing when it has no correspondence); with kPhoto also its photometric term
+template <bool kPhoto, int N>
 ODB_DEVINL void pixel_terms(const float* __restrict__ pred, const float* __restrict__ ref,
-                            const float* __restrict__ nrm, const TrkParams& P, const double* M, double s, double t,
-                            long long i, double (&acc)[kSums]) {
+                            const float* __restrict__ nrm, const PhotoIn& C, const TrkParams& P, const double* M,
+                            double s, double t, long long i, double (&acc)[N]) {
   const long long hw = (long long)P.h * P.w;
   const float af = pred[i];
   if (!isfinite(af)) return;
@@ -133,8 +241,9 @@ ODB_DEVINL void pixel_terms(const float* __restrict__ pred, const float* __restr
 #pragma unroll
   for (int k = 0; k < 3; ++k) Q[k] = __dadd_rn(dot3_rn(M + 3 * k, Pp), M[9 + k]);
   if (!(Q[2] > 0.0)) return;
-  const double u = floor(__dadd_rn(__dadd_rn(__ddiv_rn(__dmul_rn(P.fx, Q[0]), Q[2]), P.cx), 0.5));
-  const double v = floor(__dadd_rn(__dadd_rn(__ddiv_rn(__dmul_rn(P.fy, Q[1]), Q[2]), P.cy), 0.5));
+  const double uf = __dadd_rn(__ddiv_rn(__dmul_rn(P.fx, Q[0]), Q[2]), P.cx);
+  const double vf = __dadd_rn(__ddiv_rn(__dmul_rn(P.fy, Q[1]), Q[2]), P.cy);
+  const double u = floor(__dadd_rn(uf, 0.5)), v = floor(__dadd_rn(vf, 0.5));
   if (!(u >= 0.0 && u <= (double)(P.w - 1) && v >= 0.0 && v <= (double)(P.h - 1))) return;
   const long long q = (long long)v * P.w + (long long)u;
   const float dq = ref[q], c0 = nrm[q], c1 = nrm[hw + q], c2 = nrm[2 * hw + q];
@@ -148,28 +257,45 @@ ODB_DEVINL void pixel_terms(const float* __restrict__ pred, const float* __restr
   if (!(__dsqrt_rn(dot3_rn(df, df)) <= P.max_dist)) return;
   const double e = dot3_rn(n, df), ae = fabs(e);
   const double wt = ae <= P.robust ? 1.0 : __ddiv_rn(P.robust, ae);
-  double m[3];
-#pragma unroll
-  for (int j = 0; j < 3; ++j)
-    m[j] = __dadd_rn(__dadd_rn(__dmul_rn(M[j], n[0]), __dmul_rn(M[3 + j], n[1])), __dmul_rn(M[6 + j], n[2]));
-  const double ar[3] = {__dmul_rn(a, r[0]), __dmul_rn(a, r[1]), a};
-  const double J[kUnknowns] = {m[0], m[1], m[2],
-                               __dsub_rn(__dmul_rn(Pp[1], m[2]), __dmul_rn(Pp[2], m[1])),
-                               __dsub_rn(__dmul_rn(Pp[2], m[0]), __dmul_rn(Pp[0], m[2])),
-                               __dsub_rn(__dmul_rn(Pp[0], m[1]), __dmul_rn(Pp[1], m[0])),
-                               dot3_rn(m, ar), dot3_rn(m, r)};
-  int k = 0;
-#pragma unroll
-  for (int p = 0; p < kUnknowns; ++p) {
-    const double wj = wt * J[p];
-#pragma unroll
-    for (int c = p; c < kUnknowns; ++c) acc[k++] += wj * J[c];
-    acc[kG + p] += wj * e;
+  {
+    double J[kUnknowns];
+    jacobian_row(M, n, Pp, r, a, J);
+    add_row(acc, J, wt, e);
   }
   acc[kCount] += 1.0;
   acc[kWE2] += wt * e * e;
   acc[kWSum] += wt;
   acc[kDown] += ae > P.robust ? 1.0 : 0.0;
+  if constexpr (kPhoto) {
+    // bilinear lookup of (Y, g_u, g_v) at the unrounded projection (u, v), x first
+    const double bu = floor(uf), bv = floor(vf);
+    if (!(bu >= 0.0 && bu <= (double)(P.w - 2) && bv >= 0.0 && bv <= (double)(P.h - 2))) return;
+    const long long b0 = (long long)bv * P.w + (long long)bu;
+    const double fu = __dsub_rn(uf, bu), fv = __dsub_rn(vf, bv);
+    double I[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float* pl = C.ig + c * hw + b0;
+      const float x00 = pl[0], x10 = pl[1], x01 = pl[P.w], x11 = pl[P.w + 1];
+      if (!(isfinite(x00) && isfinite(x10) && isfinite(x01) && isfinite(x11))) return;
+      I[c] = lerp_rn(lerp_rn(x00, x10, fu), lerp_rn(x01, x11, fu), fv);
+    }
+    const double Yf = luminance(C.rgb[i], C.rgb[hw + i], C.rgb[2 * hw + i]);
+    if (!isfinite(Yf)) return;
+    const double ec = __dsub_rn(I[0], Yf), aec = fabs(ec);
+    const double wc = aec <= P.photometric_robust ? 1.0 : __ddiv_rn(P.photometric_robust, aec);
+    // d e_c / d Q = (g_u, g_v) d(u, v) / d Q
+    const double gfu = __dmul_rn(I[1], P.fx), gfv = __dmul_rn(I[2], P.fy);
+    const double g3[3] = {__ddiv_rn(gfu, Q[2]), __ddiv_rn(gfv, Q[2]),
+                          -__ddiv_rn(__dadd_rn(__dmul_rn(gfu, Q[0]), __dmul_rn(gfv, Q[1])), __dmul_rn(Q[2], Q[2]))};
+    double J[kUnknowns];
+    jacobian_row(M, g3, Pp, r, a, J);
+    add_row(acc, J, __dmul_rn(P.photometric, wc), ec);
+    acc[kPCount] += 1.0;
+    acc[kPWE2] += wc * ec * ec;
+    acc[kPWSum] += wc;
+    acc[kPDown] += aec > P.photometric_robust ? 1.0 : 0.0;
+  }
 }
 
 ODB_DEVINL int tri_index(int i, int j) {          // i <= j
@@ -232,36 +358,40 @@ ODB_DEVINL void track_update(const TrkParams& P, const double* tot, const double
     st[kDone] = 1.0;
 }
 
+// kPhoto: prec = the record's photometric columns 8..10, written by the last CTA of every launch that runs
+template <bool kPhoto>
 __global__ void __launch_bounds__(kTrkThreads) track_step_kernel(const float* __restrict__ pred,
                                                                  const float* __restrict__ ref,
-                                                                 const float* __restrict__ nrm, TrkParams P,
+                                                                 const float* __restrict__ nrm, PhotoIn C, TrkParams P,
                                                                  double* __restrict__ st, double* __restrict__ part,
-                                                                 unsigned int* __restrict__ ticket) {
+                                                                 unsigned int* __restrict__ ticket,
+                                                                 double* __restrict__ prec) {
+  constexpr int nsums = kPhoto ? kSumsRgbd : kSums;   // partial sums per chunk
   __shared__ double S[kDone + 1];
-  __shared__ double red[kTrkThreads / 32][kSums];
+  __shared__ double red[kTrkThreads / 32][nsums];
   __shared__ bool last;
   if (threadIdx.x <= kDone) S[threadIdx.x] = st[threadIdx.x];
   __syncthreads();
   if (S[kDone] != 0.0) return;
-  double acc[kSums];
+  double acc[nsums];
 #pragma unroll
-  for (int k = 0; k < kSums; ++k) acc[k] = 0.0;
+  for (int k = 0; k < nsums; ++k) acc[k] = 0.0;
   const long long hw = (long long)P.h * P.w;
 #pragma unroll 1
   for (int k = 0; k < kChunk / kTrkThreads; ++k) {
     const long long i = (long long)blockIdx.x * kChunk + k * kTrkThreads + threadIdx.x;
-    if (i < hw) pixel_terms(pred, ref, nrm, P, S + kM, S[kS], S[kSh], i, acc);
+    if (i < hw) pixel_terms<kPhoto>(pred, ref, nrm, C, P, S + kM, S[kS], S[kSh], i, acc);
   }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-  for (int k = 0; k < kSums; ++k) {
+  for (int k = 0; k < nsums; ++k) {
     double v = acc[k];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (lane == 0) red[warp][k] = v;
   }
   __syncthreads();
-  if (threadIdx.x < kSums) {
+  if (threadIdx.x < nsums) {
     double v = 0.0;
 #pragma unroll
     for (int q = 0; q < kTrkThreads / 32; ++q) v += red[q][threadIdx.x];
@@ -273,13 +403,13 @@ __global__ void __launch_bounds__(kTrkThreads) track_step_kernel(const float* __
   __syncthreads();
   if (!last) return;
   __threadfence();
-  // fold the partials in chunk order: columns 0..31, then 32..kSums-1
+  // fold the partials in chunk order: columns 0..31, then 32..nsums-1
   __shared__ double tot[kPart];
   const int col = threadIdx.x & 31;
   const double lo = ordered_sum8(gridDim.x, true, [&](int c) { return __ldcg(part + (long long)c * kPart + col); });
   if (threadIdx.x < 32) tot[col] = lo;
   __syncthreads();
-  const double hi = ordered_sum8(gridDim.x, 32 + col < kSums,
+  const double hi = ordered_sum8(gridDim.x, 32 + col < nsums,
                                  [&](int c) { return __ldcg(part + (long long)c * kPart + 32 + col); });
   if (threadIdx.x < 32) tot[32 + col] = hi;
   __syncthreads();
@@ -289,7 +419,7 @@ __global__ void __launch_bounds__(kTrkThreads) track_step_kernel(const float* __
   const int n = P.unknowns;
   if (threadIdx.x == 0) {
     int c = kStatusOk;
-    for (int k = 0; k < kSums; ++k)
+    for (int k = 0; k < nsums; ++k)
       if (!isfinite(tot[k])) c = kNonfinite;
     if (c == kStatusOk && !(tot[kValid] > 0.0 && tot[kCount] >= __dmul_rn(P.min_overlap, tot[kValid]) &&
                             tot[kCount] > 0.0))
@@ -314,6 +444,11 @@ __global__ void __launch_bounds__(kTrkThreads) track_step_kernel(const float* __
   if (code == kStatusOk) band_cholesky_solve(band, rhs, n, n);
   if (threadIdx.x == 0) {
     track_update(P, tot, band, rhs, scale, code, st);
+    if constexpr (kPhoto) {
+      prec[0] = tot[kPCount];
+      prec[1] = tot[kPWSum] > 0.0 ? sqrt(tot[kPWE2] / tot[kPWSum]) : 0.0;
+      prec[2] = tot[kPCount] > 0.0 ? tot[kPDown] / tot[kPCount] : 0.0;
+    }
     *ticket = 0u;                                   // re-armed for the next launch
   }
 }
@@ -359,12 +494,14 @@ extern "C" int64_t odb_track_workspace_bytes(int32_t h, int32_t w) {
   return (1 + kState + (int64_t)trk_chunks(h, w) * kPart) * (int64_t)sizeof(double);
 }
 
-extern "C" int odb_track_frame(const float* pred, const float* ref_depth, const float* ref_normals, int32_t h,
-                               int32_t w, double fx, double fy, double cx, double cy, const double* ref_pose,
-                               const double* init_pose, const double* init_nodes, int32_t affine, int32_t iterations,
-                               double tol, double robust, double max_dist, double min_overlap, void* workspace,
-                               double* pose, double* nodes, double* record, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// odb_track_frame (rgb NULL) and odb_track_frame_rgbd
+static int track_frame(const char* name, const float* pred, const float* rgb, const float* ref_depth,
+                       const float* ref_rgb, const float* ref_normals, float* ref_intensity, int32_t h, int32_t w,
+                       double fx, double fy, double cx, double cy, const double* ref_pose, const double* init_pose,
+                       const double* init_nodes, int32_t affine, int32_t iterations, double tol, double robust,
+                       double max_dist, double min_overlap, double photometric, double photometric_robust,
+                       void* workspace, double* pose, double* nodes, double* record, cudaStream_t stream) {
+  const bool photo = rgb != nullptr;
   if (!pred || !ref_depth || !ref_normals || !ref_pose || !init_pose || !workspace || !pose || !nodes || !record ||
       (affine != 0 && affine != 1) || (init_nodes == nullptr) != (affine == 0) || !planes_ok(1, h, w) ||
       !(std::isfinite(fx) && fx > 0.0 && std::isfinite(fy) && fy > 0.0 && std::isfinite(cx) && std::isfinite(cy)) ||
@@ -372,11 +509,15 @@ extern "C" int odb_track_frame(const float* pred, const float* ref_depth, const 
       !(std::isfinite(robust) && robust > 0.0) || !(std::isfinite(max_dist) && max_dist > 0.0) ||
       !(min_overlap > 0.0 && min_overlap <= 1.0) || !aligned(pred, 4) || !aligned(ref_depth, 4) ||
       !aligned(ref_normals, 4) || !aligned(init_nodes, 8) || !aligned(workspace, 8) || !aligned(pose, 8) ||
-      !aligned(nodes, 8) || !aligned(record, 8))
-    return fail(ODB_ERR_INVALID, "track_frame: bad argument");
+      !aligned(nodes, 8) || !aligned(record, 8) ||
+      (photo && (!ref_rgb || !ref_intensity || !(std::isfinite(photometric) && photometric > 0.0) ||
+                 !(std::isfinite(photometric_robust) && photometric_robust > 0.0) || !aligned(rgb, 4) ||
+                 !aligned(ref_rgb, 4) || !aligned(ref_intensity, 4))))
+    return fail(ODB_ERR_INVALID, (std::string(name) + ": bad argument").c_str());
   TrkParams P;
   if (!pose_ok(ref_pose, P.ref) || !pose_ok(init_pose, P.init))
-    return fail(ODB_ERR_INVALID, "track_frame: a pose is not a finite rigid camera-to-world matrix");
+    return fail(ODB_ERR_INVALID,
+                (std::string(name) + ": a pose is not a finite rigid camera-to-world matrix").c_str());
   P.h = h;
   P.w = w;
   P.affine = affine;
@@ -386,20 +527,58 @@ extern "C" int odb_track_frame(const float* pred, const float* ref_depth, const 
   P.robust = robust;
   P.max_dist = max_dist;
   P.min_overlap = min_overlap;
+  P.photometric = photometric;
+  P.photometric_robust = photometric_robust;
   double* ws = static_cast<double*>(workspace);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(ws);
   double* st = ws + 1;
   double* part = st + kState;
+  double* prec = photo ? record + ODB_TRACK_RECORD : nullptr;
   cudaError_t e = cudaMemsetAsync(ticket, 0, sizeof(double), stream);
-  if (e != cudaSuccess) return fail_cuda(e, "track_frame: cudaMemsetAsync");
-  track_setup_kernel<<<1, 32, 0, stream>>>(P, init_nodes, st);
-  count_launch();
+  if (e != cudaSuccess) return fail_cuda(e, (std::string(name) + ": cudaMemsetAsync").c_str());
   const int chunks = trk_chunks(h, w);
+  if (photo) {
+    track_intensity_kernel<<<(unsigned)(((long long)h * w + kTrkThreads - 1) / kTrkThreads), kTrkThreads, 0,
+                             stream>>>(ref_depth, ref_rgb, ref_normals, h, w, ref_intensity);
+    count_launch();
+  }
+  track_setup_kernel<<<1, 32, 0, stream>>>(P, init_nodes, st, prec);
+  count_launch();
+  const PhotoIn C{rgb, ref_intensity};
   for (int it = 0; it < iterations; ++it) {
-    track_step_kernel<<<chunks, kTrkThreads, 0, stream>>>(pred, ref_depth, ref_normals, P, st, part, ticket);
+    if (photo)
+      track_step_kernel<true><<<chunks, kTrkThreads, 0, stream>>>(pred, ref_depth, ref_normals, C, P, st, part,
+                                                                  ticket, prec);
+    else
+      track_step_kernel<false><<<chunks, kTrkThreads, 0, stream>>>(pred, ref_depth, ref_normals, C, P, st, part,
+                                                                   ticket, nullptr);
     count_launch();
   }
   track_output_kernel<<<1, 32, 0, stream>>>(P, init_nodes, st, pose, nodes, record);
   count_launch();
-  return check_launch("track_frame");
+  return check_launch(name);
+}
+
+extern "C" int odb_track_frame(const float* pred, const float* ref_depth, const float* ref_normals, int32_t h,
+                               int32_t w, double fx, double fy, double cx, double cy, const double* ref_pose,
+                               const double* init_pose, const double* init_nodes, int32_t affine, int32_t iterations,
+                               double tol, double robust, double max_dist, double min_overlap, void* workspace,
+                               double* pose, double* nodes, double* record, void* stream_) {
+  return track_frame("track_frame", pred, nullptr, ref_depth, nullptr, ref_normals, nullptr, h, w, fx, fy, cx, cy,
+                     ref_pose, init_pose, init_nodes, affine, iterations, tol, robust, max_dist, min_overlap, 0.0, 0.0,
+                     workspace, pose, nodes, record, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int odb_track_frame_rgbd(const float* pred, const float* rgb, const float* ref_depth, const float* ref_rgb,
+                                    const float* ref_normals, float* ref_intensity, int32_t h, int32_t w, double fx,
+                                    double fy, double cx, double cy, const double* ref_pose, const double* init_pose,
+                                    const double* init_nodes, int32_t affine, int32_t iterations, double tol,
+                                    double robust, double max_dist, double min_overlap, double photometric,
+                                    double photometric_robust, void* workspace, double* pose, double* nodes,
+                                    double* record, void* stream_) {
+  if (!rgb) return fail(ODB_ERR_INVALID, "track_frame_rgbd: bad argument");
+  return track_frame("track_frame_rgbd", pred, rgb, ref_depth, ref_rgb, ref_normals, ref_intensity, h, w, fx, fy, cx,
+                     cy, ref_pose, init_pose, init_nodes, affine, iterations, tol, robust, max_dist, min_overlap,
+                     photometric, photometric_robust, workspace, pose, nodes, record,
+                     static_cast<cudaStream_t>(stream_));
 }

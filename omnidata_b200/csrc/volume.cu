@@ -1,6 +1,7 @@
 // TSDF volumes (omnidata_b200/volume.py TSDFVolume): posed depth frames fused into a dense truncated signed-distance
 // grid, depth rendered back from it by raycasting, and a triangle mesh extracted by marching tetrahedra.  Definitions
-// in DESIGN.md §3 "TSDF volumes" and include/omnidata_b200.h; oracle/volume_oracle.py restates them in float64.
+// in DESIGN.md §3 "TSDF volumes" and include/omnidata_b200.h; oracle/volume_oracle.py restates them in float64 (the
+// coloured raycast: oracle/color_volume_oracle.py).
 //
 //   tsdf_integrate_kernel  one thread per grid point, looping over up to kFramesPerLaunch frames in order; the poses
 //                          travel by value in the kernel parameters, so a call needs no device copy of them
@@ -16,8 +17,10 @@
 // operation by operation.  Integer scans only and no atomics: every output is bit-reproducible, and a grid point's
 // result does not depend on how its frames were split into calls.  Built without fast-math.
 #include <cmath>
+#include <string>
 
 #include "common.cuh"
+#include "fp64.cuh"
 #include "host_util.h"
 #include "../../include/omnidata_b200.h"
 
@@ -54,8 +57,6 @@ __constant__ signed char kTetTri[16][2][3] = {
     {{1, 3, 4}, {1, 4, 2}},       {{0, 3, 4}, {-1, -1, -1}}, {{0, 2, 1}, {-1, -1, -1}}, {{-1, -1, -1}, {-1, -1, -1}}};
 
 ODB_DEVINL int tet_triangles(int inside) { return (inside == 0 || inside == 15) ? 0 : (__popc(inside) == 2 ? 2 : 1); }
-
-ODB_DEVINL double lerp_rn(double a, double b, double t) { return __dadd_rn(a, __dmul_rn(t, __dsub_rn(b, a))); }
 
 // ---------------------------------------------------------------------------------------------------- integrate
 __global__ void __launch_bounds__(kVolThreads) tsdf_integrate_kernel(float* __restrict__ F, float* __restrict__ W,
@@ -122,13 +123,13 @@ __global__ void __launch_bounds__(kVolThreads) tsdf_integrate_kernel(float* __re
 // ---------------------------------------------------------------------------------------------------- raycast
 struct RaySampler {
   const float *F, *W;
+  const float* C;                                 // colour planes [3][n] (the coloured raycast only)
   VolGrid G;
   double lo[3];
-  // trilinear F at world point o + t d; false when a corner has W = 0
-  ODB_DEVINL bool sample(const double o[3], const double d[3], double t, double& val) const {
+  // the trilinear cell of world point o + t d: its lowest corner's index and the fractions
+  ODB_DEVINL long long locate(const double o[3], const double d[3], double t, double fr[3]) const {
     const int n[3] = {G.nx, G.ny, G.nz};
     int c[3];
-    double fr[3];
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
       const double g = __ddiv_rn(__dsub_rn(__dadd_rn(o[a], __dmul_rn(t, d[a])), lo[a]), G.voxel);
@@ -136,23 +137,46 @@ struct RaySampler {
       c[a] = (int)fl;
       fr[a] = fmin(fmax(__dsub_rn(g, fl), 0.0), 1.0);
     }
-    const long long sx = 1, sy = G.nx, sz = (long long)G.nx * G.ny;
-    const long long base = c[0] + c[1] * sy + c[2] * sz;
+    return c[0] + c[1] * (long long)G.nx + c[2] * (long long)G.nx * G.ny;
+  }
+  // trilinear interpolation of plane V over the cell at base: the (y, z) corner pairs, x first, then y, then z
+  ODB_DEVINL double trilinear(const float* V, long long base, const double fr[3]) const {
+    const long long sy = G.nx, sz = (long long)G.nx * G.ny;
     double cv[4];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {                 // q = (y, z) corner pair; x interpolated first
+    for (int q = 0; q < 4; ++q) {
       const long long e = base + (q & 1) * sy + (q >> 1) * sz;
-      const float w0 = W[e], w1 = W[e + sx];
-      if (!(w0 > 0.f && w1 > 0.f)) return false;
-      cv[q] = lerp_rn((double)F[e], (double)F[e + sx], fr[0]);
+      cv[q] = lerp_rn((double)V[e], (double)V[e + 1], fr[0]);
     }
-    val = lerp_rn(lerp_rn(cv[0], cv[1], fr[1]), lerp_rn(cv[2], cv[3], fr[1]), fr[2]);
+    return lerp_rn(lerp_rn(cv[0], cv[1], fr[1]), lerp_rn(cv[2], cv[3], fr[1]), fr[2]);
+  }
+  // trilinear F at world point o + t d; false when a corner has W = 0
+  ODB_DEVINL bool sample(const double o[3], const double d[3], double t, double& val) const {
+    double fr[3];
+    const long long base = locate(o, d, t, fr);
+    const long long sy = G.nx, sz = (long long)G.nx * G.ny;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const long long e = base + (q & 1) * sy + (q >> 1) * sz;
+      if (!(W[e] > 0.f && W[e + 1] > 0.f)) return false;
+    }
+    val = trilinear(F, base, fr);
     return true;
+  }
+  // trilinear colour channel a at o + t d (a sample already found valid: every corner has W > 0)
+  ODB_DEVINL double color(const double o[3], const double d[3], double t, int a) const {
+    double fr[3];
+    const long long base = locate(o, d, t, fr);
+    return trilinear(C + a * ((long long)G.nx * G.ny * G.nz), base, fr);
   }
 };
 
+// kColor: also rgb [3][h][w], the colour at the hit (NaN where nothing is hit), looked up once the hit is found, so the
+// march and the depth are the depth-only kernel's operation for operation
+template <bool kColor>
 __global__ void __launch_bounds__(128) tsdf_raycast_kernel(RaySampler S, VolCam K, VolPoses P, int h, int w,
-                                                           double step, float* __restrict__ out) {
+                                                           double step, float* __restrict__ out,
+                                                           float* __restrict__ rgb) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= w) return;
   const double* m = P.m[0];
@@ -180,6 +204,8 @@ __global__ void __launch_bounds__(128) tsdf_raycast_kernel(RaySampler S, VolCam 
     }
   }
   float z = 0.f;
+  bool hit = false;
+  double t_lo = 0.0, t_hi = 0.0, frac = 0.0;
   if (!miss && t0 <= t1) {
     bool prev_ok = false;
     double prev = 0.0, tp = t0;
@@ -189,8 +215,12 @@ __global__ void __launch_bounds__(128) tsdf_raycast_kernel(RaySampler S, VolCam 
       double val;
       const bool ok = S.sample(o, d, t, val);
       if (ok && prev_ok && prev > 0.0 && val <= 0.0) {
-        const double th = __dadd_rn(tp, __dmul_rn(step, __ddiv_rn(prev, __dsub_rn(prev, val))));
+        frac = __ddiv_rn(prev, __dsub_rn(prev, val));
+        const double th = __dadd_rn(tp, __dmul_rn(step, frac));
         z = (float)__dmul_rn(th, uz);
+        hit = true;
+        t_lo = tp;
+        t_hi = t;
         break;
       }
       prev_ok = ok;
@@ -198,7 +228,13 @@ __global__ void __launch_bounds__(128) tsdf_raycast_kernel(RaySampler S, VolCam 
       tp = t;
     }
   }
-  out[(long long)y * w + x] = z;
+  const long long px = (long long)y * w + x, plane = (long long)h * w;
+  out[px] = z;
+  if constexpr (kColor) {
+#pragma unroll 1
+    for (int a = 0; a < 3; ++a)
+      rgb[a * plane + px] = hit ? (float)lerp_rn(S.color(o, d, t_lo, a), S.color(o, d, t_hi, a), frac) : NAN;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------- mesh
@@ -484,27 +520,50 @@ extern "C" int odb_tsdf_integrate(float* tsdf, float* weight, float* color, int3
   return check_launch("tsdf_integrate");
 }
 
-extern "C" int odb_tsdf_raycast(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz, double ox,
-                                double oy, double oz, double voxel, const double* cam_to_world, int32_t h, int32_t w,
-                                double fx, double fy, double cx, double cy, double step, float* out, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// odb_tsdf_raycast (color, rgb NULL) and odb_tsdf_raycast_color
+static int tsdf_raycast(const char* name, const float* tsdf, const float* weight, const float* color, int32_t nx,
+                        int32_t ny, int32_t nz, double ox, double oy, double oz, double voxel,
+                        const double* cam_to_world, int32_t h, int32_t w, double fx, double fy, double cx, double cy,
+                        double step, float* out, float* rgb, cudaStream_t stream) {
   VolGrid G;
   VolCam K;
   VolPoses P;
-  if (!tsdf || !weight || !out || !cam_to_world || !grid_ok(nx, ny, nz, ox, oy, oz, voxel, G) ||
-      !planes_ok(1, h, w) || !cam_ok(fx, fy, cx, cy, K) || !(std::isfinite(step) && step >= voxel / 64.0 &&
-      step <= voxel) || !aligned(tsdf, 4) || !aligned(weight, 4) || !aligned(out, 4))
-    return fail(ODB_ERR_INVALID, "tsdf_raycast: bad argument");
+  if (!tsdf || !weight || !out || !cam_to_world || (color == nullptr) != (rgb == nullptr) ||
+      !grid_ok(nx, ny, nz, ox, oy, oz, voxel, G) || !planes_ok(1, h, w) || !cam_ok(fx, fy, cx, cy, K) ||
+      !(std::isfinite(step) && step >= voxel / 64.0 && step <= voxel) || !aligned(tsdf, 4) || !aligned(weight, 4) ||
+      !aligned(out, 4) || !aligned(color, 4) || !aligned(rgb, 4))
+    return fail(ODB_ERR_INVALID, (std::string(name) + ": bad argument").c_str());
   if (!pose_ok(cam_to_world, P.m[0]))
-    return fail(ODB_ERR_INVALID, "tsdf_raycast: the pose is not a finite rigid camera-to-world matrix");
+    return fail(ODB_ERR_INVALID, (std::string(name) + ": the pose is not a finite rigid camera-to-world matrix").c_str());
   RaySampler S;
   S.F = tsdf;
   S.W = weight;
+  S.C = color;
   S.G = G;
   S.lo[0] = ox; S.lo[1] = oy; S.lo[2] = oz;
-  tsdf_raycast_kernel<<<dim3((w + 127) / 128, h), 128, 0, stream>>>(S, K, P, h, w, step, out);
+  const dim3 grid((w + 127) / 128, h);
+  if (color)
+    tsdf_raycast_kernel<true><<<grid, 128, 0, stream>>>(S, K, P, h, w, step, out, rgb);
+  else
+    tsdf_raycast_kernel<false><<<grid, 128, 0, stream>>>(S, K, P, h, w, step, out, nullptr);
   count_launch();
-  return check_launch("tsdf_raycast");
+  return check_launch(name);
+}
+
+extern "C" int odb_tsdf_raycast(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz, double ox,
+                                double oy, double oz, double voxel, const double* cam_to_world, int32_t h, int32_t w,
+                                double fx, double fy, double cx, double cy, double step, float* out, void* stream_) {
+  return tsdf_raycast("tsdf_raycast", tsdf, weight, nullptr, nx, ny, nz, ox, oy, oz, voxel, cam_to_world, h, w, fx, fy,
+                      cx, cy, step, out, nullptr, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int odb_tsdf_raycast_color(const float* tsdf, const float* weight, const float* color, int32_t nx,
+                                      int32_t ny, int32_t nz, double ox, double oy, double oz, double voxel,
+                                      const double* cam_to_world, int32_t h, int32_t w, double fx, double fy,
+                                      double cx, double cy, double step, float* out, float* rgb, void* stream_) {
+  if (!color || !rgb) return fail(ODB_ERR_INVALID, "tsdf_raycast_color: bad argument");
+  return tsdf_raycast("tsdf_raycast_color", tsdf, weight, color, nx, ny, nz, ox, oy, oz, voxel, cam_to_world, h, w, fx,
+                      fy, cx, cy, step, out, rgb, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int odb_tsdf_mesh_count(const float* tsdf, const float* weight, int32_t nx, int32_t ny, int32_t nz,

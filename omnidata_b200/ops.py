@@ -30,7 +30,7 @@ __all__ = [
     "boundary_workspace_bytes", "depth_edges", "edge_hysteresis", "edge_distance2", "boundary_metrics_update",
     "sparse_align_workspace_bytes", "sparse_align_fit", "sparse_align_apply",
     "fusion_workspace_bytes", "depth_normals_workspace_bytes", "depth_normal_fusion", "depth_normals",
-    "tsdf_mesh_workspace_bytes", "tsdf_integrate", "tsdf_raycast", "tsdf_mesh_count", "tsdf_mesh_emit",
+    "tsdf_mesh_workspace_bytes", "tsdf_integrate", "tsdf_raycast", "tsdf_raycast_color", "tsdf_mesh_count", "tsdf_mesh_emit",
 ]
 
 _DTYPES = {torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
@@ -1180,9 +1180,22 @@ def tsdf_integrate(tsdf, weight, color, dims, origin, voxel: float, trunc: float
 def tsdf_raycast(tsdf, weight, dims, origin, voxel: float, intrinsics, cam_to_world, step: float, out):
     """out fp32 [H,W] = the z-depth of the first surface seen from cam_to_world (host [4,4]), 0 where none
     (include/omnidata_b200.h odb_tsdf_raycast)."""
-    name = "tsdf_raycast"
+    _raycast("tsdf_raycast", tsdf, weight, None, dims, origin, voxel, intrinsics, cam_to_world, step, out, None)
+
+
+def tsdf_raycast_color(tsdf, weight, color, dims, origin, voxel: float, intrinsics, cam_to_world, step: float, out,
+                       rgb):
+    """out fp32 [H,W] as tsdf_raycast, bit for bit, and rgb fp32 [3,H,W] = the colour of color fp32 [3,nz,ny,nx] at
+    the hit, NaN where out = 0 (include/omnidata_b200.h odb_tsdf_raycast_color)."""
+    name = "tsdf_raycast_color"
+    if color is None or rgb is None:
+        raise _capi.OdbError(f"{name}: needs the volume's colour planes and an rgb output")
+    _raycast(name, tsdf, weight, color, dims, origin, voxel, intrinsics, cam_to_world, step, out, rgb)
+
+
+def _raycast(name, tsdf, weight, color, dims, origin, voxel, intrinsics, cam_to_world, step, out, rgb):
     dims, origin = check_volume_grid(name, dims, origin, voxel)
-    _volume_planes(name, tsdf, weight, None, dims)
+    _volume_planes(name, tsdf, weight, color, dims)
     fx, fy, cx, cy = check_intrinsics(name, intrinsics)
     T = check_poses(name, cam_to_world)
     if T.shape[0] != 1:
@@ -1194,9 +1207,15 @@ def tsdf_raycast(tsdf, weight, dims, origin, voxel: float, intrinsics, cam_to_wo
         raise _capi.OdbError(f"{name}: out must be a contiguous fp32 [H,W] tensor, got {tuple(out.shape)}")
     h, w = out.shape
     _check_planes(name, 1, h, w)
-    _call(name, {"bytes": 4 * h * w}, lib().odb_tsdf_raycast, _same_device(tsdf, weight, out), tsdf.data_ptr(),
-          weight.data_ptr(), *dims, *origin, float(voxel), T.ctypes.data, h, w, fx, fy, cx, cy, float(step),
-          out.data_ptr())
+    if color is None:
+        _call(name, {"bytes": 4 * h * w}, lib().odb_tsdf_raycast, _same_device(tsdf, weight, out), tsdf.data_ptr(),
+              weight.data_ptr(), *dims, *origin, float(voxel), T.ctypes.data, h, w, fx, fy, cx, cy, float(step),
+              out.data_ptr())
+        return
+    _need_shape(rgb, (3, h, w), torch.float32, "rgb")
+    _call(name, {"bytes": 16 * h * w}, lib().odb_tsdf_raycast_color, _same_device(tsdf, weight, color, out, rgb),
+          tsdf.data_ptr(), weight.data_ptr(), color.data_ptr(), *dims, *origin, float(voxel), T.ctypes.data, h, w, fx,
+          fy, cx, cy, float(step), out.data_ptr(), rgb.data_ptr())
 
 
 def tsdf_mesh_count(tsdf, weight, dims, workspace, counts):
@@ -1259,13 +1278,26 @@ def check_track_params(name: str, affine, iterations, tol: float, robust: float,
         raise _capi.OdbError(f"{name}: min_overlap must lie in (0, 1], got {min_overlap!r}")
 
 
+def check_photometric(name: str, photometric, photometric_robust):
+    """OdbError unless photometric (lambda) is finite and >= 0 and photometric_robust is finite and > 0."""
+    for what, v in (("photometric", photometric), ("photometric_robust", photometric_robust)):
+        if isinstance(v, bool) or not (isinstance(v, numbers.Real) and math.isfinite(v)):
+            raise _capi.OdbError(f"{name}: {what} must be a finite number, got {v!r}")
+    if photometric < 0 or photometric_robust <= 0:
+        raise _capi.OdbError(f"{name}: need photometric >= 0 and photometric_robust > 0, got {photometric!r}, "
+                             f"{photometric_robust!r}")
+
+
 def track_frame(pred, ref_depth, ref_normals, intrinsics, ref_pose, init_pose, init_nodes, affine: bool,
                 iterations: int, tol: float, robust: float, max_dist: float, min_overlap: float, workspace, pose,
-                nodes, record):
+                nodes, record, rgb=None, ref_rgb=None, ref_intensity=None, photometric: float = 0.0,
+                photometric_robust: float = 0.1):
     """pose fp64 [4,4], nodes fp64 [1,1,1,2] and record fp64 [TRACK_RECORD] of pred fp32 [(1,)H,W] tracked against
     ref_depth fp32 [H,W] and its normals ref_normals fp32 [(1,)3,H,W] (depth_normals with axes (1, 1, 1)) rendered at
     ref_pose, from init_pose (both host [4,4]) and init_nodes fp64 [1,1,1,2] (exactly when affine)
-    (include/omnidata_b200.h odb_track_frame)."""
+    (include/omnidata_b200.h odb_track_frame).  With photometric > 0: also rgb fp32 [3,H,W] (the frame's image),
+    ref_rgb fp32 [3,H,W] (the model's colour at ref_pose), the scratch ref_intensity fp32 [3,H,W], and record fp64
+    [TRACK_RGBD_RECORD] (odb_track_frame_rgbd)."""
     name = "track_frame"
     _need(pred, torch.float32, "pred")
     if pred.dim() == 3 and pred.shape[0] == 1:
@@ -1295,7 +1327,22 @@ def track_frame(pred, ref_depth, ref_normals, intrinsics, ref_pose, init_pose, i
     _check_workspace(name, workspace, track_workspace_bytes(h, w))
     _need_shape(pose, (4, 4), torch.float64, "pose")
     _need_shape(nodes, (1, 1, 1, 2), torch.float64, "nodes")
-    _need_shape(record, (_capi.TRACK_RECORD,), torch.float64, "record")
+    check_photometric(name, photometric, photometric_robust)
+    photo = photometric > 0
+    if any((t is None) == photo for t in (rgb, ref_rgb, ref_intensity)):
+        raise _capi.OdbError(f"{name}: rgb, ref_rgb and ref_intensity are required exactly when photometric > 0")
+    _need_shape(record, (_capi.TRACK_RGBD_RECORD if photo else _capi.TRACK_RECORD,), torch.float64, "record")
+    if photo:
+        for what, t in (("rgb", rgb), ("ref_rgb", ref_rgb), ("ref_intensity", ref_intensity)):
+            _need_shape(t, (3, h, w), torch.float32, what)
+        _call("track_frame_rgbd", {"bytes": 44 * h * w * iterations}, lib().odb_track_frame_rgbd,
+              _same_device(pred, rgb, ref_depth, ref_rgb, ref_normals, ref_intensity, init_nodes, workspace, pose,
+                           nodes, record), pred.data_ptr(), rgb.data_ptr(), ref_depth.data_ptr(), ref_rgb.data_ptr(),
+              ref_normals.data_ptr(), ref_intensity.data_ptr(), h, w, fx, fy, cx, cy, poses[0].ctypes.data,
+              poses[1].ctypes.data, _ptr(init_nodes), 1 if affine else 0, int(iterations), float(tol), float(robust),
+              float(max_dist), float(min_overlap), float(photometric), float(photometric_robust),
+              workspace.data_ptr(), pose.data_ptr(), nodes.data_ptr(), record.data_ptr())
+        return
     _call(name, {"bytes": 20 * h * w * iterations}, lib().odb_track_frame,
           _same_device(pred, ref_depth, ref_normals, init_nodes, workspace, pose, nodes, record), pred.data_ptr(),
           ref_depth.data_ptr(), ref_normals.data_ptr(), h, w, fx, fy, cx, cy, poses[0].ctypes.data,

@@ -1,9 +1,10 @@
 """Track the camera through unposed frames: one frame's pose (and the scale and shift of its depth) solved against a
 model depth map rendered at a reference pose, by point-to-plane ICP with projective association (KinectFusion,
-Newcombe et al. 2011), on the device (csrc/track.cu).
+Newcombe et al. 2011), optionally with a photometric term, on the device (csrc/track.cu).
 
     from omnidata_b200.track import FrameTracker
-    tracker = FrameTracker(affine=True, iterations=20, tol=1e-6, robust=0.02, max_dist=0.1, min_overlap=0.1)
+    tracker = FrameTracker(affine=True, iterations=20, tol=1e-6, robust=0.02, max_dist=0.1, min_overlap=0.1,
+                           photometric=0.0, photometric_robust=0.1)
     ref = volume.raycast((fx, fy, cx, cy), ref_pose, (h, w))            # the model's z-depth at ref_pose
     nodes0, _ = SparseDepthAligner(grid=(1, 1), robust=0.05).fit(pred, ref.unsqueeze(0))
     pose, nodes, record = tracker.track(pred, ref, (fx, fy, cx, cy), ref_pose, init_pose=None, init_nodes=nodes0)
@@ -24,7 +25,20 @@ nonfinite: NaN in init_nodes or the update) returns init_pose and init_nodes unc
 
 The defaults max_dist = 0.1 m, robust = 0.02 m, min_overlap = 0.1, the pivot threshold 1e-6 and iterations = 20 are
 not tuned.  Tracking is frame-to-model only: drift is bounded by the model, not corrected (no loop closure).
-Definition: DESIGN.md §3 "Camera tracking" and include/omnidata_b200.h; oracle/track_oracle.py restates it in float64.
+Photometric term (RGB-D odometry, Whelan et al. 2013; the joint cost of ElasticFusion): with `photometric` = lambda > 0
+each geometric correspondence also asks the reference image's luminance at the frame point's projection to equal the
+frame's, which fixes the motions that geometry alone leaves free (a textured wall).  Then
+`track(..., rgb=image, ref_rgb=model_colour)` is required: rgb fp32 [3,H,W] or [1,3,H,W] the frame's image in [0, 1],
+ref_rgb the model's colour at ref_pose, normally `volume.raycast(K, ref_pose, (h, w), color=True)[1]` (NaN: no
+colour).  lambda is in m^2 per squared intensity step; photometric_robust is the Huber threshold of the intensity
+residual.  The record then has 11 columns: the 8 above, then (photometric terms in the last iteration, weighted RMS of
+the intensity residual, fraction of them the Huber weight reduced).  The reference's luminance and Sobel gradient go to
+a buffer the tracker keeps; a call is one launch longer.  There is no exposure or brightness compensation between
+frames: real video will need it.  lambda = 1e-2 is what the sweep on the analytic scene chose (DESIGN.md §6); it is not
+tuned on real data.  photometric = 0 (the default) is the geometric tracker unchanged.
+
+Definition: DESIGN.md §3 "Camera tracking" and include/omnidata_b200.h; oracle/track_oracle.py restates it in float64,
+and oracle/photometric_oracle.py the photometric term.
 Bit-reproducible; after the first call at a shape a call neither synchronises nor allocates beyond its outputs, so it
 can be captured in a CUDA graph.
 """
@@ -54,8 +68,11 @@ class FrameTracker(_StepBuffers):
     """Solves a frame's camera pose against a model depth map (module docstring)."""
 
     def __init__(self, affine: bool = True, iterations: int = 20, tol: float = 1e-6, robust: float = 0.02,
-                 max_dist: float = 0.1, min_overlap: float = 0.1):
+                 max_dist: float = 0.1, min_overlap: float = 0.1, photometric: float = 0.0,
+                 photometric_robust: float = 0.1):
         _value_error(ops.check_track_params, "FrameTracker", affine, iterations, tol, robust, max_dist, min_overlap)
+        _value_error(ops.check_photometric, "FrameTracker", photometric, photometric_robust)
+        self.photometric, self.photometric_robust = float(photometric), float(photometric_robust)
         self.affine, self.iterations = affine, int(iterations)
         self.tol, self.robust, self.max_dist, self.min_overlap = float(tol), float(robust), float(max_dist), \
             float(min_overlap)
@@ -65,10 +82,16 @@ class FrameTracker(_StepBuffers):
     @_capi.on_tensor_device
     @torch.no_grad()
     def track(self, pred: torch.Tensor, ref_depth: torch.Tensor, intrinsics, ref_pose, init_pose=None,
-              init_nodes: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-        """(pose fp64 [4,4], nodes fp64 [1,1,1,2], record fp64 [8]) on pred's device; kept for the next call at this
-        shape, which overwrites them."""
+              init_nodes: Optional[torch.Tensor] = None, rgb: Optional[torch.Tensor] = None,
+              ref_rgb: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """(pose fp64 [4,4], nodes fp64 [1,1,1,2], record fp64 [8], or [11] with the photometric term) on pred's
+        device; kept for the next call at this shape, which overwrites them.  rgb and ref_rgb (fp32 [3,H,W] or
+        [1,3,H,W]) exactly when photometric > 0."""
         name = "FrameTracker.track"
+        photo = self.photometric > 0
+        if (rgb is None) == photo or (ref_rgb is None) == photo:
+            raise ValueError(f"{name}: rgb and ref_rgb are required exactly when photometric > 0 "
+                             f"(photometric={self.photometric})")
         if pred.dim() == 3 and pred.shape[0] == 1:
             pred = pred[0]
         if pred.dim() != 2:
@@ -76,13 +99,21 @@ class FrameTracker(_StepBuffers):
         h, w = pred.shape
         if tuple(ref_depth.shape) != (h, w):
             raise ValueError(f"{name}: ref_depth must be [{h}, {w}] like pred, got {tuple(ref_depth.shape)}")
-        for what, t in (("pred", pred), ("ref_depth", ref_depth)):
+        tensors = [("pred", pred), ("ref_depth", ref_depth)]
+        if photo:
+            rgb, ref_rgb = (t[0] if t.dim() == 4 and t.shape[0] == 1 else t for t in (rgb, ref_rgb))
+            for what, t in (("rgb", rgb), ("ref_rgb", ref_rgb)):
+                if tuple(t.shape) != (3, h, w):
+                    raise ValueError(f"{name}: {what} must be [3, {h}, {w}] or [1, 3, {h}, {w}] like pred, got "
+                                     f"{tuple(t.shape)}")
+            tensors += [("rgb", rgb), ("ref_rgb", ref_rgb)]
+        for what, t in tensors:
             if not t.is_cuda or t.dtype != torch.float32:
                 raise ValueError(f"{name}: {what} must be fp32 on a CUDA device, got {t.dtype} on {t.device}")
-        if ref_depth.device != pred.device:
-            raise ValueError(f"{name}: pred and ref_depth live on different devices")
-        if not (pred.is_contiguous() and ref_depth.is_contiguous()):
-            raise ValueError(f"{name}: pred and ref_depth must be contiguous (a copy would allocate on every call)")
+            if t.device != pred.device:
+                raise ValueError(f"{name}: pred and {what} live on different devices")
+            if not t.is_contiguous():
+                raise ValueError(f"{name}: {what} must be contiguous (a copy would allocate on every call)")
         if self.affine != (init_nodes is not None):
             raise ValueError(f"{name}: init_nodes (the initial (s, t), e.g. SparseDepthAligner(grid=(1, 1)).fit) is "
                              f"required exactly when affine (affine={self.affine})")
@@ -105,9 +136,10 @@ class FrameTracker(_StepBuffers):
         ws = self._buf("workspace", (-(-ops.track_workspace_bytes(h, w) // 8),), torch.float64, dev)
         pose = self._buf("pose", (4, 4), torch.float64, dev)
         nodes = self._buf("nodes", (1, 1, 1, 2), torch.float64, dev)
-        rec = self._buf("record", (_capi.TRACK_RECORD,), torch.float64, dev)
+        rec = self._buf("record", (_capi.TRACK_RGBD_RECORD if photo else _capi.TRACK_RECORD,), torch.float64, dev)
+        intensity = self._buf("intensity", (3, h, w), torch.float32, dev) if photo else None
         ops.depth_normals(ref_depth.unsqueeze(0), mask, k, NORMAL_AXES, self._jump, nws, normals)
         ops.track_frame(pred, ref_depth, normals, k, ref_pose.reshape(4, 4), init_pose.reshape(4, 4), init_nodes,
                         self.affine, self.iterations, self.tol, self.robust, self.max_dist, self.min_overlap, ws,
-                        pose, nodes, rec)
+                        pose, nodes, rec, rgb, ref_rgb, intensity, self.photometric, self.photometric_robust)
         return pose, nodes, rec

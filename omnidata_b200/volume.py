@@ -6,6 +6,7 @@ integration of depth frames, raycasting of depth from the model and marching-tet
     vol = TSDFVolume(origin=(x0, y0, z0), voxel=0.02, dims=(nx, ny, nz), trunc=None, color=False)
     vol.integrate(depth, (fx, fy, cx, cy), cam_to_world, rgb=None)  # depth fp32 [B,H,W] metres; poses [B,4,4] host
     rendered = vol.raycast((fx, fy, cx, cy), cam_to_world, (h, w))    # fp32 [h,w] z-depth, 0 where nothing is hit
+    depth, rgb = vol.raycast(K, cam_to_world, (h, w), color=True)     # color=True volumes: also fp32 [3,h,w], NaN: none
     vertices, faces, colors = vol.extract_mesh()                      # fp32 [V,3], int32 [F,3], fp32 [V,3] | None
     write_ply("mesh.ply", vertices, faces, colors)
 
@@ -116,10 +117,17 @@ class TSDFVolume(_StepBuffers):
                                depth.contiguous(), None if rgb is None else rgb.contiguous(), k, cam_to_world)
 
     @torch.no_grad()
-    def raycast(self, intrinsics, cam_to_world, size: Tuple[int, int], step: Optional[float] = None) -> torch.Tensor:
+    def raycast(self, intrinsics, cam_to_world, size: Tuple[int, int], step: Optional[float] = None,
+                color: bool = False):
         """The z-depth fp32 [H,W] (size = (H, W)) of the first surface seen from cam_to_world ([4,4] host), 0 where no
-        surface is hit.  step: the march's sample spacing along the ray (default half a voxel)."""
+        surface is hit.  step: the march's sample spacing along the ray (default half a voxel).  color=True (a volume
+        that keeps colour): (depth, rgb fp32 [3,H,W]), the same depth and the mean colour at the hit, NaN where there
+        is none."""
         name = "TSDFVolume.raycast"
+        if not isinstance(color, bool):
+            raise ValueError(f"{name}: color must be a bool, got {color!r}")
+        if color and self.color is None:
+            raise ValueError(f"{name}: color=True needs a volume that keeps colour (TSDFVolume(..., color=True))")
         k = _value_error(ops.check_intrinsics, name, intrinsics)
         T = _value_error(ops.check_poses, name, cam_to_world)
         if T.shape[0] != 1:
@@ -133,9 +141,16 @@ class TSDFVolume(_StepBuffers):
         if not (math.isfinite(step) and self.voxel / 64 <= step <= self.voxel):
             raise ValueError(f"{name}: step must lie in [voxel / 64, voxel], got {step}")
         out = torch.empty(h, w, dtype=torch.float32, device=self.device)
+        if not color:
+            with torch.cuda.device(self.device):
+                ops.tsdf_raycast(self.tsdf, self.weight, self.dims, self.origin, self.voxel, k, cam_to_world, step,
+                                 out)
+            return out
+        rgb = torch.empty(3, h, w, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            ops.tsdf_raycast(self.tsdf, self.weight, self.dims, self.origin, self.voxel, k, cam_to_world, step, out)
-        return out
+            ops.tsdf_raycast_color(self.tsdf, self.weight, self.color, self.dims, self.origin, self.voxel, k,
+                                   cam_to_world, step, out, rgb)
+        return out, rgb
 
     @torch.no_grad()
     def extract_mesh(self) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:

@@ -7,7 +7,7 @@ extracted mesh as a PLY:
                           --bounds X0,Y0,Z0,X1,Y1,Z1 --out mesh.ply [--pose_out DIR]
                           [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
                           [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--guided_size HxW]
-                          [--sparse_path DIR [--depth_scale 1000]] [--trunc T]
+                          [--sparse_path DIR [--depth_scale 1000]] [--trunc T] [--color] [--photometric LAMBDA]
 
 Frames are the images of --img_path (PNG / JPEG) in file-name order.  Each has a pose, the 4 x 4 camera-to-world matrix
 as text (ScanNet's pose/<stem>.txt), in --pose_path by file stem.  The intrinsics are in pixels of the images.  The grid
@@ -24,7 +24,8 @@ named in the summary.
 
 Without --pose_path the cameras are tracked (`FrameTracker`, point-to-plane ICP against the volume).  This mode and
 --track are experimental: tracking against the fused model drifts (on the analytic test scene at 12.5 mm voxels, 13.5
-mm over 48 frames, and refined poses end a mean 6.8 mm from the truth when given 20 mm off; DESIGN.md §6).  Frame 0's pose is
+mm over 48 frames, and refined poses end a mean 6.8 mm from the truth when given 20 mm off; with --photometric 1e-2 on
+its textured version 3.4 mm and 1.45 mm; DESIGN.md §6).  Frame 0's pose is
 the identity, so --bounds are in frame 0's camera coordinates (x right, y down, z forward); frame 0 still needs sparse
 depths.  Every later frame starts from the last tracked pose: the volume is raycast there, one scale and shift is fitted
 as above (to the frame's sparse depths when it has them, then the aligned metres are tracked with the pose alone;
@@ -32,6 +33,13 @@ otherwise to that raycast, then the scale and shift are tracked with the pose), 
 tracked pose.  A frame whose fit or tracking fails is skipped and named with its status; the next frame starts from the
 last good pose.  With --pose_path and --track the given poses are the initial guesses (pose refinement).  --pose_out
 DIR writes each used frame's pose as <stem>.txt, in the format --pose_path reads.
+
+--color also fuses each frame's image (RGB in [0, 1] at the prediction's size, before the network's normalisation)
+into a colour volume and writes a coloured PLY.  --photometric LAMBDA (implies --color; needs tracking, so no
+--pose_path without --track) adds a photometric term to the tracking (`FrameTracker(photometric=LAMBDA)`): each frame's
+image against the volume's coloured raycast at the initial pose.  It constrains motions the geometry leaves free (a
+textured wall); 1e-2 is what the sweep on the analytic scene chose (DESIGN.md §6), not tuned on real data, and there is
+no exposure compensation between frames.  It is experimental like the tracking it refines.
 
 Prints one JSON line: frames used and skipped, vertices, faces and seconds.  Runs on cuda:0; there is no CPU path.
 """
@@ -105,6 +113,10 @@ def parse_args(argv=None):
                     help="sparse depths by file stem (16-bit PNG or .npy in metres); frame 0 must have one")
     ap.add_argument("--depth_scale", type=float, default=1000.0, help="16-bit PNG units per metre (default mm)")
     ap.add_argument("--trunc", type=float, default=None, help="truncation distance in metres (default 3 voxels)")
+    ap.add_argument("--color", action="store_true", help="fuse the images' colour and write a coloured PLY")
+    ap.add_argument("--photometric", type=float, default=None, metavar="LAMBDA",
+                    help="experimental: track with a photometric term of this weight (m^2 per squared intensity "
+                         "step; implies --color)")
     args = ap.parse_args(argv)
     if not (math.isfinite(args.voxel) and args.voxel > 0):
         ap.error(f"--voxel must be finite and > 0, got {args.voxel}")
@@ -124,6 +136,13 @@ def parse_args(argv=None):
         ap.error(f"--trunc must be finite and > 0, got {args.trunc}")
     if args.track and args.pose_path is None:
         ap.error("--track refines the poses of --pose_path; without --pose_path every frame is tracked already")
+    if args.photometric is not None:
+        if not (math.isfinite(args.photometric) and args.photometric > 0):
+            ap.error(f"--photometric must be finite and > 0, got {args.photometric}")
+        if args.pose_path is not None and not args.track:
+            ap.error("--photometric weights a term of the tracking; with --pose_path nothing is tracked without "
+                     "--track")
+        args.color = True
     if args.pose_out is not None and Path(args.pose_out).exists() and not Path(args.pose_out).is_dir():
         ap.error(f"--pose_out must be a directory, got the file {args.pose_out}")
     if args.mode == "guided":
@@ -134,45 +153,50 @@ def parse_args(argv=None):
     return args
 
 
-def align_and_integrate(volume, aligner, pred: torch.Tensor, intrinsics, pose: np.ndarray, sparse=None):
+def align_and_integrate(volume, aligner, pred: torch.Tensor, intrinsics, pose: np.ndarray, sparse=None, rgb=None):
     """One frame of the loop: fit pred fp32 [1,H,W] to sparse [1,H,W] (metres, 0 = none) or, without it, to the
-    volume's raycast at pose; integrate the aligned depth when the fit is ok.  Returns the aligner's record (fp64 [8],
-    on the host) and the nodes (scale, shift)."""
+    volume's raycast at pose; integrate the aligned depth (and rgb fp32 [3,H,W] into a colour volume) when the fit is
+    ok.  Returns the aligner's record (fp64 [8], on the host) and the nodes (scale, shift)."""
     h, w = pred.shape[-2:]
     target = sparse if sparse is not None else volume.raycast(intrinsics, pose, (h, w)).unsqueeze(0)
     nodes, rec = aligner.fit(pred, target)
     rec, st = rec[0].cpu(), nodes.reshape(2).cpu()
     if int(rec[1]) == 0:
-        volume.integrate(aligner.apply(pred, nodes), intrinsics, pose)
+        volume.integrate(aligner.apply(pred, nodes), intrinsics, pose, None if rgb is None else rgb.unsqueeze(0))
     return rec, (float(st[0]), float(st[1]))
 
 
 def track_and_integrate(volume, aligner, trackers, pred: torch.Tensor, intrinsics, init_pose: np.ndarray,
-                        sparse=None):
+                        sparse=None, rgb=None):
     """One frame of the tracking loop: raycast the volume at init_pose, fit pred fp32 [1,H,W] with the aligner to
     sparse [1,H,W] (metres, 0 = none) or, without it, to that raycast, track it (trackers[False] on the aligned metres
     with sparse, else trackers[True] on pred with the fitted (s, t) as initial nodes), and integrate the aligned depth at
-    the tracked pose.  Returns (failure, pose, (s, t)): failure None when the frame was integrated, else
-    "fit: <status>" or "track: <status>"; pose the tracked host float64 [4,4] (None on failure)."""
+    the tracked pose.  rgb fp32 [3,H,W] (a colour volume): integrated with the depth and, for trackers with a
+    photometric term, tracked against the coloured raycast.  Returns (failure, pose, (s, t)): failure None when the
+    frame was integrated, else "fit: <status>" or "track: <status>"; pose the tracked host float64 [4,4] (None on
+    failure)."""
     from omnidata_b200.sparse import STATUS as FIT_STATUS
     from omnidata_b200.track import STATUS as TRACK_STATUS
     h, w = pred.shape[-2:]
-    ref = volume.raycast(intrinsics, init_pose, (h, w))
+    photo = trackers[True].photometric > 0
+    ref, ref_rgb = volume.raycast(intrinsics, init_pose, (h, w), color=True) if photo else \
+        (volume.raycast(intrinsics, init_pose, (h, w)), None)
+    colour = dict(rgb=rgb, ref_rgb=ref_rgb) if photo else {}
     nodes, rec = aligner.fit(pred, sparse if sparse is not None else ref.unsqueeze(0))
     status = int(rec[0, 1].item())
     if status != 0:
         return f"fit: {FIT_STATUS[status]}", None, None
     if sparse is not None:
         metres = aligner.apply(pred, nodes)
-        pose, _, trec = trackers[False].track(metres, ref, intrinsics, init_pose)
+        pose, _, trec = trackers[False].track(metres, ref, intrinsics, init_pose, **colour)
     else:
-        pose, nodes, trec = trackers[True].track(pred, ref, intrinsics, init_pose, init_nodes=nodes)
+        pose, nodes, trec = trackers[True].track(pred, ref, intrinsics, init_pose, init_nodes=nodes, **colour)
         metres = aligner.apply(pred, nodes)
     status = int(trec[1].item())
     if status != 0:
         return f"track: {TRACK_STATUS[status]}", None, None
     pose = pose.cpu().numpy()
-    volume.integrate(metres, intrinsics, pose)
+    volume.integrate(metres, intrinsics, pose, None if rgb is None else rgb.unsqueeze(0))
     st = nodes.reshape(2).cpu()
     return None, pose, (float(st[0]), float(st[1]))
 
@@ -192,16 +216,19 @@ def reconstruct(args) -> dict:
     model = evaluate.build_model("depth", args.backbone, args.checkpoint, args.synthetic_weights, args.precision,
                                  device)
     guided = (args.guided_size, 4, 1e-3) if args.mode == "guided" else None
-    volume = TSDFVolume(args.origin, args.voxel, args.dims, trunc=args.trunc, device=device)
+    volume = TSDFVolume(args.origin, args.voxel, args.dims, trunc=args.trunc, color=args.color, device=device)
     aligner = SparseDepthAligner(grid=(1, 1), robust=ROBUST)
     tracking = args.track or not posed
-    trackers = {a: FrameTracker(affine=a) for a in (False, True)} if tracking else None
+    lam = 0.0 if args.photometric is None else args.photometric
+    trackers = {a: FrameTracker(affine=a, photometric=lam) for a in (False, True)} if tracking else None
     if args.pose_out is not None:
         Path(args.pose_out).mkdir(parents=True, exist_ok=True)
     last = np.eye(4)                                  # the last good pose: frame 0's without --pose_path
     used, skipped = [], []
     for q, (p, pose) in enumerate(zip(images, poses)):
-        x = evaluate.image_tensor(p, "depth").to(device)
+        image = evaluate.image_tensor(p, "rgb")                   # [1,3,H,W] in [0, 1]
+        x = ((image - 0.5) / 0.5).to(device)                       # image_tensor(p, "depth")'s normalisation
+        rgb = image[0].to(device) if args.color else None
         pred = evaluate.predict(model, x, args.mode, (args.tile, args.tile), args.overlap, p.name, guided=guided)
         sparse = None
         try:
@@ -216,10 +243,10 @@ def reconstruct(args) -> dict:
             sparse = torch.from_numpy(sp).unsqueeze(0).to(device)
         if tracking and used:
             failure, pose, _ = track_and_integrate(volume, aligner, trackers, pred, args.intrinsics,
-                                                   pose if posed else last, sparse)
+                                                   pose if posed else last, sparse, rgb)
         else:
             pose = last if pose is None else pose
-            rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse)
+            rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse, rgb)
             failure = None if int(rec[1]) == 0 else STATUS[int(rec[1])]
         if failure is None:
             used.append(p.name)
@@ -228,8 +255,8 @@ def reconstruct(args) -> dict:
                 np.savetxt(Path(args.pose_out) / (p.stem + ".txt"), pose)
         else:
             skipped.append({"frame": p.name, "status": failure})
-    vertices, faces, _ = volume.extract_mesh()
-    write_ply(args.out, vertices, faces)
+    vertices, faces, colors = volume.extract_mesh()
+    write_ply(args.out, vertices, faces, colors)
     return {"frames": len(images), "frames_used": len(used), "frames_skipped": skipped,
             "vertices": int(vertices.shape[0]), "faces": int(faces.shape[0]), "dims": list(args.dims),
             "voxel": args.voxel, "out": str(args.out), "seconds": round(time.perf_counter() - t0, 3)}
