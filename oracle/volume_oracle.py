@@ -36,19 +36,28 @@ def kuhn_volumes() -> np.ndarray:
     return np.array(out)
 
 
-def _points(dims, origin, voxel):
+def _indices(dims, index_offset=(0, 0, 0)):
+    """float64 (i, j, k) [nz, ny, nx] of the points of a dims grid whose first point is index_offset of a larger
+    grid (integers, so exact)."""
     nx, ny, nz = dims
     k, j, i = np.meshgrid(np.arange(nz), np.arange(ny), np.arange(nx), indexing="ij")
-    return [origin[0] + voxel * i.astype(np.float64), origin[1] + voxel * j.astype(np.float64),
-            origin[2] + voxel * k.astype(np.float64)]
+    return [(q + int(o)).astype(np.float64) for q, o in zip((i, j, k), index_offset)]
 
 
-def integrate(F, W, C, origin, voxel, trunc, depth, K, poses, rgb=None):
-    """(F, W, C) after integrating depth [B,H,W] (rgb [B,3,H,W] with C) from poses [B,4,4]; new arrays."""
+def _points(dims, origin, voxel, index_offset=(0, 0, 0)):
+    """X = origin + voxel (i, j, k) of the points of a dims grid; index_offset: the grid is the sub-box of a larger grid
+    starting at that point, whose positions the kernels compute from the larger grid's indices."""
+    idx = _indices(dims, index_offset)
+    return [origin[a] + voxel * idx[a] for a in range(3)]
+
+
+def integrate(F, W, C, origin, voxel, trunc, depth, K, poses, rgb=None, index_offset=(0, 0, 0)):
+    """(F, W, C) after integrating depth [B,H,W] (rgb [B,3,H,W] with C) from poses [B,4,4]; new arrays.
+    index_offset: F, W, C are the sub-box from that point of a larger grid with this origin and voxel."""
     F, W = F.astype(np.float32).copy(), W.astype(np.float32).copy()
     C = None if C is None else C.astype(np.float32).copy()
     nz, ny, nx = F.shape
-    X, Y, Z = _points((nx, ny, nz), origin, voxel)
+    X, Y, Z = _points((nx, ny, nz), origin, voxel, index_offset)
     fx, fy, cx, cy = (float(v) for v in K)
     depth = np.asarray(depth, np.float32)
     _, h, w = depth.shape
@@ -153,8 +162,11 @@ def _shift(a, code, fill):
     return out
 
 
-def extract_mesh(F, W, C, origin, voxel):
-    """(vertices float32 [V,3], faces int32 [F,3], colors float32 [V,3] or None) in the kernels' order."""
+def extract_mesh(F, W, C, origin, voxel, index_offset=(0, 0, 0)):
+    """(vertices float32 [V,3], faces int32 [F,3], colors float32 [V,3] or None) in the kernels' order.
+    index_offset: F, W, C are the sub-box from that point of a larger grid with this origin and voxel, whose points
+    outside the sub-box have W = 0; the vertices are the larger grid's, and the face ids count from the sub-box's
+    first vertex."""
     nz, ny, nx = F.shape
     N = F.size
     obs = [_shift(W, c, 0.0).reshape(-1) > 0 for c in range(8)]
@@ -165,7 +177,7 @@ def extract_mesh(F, W, C, origin, voxel):
     counts = bits.sum(1)
     vbase = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
     k, j, i = np.meshgrid(np.arange(nz), np.arange(ny), np.arange(nx), indexing="ij")
-    idx = [i.reshape(-1).astype(np.float64), j.reshape(-1).astype(np.float64), k.reshape(-1).astype(np.float64)]
+    idx = [q.reshape(-1) for q in _indices((nx, ny, nz), index_offset)]
     verts, cols = [], []
     fp = fv[0].astype(np.float64)
     for c in range(1, 8):

@@ -138,3 +138,44 @@ def test_volume_kernels_do_not_spill(tmp_path):
     frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", out)
     assert len(frames) >= 6, out
     assert all(f == ("0", "0", "0") for f in frames), out
+
+
+def test_oracle_index_offset():
+    """A sub-box of a larger grid with index_offset: offset 0 is the plain call bit for bit; a box holding every W > 0
+    point of the grid gives the grid's vertices and colours bit for bit and its faces less the box's first vertex;
+    integrating the box gives the grid's integration of it bit for bit."""
+    rng = np.random.default_rng(5)
+    dims, origin, voxel = (13, 11, 12), (-0.45, -0.41, -0.43), 0.07
+    F, W = VO.sphere_sdf_volume(dims, origin, voxel, (0.02, -0.03, 0.01), 0.25, 2 * voxel)
+    C = rng.random((3,) + F.shape).astype(np.float32)
+    W[rng.random(F.shape) < 0.05] = 0.0
+    plain = VO.extract_mesh(F, W, C, origin, voxel)
+    zero = VO.extract_mesh(F, W, C, origin, voxel, index_offset=(0, 0, 0))
+    assert len(plain[1]) > 100
+    for a, b in zip(plain, zero):
+        assert a.dtype == b.dtype and np.array_equal(a, b)
+    big = (dims[0] + 5, dims[1] + 3, dims[2] + 4)
+    off = (5, 2, 3)
+    box = (slice(off[2], off[2] + dims[2]), slice(off[1], off[1] + dims[1]), slice(off[0], off[0] + dims[0]))
+    Fb, Wb, Cb = np.ones(big[::-1], np.float32), np.zeros(big[::-1], np.float32), np.zeros((3,) + big[::-1], np.float32)
+    Fb[box], Wb[box], Cb[(slice(None),) + box] = F, W, C
+    borigin = tuple(o - voxel * q for o, q in zip(origin, off))
+    whole = VO.extract_mesh(Fb, Wb, Cb, borigin, voxel)
+    sub = VO.extract_mesh(F, W, C, borigin, voxel, index_offset=off)
+    assert np.array_equal(whole[0], sub[0]) and np.array_equal(whole[2], sub[2])
+    assert np.array_equal(whole[1], sub[1])                       # no W > 0 point before the box: first vertex 0
+    assert np.array_equal(VO._points(dims, borigin, voxel, off)[0], VO._points(big, borigin, voxel)[0][box])
+    K = (40.0, 42.0, 15.5, 11.0)
+    T = np.stack([VO.look_at((0.1, -1.2, 0.3), (0.0, 0.0, 0.0)), VO.look_at((1.0, 0.4, -0.6), (0.05, 0.0, 0.0))])
+    depth = rng.uniform(0.8, 1.6, (2, 24, 32)).astype(np.float32)
+    rgb = rng.random((2, 3, 24, 32)).astype(np.float32)
+    z = np.zeros(big[::-1], np.float32)
+    gF, gW, gC = VO.integrate(z, z, np.zeros((3,) + z.shape, np.float32), borigin, voxel, 0.2, depth, K, T, rgb)
+    zb = np.zeros(dims[::-1], np.float32)
+    bF, bW, bC = VO.integrate(zb, zb, np.zeros((3,) + zb.shape, np.float32), borigin, voxel, 0.2, depth, K, T, rgb,
+                              index_offset=off)
+    assert (bW > 0).any() and np.array_equal(bW, gW[box]) and np.array_equal(bF, gF[box])
+    assert np.array_equal(bC, gC[(slice(None),) + box])
+    pF, pW, pC = VO.integrate(zb, zb, None, origin, voxel, 0.2, depth, K, T)
+    qF, qW, qC = VO.integrate(zb, zb, None, origin, voxel, 0.2, depth, K, T, index_offset=(0, 0, 0))
+    assert pC is None and qC is None and np.array_equal(pF, qF) and np.array_equal(pW, qW)
