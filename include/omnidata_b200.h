@@ -827,6 +827,45 @@ int odb_track_frame_rgbd(const float* pred, const float* rgb, const float* ref_d
                          double max_dist, double min_overlap, double photometric, double photometric_robust,
                          void* workspace, double* pose, double* nodes, double* record, void* stream);
 
+/* odb_track_information: info fp64 [unknowns][unknowns] (unknowns 6, or 8 with affine) = the normal matrix
+ * sum w J J^T of the last Gauss-Newton step that ran in the last odb_track_frame / odb_track_frame_rgbd call on this
+ * workspace at h x w (the photometric terms included), unscaled, in the (v, omega[, s, t]) increment coordinates: the
+ * per-chunk partials that step left in the workspace, folded in the same order as the step folded them.  Meaningful
+ * when that call's status is ok.  One launch; the tracking entry points are unchanged by it. */
+int odb_track_information(const void* workspace, int32_t h, int32_t w, int32_t unknowns, double* info, void* stream);
+
+/* ---- SE(3) pose graphs (omnidata_b200/posegraph.py PoseGraph) -----------------------------------------------------
+ *
+ * No reference counterpart.  Gauss-Newton over N camera-to-world poses T_k with E relative-pose edges (i, j),
+ * measurement Z_ij ~ T_i^-1 T_j and information W_ij; node 0 is fixed.  Definition in DESIGN.md §3 "Loop closure and
+ * pose graphs"; oracle/posegraph_oracle.py restates it in float64.  All inputs are DEVICE arrays: edges int32 [E][2]
+ * (0 <= i, j < N, i != j; the kernels ignore any other edge), poses fp64 [N][16] and measurements fp64 [E][16]
+ * (row-major 4 x 4, rigid), information fp64 [E][36] (symmetric).  2 <= N <= ODB_POSEGRAPH_MAX_NODES, 1 <= E <= 8 N.
+ *
+ * Residual r = Log(Z^-1 T_i^-1 T_j) in (v, omega) order, explicit round-to-nearest fp64: with M = Z^-1 T_i^-1 T_j,
+ * w = vee(R_M - R_M^T) / 2, theta = atan2(|w|, (tr R_M - 1) / 2), omega = (theta / |w|) w, v = V^-1 t_M with V^-1 = I -
+ * W / 2 + ((1 - A / (2 B)) / theta^2) W^2, W = [omega]x, A = sin(theta) / theta, B = (1 - cos(theta)) / theta^2; below
+ * theta = 1e-2 the series theta / |w| = 1 + theta^2 / 6 + 7 theta^4 / 360 and 1 / 12 + theta^2 / 720 + theta^4 / 30240.
+ * Increments T_k <- T_k exp(delta_k) (odb_track_frame's exponential); Jacobians d r / d delta_j = I and d r / d delta_i =
+ * -Ad(T_j^-1 T_i), Ad(T) = [[R, [t]x R], [0, R]] (Gauss-Newton with J_r^-1(r) ~ I).  H = S J^T W J and g = S J^T W r
+ * over the 6 (N - 1) free unknowns, scaled to a unit diagonal, solved by a blocked Cholesky in fp64; a solve stops when
+ * every node has |delta_v| <= tol and |delta_omega| <= tol (tol finite > 0), after at most iterations (1..100).
+ * Status (record[0]): 0 ok; 1 degenerate (a diagonal entry <= 0, as for a node no edge reaches, or a scaled pivot below
+ * 1e-12); 2 nonfinite (a NaN or infinity, or a residual rotation above pi / 2).  A failed solve returns the input poses
+ * bit for bit.  poses_out fp64 [N][16]; record fp64 [ODB_POSEGRAPH_RECORD] = (status, iterations run, S r^T W r at the
+ * input poses, the same at poses_out, the largest |delta| of the last step, N, E).
+ *
+ * workspace: odb_posegraph_workspace_bytes(N, E) bytes, 8-byte aligned (negative: refused); it holds the dense fp64
+ * matrix, 8 (6 (N - 1))^2 bytes.  A call is 2 + iterations (4 P + 2) launches, P = ceil(6 (N - 1) / 64), with no host
+ * synchronisation, so it can be captured in a CUDA graph.  Fixed-order sums, no floating-point atomics: results are
+ * bit-reproducible.  Arguments are checked before any launch. */
+#define ODB_POSEGRAPH_MAX_NODES 1024
+#define ODB_POSEGRAPH_RECORD 7
+int64_t odb_posegraph_workspace_bytes(int32_t n_nodes, int32_t n_edges);
+int odb_posegraph_optimize(int32_t n_nodes, int32_t n_edges, const int32_t* edges, const double* poses,
+                           const double* measurements, const double* information, int32_t iterations, double tol,
+                           void* workspace, double* poses_out, double* record, void* stream);
+
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *
  * The depth-boundary error (DBE) of iBims-1 (Koch et al., ECCV Workshops 2018): how far predicted depth edges lie from

@@ -31,6 +31,8 @@ TSDF_MAX_DIM = 2048                             # ODB_TSDF_MAX_DIM
 TSDF_MAX_POINTS = 1 << 28                       # ODB_TSDF_MAX_POINTS
 TRACK_RECORD = 8                                # ODB_TRACK_RECORD
 TRACK_RGBD_RECORD = 11                          # ODB_TRACK_RGBD_RECORD
+POSEGRAPH_MAX_NODES = 1024                      # ODB_POSEGRAPH_MAX_NODES
+POSEGRAPH_RECORD = 7                            # ODB_POSEGRAPH_RECORD
 
 
 class OdbError(RuntimeError):
@@ -258,6 +260,10 @@ _SIGNATURES = {
                         [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 5),
     "odb_track_frame_rgbd": (C.c_int, [C.c_void_p] * 6 + [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 3 +
                              [C.c_int32] * 2 + [C.c_double] * 6 + [C.c_void_p] * 5),
+    "odb_track_information": (C.c_int, [C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 2),
+    "odb_posegraph_workspace_bytes": (C.c_int64, [C.c_int32] * 2),
+    "odb_posegraph_optimize": (C.c_int, [C.c_int32] * 2 + [C.c_void_p] * 4 + [C.c_int32, C.c_double] +
+                               [C.c_void_p] * 4),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "fp64.cuh"
 #include "host_util.h"
+#include "se3.cuh"
 #include "../../include/omnidata_b200.h"
 
 namespace odb {
@@ -44,8 +45,6 @@ constexpr int kG = kTri, kCount = kG + kUnknowns, kWE2 = kCount + 1, kWSum = kCo
 constexpr int kPCount = kSums, kPWE2 = kSums + 1, kPWSum = kSums + 2, kPDown = kSums + 3, kSumsRgbd = kSums + 4;
 constexpr int kPart = 64;                         // doubles per chunk partial (two ordered_sum8 column blocks)
 constexpr double kPivotMin = 1e-6;                // smallest Cholesky pivot of the unit-diagonal matrix (not tuned)
-constexpr double kSeriesTheta = 1e-2;             // |omega| below this: series for the exponential's coefficients
-constexpr double kPi = 3.141592653589793;
 // state [kState] doubles
 constexpr int kT = 0, kM = 12, kS = 24, kSh = 25, kDone = 26, kStatus = 27, kIters = 28, kCorr = 29, kRms = 30,
               kFrac = 31, kNValid = 32, kState = 34;
@@ -62,61 +61,9 @@ struct TrkParams {
 
 static int trk_chunks(int h, int w) { return (int)(((long long)h * w + kChunk - 1) / kChunk); }
 
-ODB_DEVINL double dot3_rn(const double u[3], const double v[3]) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(u[0], v[0]), __dmul_rn(u[1], v[1])), __dmul_rn(u[2], v[2]));
-}
-
 // Y = (0.299 R + 0.587 G) + 0.114 B
 ODB_DEVINL double luminance(float r, float g, float b) {
   return __dadd_rn(__dadd_rn(__dmul_rn(kLumR, (double)r), __dmul_rn(kLumG, (double)g)), __dmul_rn(kLumB, (double)b));
-}
-
-// M = ref^-1 T: Rm = Rref^T R, tm = Rref^T (t - tref)
-ODB_DEVINL void relative_pose(const double* ref, const double* T, double* M) {
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-#pragma unroll
-    for (int j = 0; j < 3; ++j)
-      M[3 * i + j] = __dadd_rn(__dadd_rn(__dmul_rn(ref[i], T[j]), __dmul_rn(ref[3 + i], T[3 + j])),
-                               __dmul_rn(ref[6 + i], T[6 + j]));
-    M[9 + i] = __dadd_rn(__dadd_rn(__dmul_rn(ref[i], __dsub_rn(T[9], ref[9])),
-                                   __dmul_rn(ref[3 + i], __dsub_rn(T[10], ref[10]))),
-                         __dmul_rn(ref[6 + i], __dsub_rn(T[11], ref[11])));
-  }
-}
-
-// exp of the twist (v, omega): R = I + A W + B W^2, u = (I + B W + C W^2) v with W = [omega]x, W^2 = omega omega^T -
-// theta^2 I, A = sin(theta) / theta, B = (1 - cos(theta)) / theta^2, C = (theta - sin(theta)) / theta^3; below
-// kSeriesTheta the Taylor series to theta^4
-ODB_DEVINL void se3_exp(const double xi[6], double R[9], double u[3]) {
-  const double om[3] = {xi[3], xi[4], xi[5]};
-  const double th2 = dot3_rn(om, om), th = __dsqrt_rn(th2);
-  double A, B, C;
-  if (th < kSeriesTheta) {
-    const double th4 = __dmul_rn(th2, th2);
-    A = __dadd_rn(__dsub_rn(1.0, __ddiv_rn(th2, 6.0)), __ddiv_rn(th4, 120.0));
-    B = __dadd_rn(__dsub_rn(0.5, __ddiv_rn(th2, 24.0)), __ddiv_rn(th4, 720.0));
-    C = __dadd_rn(__dsub_rn(1.0 / 6.0, __ddiv_rn(th2, 120.0)), __ddiv_rn(th4, 5040.0));
-  } else {
-    double sn, cs;                                  // sin(theta), cos(theta); no Payne-Hanek path (no stack frame)
-    sincospi(__ddiv_rn(th, kPi), &sn, &cs);
-    A = __ddiv_rn(sn, th);
-    B = __ddiv_rn(__dsub_rn(1.0, cs), th2);
-    C = __ddiv_rn(__dsub_rn(th, sn), __dmul_rn(th2, th));
-  }
-  const double W[9] = {0.0, -om[2], om[1], om[2], 0.0, -om[0], -om[1], om[0], 0.0};
-  double V[9];
-#pragma unroll
-  for (int i = 0; i < 3; ++i)
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double w2 = i == j ? __dsub_rn(__dmul_rn(om[i], om[j]), th2) : __dmul_rn(om[i], om[j]);
-      const double id = i == j ? 1.0 : 0.0;
-      R[3 * i + j] = __dadd_rn(__dadd_rn(id, __dmul_rn(A, W[3 * i + j])), __dmul_rn(B, w2));
-      V[3 * i + j] = __dadd_rn(__dadd_rn(id, __dmul_rn(B, W[3 * i + j])), __dmul_rn(C, w2));
-    }
-#pragma unroll
-  for (int i = 0; i < 3; ++i) u[i] = dot3_rn(V + 3 * i, xi);
 }
 
 // A reference pixel is usable with a surface, a finite colour and a usable normal; its luminance Y in fp64
@@ -485,9 +432,40 @@ __global__ void track_output_kernel(TrkParams P, const double* __restrict__ init
   record[7] = st[kNValid];
 }
 
+// info [n][n] = sum w J J^T of the last step that ran: columns 0..kTri-1 of the chunk partials folded in chunk order by
+// ordered_sum8 exactly as that step's last CTA folded them, so the matrix is the one its Cholesky factored (unscaled)
+__global__ void __launch_bounds__(kTrkThreads) track_information_kernel(const double* __restrict__ part, int chunks,
+                                                                        int n, double* __restrict__ info) {
+  __shared__ double tot[kPart];
+  const int col = threadIdx.x & 31;
+  const double lo = ordered_sum8(chunks, true, [&](int c) { return __ldcg(part + (long long)c * kPart + col); });
+  if (threadIdx.x < 32) tot[col] = lo;
+  __syncthreads();
+  const double hi = ordered_sum8(chunks, 32 + col < kTri,
+                                 [&](int c) { return __ldcg(part + (long long)c * kPart + 32 + col); });
+  if (threadIdx.x < 32) tot[32 + col] = hi;
+  __syncthreads();
+  if (threadIdx.x < n * n) {
+    const int p = threadIdx.x / n, q = threadIdx.x - p * n;
+    info[threadIdx.x] = tot[p <= q ? tri_index(p, q) : tri_index(q, p)];
+  }
+}
+
 }  // namespace odb
 
 using namespace odb;
+
+extern "C" int odb_track_information(const void* workspace, int32_t h, int32_t w, int32_t unknowns, double* info,
+                                     void* stream_) {
+  if (!workspace || !info || !planes_ok(1, h, w) || (unknowns != 6 && unknowns != 8) || !aligned(workspace, 8) ||
+      !aligned(info, 8))
+    return fail(ODB_ERR_INVALID, "track_information: bad argument");
+  const double* part = static_cast<const double*>(workspace) + 1 + kState;
+  track_information_kernel<<<1, kTrkThreads, 0, static_cast<cudaStream_t>(stream_)>>>(part, trk_chunks(h, w),
+                                                                                      unknowns, info);
+  count_launch();
+  return check_launch("track_information");
+}
 
 extern "C" int64_t odb_track_workspace_bytes(int32_t h, int32_t w) {
   if (!planes_ok(1, h, w)) return -1;

@@ -1349,3 +1349,86 @@ def track_frame(pred, ref_depth, ref_normals, intrinsics, ref_pose, init_pose, i
           poses[1].ctypes.data, _ptr(init_nodes), 1 if affine else 0, int(iterations), float(tol), float(robust),
           float(max_dist), float(min_overlap), workspace.data_ptr(), pose.data_ptr(), nodes.data_ptr(),
           record.data_ptr())
+
+
+def track_information(workspace, h: int, w: int, unknowns: int, info):
+    """info fp64 [n,n] (n = unknowns, 6 or 8) = the normal matrix of the last step of the last track_frame call on
+    workspace at h x w (include/omnidata_b200.h odb_track_information)."""
+    name = "track_information"
+    if unknowns not in (6, 8):
+        raise _capi.OdbError(f"{name}: unknowns must be 6 or 8, got {unknowns!r}")
+    _check_workspace(name, workspace, track_workspace_bytes(h, w))
+    _need_shape(info, (unknowns, unknowns), torch.float64, "info")
+    _call(name, {"bytes": 8 * unknowns * unknowns}, lib().odb_track_information, _same_device(workspace, info),
+          workspace.data_ptr(), h, w, unknowns, info.data_ptr())
+
+
+# ---------------------------------------------------------------- pose graphs (csrc/posegraph.cu)
+POSEGRAPH_MAX_ITERATIONS = 100
+
+
+def check_posegraph_sizes(name: str, n_nodes: int, n_edges: int):
+    """OdbError unless 2 <= n_nodes <= POSEGRAPH_MAX_NODES and 1 <= n_edges <= 8 n_nodes."""
+    if not 2 <= n_nodes <= _capi.POSEGRAPH_MAX_NODES or not 1 <= n_edges <= 8 * n_nodes:
+        raise _capi.OdbError(f"{name}: need 2 <= N <= {_capi.POSEGRAPH_MAX_NODES} nodes and 1 <= E <= 8 N edges, got "
+                             f"N = {n_nodes}, E = {n_edges}")
+
+
+def posegraph_workspace_bytes(n_nodes: int, n_edges: int) -> int:
+    check_posegraph_sizes("posegraph_workspace_bytes", n_nodes, n_edges)
+    return int(lib().odb_posegraph_workspace_bytes(n_nodes, n_edges))
+
+
+def check_posegraph(name: str, poses, edges, measurements, information):
+    """Host (poses float64 [N,16], edges int32 [E,2], measurements float64 [E,16], information float64 [E,36]) from
+    numpy or CPU tensors; OdbError unless the poses pass check_poses, every edge (i, j) has 0 <= i, j < N and i != j,
+    every measurement is rigid (check_poses) and every information matrix is a finite symmetric 6 x 6 matrix."""
+    T = check_poses(f"{name} poses", poses)
+    n = T.shape[0]
+    E = np.asarray(edges.numpy() if isinstance(edges, torch.Tensor) else edges)
+    if E.ndim != 2 or E.shape[1] != 2 or not np.issubdtype(E.dtype, np.integer):
+        raise _capi.OdbError(f"{name}: edges must be an integer [E,2] array, got {E.dtype} {E.shape}")
+    check_posegraph_sizes(name, n, E.shape[0])
+    if (E < 0).any() or (E >= n).any():
+        raise _capi.OdbError(f"{name}: an edge index lies outside [0, {n})")
+    if (E[:, 0] == E[:, 1]).any():
+        raise _capi.OdbError(f"{name}: an edge joins a node to itself")
+    Z = check_poses(f"{name} measurements", measurements)
+    W = np.asarray(information.numpy() if isinstance(information, torch.Tensor) else information, np.float64)
+    if Z.shape[0] != E.shape[0] or W.shape != (E.shape[0], 6, 6):
+        raise _capi.OdbError(f"{name}: need [{E.shape[0]},4,4] measurements and [{E.shape[0]},6,6] information "
+                             f"matrices, got {Z.shape[0]} and {W.shape}")
+    if not np.isfinite(W).all():
+        raise _capi.OdbError(f"{name}: information matrices must be finite")
+    if not (W == W.transpose(0, 2, 1)).all():
+        raise _capi.OdbError(f"{name}: information matrices must be symmetric")
+    return T, np.ascontiguousarray(E, np.int32), Z, np.ascontiguousarray(W.reshape(-1, 36))
+
+
+def posegraph_optimize(edges, poses, measurements, information, iterations: int, tol: float, workspace, poses_out,
+                       record):
+    """poses_out fp64 [N,4,4] and record fp64 [POSEGRAPH_RECORD] of the pose graph of device edges int32 [E,2], poses
+    fp64 [N,4,4], measurements fp64 [E,4,4] and information fp64 [E,6,6], checked on the host by check_posegraph
+    (include/omnidata_b200.h odb_posegraph_optimize)."""
+    name = "posegraph_optimize"
+    _need(edges, torch.int32, "edges")
+    n, e = poses.shape[0], edges.shape[0]
+    check_posegraph_sizes(name, n, e)
+    _need_shape(edges, (e, 2), torch.int32, "edges")
+    _need_shape(poses, (n, 4, 4), torch.float64, "poses")
+    _need_shape(measurements, (e, 4, 4), torch.float64, "measurements")
+    _need_shape(information, (e, 6, 6), torch.float64, "information")
+    if isinstance(iterations, bool) or not isinstance(iterations, (int, np.integer)) or \
+            not 1 <= iterations <= POSEGRAPH_MAX_ITERATIONS:
+        raise _capi.OdbError(f"{name}: iterations must be an integer in [1, {POSEGRAPH_MAX_ITERATIONS}], got "
+                             f"{iterations!r}")
+    if isinstance(tol, bool) or not (isinstance(tol, numbers.Real) and math.isfinite(tol) and tol > 0):
+        raise _capi.OdbError(f"{name}: tol must be finite and > 0, got {tol!r}")
+    _check_workspace(name, workspace, posegraph_workspace_bytes(n, e))
+    _need_shape(poses_out, (n, 4, 4), torch.float64, "poses_out")
+    _need_shape(record, (_capi.POSEGRAPH_RECORD,), torch.float64, "record")
+    m = 6 * (n - 1)
+    _call(name, {"flops": iterations * m ** 3 / 3}, lib().odb_posegraph_optimize,
+          _same_device(edges, poses, measurements, information, workspace, poses_out, record), n, e,
+          edges.data_ptr(), poses.data_ptr(), measurements.data_ptr(), information.data_ptr(), int(iterations),
+          float(tol), workspace.data_ptr(), poses_out.data_ptr(), record.data_ptr())

@@ -24,7 +24,8 @@ correspondence, also for an empty model; degenerate: the scene does not fix ever
 nonfinite: NaN in init_nodes or the update) returns init_pose and init_nodes unchanged.
 
 The defaults max_dist = 0.1 m, robust = 0.02 m, min_overlap = 0.1, the pivot threshold 1e-6 and iterations = 20 are
-not tuned.  Tracking is frame-to-model only: drift is bounded by the model, not corrected (no loop closure).
+not tuned.  Tracking is frame-to-model: drift is bounded by the model and not corrected here; LoopClosure
+(omnidata_b200/loop.py) corrects it when the camera revisits a place, from the information matrices below.
 Photometric term (RGB-D odometry, Whelan et al. 2013; the joint cost of ElasticFusion): with `photometric` = lambda > 0
 each geometric correspondence also asks the reference image's luminance at the frame point's projection to equal the
 frame's, which fixes the motions that geometry alone leaves free (a textured wall).  Then
@@ -36,6 +37,11 @@ the intensity residual, fraction of them the Huber weight reduced).  The referen
 a buffer the tracker keeps; a call is one launch longer.  There is no exposure or brightness compensation between
 frames: real video will need it.  lambda = 1e-2 is what the sweep on the analytic scene chose (DESIGN.md §6); it is not
 tuned on real data.  photometric = 0 (the default) is the geometric tracker unchanged.
+
+`information()` after a call returns the normal matrix sum w J J^T of that call's last Gauss-Newton step, fp64 [n,n]
+on the device (n = 8 with affine, else 6; the photometric terms included, unscaled, in the tracker's (v, omega[, s,
+t]) increment coordinates): the information of the solved pose, as a pose-graph edge needs it.  It is meaningful only
+when that call's status is ok, and it reads the workspace of the last `track` call, so call it before the next one.
 
 Definition: DESIGN.md §3 "Camera tracking" and include/omnidata_b200.h; oracle/track_oracle.py restates it in float64,
 and oracle/photometric_oracle.py the photometric term.
@@ -78,6 +84,7 @@ class FrameTracker(_StepBuffers):
             float(min_overlap)
         self._jump = _check_jump(NORMAL_JUMP)
         self._bufs = {}
+        self._last_hw = None
 
     @_capi.on_tensor_device
     @torch.no_grad()
@@ -142,4 +149,20 @@ class FrameTracker(_StepBuffers):
         ops.track_frame(pred, ref_depth, normals, k, ref_pose.reshape(4, 4), init_pose.reshape(4, 4), init_nodes,
                         self.affine, self.iterations, self.tol, self.robust, self.max_dist, self.min_overlap, ws,
                         pose, nodes, rec, rgb, ref_rgb, intensity, self.photometric, self.photometric_robust)
+        self._last_hw = (h, w)
         return pose, nodes, rec
+
+    @torch.no_grad()
+    def information(self) -> torch.Tensor:
+        """fp64 [n,n] on the device (n = 8 with affine, else 6): sum w J J^T of the last Gauss-Newton step of the last
+        `track` call, meaningful when its status is ok (module docstring).  Kept for the next call, which overwrites
+        it."""
+        if self._last_hw is None:
+            raise ValueError("FrameTracker.information: no track call yet")
+        h, w = self._last_hw
+        ws = self._bufs["workspace"]
+        n = 8 if self.affine else 6
+        info = self._buf("information", (n, n), torch.float64, ws.device)
+        with torch.cuda.device(ws.device):
+            ops.track_information(ws, h, w, n, info)
+        return info

@@ -8,6 +8,7 @@ extracted mesh as a PLY:
                           [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
                           [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--guided_size HxW]
                           [--sparse_path DIR [--depth_scale 1000]] [--trunc T] [--color] [--photometric LAMBDA]
+                          [--loop_closure]
 
 Frames are the images of --img_path (PNG / JPEG) in file-name order.  Each has a pose, the 4 x 4 camera-to-world matrix
 as text (ScanNet's pose/<stem>.txt), in --pose_path by file stem.  The intrinsics are in pixels of the images.  The grid
@@ -41,7 +42,15 @@ image against the volume's coloured raycast at the initial pose.  It constrains 
 textured wall); 1e-2 is what the sweep on the analytic scene chose (DESIGN.md §6), not tuned on real data, and there is
 no exposure compensation between frames.  It is experimental like the tracking it refines.
 
-Prints one JSON line: frames used and skipped, vertices, faces and seconds.  Runs on cuda:0; there is no CPU path.
+--loop_closure (needs tracking, so no --pose_path or --track, and --photometric) corrects drift when the camera comes back to a place it has
+seen (`LoopClosure`, DESIGN.md §3 "Loop closure and pose graphs"): keyframes, loop candidates by pose proximity
+verified by tracking, an SE(3) pose-graph solve over the keyframes, and re-fusion of the volume from every stored frame
+at the corrected poses.  The next frame is tracked from the corrected last pose, and --pose_out writes the final poses.
+It keeps every frame's aligned depth on the device (4 bytes per pixel, 16 with --color).  Experimental like the
+tracking it corrects.
+
+Prints one JSON line: frames used and skipped, vertices, faces and seconds (with --loop_closure also the keyframes,
+the accepted loops as (frame i, frame j) index pairs of the used frames, and the number of re-fusions).  Runs on cuda:0; there is no CPU path.
 """
 from __future__ import annotations
 
@@ -117,6 +126,9 @@ def parse_args(argv=None):
     ap.add_argument("--photometric", type=float, default=None, metavar="LAMBDA",
                     help="experimental: track with a photometric term of this weight (m^2 per squared intensity "
                          "step; implies --color)")
+    ap.add_argument("--loop_closure", action="store_true",
+                    help="experimental: correct tracking drift at revisits (pose graph over keyframes, re-fusion; "
+                         "needs --photometric)")
     args = ap.parse_args(argv)
     if not (math.isfinite(args.voxel) and args.voxel > 0):
         ap.error(f"--voxel must be finite and > 0, got {args.voxel}")
@@ -143,6 +155,11 @@ def parse_args(argv=None):
             ap.error("--photometric weights a term of the tracking; with --pose_path nothing is tracked without "
                      "--track")
         args.color = True
+    if args.loop_closure and args.pose_path is not None and not args.track:
+        ap.error("--loop_closure corrects tracked poses; with --pose_path nothing is tracked without --track")
+    if args.loop_closure and args.photometric is None:
+        ap.error("--loop_closure needs --photometric: pose-graph edges from geometry alone bent the analytic test "
+                 "scene's trajectory instead of correcting it (DESIGN.md §6)")
     if args.pose_out is not None and Path(args.pose_out).exists() and not Path(args.pose_out).is_dir():
         ap.error(f"--pose_out must be a directory, got the file {args.pose_out}")
     if args.mode == "guided":
@@ -153,28 +170,34 @@ def parse_args(argv=None):
     return args
 
 
-def align_and_integrate(volume, aligner, pred: torch.Tensor, intrinsics, pose: np.ndarray, sparse=None, rgb=None):
+def align_and_integrate(volume, aligner, pred: torch.Tensor, intrinsics, pose: np.ndarray, sparse=None, rgb=None,
+                        loop=None):
     """One frame of the loop: fit pred fp32 [1,H,W] to sparse [1,H,W] (metres, 0 = none) or, without it, to the
     volume's raycast at pose; integrate the aligned depth (and rgb fp32 [3,H,W] into a colour volume) when the fit is
-    ok.  Returns the aligner's record (fp64 [8], on the host) and the nodes (scale, shift)."""
+    ok, and store it in loop (a LoopClosure) when given.  Returns the aligner's record (fp64 [8], on the host) and the
+    nodes (scale, shift)."""
     h, w = pred.shape[-2:]
     target = sparse if sparse is not None else volume.raycast(intrinsics, pose, (h, w)).unsqueeze(0)
     nodes, rec = aligner.fit(pred, target)
     rec, st = rec[0].cpu(), nodes.reshape(2).cpu()
     if int(rec[1]) == 0:
-        volume.integrate(aligner.apply(pred, nodes), intrinsics, pose, None if rgb is None else rgb.unsqueeze(0))
+        metres = aligner.apply(pred, nodes)
+        volume.integrate(metres, intrinsics, pose, None if rgb is None else rgb.unsqueeze(0))
+        if loop is not None and loop.add(metres, pose, rgb):
+            loop.refuse(volume)
     return rec, (float(st[0]), float(st[1]))
 
 
 def track_and_integrate(volume, aligner, trackers, pred: torch.Tensor, intrinsics, init_pose: np.ndarray,
-                        sparse=None, rgb=None):
+                        sparse=None, rgb=None, loop=None):
     """One frame of the tracking loop: raycast the volume at init_pose, fit pred fp32 [1,H,W] with the aligner to
     sparse [1,H,W] (metres, 0 = none) or, without it, to that raycast, track it (trackers[False] on the aligned metres
     with sparse, else trackers[True] on pred with the fitted (s, t) as initial nodes), and integrate the aligned depth at
     the tracked pose.  rgb fp32 [3,H,W] (a colour volume): integrated with the depth and, for trackers with a
     photometric term, tracked against the coloured raycast.  Returns (failure, pose, (s, t)): failure None when the
     frame was integrated, else "fit: <status>" or "track: <status>"; pose the tracked host float64 [4,4] (None on
-    failure)."""
+    failure).  With loop (a LoopClosure) the integrated frame is stored there; when that closes a loop the volume is
+    re-fused and pose is the frame's corrected pose."""
     from omnidata_b200.sparse import STATUS as FIT_STATUS
     from omnidata_b200.track import STATUS as TRACK_STATUS
     h, w = pred.shape[-2:]
@@ -197,11 +220,15 @@ def track_and_integrate(volume, aligner, trackers, pred: torch.Tensor, intrinsic
         return f"track: {TRACK_STATUS[status]}", None, None
     pose = pose.cpu().numpy()
     volume.integrate(metres, intrinsics, pose, None if rgb is None else rgb.unsqueeze(0))
+    if loop is not None and loop.add(metres, pose, rgb):
+        loop.refuse(volume)
+        pose = loop.poses[-1]
     st = nodes.reshape(2).cpu()
     return None, pose, (float(st[0]), float(st[1]))
 
 
 def reconstruct(args) -> dict:
+    from omnidata_b200.loop import LoopClosure
     from omnidata_b200.sparse import STATUS, SparseDepthAligner
     from omnidata_b200.track import FrameTracker
     from omnidata_b200.volume import TSDFVolume, write_ply
@@ -223,6 +250,7 @@ def reconstruct(args) -> dict:
     trackers = {a: FrameTracker(affine=a, photometric=lam) for a in (False, True)} if tracking else None
     if args.pose_out is not None:
         Path(args.pose_out).mkdir(parents=True, exist_ok=True)
+    loop = None
     last = np.eye(4)                                  # the last good pose: frame 0's without --pose_path
     used, skipped = [], []
     for q, (p, pose) in enumerate(zip(images, poses)):
@@ -241,25 +269,35 @@ def reconstruct(args) -> dict:
                 raise ValueError(f"{p.name}: the sparse depth is {sp.shape[0]}x{sp.shape[1]}, the image "
                                  f"{pred.shape[-2]}x{pred.shape[-1]}")
             sparse = torch.from_numpy(sp).unsqueeze(0).to(device)
+        if args.loop_closure and loop is None:
+            loop = LoopClosure(args.intrinsics, tuple(pred.shape[-2:]), photometric=lam, device=device)
         if tracking and used:
             failure, pose, _ = track_and_integrate(volume, aligner, trackers, pred, args.intrinsics,
-                                                   pose if posed else last, sparse, rgb)
+                                                   pose if posed else last, sparse, rgb, loop)
         else:
             pose = last if pose is None else pose
-            rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse, rgb)
+            rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse, rgb, loop)
             failure = None if int(rec[1]) == 0 else STATUS[int(rec[1])]
         if failure is None:
-            used.append(p.name)
+            used.append(p)
             last = pose
-            if args.pose_out is not None:
+            if args.pose_out is not None and loop is None:
                 np.savetxt(Path(args.pose_out) / (p.stem + ".txt"), pose)
         else:
             skipped.append({"frame": p.name, "status": failure})
+    if args.pose_out is not None and loop is not None:
+        for p, pose in zip(used, loop.poses):                     # the final poses, after the last closure
+            np.savetxt(Path(args.pose_out) / (p.stem + ".txt"), pose)
     vertices, faces, colors = volume.extract_mesh()
     write_ply(args.out, vertices, faces, colors)
-    return {"frames": len(images), "frames_used": len(used), "frames_skipped": skipped,
-            "vertices": int(vertices.shape[0]), "faces": int(faces.shape[0]), "dims": list(args.dims),
-            "voxel": args.voxel, "out": str(args.out), "seconds": round(time.perf_counter() - t0, 3)}
+    result = {"frames": len(images), "frames_used": len(used), "frames_skipped": skipped,
+              "vertices": int(vertices.shape[0]), "faces": int(faces.shape[0]), "dims": list(args.dims),
+              "voxel": args.voxel, "out": str(args.out), "seconds": round(time.perf_counter() - t0, 3)}
+    if loop is not None:
+        result.update(keyframes=len(loop.keyframes), loops=[list(pair) for pair in loop.loops],
+                      refusions=loop.refusions)
+        result["seconds"] = round(time.perf_counter() - t0, 3)
+    return result
 
 
 def main(argv=None) -> dict:
