@@ -131,6 +131,14 @@ def _stats(corr, e, wt, robust):
     return count, np.sqrt(we2 / wsum) if wsum > 0 else 0.0, down / count if count > 0 else 0.0
 
 
+def normal_matrix(A, Ph, lam):
+    """(H [8,8], g [8]) of one step with both terms: track_oracle.normal_matrix of the geometric association A plus
+    lam times sum w_c J_c J_c^T (and sum w_c J_c e_c) over the photometric terms Ph (photometric)."""
+    H, g = TO.normal_matrix(A)
+    Jc, ec, wc = Ph["J"].reshape(-1, 8), Ph["e"].reshape(-1), Ph["w"].reshape(-1)
+    return H + (Jc * (lam * wc)[:, None]).T @ Jc, g + (Jc * (lam * wc)[:, None]).T @ ec
+
+
 def step(pred, ref_depth, normals, K, ref, T, s, t, affine, robust, max_dist, min_overlap, rgb, intensity, lam,
          robust_c):
     """One Gauss-Newton iteration with both terms: (status, T', s', t', stats, xi) with stats = (correspondences,
@@ -139,10 +147,9 @@ def step(pred, ref_depth, normals, K, ref, T, s, t, affine, robust, max_dist, mi
     Rm, tm = TO.relative_pose(ref, T)
     A = associate(pred, ref_depth, normals, K, Rm, tm, s, t, max_dist, robust)
     Ph = photometric(A, rgb, intensity, K, Rm, robust_c)
-    J, e, wt = A["J"].reshape(-1, 8), A["e"].reshape(-1), A["w"].reshape(-1)
-    Jc, ec, wc = Ph["J"].reshape(-1, 8), Ph["e"].reshape(-1), Ph["w"].reshape(-1)
-    H = (J * wt[:, None]).T @ J + (Jc * (lam * wc)[:, None]).T @ Jc
-    g = (J * wt[:, None]).T @ e + (Jc * (lam * wc)[:, None]).T @ ec
+    e, wt = A["e"].reshape(-1), A["w"].reshape(-1)
+    ec, wc = Ph["e"].reshape(-1), Ph["w"].reshape(-1)
+    H, g = normal_matrix(A, Ph, lam)
     count, valid = float(A["corr"].sum()), float(A["valid"].sum())
     stats = _stats(A["corr"], e, wt, robust) + (valid,) + _stats(Ph["corr"], ec, wc, robust_c)
     n = 8 if affine else 6

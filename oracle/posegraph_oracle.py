@@ -179,13 +179,7 @@ def chain_graph(n, rng, loops=0, step=0.05, turn=0.05, noise=(0.0, 0.0), info_sc
     random loop edges (i, j), j >= i + 2, with measurements the true relative poses times exp of Gaussian noise of
     (position, rotation) standard deviations `noise`, and diagonal information (info_scale[0] on v, [1] on omega,
     each entry scaled by a random factor in [0.5, 2]).  Returns (truth [n,4,4], edges [E,2], Z [E,4,4], W [E,6,6])."""
-    T = [np.eye(4)]
-    for _ in range(n - 1):
-        d = rng.standard_normal(3)
-        inc = random_rotation(turn, rng)
-        inc[:3, 3] = step * d / np.linalg.norm(d)
-        T.append(T[-1] @ inc)
-    T = np.stack(T)
+    T = _walk(n, rng, step, turn)
     edges = [(k, k + 1) for k in range(n - 1)]
     while len(edges) < n - 1 + loops and n > 2:
         i = int(rng.integers(0, n - 2))
@@ -196,6 +190,59 @@ def chain_graph(n, rng, loops=0, step=0.05, turn=0.05, noise=(0.0, 0.0), info_sc
         xi = np.r_[noise[0] * rng.standard_normal(3), noise[1] * rng.standard_normal(3)]
         Z.append(np.linalg.inv(T[i]) @ T[j] @ se3_exp_matrix(xi))
         W.append(np.diag(np.r_[[info_scale[0]] * 3, [info_scale[1]] * 3] * rng.uniform(0.5, 2.0, 6)))
+    Z = np.stack(Z)
+    Z[:, :3, :3] = [_orthonormal(R) for R in Z[:, :3, :3]]
+    return T, np.array(edges, np.int64), Z, np.stack(W)
+
+
+def _walk(n, rng, step, turn):
+    T = [np.eye(4)]
+    for _ in range(n - 1):
+        d = rng.standard_normal(3)
+        inc = random_rotation(turn, rng)
+        inc[:3, 3] = step * d / np.linalg.norm(d)
+        T.append(T[-1] @ inc)
+    return np.stack(T)
+
+
+def full_information(rng, scale=1e3, spread=1e2):
+    """A random SPD 6 x 6 W = Q diag(lam) Q^T, exactly symmetric, with eigenvalues from scale to scale * spread
+    (log-uniform between the two ends, both of which occur) and random eigenvectors Q: v-omega coupling in every
+    entry."""
+    lam = scale * spread ** np.r_[0.0, 1.0, rng.uniform(0.0, 1.0, 4)]
+    Q, _ = np.linalg.qr(rng.standard_normal((6, 6)))
+    W = (Q * lam) @ Q.T
+    return (W + W.T) / 2
+
+
+def loop_graph(n, rng, n_edges=None, hubs=(), star=False, reverse=False, step=0.05, turn=0.05, noise=(0.01, 0.01),
+               scale=1e3, spread=1e2):
+    """A keyframe graph as loop closure builds it: a random walk of n poses (chain_graph's) with
+    - odometry edges (k, k + 1), or with `star` one edge between every node and node 0 (and nothing else), so that the
+      normal matrix is block-diagonal;
+    - for every node h in `hubs`, an edge between h and every other node;
+    - random loop edges (i, j), i < j, between any two distinct nodes until there are n_edges edges (parallel edges
+      included; at n = 2 every edge joins nodes 0 and 1);
+    - with `reverse`, every odd edge listed as (j, i) instead of (i, j) (its measurement taken the other way).
+    Measurements are the true relative poses times exp of Gaussian noise of (position, rotation) standard deviations
+    `noise`; every W is full_information(rng, scale, spread).  Returns (truth [n,4,4], edges [E,2], Z [E,4,4],
+    W [E,6,6]); E <= 8 n is the caller's to respect."""
+    T = _walk(n, rng, step, turn)
+    if star:
+        edges = [(0, k) if rng.random() < 0.5 else (k, 0) for k in range(1, n)]
+    else:
+        edges = [(k, k + 1) for k in range(n - 1)]
+    edges += [(h, k) for h in hubs for k in range(n) if k != h]
+    while n_edges is not None and len(edges) < n_edges:
+        i, j = sorted(int(v) for v in rng.choice(n, 2, replace=False))
+        edges.append((i, j))
+    if reverse:
+        edges = [(j, i) if e % 2 else (i, j) for e, (i, j) in enumerate(edges)]
+    Z, W = [], []
+    for i, j in edges:
+        xi = np.r_[noise[0] * rng.standard_normal(3), noise[1] * rng.standard_normal(3)]
+        Z.append(np.linalg.inv(T[i]) @ T[j] @ se3_exp_matrix(xi))
+        W.append(full_information(rng, scale, spread))
     Z = np.stack(Z)
     Z[:, :3, :3] = [_orthonormal(R) for R in Z[:, :3, :3]]
     return T, np.array(edges, np.int64), Z, np.stack(W)

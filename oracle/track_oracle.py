@@ -125,14 +125,36 @@ def residual(pred, ref_depth, normals, K, Rm, tm, s, t, assoc):
     return _dot(n, [Q[k] - V[k] for k in range(3)])
 
 
+def normal_matrix(A):
+    """(H [8,8], g [8]) = (sum w J J^T, sum w J e) over the correspondences of an association A (associate)."""
+    J, e, wt = A["J"].reshape(-1, 8), A["e"].reshape(-1), A["w"].reshape(-1)
+    return (J * wt[:, None]).T @ J, (J * wt[:, None]).T @ e
+
+
+def ordered_sum8(parts):
+    """Sum over the first axis of parts [P, ...] in common.cuh ordered_sum8's order: lane l adds parts l, l + 8, ... in
+    ascending order from 0.0, then the eight lane sums are added in lane order from 0.0 (how track.cu folds its chunk
+    partials)."""
+    parts = np.asarray(parts, np.float64)
+    lanes = []
+    for lane in range(8):
+        t = np.zeros(parts.shape[1:])
+        for p in range(lane, parts.shape[0], 8):
+            t = t + parts[p]
+        lanes.append(t)
+    s = np.zeros(parts.shape[1:])
+    for t in lanes:
+        s = s + t
+    return s
+
+
 def step(pred, ref_depth, normals, K, ref, T, s, t, affine, robust, max_dist, min_overlap):
     """One Gauss-Newton iteration: (status, T', s', t', stats, xi) with stats = (correspondences, weighted RMS, fraction
     down-weighted, valid pixels) and xi the solved increment (None unless solved)."""
     Rm, tm = relative_pose(ref, T)
     A = associate(pred, ref_depth, normals, K, Rm, tm, s, t, max_dist, robust)
-    J, e, wt = A["J"].reshape(-1, 8), A["e"].reshape(-1), A["w"].reshape(-1)
-    H = (J * wt[:, None]).T @ J
-    g = (J * wt[:, None]).T @ e
+    e, wt = A["e"].reshape(-1), A["w"].reshape(-1)
+    H, g = normal_matrix(A)
     count, valid = float(A["corr"].sum()), float(A["valid"].sum())
     wsum, we2 = float(wt.sum()), float((wt * e * e).sum())
     down = float((A["corr"].reshape(-1) & (np.abs(e) > robust)).sum())

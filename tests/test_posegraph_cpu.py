@@ -1,6 +1,6 @@
 """The pose-graph oracle and the host side of the pose graph and loop closure (no GPU needed): the SE(3) logarithm
 against scipy and the exponential, the first-order Jacobians against central differences, recovery of a consistent
-graph, the host refusals of ops.check_posegraph, the reconstruct.py --loop_closure rules, and the ptxas check of
+graph, loop_graph's graphs accepted by the host checks and recovered, the host refusals of ops.check_posegraph, the reconstruct.py --loop_closure rules, and the ptxas check of
 csrc/posegraph.cu and csrc/track.cu (no spills or stack frames)."""
 import re
 import subprocess
@@ -61,6 +61,35 @@ def test_oracle_recovers_a_consistent_graph():
     P, rec = PG.optimize(P0, E, Z, W, iterations=20)
     assert rec[0] == PG.OK and rec[1] < 20 and np.abs(P - T).max() <= 1e-9
     assert rec[3] < 1e-15 * rec[2]
+
+
+@pytest.mark.parametrize("kw", [dict(n=2, n_edges=16, reverse=True), dict(n=12, hubs=(0, 5), reverse=True),
+                                dict(n=12, star=True), dict(n=65, n_edges=8 * 65, spread=1e6)],
+                         ids=["parallel", "hubs", "star", "8N"])
+def test_loop_graph_is_accepted_and_recovered(kw):
+    """loop_graph's graphs pass the host checks (full, exactly symmetric W), have the asked-for topology, and without
+    noise the oracle recovers the truth from perturbed poses."""
+    from omnidata_b200 import ops
+    rng = np.random.default_rng(7)
+    n = kw["n"]
+    T, E, Z, W = PG.loop_graph(n, rng, noise=(0.0, 0.0), **{k: v for k, v in kw.items() if k != "n"})
+    ops.check_posegraph("t", T, E, Z, W)
+    lam = np.linalg.eigvalsh(W)
+    spread = kw.get("spread", 1e2)
+    assert np.allclose(lam.min(1), 1e3) and np.allclose(lam.max(1), 1e3 * spread)
+    assert (np.abs(W[:, :3, 3:]) > 0).all()                    # v-omega coupling
+    if "n_edges" in kw:
+        assert len(E) == kw["n_edges"]
+    if n == 2:
+        assert (E == [1, 0]).all(1).sum() == (E == [0, 1]).all(1).sum() == 8
+    if kw.get("hubs"):
+        for h in kw["hubs"]:
+            assert {int(k) for k in E[(E == h).any(1)].reshape(-1)} == set(range(n))
+    if kw.get("star"):
+        assert len(E) == n - 1 and (E == 0).any(1).all()
+    P0 = np.stack([T[0]] + [TO.perturb(t, 0.02, np.radians(1.0), rng) for t in T[1:]])
+    P, rec = PG.optimize(P0, E, Z, W, iterations=20)
+    assert rec[0] == PG.OK and rec[1] < 20 and np.abs(P - T).max() <= 1e-9
 
 
 def test_oracle_status_rules():

@@ -1,6 +1,6 @@
 """Camera tracking on the CPU: the float64 oracle's SE(3) exponential against scipy's expm, its Jacobian against
 central differences, recovery of a perturbed pose and a corrupted scale and shift on the analytic sphere-in-a-room
-scene, the degenerate single-wall view, the host-side refusals of FrameTracker, ops.track_frame and reconstruct.py, and
+scene, the degenerate single-wall view, the chunk-partial fold ordered_sum8, the host-side refusals of FrameTracker, ops.track_frame and reconstruct.py, and
 the ptxas check of csrc/track.cu (no spills or stack frames)."""
 import re
 import subprocess
@@ -86,6 +86,24 @@ def _oracle_recovery(h, w):
     assert rec[1] == TO.OK and rec[4] < 30
     assert abs(s * 1.7 - 1) < 1e-3 and abs(t - 0.2 / 1.7) < 2e-3
     return dp, dr
+
+
+def test_ordered_sum8_adds_in_the_folds_order():
+    """Inputs whose sum depends on the order: lane l adds parts l, l + 8, ... from 0.0, then lanes 0..7 in order."""
+    big = 1e16                                   # big + 1.0 rounds back to big
+    # lane 0: big + (-big) = 0, lanes 1..7: 1.0 each -> 7.0; added in index order every 1.0 is lost -> 0.0
+    a = np.r_[big, [1.0] * 7, -big]
+    # one part per lane: 7.0 from lanes 0..6 is added to lane 7's big at once; one at a time it would be lost
+    b = np.r_[[1.0] * 7, big]
+    assert TO.ordered_sum8(a) == 7.0
+    assert TO.ordered_sum8(b) == 7.0 + big != big
+    seq = 0.0
+    for v in a:
+        seq += v
+    assert seq == 0.0                            # the plain ascending order gives another value
+    cols = TO.ordered_sum8(np.stack([a, np.r_[b, 0.0]], 1))     # columns are independent
+    assert cols.shape == (2,) and cols[0] == 7.0 and cols[1] == 7.0 + big
+    assert TO.ordered_sum8(np.ones((3, 2, 2))).tolist() == [[3.0, 3.0], [3.0, 3.0]]
 
 
 def test_oracle_recovers_pose_scale_and_shift():
