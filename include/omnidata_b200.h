@@ -866,6 +866,48 @@ int odb_posegraph_optimize(int32_t n_nodes, int32_t n_edges, const int32_t* edge
                            const double* measurements, const double* information, int32_t iterations, double tol,
                            void* workspace, double* poses_out, double* record, void* stream);
 
+/* ---- place recognition by randomized ferns (omnidata_b200/places.py FernDatabase) ---------------------------------
+ *
+ * No reference counterpart.  Glocker et al., "Real-time RGB-D camera relocalization via randomized ferns" (2015), as
+ * ElasticFusion uses it.  Definition in DESIGN.md §3 "Place recognition and relocalisation"; oracle/places_oracle.py
+ * restates it in float64.  All arrays are DEVICE arrays.
+ *
+ * odb_fern_encode: codes uint8 [n][F] of n frames, depth fp32 [n][h][w] (metres or a relative prediction) and rgb fp32
+ * [n][3][h][w]; 1 <= n <= 65535, ODB_FERN_GRID_ROWS <= h <= 65535, ODB_FERN_GRID_COLS <= w <= 65535,
+ * 1 <= F <= ODB_FERN_MAX_FERNS.
+ *   Thumbnail: cell (r, c) of the 60 x 80 grid covers rows floor(r h / 60) .. floor((r + 1) h / 60) - 1 and columns
+ *   floor(c w / 80) .. floor((c + 1) w / 80) - 1.  Each channel (depth, R, G, B) of a cell is the mean of its usable
+ *   samples (finite; depth also > 0): summed in fp64 with round-to-nearest adds, rows top to bottom and columns left to
+ *   right, divided by the count in fp64 and rounded to fp32; NaN without a usable sample.
+ *   Normalisation per frame and channel: m = the lower median (rank floor((n_f - 1) / 2)) of the n_f non-NaN cells,
+ *   s = the lower median of |v - m| over them, the difference an fp32 round-to-nearest subtraction.
+ *   Ferns: fern f has a cell p_f (fern_cells int32 [F]) and thresholds theta_f,c (fern_thresholds fp64 [F][4]).  Bit c
+ *   of code f is (double(v_c(p_f)) - double(m_c)) > theta_f,c double(s_c), both operations round-to-nearest fp64; a
+ *   NaN cell, a channel without non-NaN cells or with s = 0, and a cell index outside [0, 4800) give 0.
+ *   workspace: odb_fern_encode_workspace_bytes(n) bytes, 8-byte aligned.  3 launches.
+ *
+ * odb_fern_query: the k entries i < limit of db_codes uint8 [n_db][F] with the smallest distance to code uint8 [F],
+ * the distance being the number of ferns whose codes differ; ties to the lower index.  out_index and out_distance
+ * int32 [k], in (distance, index) order, padded with -1 beyond min(k, limit).  1 <= n_db <= ODB_FERN_MAX_ENTRIES,
+ * 0 <= limit <= n_db,
+ * 1 <= k <= ODB_FERN_MAX_K.  workspace: odb_fern_query_workspace_bytes(n_db) bytes, 8-byte aligned.  2 launches.
+ *
+ * Both only enqueue a fixed launch sequence (no host synchronisation), so they can be captured in a CUDA graph.
+ * Integer histograms and scans, no floating-point atomics: outputs are bit-reproducible.  Arguments are checked before
+ * any launch. */
+#define ODB_FERN_GRID_ROWS 60
+#define ODB_FERN_GRID_COLS 80
+#define ODB_FERN_MAX_FERNS 4096
+#define ODB_FERN_MAX_K 1024
+#define ODB_FERN_MAX_ENTRIES (1 << 28)
+int64_t odb_fern_encode_workspace_bytes(int32_t n);
+int odb_fern_encode(int32_t n, int32_t h, int32_t w, const float* depth, const float* rgb, int32_t n_ferns,
+                    const int32_t* fern_cells, const double* fern_thresholds, uint8_t* codes, void* workspace,
+                    void* stream);
+int64_t odb_fern_query_workspace_bytes(int32_t n_db);
+int odb_fern_query(int32_t n_db, int32_t n_ferns, const uint8_t* db_codes, const uint8_t* code, int32_t limit,
+                   int32_t k, int32_t* out_index, int32_t* out_distance, void* workspace, void* stream);
+
 /* ---- depth-boundary errors (omnidata_b200/metrics.py BoundaryMetrics) ---------------------------------------------
  *
  * The depth-boundary error (DBE) of iBims-1 (Koch et al., ECCV Workshops 2018): how far predicted depth edges lie from

@@ -33,6 +33,10 @@ TRACK_RECORD = 8                                # ODB_TRACK_RECORD
 TRACK_RGBD_RECORD = 11                          # ODB_TRACK_RGBD_RECORD
 POSEGRAPH_MAX_NODES = 1024                      # ODB_POSEGRAPH_MAX_NODES
 POSEGRAPH_RECORD = 7                            # ODB_POSEGRAPH_RECORD
+FERN_GRID = (60, 80)                            # ODB_FERN_GRID_ROWS, ODB_FERN_GRID_COLS
+FERN_MAX_FERNS = 4096                           # ODB_FERN_MAX_FERNS
+FERN_MAX_K = 1024                               # ODB_FERN_MAX_K
+FERN_MAX_ENTRIES = 1 << 28                      # ODB_FERN_MAX_ENTRIES
 
 
 class OdbError(RuntimeError):
@@ -264,6 +268,10 @@ _SIGNATURES = {
     "odb_posegraph_workspace_bytes": (C.c_int64, [C.c_int32] * 2),
     "odb_posegraph_optimize": (C.c_int, [C.c_int32] * 2 + [C.c_void_p] * 4 + [C.c_int32, C.c_double] +
                                [C.c_void_p] * 4),
+    "odb_fern_encode_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "odb_fern_encode": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 2 + [C.c_int32] + [C.c_void_p] * 5),
+    "odb_fern_query_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "odb_fern_query": (C.c_int, [C.c_int32] * 2 + [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 4),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -1,6 +1,6 @@
-"""Correct tracking drift when the camera revisits a place: keyframes, loop detection by pose proximity, verification
-by tracking, an SE(3) pose-graph solve (omnidata_b200/posegraph.py) and re-fusion of the TSDF volume at the corrected
-poses.  Host orchestration over the existing kernels.
+"""Correct tracking drift when the camera revisits a place: keyframes, loop detection by pose proximity (and, with
+places=True, by appearance), verification by tracking, an SE(3) pose-graph solve (omnidata_b200/posegraph.py) and
+re-fusion of the TSDF volume at the corrected poses.  Host orchestration over the existing kernels.
 
     from omnidata_b200.loop import LoopClosure
     loop = LoopClosure((fx, fy, cx, cy), (h, w))
@@ -31,10 +31,32 @@ and `add` returns True.  `refuse(volume)` then resets the volume and integrates 
 poses; integration loops over the frames in order at every point, so the result is bit-identical to a fresh volume
 integrating the same frames at those poses.  When no loop is accepted nothing changes.
 
+Place recognition (places=True; every frame then needs rgb).  Each new keyframe is encoded from its stored metres and
+rgb into a randomized-fern code (omnidata_b200/places.py FernDatabase), so candidates no longer depend on poses that
+may have drifted.  After the pose candidates, which are unchanged, up to `candidates` more come from the fern lookup
+over the keyframes i <= j - min_gap whose dissimilarity (the fraction of ferns whose codes differ) is at most
+max_dissimilarity, skipping those already proposed.  A fern candidate is verified by the same tracking but from init
+pose T_i, keyframe i's own pose: the match says that the views are alike, the drifted pose says nothing.  The
+acceptance rule, the solve and the re-posing are unchanged.
+
+Relocalisation (places=True).  `relocalise(pred, rgb, sparse=None)` finds the pose of a frame whose tracking failed:
+it encodes the frame and tries the nearest `candidates` keyframes under max_dissimilarity in order of distance,
+tracking pred from keyframe i's pose T_i against its stored metres and rgb (with sparse depths: pred fitted to them,
+then the metres with the metric tracker; without: FrameTracker(affine=True) from a SparseDepthAligner(grid=(1, 1),
+robust=0.05) fit of pred to keyframe i's metres).  The first candidate that passes the loop-edge test gives the pose,
+host [4,4]; None when none does.  The next `add` must then be of that frame: it always becomes a keyframe, and its
+first edge goes to keyframe i with the relocalisation's Z = T_i^-1 T^ and W (with affine tracking the information of
+the pose with the scale and shift marginalised out), not an odometry edge to keyframe j - 1, which it could not track
+against; that keyframe is not proposed again as a loop candidate in the same `add`, so the one constraint is not
+counted twice.  `cancel_relocalisation()` forgets a relocalisation whose frame is not added.  `relocalisations` lists
+(keyframe frame index, frame index) pairs.  Relocalisation starts only from a failure status: a frame that tracks to
+a wrong pose with status ok is not detected.
+
 Every default (keyframe_dist = 0.1 m, keyframe_angle = 5 degrees, min_gap = 10 keyframes, radius = 0.3 m, angle = 30
-degrees, candidates = 3, min_overlap = 0.3, max_rms = 0.01 m, the fallback sigmas) is untuned.  Loop edges are not
-robust (one wrong accepted edge bends the whole graph), the graph is SE(3) (no scale drift), candidates come from the
-poses alone (no place recognition) and a closure re-fuses every frame instead of de-integrating: DESIGN.md §8.
+degrees, candidates = 3, min_overlap = 0.3, max_rms = 0.01 m, the fallback sigmas, max_dissimilarity = MAX_DISSIMILARITY
+from the analytic orbit, DESIGN.md §6) is untuned on real data.  Loop edges are not robust (one wrong accepted edge
+bends the whole graph), the graph is SE(3) (no scale drift) and a closure re-fuses every frame instead of
+de-integrating: DESIGN.md §8.
 
 Use the photometric term (photometric = 1e-2, as the tracking): on the analytic scene's closed orbit, edges from
 geometry alone leave rotations about weakly seen axes nearly free, and a closure then bends the graph along them and
@@ -50,9 +72,13 @@ import torch
 
 from . import ops
 from .posegraph import PoseGraph
+from .places import FernDatabase
+from .sparse import SparseDepthAligner
 from .track import FrameTracker, _value_error
 
 FALLBACK_SIGMA = (0.01, math.radians(0.5))      # metres, radians: a failed odometry edge's information (untuned)
+MAX_DISSIMILARITY = 0.6                         # fern candidates' largest dissimilarity (DESIGN.md §6; untuned)
+RELOCALISE_ROBUST = 0.05                        # Huber threshold of relocalisation's scale-and-shift fit (untuned)
 
 
 def _angle_deg(Ra, Rb):
@@ -70,7 +96,8 @@ class LoopClosure:
 
     def __init__(self, intrinsics, size: Tuple[int, int], keyframe_dist: float = 0.1, keyframe_angle: float = 5.0,
                  min_gap: int = 10, radius: float = 0.3, angle: float = 30.0, candidates: int = 3,
-                 min_overlap: float = 0.3, max_rms: float = 0.01, photometric: float = 0.0, device=None):
+                 min_overlap: float = 0.3, max_rms: float = 0.01, photometric: float = 0.0, places: bool = False,
+                 max_dissimilarity: float = MAX_DISSIMILARITY, device=None):
         self.intrinsics = _value_error(ops.check_intrinsics, "LoopClosure", intrinsics)
         h, w = (int(v) for v in size)
         _value_error(ops._check_planes, "LoopClosure", 1, h, w)
@@ -83,6 +110,11 @@ class LoopClosure:
                              f"{candidates!r}")
         if not 0 < min_overlap <= 1:
             raise ValueError(f"LoopClosure: min_overlap must lie in (0, 1], got {min_overlap!r}")
+        if not isinstance(places, bool):
+            raise ValueError(f"LoopClosure: places must be a bool, got {places!r}")
+        if isinstance(max_dissimilarity, bool) or not (isinstance(max_dissimilarity, (int, float)) and
+                                                       0 <= max_dissimilarity <= 1):
+            raise ValueError(f"LoopClosure: max_dissimilarity must lie in [0, 1], got {max_dissimilarity!r}")
         self.size = (h, w)
         self.keyframe_dist, self.keyframe_angle = float(keyframe_dist), float(keyframe_angle)
         self.min_gap, self.radius, self.angle, self.candidates = min_gap, float(radius), float(angle), candidates
@@ -103,6 +135,12 @@ class LoopClosure:
         self.loops: List[Tuple[int, int]] = []        # accepted loop edges as (frame i, frame j)
         self.refusions = 0
         self.closures = 0
+        self.max_dissimilarity = float(max_dissimilarity)
+        self.places: Optional[FernDatabase] = FernDatabase((h, w), device=self.device) if places else None
+        self.relocalisations: List[Tuple[int, int]] = []   # (keyframe frame index, relocalised frame index)
+        self._reloc = None                            # (keyframe index i, Z, W) of the pending relocalisation
+        self._affine_tracker = FrameTracker(affine=True, photometric=photometric) if places else None
+        self._aligner = SparseDepthAligner(grid=(1, 1), robust=RELOCALISE_ROBUST) if places else None
 
     @property
     def frames(self) -> int:
@@ -139,6 +177,22 @@ class LoopClosure:
             return False, None, None, rec
         return True, pose.cpu().numpy(), self.tracker.information().cpu().numpy(), rec
 
+    def _edge_ok(self, rec) -> bool:
+        """The loop-edge test: status ok, correspondences >= min_overlap of the valid pixels, RMS <= max_rms."""
+        return int(rec[1]) == 0 and rec[0] >= self.min_overlap * rec[7] and rec[2] <= self.max_rms
+
+    def _fern_candidates(self, code: torch.Tensor, limit: int, count: int, skip=()) -> List[int]:
+        """Up to `count` keyframe indices i < limit in order of fern distance to code, at most max_dissimilarity, not
+        in skip."""
+        if limit <= 0:
+            return []
+        idx, dist = self.places.query(code, min(count + len(skip), limit), limit=limit)
+        out = []
+        for i, d in zip(idx.cpu().tolist(), dist.cpu().tolist()):
+            if i >= 0 and i not in skip and self.places.dissimilarity(d) <= self.max_dissimilarity:
+                out.append(i)
+        return out[:count]
+
     @torch.no_grad()
     def add(self, metres: torch.Tensor, pose, rgb: Optional[torch.Tensor] = None) -> bool:
         """Stores a frame integrated at pose (host [4,4]): metres fp32 [H,W] or [1,H,W] on the device, rgb fp32 [3,H,W]
@@ -148,8 +202,10 @@ class LoopClosure:
         if metres.numel() != h * w or metres.dtype != torch.float32 or metres.device != self.device:
             raise ValueError(f"{name}: metres must be fp32 [{h}, {w}] on {self.device}, got {metres.dtype} "
                              f"{tuple(metres.shape)} on {metres.device}")
-        if (self.frames and (rgb is None) != (self._rgb is None)) or (self.photometric > 0 and rgb is None):
-            raise ValueError(f"{name}: pass rgb for every frame or for none, and for every frame when photometric > 0")
+        if (self.frames and (rgb is None) != (self._rgb is None)) or \
+                ((self.photometric > 0 or self.places is not None) and rgb is None):
+            raise ValueError(f"{name}: pass rgb for every frame or for none, and for every frame when photometric > 0 "
+                             f"or with places")
         if rgb is not None and (rgb.numel() != 3 * h * w or rgb.dtype != torch.float32 or rgb.device != self.device):
             raise ValueError(f"{name}: rgb must be fp32 [3, {h}, {w}] on {self.device}")
         T = _value_error(ops.check_poses, name, pose).reshape(-1, 4, 4)
@@ -159,7 +215,8 @@ class LoopClosure:
         f = self.frames
         self._store(metres, rgb)
         self._poses.append(T.copy())
-        new_kf = not self.keyframes
+        reloc, self._reloc = self._reloc, None
+        new_kf = not self.keyframes or reloc is not None
         if not new_kf:
             last = self._kf_poses[-1]
             new_kf = np.linalg.norm(T[:3, 3] - last[:3, 3]) >= self.keyframe_dist or \
@@ -171,26 +228,47 @@ class LoopClosure:
         self._kf_poses.append(T.copy())
         self._attach.append((len(self.keyframes) - 1, np.eye(4)))
         j = len(self.keyframes) - 1
+        code = None
+        if self.places is not None:
+            code = self.places.encode(self._metres[f], self._rgb[f])[0]
+            self.places.add(code)
         if j == 0:
             return False
-        prev = self._kf_poses[j - 1]
-        ok, That, W, _ = self._track(f, self.keyframes[j - 1], prev, T)
-        if not ok:
-            That, W = T, np.diag([FALLBACK_SIGMA[0] ** -2] * 3 + [FALLBACK_SIGMA[1] ** -2] * 3)
-        self._edges.append((j - 1, j))
-        self._Z.append(np.linalg.inv(prev) @ That)
-        self._W.append(W)
+        if reloc is not None:
+            i, Z, W = reloc
+            self._edges.append((i, j))
+            self._Z.append(Z)
+            self._W.append(W)
+            self.relocalisations.append((self.keyframes[i], f))
+        else:
+            prev = self._kf_poses[j - 1]
+            ok, That, W, _ = self._track(f, self.keyframes[j - 1], prev, T)
+            if not ok:
+                That, W = T, np.diag([FALLBACK_SIGMA[0] ** -2] * 3 + [FALLBACK_SIGMA[1] ** -2] * 3)
+            self._edges.append((j - 1, j))
+            self._Z.append(np.linalg.inv(prev) @ That)
+            self._W.append(W)
+        # a relocalised keyframe already has its edge to the keyframe it was found against: not proposed again
+        skip = [] if reloc is None else [reloc[0]]
         accepted = []
         cands = []
         for i in range(0, j - self.min_gap + 1):
+            if i in skip:
+                continue
             Ti = self._kf_poses[i]
             d = float(np.linalg.norm(Ti[:3, 3] - T[:3, 3]))
             if d <= self.radius and _axis_angle_deg(Ti[:3, :3], T[:3, :3]) <= self.angle:
                 cands.append((d, i))
-        for _, i in sorted(cands)[:self.candidates]:
+        proposals = [(i, T) for _, i in sorted(cands)[:self.candidates]]
+        if code is not None:
+            # fern candidates, tracked from keyframe i's own pose
+            near = [i for i, _ in proposals] + skip
+            proposals += [(i, self._kf_poses[i]) for i in
+                          self._fern_candidates(code, j - self.min_gap + 1, self.candidates, near)]
+        for i, init in proposals:
             Ti = self._kf_poses[i]
-            ok, That, W, rec = self._track(f, self.keyframes[i], Ti, T)
-            if ok and rec[0] >= self.min_overlap * rec[7] and rec[2] <= self.max_rms:
+            ok, That, W, rec = self._track(f, self.keyframes[i], Ti, init)
+            if ok and self._edge_ok(rec):
                 accepted.append((i, np.linalg.inv(Ti) @ That, W))
         if not accepted:
             return False
@@ -206,6 +284,61 @@ class LoopClosure:
         self._poses = [self._kf_poses[k] @ rel for k, rel in self._attach]
         self.closures += 1
         return True
+
+    @torch.no_grad()
+    def relocalise(self, pred: torch.Tensor, rgb: torch.Tensor, sparse: Optional[torch.Tensor] = None):
+        """The camera-to-world pose (host float64 [4,4]) of a lost frame found against the keyframes, or None: pred
+        fp32 [H,W] or [1,H,W] (the relative prediction), rgb fp32 [3,H,W], sparse fp32 [1,H,W] metres (0: none) or
+        None (module docstring).  The next `add` must be of this frame."""
+        name = "LoopClosure.relocalise"
+        if self.places is None:
+            raise ValueError(f"{name}: needs places=True")
+        h, w = self.size
+        if pred.numel() != h * w or pred.dtype != torch.float32 or pred.device != self.device:
+            raise ValueError(f"{name}: pred must be fp32 [{h}, {w}] on {self.device}")
+        if rgb is None or rgb.numel() != 3 * h * w or rgb.dtype != torch.float32 or rgb.device != self.device:
+            raise ValueError(f"{name}: rgb must be fp32 [3, {h}, {w}] on {self.device}")
+        pred, rgb = pred.reshape(1, h, w), rgb.reshape(3, h, w)
+        self._reloc = None
+        if not self.keyframes:
+            return None
+        code = self.places.encode(pred[0], rgb)[0]
+        cands = self._fern_candidates(code, len(self.keyframes), self.candidates)
+        metres = None
+        if sparse is not None:
+            nodes, rec = self._aligner.fit(pred, sparse.reshape(1, h, w))
+            if int(rec[0, 1].item()) != 0:
+                return None
+            metres = self._aligner.apply(pred, nodes)[0]
+        for i in cands:
+            Ti = self._kf_poses[i]
+            kf = self.keyframes[i]
+            colour = dict(rgb=rgb, ref_rgb=self._rgb[kf]) if self.photometric > 0 else {}
+            if metres is not None:
+                tracker = self.tracker
+                pose, _, rec = tracker.track(metres, self._metres[kf], self.intrinsics, Ti, Ti, **colour)
+            else:
+                nodes, frec = self._aligner.fit(pred, self._metres[kf].unsqueeze(0))
+                if int(frec[0, 1].item()) != 0:
+                    continue
+                tracker = self._affine_tracker
+                pose, _, rec = tracker.track(pred[0], self._metres[kf], self.intrinsics, Ti, Ti,
+                                             init_nodes=nodes, **colour)
+            rec = rec.cpu().numpy()
+            if not self._edge_ok(rec):
+                continue
+            W = tracker.information().cpu().numpy()
+            if W.shape[0] == 8:                      # marginalise the scale and shift out of the pose's information
+                W = W[:6, :6] - W[:6, 6:] @ np.linalg.solve(W[6:, 6:], W[6:, :6])
+                W = (W + W.T) / 2
+            pose = pose.cpu().numpy()
+            self._reloc = (i, np.linalg.inv(Ti) @ pose, W)
+            return pose
+        return None
+
+    def cancel_relocalisation(self):
+        """Forgets the last relocalisation, for a frame that is not added after all."""
+        self._reloc = None
 
     @torch.no_grad()
     def refuse(self, volume):

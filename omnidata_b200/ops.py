@@ -1432,3 +1432,76 @@ def posegraph_optimize(edges, poses, measurements, information, iterations: int,
           _same_device(edges, poses, measurements, information, workspace, poses_out, record), n, e,
           edges.data_ptr(), poses.data_ptr(), measurements.data_ptr(), information.data_ptr(), int(iterations),
           float(tol), workspace.data_ptr(), poses_out.data_ptr(), record.data_ptr())
+
+
+# ---------------------------------------------------------------- place recognition (csrc/places.cu)
+def _check_fern_count(name: str, n_ferns):
+    if isinstance(n_ferns, bool) or not isinstance(n_ferns, (int, np.integer)) or \
+            not 1 <= n_ferns <= _capi.FERN_MAX_FERNS:
+        raise _capi.OdbError(f"{name}: the number of ferns must be an integer in [1, {_capi.FERN_MAX_FERNS}], got "
+                             f"{n_ferns!r}")
+
+
+def check_fern_frames(name: str, n: int, h: int, w: int):
+    """OdbError unless 1 <= n <= 65535 frames of h x w with FERN_GRID <= (h, w) <= 65535."""
+    _check_planes(name, n, h, w)
+    if h < _capi.FERN_GRID[0] or w < _capi.FERN_GRID[1]:
+        raise _capi.OdbError(f"{name}: frames must be at least {_capi.FERN_GRID[0]}x{_capi.FERN_GRID[1]} (the "
+                             f"thumbnail grid), got {h}x{w}")
+
+
+def fern_encode_workspace_bytes(n: int) -> int:
+    _check_planes("fern_encode_workspace_bytes", n, 1, 1)
+    return int(lib().odb_fern_encode_workspace_bytes(n))
+
+
+def fern_encode(depth, rgb, fern_cells, fern_thresholds, codes, workspace):
+    """codes uint8 [n,F] of depth fp32 [n,H,W] and rgb fp32 [n,3,H,W] under the fern table fern_cells int32 [F] and
+    fern_thresholds fp64 [F,4] (include/omnidata_b200.h odb_fern_encode).  Contiguous tensors on one device."""
+    name = "fern_encode"
+    _need(depth, torch.float32, "depth")
+    if depth.dim() != 3:
+        raise _capi.OdbError(f"{name}: depth must be [n,H,W], got {tuple(depth.shape)}")
+    n, h, w = depth.shape
+    check_fern_frames(name, n, h, w)
+    f = fern_cells.shape[0] if fern_cells.dim() == 1 else -1
+    _check_fern_count(name, f)
+    _need_shape(rgb, (n, 3, h, w), torch.float32, "rgb")
+    _need_shape(fern_cells, (f,), torch.int32, "fern_cells")
+    _need_shape(fern_thresholds, (f, 4), torch.float64, "fern_thresholds")
+    _need_shape(codes, (n, f), torch.uint8, "codes")
+    if not depth.is_contiguous():
+        raise _capi.OdbError(f"{name}: depth must be contiguous")
+    _check_workspace(name, workspace, fern_encode_workspace_bytes(n))
+    _call(name, {"bytes": 16 * n * h * w}, lib().odb_fern_encode,
+          _same_device(depth, rgb, fern_cells, fern_thresholds, codes, workspace), n, h, w, depth.data_ptr(),
+          rgb.data_ptr(), f, fern_cells.data_ptr(), fern_thresholds.data_ptr(), codes.data_ptr(), workspace.data_ptr())
+
+
+def fern_query_workspace_bytes(n_db: int) -> int:
+    if isinstance(n_db, bool) or not isinstance(n_db, (int, np.integer)) or not 1 <= n_db <= _capi.FERN_MAX_ENTRIES:
+        raise _capi.OdbError(f"fern_query_workspace_bytes: need 1 <= n_db <= {_capi.FERN_MAX_ENTRIES}, got {n_db!r}")
+    return int(lib().odb_fern_query_workspace_bytes(int(n_db)))
+
+
+def fern_query(db_codes, code, limit: int, k: int, out_index, out_distance, workspace):
+    """out_index and out_distance int32 [k]: the k entries i < limit of db_codes uint8 [n_db,F] nearest to code uint8
+    [F] in the number of differing ferns, in (distance, index) order, padded with -1 (include/omnidata_b200.h
+    odb_fern_query)."""
+    name = "fern_query"
+    _need(db_codes, torch.uint8, "db_codes")
+    if db_codes.dim() != 2 or not db_codes.is_contiguous():
+        raise _capi.OdbError(f"{name}: db_codes must be a contiguous [n_db,F] array, got {tuple(db_codes.shape)}")
+    n_db, f = db_codes.shape
+    _check_fern_count(name, f)
+    ws_bytes = fern_query_workspace_bytes(n_db)
+    _need_shape(code, (f,), torch.uint8, "code")
+    for what, v, lo, hi in (("limit", limit, 0, n_db), ("k", k, 1, _capi.FERN_MAX_K)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+            raise _capi.OdbError(f"{name}: {what} must be an integer in [{lo}, {hi}], got {v!r}")
+    _need_shape(out_index, (k,), torch.int32, "out_index")
+    _need_shape(out_distance, (k,), torch.int32, "out_distance")
+    _check_workspace(name, workspace, ws_bytes)
+    _call(name, {"bytes": int(limit) * f}, lib().odb_fern_query,
+          _same_device(db_codes, code, out_index, out_distance, workspace), n_db, f, db_codes.data_ptr(),
+          code.data_ptr(), int(limit), int(k), out_index.data_ptr(), out_distance.data_ptr(), workspace.data_ptr())

@@ -8,7 +8,7 @@ extracted mesh as a PLY:
                           [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
                           [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--guided_size HxW]
                           [--sparse_path DIR [--depth_scale 1000]] [--trunc T] [--color] [--photometric LAMBDA]
-                          [--loop_closure]
+                          [--loop_closure [--place_recognition]]
 
 Frames are the images of --img_path (PNG / JPEG) in file-name order.  Each has a pose, the 4 x 4 camera-to-world matrix
 as text (ScanNet's pose/<stem>.txt), in --pose_path by file stem.  The intrinsics are in pixels of the images.  The grid
@@ -49,8 +49,17 @@ at the corrected poses.  The next frame is tracked from the corrected last pose,
 It keeps every frame's aligned depth on the device (4 bytes per pixel, 16 with --color).  Experimental like the
 tracking it corrects.
 
+--place_recognition (needs --loop_closure) adds appearance to it (`LoopClosure(places=True)`, DESIGN.md §3 "Place
+recognition and relocalisation"): every keyframe gets a randomized-fern code, loop candidates also come from the
+keyframes that look alike, whatever the drifted poses say, and a frame whose fit or tracking fails is relocalised:
+`LoopClosure.relocalise` finds its pose against the most similar keyframes, and the frame then runs through the
+tracking from that pose (raycast, fit, tracking against the model, integration).  A frame that cannot be relocalised is
+skipped with status "relocalise: failed".  So a covered lens, a fast turn or a cut in the video no longer loses the
+rest of it.  Relocalisation starts only from a failure: a frame that tracks to a wrong pose is not detected.
+
 Prints one JSON line: frames used and skipped, vertices, faces and seconds (with --loop_closure also the keyframes,
-the accepted loops as (frame i, frame j) index pairs of the used frames, and the number of re-fusions).  Runs on cuda:0; there is no CPU path.
+the accepted loops as (frame i, frame j) index pairs of the used frames, and the number of re-fusions; with
+--place_recognition also the names of the relocalised frames).  Runs on cuda:0; there is no CPU path.
 """
 from __future__ import annotations
 
@@ -129,6 +138,9 @@ def parse_args(argv=None):
     ap.add_argument("--loop_closure", action="store_true",
                     help="experimental: correct tracking drift at revisits (pose graph over keyframes, re-fusion; "
                          "needs --photometric)")
+    ap.add_argument("--place_recognition", action="store_true",
+                    help="experimental: with --loop_closure, find loops by appearance and relocalise frames whose "
+                         "tracking fails")
     args = ap.parse_args(argv)
     if not (math.isfinite(args.voxel) and args.voxel > 0):
         ap.error(f"--voxel must be finite and > 0, got {args.voxel}")
@@ -160,6 +172,8 @@ def parse_args(argv=None):
     if args.loop_closure and args.photometric is None:
         ap.error("--loop_closure needs --photometric: pose-graph edges from geometry alone bent the analytic test "
                  "scene's trajectory instead of correcting it (DESIGN.md §6)")
+    if args.place_recognition and not args.loop_closure:
+        ap.error("--place_recognition needs --loop_closure (it keeps the keyframes it looks up)")
     if args.pose_out is not None and Path(args.pose_out).exists() and not Path(args.pose_out).is_dir():
         ap.error(f"--pose_out must be a directory, got the file {args.pose_out}")
     if args.mode == "guided":
@@ -227,6 +241,20 @@ def track_and_integrate(volume, aligner, trackers, pred: torch.Tensor, intrinsic
     return None, pose, (float(st[0]), float(st[1]))
 
 
+def relocalise_and_integrate(volume, aligner, trackers, loop, pred: torch.Tensor, intrinsics, sparse=None, rgb=None):
+    """A lost frame: its pose from loop.relocalise (a LoopClosure with places=True), then track_and_integrate from
+    there.  Returns (failure, pose, (s, t)) as track_and_integrate does; failure is "relocalise: failed" when no
+    keyframe gives a pose or the frame fails from the pose it gives."""
+    init = loop.relocalise(pred, rgb, sparse)
+    if init is None:
+        return "relocalise: failed", None, None
+    failure, pose, st = track_and_integrate(volume, aligner, trackers, pred, intrinsics, init, sparse, rgb, loop)
+    if failure is not None:
+        loop.cancel_relocalisation()
+        return "relocalise: failed", None, None
+    return None, pose, st
+
+
 def reconstruct(args) -> dict:
     from omnidata_b200.loop import LoopClosure
     from omnidata_b200.sparse import STATUS, SparseDepthAligner
@@ -252,7 +280,7 @@ def reconstruct(args) -> dict:
         Path(args.pose_out).mkdir(parents=True, exist_ok=True)
     loop = None
     last = np.eye(4)                                  # the last good pose: frame 0's without --pose_path
-    used, skipped = [], []
+    used, skipped, relocalised = [], [], []
     for q, (p, pose) in enumerate(zip(images, poses)):
         image = evaluate.image_tensor(p, "rgb")                   # [1,3,H,W] in [0, 1]
         x = ((image - 0.5) / 0.5).to(device)                       # image_tensor(p, "depth")'s normalisation
@@ -270,10 +298,16 @@ def reconstruct(args) -> dict:
                                  f"{pred.shape[-2]}x{pred.shape[-1]}")
             sparse = torch.from_numpy(sp).unsqueeze(0).to(device)
         if args.loop_closure and loop is None:
-            loop = LoopClosure(args.intrinsics, tuple(pred.shape[-2:]), photometric=lam, device=device)
+            loop = LoopClosure(args.intrinsics, tuple(pred.shape[-2:]), photometric=lam,
+                               places=args.place_recognition, device=device)
         if tracking and used:
             failure, pose, _ = track_and_integrate(volume, aligner, trackers, pred, args.intrinsics,
                                                    pose if posed else last, sparse, rgb, loop)
+            if failure is not None and args.place_recognition:
+                failure, pose, _ = relocalise_and_integrate(volume, aligner, trackers, loop, pred, args.intrinsics,
+                                                            sparse, rgb)
+                if failure is None:
+                    relocalised.append(p.name)
         else:
             pose = last if pose is None else pose
             rec, _ = align_and_integrate(volume, aligner, pred, args.intrinsics, pose, sparse, rgb, loop)
@@ -296,6 +330,8 @@ def reconstruct(args) -> dict:
     if loop is not None:
         result.update(keyframes=len(loop.keyframes), loops=[list(pair) for pair in loop.loops],
                       refusions=loop.refusions)
+        if args.place_recognition:
+            result["relocalised"] = relocalised
         result["seconds"] = round(time.perf_counter() - t0, 3)
     return result
 
