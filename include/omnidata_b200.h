@@ -768,6 +768,75 @@ int odb_tsdf_mesh_emit(const float* tsdf, const float* weight, const float* colo
                        double ox, double oy, double oz, double voxel, const void* workspace, float* vertices,
                        int32_t* faces, float* colors, void* stream);
 
+/* ---- Sparse TSDF volumes (omnidata_b200/volume.py SparseTSDFVolume) ----------------------------------------------
+ *
+ * No reference counterpart.  The TSDF volume above without a box: definitions in DESIGN.md §3 "Sparse TSDF volumes";
+ * oracle/sparse_volume_oracle.py restates them in float64.  Frames, intrinsics and poses as for the TSDF volumes.
+ *
+ * Lattice: points X(p) = origin + voxel p, p in Z^3, stored in blocks of 8^3: block b holds p = 8 b + (0..7)^3, laid
+ * out [k][j][i], with |b| < ODB_SPARSE_TSDF_BLOCK_RANGE per axis.  A block's key packs (bz, by, bx) + RANGE into 21
+ * bits each, bz highest, so keys order blocks by (bz, by, bx).  odb_sparse_tsdf describes one volume, all device
+ * arrays: data fp32 [capacity][channels][512] (channel 0 F, 1 W, 2-4 the colour means when channels = 5); keys int64
+ * [capacity] and birth int32 [capacity] of blocks 0..blocks-1 in id order; nbr int32 [capacity][8], entry c the id of
+ * block b + (c & 1, c >> 1 & 1, c >> 2) (-1: unallocated); the hash table table_keys int64 / table_ids int32 /
+ * table_birth int32 [table_size] (a power of two >= 1024, -1 / -1 / INT_MAX empty, at most half full between calls);
+ * bbox int32 [6] = the allocated blocks' min (x, y, z) and max (x, y, z), (INT_MAX x 3, INT_MIN x 3) when empty;
+ * scratch int32 [2 + table_size].
+ *
+ * Allocation of a call of b frames numbered frame0.. (frames count from the volume's construction or reset):
+ * odb_sparse_tsdf_mark: a pixel with finite depth d, 0 < d <= max_depth, covers its ray from z = d - trunc to
+ * z = d + trunc; in fp64 round-to-nearest, r = ((x - cx) / fx, (y - cy) / fy), the endpoint at z is X = R (z r_x,
+ * z r_y, z) + t, summed in the order x, y, z, then t; its block is floor(((X - origin) / voxel) * 0.125) per axis.  Every
+ * block of the box of the two endpoints' blocks is inserted into the table (integer CAS) with the earliest frame that
+ * covers it (integer atomicMin); blocks outside the range are not.  scratch[0] = the number of new blocks; scratch[1]
+ * = 1 when the table passed half full (the caller doubles the table, rebuilds it and marks again).
+ * odb_sparse_tsdf_rebuild: clears the table and inserts blocks 0..blocks-1 with their ids (after growing the table,
+ * and to forget a mark that is not committed).
+ * odb_sparse_tsdf_commit: gives the n_new marked blocks the ids blocks.. blocks+n_new-1 in the order (birth frame,
+ * key), zeroes their data, widens bbox and refreshes nbr; workspace: odb_sparse_tsdf_commit_workspace_bytes(n_new),
+ * 16-byte aligned.  capacity >= blocks + n_new.
+ * odb_sparse_tsdf_integrate: odb_tsdf_integrate's per-point arithmetic at every point of blocks 0..blocks-1, where a
+ * point updates from frame g only when g >= its block's birth frame.
+ * odb_sparse_tsdf_raycast: odb_tsdf_raycast (and, with rgb, odb_tsdf_raycast_color) over the grid of bbox: origin
+ * lo = origin + voxel 8 bmin, n = 8 (bmax - bmin + 1) points per axis, with unallocated points W = 0.  Samples of
+ * unallocated blocks are skipped without changing a bit.  Reads bbox on the device: no synchronisation.
+ * odb_sparse_tsdf_mesh_count + _emit: odb_tsdf_mesh_count / _emit over the allocated points (unallocated: W = 0), with
+ * vertices at origin + voxel (p + d s), vertex ids in (block id, point, direction) order and faces in (block id, cell,
+ * tetrahedron, triangle) order; workspace odb_sparse_tsdf_mesh_workspace_bytes(blocks), 8-byte aligned.
+ *
+ * Integer atomics only in the table, its birth stamps and the bounding box; every output is bit-reproducible and does
+ * not depend on how frames are split into calls. */
+#define ODB_SPARSE_TSDF_BLOCK_RANGE 1048576
+#define ODB_SPARSE_TSDF_MAX_BLOCKS 2097152
+typedef struct {
+  float* data;
+  int64_t* keys;
+  int32_t* birth;
+  int32_t* nbr;
+  int64_t* table_keys;
+  int32_t* table_ids;
+  int32_t* table_birth;
+  int32_t* bbox;
+  int32_t* scratch;
+  int32_t blocks, capacity, table_size, channels;
+  double ox, oy, oz, voxel;
+} odb_sparse_tsdf;
+int odb_sparse_tsdf_rebuild(const odb_sparse_tsdf* vol, void* stream);
+int odb_sparse_tsdf_mark(const odb_sparse_tsdf* vol, double trunc, double max_depth, const float* depth, int32_t b,
+                         int32_t h, int32_t w, double fx, double fy, double cx, double cy, const double* cam_to_world,
+                         int32_t frame0, void* stream);
+int64_t odb_sparse_tsdf_commit_workspace_bytes(int32_t n_new);
+int odb_sparse_tsdf_commit(const odb_sparse_tsdf* vol, int32_t n_new, void* workspace, void* stream);
+int odb_sparse_tsdf_integrate(const odb_sparse_tsdf* vol, double trunc, const float* depth, const float* rgb,
+                              int32_t b, int32_t h, int32_t w, double fx, double fy, double cx, double cy,
+                              const double* cam_to_world, int32_t frame0, void* stream);
+int odb_sparse_tsdf_raycast(const odb_sparse_tsdf* vol, const double* cam_to_world, int32_t h, int32_t w, double fx,
+                            double fy, double cx, double cy, double step, float* out, float* rgb, void* stream);
+int64_t odb_sparse_tsdf_mesh_workspace_bytes(int32_t blocks);
+int odb_sparse_tsdf_mesh_count(const odb_sparse_tsdf* vol, void* workspace, int64_t* counts, void* stream);
+int odb_sparse_tsdf_mesh_emit(const odb_sparse_tsdf* vol, const void* workspace, float* vertices, int32_t* faces,
+                              float* colors, void* stream);
+
 /* ---- camera tracking (omnidata_b200/track.py FrameTracker) ---------------------------------------------------------
  *
  * No reference counterpart.  Solves one frame's camera pose (and, with affine, the scale and shift of its depth) against

@@ -29,6 +29,8 @@ SPARSE_RECORD = 8                               # ODB_SPARSE_RECORD
 FUSION_RECORD = 8                               # ODB_FUSION_RECORD
 TSDF_MAX_DIM = 2048                             # ODB_TSDF_MAX_DIM
 TSDF_MAX_POINTS = 1 << 28                       # ODB_TSDF_MAX_POINTS
+SPARSE_TSDF_BLOCK_RANGE = 1 << 20               # ODB_SPARSE_TSDF_BLOCK_RANGE
+SPARSE_TSDF_MAX_BLOCKS = 1 << 21                # ODB_SPARSE_TSDF_MAX_BLOCKS
 TRACK_RECORD = 8                                # ODB_TRACK_RECORD
 TRACK_RGBD_RECORD = 11                          # ODB_TRACK_RGBD_RECORD
 POSEGRAPH_MAX_NODES = 1024                      # ODB_POSEGRAPH_MAX_NODES
@@ -49,6 +51,14 @@ class View(C.Structure):
         ("c", C.c_int32), ("w", C.c_int32), ("h", C.c_int32), ("b", C.c_int32),
         ("sx", C.c_int64), ("sy", C.c_int64), ("sb", C.c_int64),
     ]
+
+
+class SparseTSDF(C.Structure):
+    """odb_sparse_tsdf: one sparse TSDF volume's device arrays and geometry."""
+    _fields_ = [(n, C.c_void_p) for n in ("data", "keys", "birth", "nbr", "table_keys", "table_ids", "table_birth",
+                                          "bbox", "scratch")] + \
+               [(n, C.c_int32) for n in ("blocks", "capacity", "table_size", "channels")] + \
+               [(n, C.c_double) for n in ("ox", "oy", "oz", "voxel")]
 
 
 class ConvGemmDesc(C.Structure):
@@ -259,6 +269,17 @@ _SIGNATURES = {
                                [C.c_int32] * 2 + [C.c_double] * 5 + [C.c_void_p] * 3),
     "odb_tsdf_mesh_count": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 3 + [C.c_void_p] * 3),
     "odb_tsdf_mesh_emit": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_double] * 4 + [C.c_void_p] * 5),
+    "odb_sparse_tsdf_rebuild": (C.c_int, [C.c_void_p] * 2),
+    "odb_sparse_tsdf_mark": (C.c_int, [C.c_void_p] + [C.c_double] * 2 + [C.c_void_p] + [C.c_int32] * 3 +
+                             [C.c_double] * 4 + [C.c_void_p, C.c_int32, C.c_void_p]),
+    "odb_sparse_tsdf_commit_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "odb_sparse_tsdf_commit": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 2),
+    "odb_sparse_tsdf_integrate": (C.c_int, [C.c_void_p, C.c_double] + [C.c_void_p] * 2 + [C.c_int32] * 3 +
+                                  [C.c_double] * 4 + [C.c_void_p, C.c_int32, C.c_void_p]),
+    "odb_sparse_tsdf_raycast": (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_double] * 5 + [C.c_void_p] * 3),
+    "odb_sparse_tsdf_mesh_workspace_bytes": (C.c_int64, [C.c_int32]),
+    "odb_sparse_tsdf_mesh_count": (C.c_int, [C.c_void_p] * 4),
+    "odb_sparse_tsdf_mesh_emit": (C.c_int, [C.c_void_p] * 6),
     "odb_track_workspace_bytes": (C.c_int64, [C.c_int32] * 2),
     "odb_track_frame": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 3 +
                         [C.c_int32] * 2 + [C.c_double] * 4 + [C.c_void_p] * 5),

@@ -1253,6 +1253,148 @@ def tsdf_mesh_emit(tsdf, weight, color, dims, origin, voxel: float, workspace, v
           _ptr(colors))
 
 
+# ---------------------------------------------------------------- sparse TSDF volumes (csrc/sparse_volume.cu)
+def sparse_tsdf_desc(data, keys, birth, nbr, table_keys, table_ids, table_birth, bbox, scratch, blocks: int,
+                     origin, voxel: float) -> _capi.SparseTSDF:
+    """The odb_sparse_tsdf descriptor of one volume's device arrays (include/omnidata_b200.h): data fp32
+    [capacity, 2 or 5, 512], keys int64 / birth int32 [capacity], nbr int32 [capacity, 8], the table int64 / int32 /
+    int32 [table_size], bbox int32 [6], scratch int32 [2 + table_size]; OdbError on any mismatch."""
+    name = "sparse_tsdf"
+    _need(data, torch.float32, "data")
+    if data.dim() != 3 or data.shape[1] not in (2, 5) or data.shape[2] != 512 or not data.is_contiguous():
+        raise _capi.OdbError(f"{name}: data must be a contiguous fp32 [capacity, 2 or 5, 512], got {tuple(data.shape)}")
+    cap, tsize = data.shape[0], table_keys.numel()
+    for t, shape, dt, n in ((keys, (cap,), torch.int64, "keys"), (birth, (cap,), torch.int32, "birth"),
+                            (nbr, (cap, 8), torch.int32, "nbr"), (table_keys, (tsize,), torch.int64, "table_keys"),
+                            (table_ids, (tsize,), torch.int32, "table_ids"),
+                            (table_birth, (tsize,), torch.int32, "table_birth"), (bbox, (6,), torch.int32, "bbox"),
+                            (scratch, (2 + tsize,), torch.int32, "scratch")):
+        _need_shape(t, shape, dt, n)
+    _same_device(data, keys, birth, nbr, table_keys, table_ids, table_birth, bbox, scratch)
+    if not 0 <= blocks <= cap or cap > _capi.SPARSE_TSDF_MAX_BLOCKS or tsize < 1024 or tsize & (tsize - 1) or \
+            blocks > tsize // 2:
+        raise _capi.OdbError(f"{name}: {blocks} blocks do not fit capacity {cap} and table size {tsize}")
+    ox, oy, oz = (float(v) for v in origin)
+    if not all(math.isfinite(v) for v in (ox, oy, oz)) or not (math.isfinite(voxel) and voxel > 0):
+        raise _capi.OdbError(f"{name}: need a finite origin and a finite voxel > 0, got {origin!r}, {voxel}")
+    return _capi.SparseTSDF(data.data_ptr(), keys.data_ptr(), birth.data_ptr(), nbr.data_ptr(), table_keys.data_ptr(),
+                            table_ids.data_ptr(), table_birth.data_ptr(), bbox.data_ptr(), scratch.data_ptr(),
+                            int(blocks), int(cap), int(tsize), int(data.shape[1]), ox, oy, oz, float(voxel))
+
+
+def _sparse_frames(name, depth, rgb, channels, intrinsics, cam_to_world):
+    _need(depth, torch.float32, "depth")
+    if depth.dim() != 3 or not depth.is_contiguous():
+        raise _capi.OdbError(f"{name}: depth must be a contiguous fp32 [B,H,W] tensor, got {tuple(depth.shape)}")
+    b, h, w = depth.shape
+    _check_planes(name, b, h, w)
+    if (channels == 5) != (rgb is not None):
+        raise _capi.OdbError(f"{name}: rgb is required exactly when the volume stores colour")
+    if rgb is not None:
+        _need_shape(rgb, (b, 3, h, w), torch.float32, "rgb")
+    k = check_intrinsics(name, intrinsics)
+    T = check_poses(name, cam_to_world)
+    if T.shape[0] != b:
+        raise _capi.OdbError(f"{name}: {b} depth frames but {T.shape[0]} poses")
+    return b, h, w, k, T
+
+
+def sparse_tsdf_rebuild(desc: _capi.SparseTSDF, device):
+    """Clears the hash table and inserts the allocated blocks with their ids (odb_sparse_tsdf_rebuild)."""
+    _call("sparse_tsdf_rebuild", {}, lib().odb_sparse_tsdf_rebuild, device, C.byref(desc))
+
+
+def sparse_tsdf_mark(desc: _capi.SparseTSDF, device, trunc: float, max_depth: float, depth, intrinsics, cam_to_world,
+                     frame0: int):
+    """Inserts the blocks covered by depth fp32 [B,H,W] seen from cam_to_world into the table; scratch[0:2] = (new
+    blocks, table half full) (odb_sparse_tsdf_mark)."""
+    name = "sparse_tsdf_mark"
+    b, h, w, (fx, fy, cx, cy), T = _sparse_frames(name, depth, None, 2, intrinsics, cam_to_world)
+    if not (math.isfinite(trunc) and trunc > 0 and math.isfinite(max_depth) and max_depth > 0):
+        raise _capi.OdbError(f"{name}: trunc and max_depth must be finite and > 0, got {trunc}, {max_depth}")
+    _call(name, {"bytes": 4 * b * h * w}, lib().odb_sparse_tsdf_mark, _same_device(depth), C.byref(desc),
+          float(trunc), float(max_depth), depth.data_ptr(), b, h, w, fx, fy, cx, cy, T.ctypes.data, int(frame0))
+
+
+def sparse_tsdf_commit_workspace_bytes(n_new: int) -> int:
+    return int(lib().odb_sparse_tsdf_commit_workspace_bytes(int(n_new)))
+
+
+def sparse_tsdf_commit(desc: _capi.SparseTSDF, device, n_new: int, workspace):
+    """Gives the n_new marked blocks their ids (odb_sparse_tsdf_commit)."""
+    name = "sparse_tsdf_commit"
+    _check_workspace(name, workspace, sparse_tsdf_commit_workspace_bytes(n_new))
+    _call(name, {}, lib().odb_sparse_tsdf_commit, device, C.byref(desc), int(n_new), workspace.data_ptr())
+
+
+def sparse_tsdf_integrate(desc: _capi.SparseTSDF, device, trunc: float, depth, rgb, intrinsics, cam_to_world,
+                          frame0: int):
+    """Integrates depth fp32 [B,H,W] (rgb fp32 [B,3,H,W] exactly when the volume stores colour), frames numbered
+    frame0.., into the allocated blocks (odb_sparse_tsdf_integrate)."""
+    name = "sparse_tsdf_integrate"
+    b, h, w, (fx, fy, cx, cy), T = _sparse_frames(name, depth, rgb, desc.channels, intrinsics, cam_to_world)
+    if not (math.isfinite(trunc) and trunc > 0):
+        raise _capi.OdbError(f"{name}: trunc must be finite and > 0, got {trunc}")
+    _call(name, {"bytes": 4 * desc.channels * 512 * desc.blocks + 4 * b * h * w}, lib().odb_sparse_tsdf_integrate,
+          _same_device(depth, rgb), C.byref(desc), float(trunc), depth.data_ptr(), _ptr(rgb), b, h, w, fx, fy, cx, cy,
+          T.ctypes.data, int(frame0))
+
+
+def sparse_tsdf_raycast(desc: _capi.SparseTSDF, device, intrinsics, cam_to_world, step: float, out, rgb=None):
+    """out fp32 [H,W] (and rgb fp32 [3,H,W] for a colour volume) as tsdf_raycast / tsdf_raycast_color over the
+    allocated blocks' bounding box (odb_sparse_tsdf_raycast)."""
+    name = "sparse_tsdf_raycast"
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    T = check_poses(name, cam_to_world)
+    if T.shape[0] != 1:
+        raise _capi.OdbError(f"{name}: one pose, got {T.shape[0]}")
+    if not (math.isfinite(step) and desc.voxel / 64 <= step <= desc.voxel):
+        raise _capi.OdbError(f"{name}: step must lie in [voxel / 64, voxel], got {step}")
+    _need(out, torch.float32, "out")
+    if out.dim() != 2 or not out.is_contiguous():
+        raise _capi.OdbError(f"{name}: out must be a contiguous fp32 [H,W] tensor, got {tuple(out.shape)}")
+    h, w = out.shape
+    _check_planes(name, 1, h, w)
+    if rgb is not None:
+        if desc.channels != 5:
+            raise _capi.OdbError(f"{name}: rgb needs a volume that stores colour")
+        _need_shape(rgb, (3, h, w), torch.float32, "rgb")
+    _call(name, {"bytes": (16 if rgb is not None else 4) * h * w}, lib().odb_sparse_tsdf_raycast,
+          _same_device(out, rgb), C.byref(desc), T.ctypes.data, h, w, fx, fy, cx, cy, float(step), out.data_ptr(),
+          _ptr(rgb))
+
+
+def sparse_tsdf_mesh_workspace_bytes(blocks: int) -> int:
+    return int(lib().odb_sparse_tsdf_mesh_workspace_bytes(int(blocks)))
+
+
+def sparse_tsdf_mesh_count(desc: _capi.SparseTSDF, device, workspace, counts):
+    """counts int64 [2] = (vertices, faces) of the volume's mesh; fills workspace (odb_sparse_tsdf_mesh_count)."""
+    name = "sparse_tsdf_mesh_count"
+    _check_workspace(name, workspace, sparse_tsdf_mesh_workspace_bytes(desc.blocks))
+    _need_shape(counts, (2,), torch.int64, "counts")
+    _call(name, {"bytes": 10 * 512 * desc.blocks}, lib().odb_sparse_tsdf_mesh_count,
+          _same_device(workspace, counts), C.byref(desc), workspace.data_ptr(), counts.data_ptr())
+
+
+def sparse_tsdf_mesh_emit(desc: _capi.SparseTSDF, device, workspace, vertices, faces, colors):
+    """vertices fp32 [V,3], faces int32 [F,3] and colors fp32 [V,3] (exactly for a colour volume), sized from
+    sparse_tsdf_mesh_count on the same workspace (odb_sparse_tsdf_mesh_emit)."""
+    name = "sparse_tsdf_mesh_emit"
+    _check_workspace(name, workspace, sparse_tsdf_mesh_workspace_bytes(desc.blocks))
+    for t, dt, n in ((vertices, torch.float32, "vertices"), (faces, torch.int32, "faces")):
+        _need(t, dt, n)
+        if t.dim() != 2 or t.shape[1] != 3 or not t.is_contiguous():
+            raise _capi.OdbError(f"{name}: {n} must be a contiguous [N, 3] tensor, got {tuple(t.shape)}")
+    if (desc.channels == 5) != (colors is not None):
+        raise _capi.OdbError(f"{name}: colors is required exactly when the volume stores colour")
+    if colors is not None:
+        _need_shape(colors, tuple(vertices.shape), torch.float32, "colors")
+    _call(name, {"bytes": 10 * 512 * desc.blocks}, lib().odb_sparse_tsdf_mesh_emit,
+          _same_device(workspace, vertices, faces, colors), C.byref(desc), workspace.data_ptr(), vertices.data_ptr(),
+          faces.data_ptr(), _ptr(colors))
+
+
 # ---------------------------------------------------------------- camera tracking (csrc/track.cu)
 TRACK_MAX_ITERATIONS = 100
 

@@ -171,6 +171,266 @@ class TSDFVolume(_StepBuffers):
         return verts, faces, colors
 
 
+BLOCK_RANGE = _capi.SPARSE_TSDF_BLOCK_RANGE
+MAX_BLOCKS = _capi.SPARSE_TSDF_MAX_BLOCKS
+
+
+class SparseTSDFVolume(_StepBuffers):
+    """A TSDF volume without a box (csrc/sparse_volume.cu): the points X(p) = origin + voxel p, p in Z^3, stored in
+    blocks of 8^3 that are allocated where depth is seen, so a scene of any extent fuses without knowing its bounds.
+    A drop-in for TSDFVolume's integrate, raycast, extract_mesh and reset, with the same per-point arithmetic.
+
+    A pixel with finite depth d, 0 < d <= max_depth, allocates every block meeting the box of its ray segment from
+    z = d - trunc to z = d + trunc (max_depth, default 10 m and not tuned, limits allocation only).  Each block
+    records the frame that first allocated it, counting frames from construction or reset(), and its points update
+    only from that frame on, so the result does not depend on how frames are split into calls.  Block ids follow
+    (birth frame, block key).  Storage is 2 KB per block (5 KB with colour); at most MAX_BLOCKS = 2^21 blocks (4.3 GB,
+    10.7 GB with colour, 2^30 points), and block coordinates stay within +-BLOCK_RANGE = 2^20.  `integrate`
+    synchronises once to read the number of new blocks (again when its hash table has to grow); `raycast` neither
+    synchronises nor allocates beyond its output, so it can be captured in a CUDA graph.  Definitions: DESIGN.md §3
+    "Sparse TSDF volumes"; oracle/sparse_volume_oracle.py restates them in float64."""
+
+    _INITIAL_BLOCKS = 1024
+    _INITIAL_TABLE = 1 << 14
+
+    def __init__(self, voxel: float, trunc: Optional[float] = None, color: bool = False,
+                 origin: Sequence[float] = (0.0, 0.0, 0.0), max_depth: float = 10.0, device=None):
+        voxel = float(voxel)
+        self.origin = _value_error(ops.check_volume_grid, "SparseTSDFVolume", (2, 2, 2), origin, voxel)[1]
+        self.voxel = voxel
+        self.trunc = 3.0 * voxel if trunc is None else float(trunc)
+        if not (math.isfinite(self.trunc) and self.trunc > 0):
+            raise ValueError(f"trunc must be finite and > 0, got {trunc}")
+        self.max_depth = float(max_depth)
+        if not (math.isfinite(self.max_depth) and self.max_depth > 0):
+            raise ValueError(f"max_depth must be finite and > 0, got {max_depth}")
+        if not isinstance(color, bool):
+            raise ValueError(f"color must be a bool, got {color!r}")
+        if any(abs(math.floor(o / (8.0 * voxel))) >= BLOCK_RANGE for o in self.origin):
+            raise ValueError(f"SparseTSDFVolume: the origin {self.origin} lies {BLOCK_RANGE} or more blocks of "
+                             f"8 x {voxel} m from the world's zero")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.type != "cuda":
+            raise ValueError(f"SparseTSDFVolume lives on a CUDA device (no CPU path exists), got {self.device}")
+        self._channels = 5 if color else 2
+        self._bufs = {}
+        self._alloc_pool(self._INITIAL_BLOCKS)
+        self._alloc_table(self._INITIAL_TABLE)
+        self._bbox = torch.empty(6, dtype=torch.int32, device=self.device)
+        self.reset()
+
+    # -------------------------------------------------------------- state
+    def _alloc_pool(self, cap: int):
+        dev = self.device
+        self._data = torch.empty(cap, self._channels, 512, dtype=torch.float32, device=dev)
+        self._keys = torch.empty(cap, dtype=torch.int64, device=dev)
+        self._birth = torch.empty(cap, dtype=torch.int32, device=dev)
+        self._nbr = torch.empty(cap, 8, dtype=torch.int32, device=dev)
+
+    def _alloc_table(self, size: int):
+        dev = self.device
+        self._tkeys = torch.empty(size, dtype=torch.int64, device=dev)
+        self._tids = torch.empty(size, dtype=torch.int32, device=dev)
+        self._tbirth = torch.empty(size, dtype=torch.int32, device=dev)
+        self._scratch = torch.zeros(2 + size, dtype=torch.int32, device=dev)
+
+    def _desc(self, blocks: Optional[int] = None):
+        return ops.sparse_tsdf_desc(self._data, self._keys, self._birth, self._nbr, self._tkeys, self._tids,
+                                    self._tbirth, self._bbox, self._scratch, self.blocks if blocks is None else blocks,
+                                    self.origin, self.voxel)
+
+    def reset(self):
+        """Forgets every block and observation; frames count from 0 again."""
+        self.blocks = 0
+        self.frames = 0
+        big = torch.iinfo(torch.int32)
+        self._bbox.copy_(torch.tensor([big.max] * 3 + [big.min] * 3, dtype=torch.int32))
+        with torch.cuda.device(self.device):
+            ops.sparse_tsdf_rebuild(self._desc(), self.device)
+
+    @property
+    def block_keys(self) -> torch.Tensor:
+        """int64 [blocks]: the packed block coordinates in id order (include/omnidata_b200.h)."""
+        return self._keys[:self.blocks]
+
+    @property
+    def block_coords(self) -> torch.Tensor:
+        """int64 [blocks, 3]: the (x, y, z) block coordinates in id order; block b holds the points 8 b + (0..7)^3."""
+        k = self.block_keys
+        m = (1 << 21) - 1
+        return torch.stack([k & m, (k >> 21) & m, k >> 42], 1) - BLOCK_RANGE
+
+    @property
+    def block_birth(self) -> torch.Tensor:
+        """int32 [blocks]: the frame that allocated each block."""
+        return self._birth[:self.blocks]
+
+    @property
+    def tsdf(self) -> torch.Tensor:
+        """F fp32 [blocks, 8, 8, 8] (a view; index [id, k, j, i])."""
+        return self._data[:self.blocks, 0].view(-1, 8, 8, 8)
+
+    @property
+    def weight(self) -> torch.Tensor:
+        """W fp32 [blocks, 8, 8, 8] (a view)."""
+        return self._data[:self.blocks, 1].view(-1, 8, 8, 8)
+
+    @property
+    def color(self) -> Optional[torch.Tensor]:
+        """Mean RGB fp32 [blocks, 3, 8, 8, 8] (a view), or None without colour."""
+        return self._data[:self.blocks, 2:5].view(-1, 3, 8, 8, 8) if self._channels == 5 else None
+
+    def bounds(self):
+        """((x0, y0, z0), (x1, y1, z1)): the first and last point of the allocated blocks' bounding box in world
+        coordinates, or None when nothing is allocated.  Synchronises."""
+        if self.blocks == 0:
+            return None
+        b = self._bbox.tolist()
+        lo = tuple(o + self.voxel * (8 * b[a]) for a, o in enumerate(self.origin))
+        return lo, tuple(o + self.voxel * (8 * b[3 + a] + 7) for a, o in enumerate(self.origin))
+
+    @torch.no_grad()
+    def to_dense(self):
+        """(origin, dims, F, W, C) of the allocated blocks' bounding box as a dense grid: origin = the volume's origin +
+        voxel 8 bmin, dims = (nx, ny, nz), F, W fp32 [nz, ny, nx] and C fp32 [3, nz, ny, nx] or None, with F = W = 0
+        (and colour 0) at unallocated points.  For tests and interop; synchronises."""
+        if self.blocks == 0:
+            return self.origin, (0, 0, 0), None, None, None
+        b = self._bbox.tolist()
+        nb = [b[3 + a] - b[a] + 1 for a in range(3)]
+        ch = self._channels
+        dense = torch.zeros(ch, 8 * nb[2], 8 * nb[1], 8 * nb[0], dtype=torch.float32, device=self.device)
+        rel = self.block_coords - torch.tensor(b[:3], device=self.device)
+        view = dense.view(ch, nb[2], 8, nb[1], 8, nb[0], 8).permute(1, 3, 5, 0, 2, 4, 6)
+        view[rel[:, 2], rel[:, 1], rel[:, 0]] = self._data[:self.blocks].view(-1, ch, 8, 8, 8)
+        origin = tuple(o + self.voxel * (8 * b[a]) for a, o in enumerate(self.origin))
+        dims = (8 * nb[0], 8 * nb[1], 8 * nb[2])
+        return origin, dims, dense[0], dense[1], dense[2:5] if ch == 5 else None
+
+    def _check_centres(self, name, T):
+        """ValueError unless every camera centre lies, with max_depth + trunc around it, inside the block range."""
+        reach = (self.max_depth + self.trunc) / (8.0 * self.voxel)
+        for t in T.reshape(-1, 16)[:, [3, 7, 11]]:
+            for a in range(3):
+                b = (t[a] - self.origin[a]) / (8.0 * self.voxel)
+                if not abs(b) + reach < BLOCK_RANGE - 1:
+                    raise ValueError(f"{name}: a camera centre {tuple(t)} lies outside the sparse volume's block "
+                                     f"range (+-{BLOCK_RANGE} blocks of 8 x {self.voxel} m around the origin, less "
+                                     f"max_depth + trunc)")
+
+    # -------------------------------------------------------------- integrate / raycast / extract
+    @torch.no_grad()
+    def integrate(self, depth: torch.Tensor, intrinsics, cam_to_world, rgb: Optional[torch.Tensor] = None):
+        """TSDFVolume.integrate's arguments and arithmetic; allocates the frames' blocks first.  ValueError, with the
+        volume unchanged, when the blocks would exceed MAX_BLOCKS or a camera centre lies outside the block range."""
+        name = "SparseTSDFVolume.integrate"
+        if depth.dim() == 2:
+            depth = depth.unsqueeze(0)
+            rgb = None if rgb is None else rgb.unsqueeze(0)
+        if depth.dim() != 3:
+            raise ValueError(f"{name}: depth must be [B,H,W] or [H,W], got {tuple(depth.shape)}")
+        b, h, w = depth.shape
+        if depth.device != self.device or depth.dtype != torch.float32:
+            raise ValueError(f"{name}: depth must be fp32 on {self.device}, got {depth.dtype} on {depth.device}")
+        if (rgb is None) != (self._channels == 2):
+            raise ValueError(f"{name}: pass rgb exactly when the volume keeps colour (color={self._channels == 5})")
+        if rgb is not None and (tuple(rgb.shape) != (b, 3, h, w) or rgb.device != self.device or
+                                rgb.dtype != torch.float32):
+            raise ValueError(f"{name}: rgb must be fp32 [{b}, 3, {h}, {w}] on {self.device}, got {rgb.dtype} "
+                             f"{tuple(rgb.shape)} on {rgb.device}")
+        k = _value_error(ops.check_intrinsics, name, intrinsics)
+        T = _value_error(ops.check_poses, name, cam_to_world)
+        if T.shape[0] != b:
+            raise ValueError(f"{name}: {b} depth frames but {T.shape[0]} poses")
+        _value_error(ops._check_planes, name, b, h, w)
+        self._check_centres(name, T)
+        if self.frames + b > torch.iinfo(torch.int32).max:
+            raise ValueError(f"{name}: more than 2^31 - 1 frames since the last reset")
+        depth = depth.contiguous()
+        T = T.reshape(-1, 4, 4)
+        dev = self.device
+        with torch.cuda.device(dev):
+            while True:
+                ops.sparse_tsdf_mark(self._desc(), dev, self.trunc, self.max_depth, depth, k, T, self.frames)
+                n_new, full = self._scratch[:2].tolist()
+                if not full and self.blocks + n_new <= self._tkeys.numel() // 2:
+                    break
+                if self._tkeys.numel() >= 2 * MAX_BLOCKS:
+                    n_new = MAX_BLOCKS + 1 - self.blocks          # the limit is exceeded whatever the exact count
+                    break
+                self._alloc_table(2 * self._tkeys.numel())
+                ops.sparse_tsdf_rebuild(self._desc(), dev)
+            if self.blocks + n_new > MAX_BLOCKS:
+                ops.sparse_tsdf_rebuild(self._desc(), dev)      # forget the uncommitted marks
+                raise ValueError(f"{name}: the frames need more than MAX_BLOCKS = {MAX_BLOCKS} blocks of 8^3 points "
+                                 f"({self.blocks} allocated); use a coarser voxel or a smaller max_depth")
+            if self.blocks + n_new > self._data.shape[0]:
+                cap = self._data.shape[0]
+                while cap < self.blocks + n_new:
+                    cap *= 2
+                old = (self._data, self._keys, self._birth, self._nbr)
+                self._alloc_pool(min(cap, MAX_BLOCKS))
+                for new, o in zip((self._data, self._keys, self._birth, self._nbr), old):
+                    new[:self.blocks] = o[:self.blocks]
+            if n_new:
+                ws = self._buf("commit_ws", (-(-ops.sparse_tsdf_commit_workspace_bytes(n_new) // 8),), torch.float64,
+                               dev)
+                ops.sparse_tsdf_commit(self._desc(), dev, n_new, ws)
+                self.blocks += n_new
+            ops.sparse_tsdf_integrate(self._desc(), dev, self.trunc, depth, None if rgb is None else rgb.contiguous(),
+                                      k, T, self.frames)
+        self.frames += b
+
+    @torch.no_grad()
+    def raycast(self, intrinsics, cam_to_world, size: Tuple[int, int], step: Optional[float] = None,
+                color: bool = False):
+        """TSDFVolume.raycast over the allocated blocks' bounding box, with unallocated points unobserved; the march
+        skips unallocated blocks without changing a bit of the result."""
+        name = "SparseTSDFVolume.raycast"
+        if not isinstance(color, bool):
+            raise ValueError(f"{name}: color must be a bool, got {color!r}")
+        if color and self._channels != 5:
+            raise ValueError(f"{name}: color=True needs a volume that keeps colour (SparseTSDFVolume(..., color=True))")
+        k = _value_error(ops.check_intrinsics, name, intrinsics)
+        T = _value_error(ops.check_poses, name, cam_to_world)
+        if T.shape[0] != 1:
+            raise ValueError(f"{name}: one pose [4,4], got {T.shape[0]}")
+        self._check_centres(name, T)
+        try:
+            h, w = (int(v) for v in size)
+        except (TypeError, ValueError):
+            raise ValueError(f"{name}: size must be (H, W), got {size!r}") from None
+        _value_error(ops._check_planes, name, 1, h, w)
+        step = 0.5 * self.voxel if step is None else float(step)
+        if not (math.isfinite(step) and self.voxel / 64 <= step <= self.voxel):
+            raise ValueError(f"{name}: step must lie in [voxel / 64, voxel], got {step}")
+        out = torch.empty(h, w, dtype=torch.float32, device=self.device)
+        rgb = torch.empty(3, h, w, dtype=torch.float32, device=self.device) if color else None
+        with torch.cuda.device(self.device):
+            ops.sparse_tsdf_raycast(self._desc(), self.device, k, T.reshape(4, 4), step, out, rgb)
+        return (out, rgb) if color else out
+
+    @torch.no_grad()
+    def extract_mesh(self) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
+        """TSDFVolume.extract_mesh over the allocated points: vertex ids in (block id, point, direction) order, faces
+        in (block id, cell, tetrahedron, triangle) order.  Synchronises once to read the two counts."""
+        dev = self.device
+        ws = self._buf("mesh_ws", (-(-ops.sparse_tsdf_mesh_workspace_bytes(self.blocks) // 8),), torch.float64, dev)
+        counts = self._buf("mesh_counts", (2,), torch.int64, dev)
+        desc = self._desc()
+        with torch.cuda.device(dev):
+            ops.sparse_tsdf_mesh_count(desc, dev, ws, counts)
+            nv, nf = counts.tolist()
+            if nv >= 2 ** 31:
+                raise ValueError(f"SparseTSDFVolume.extract_mesh: {nv} vertices exceed int32 face indices")
+            verts = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+            faces = torch.empty(nf, 3, dtype=torch.int32, device=dev)
+            colors = None if self._channels == 2 else torch.empty(nv, 3, dtype=torch.float32, device=dev)
+            if nv:
+                ops.sparse_tsdf_mesh_emit(desc, dev, ws, verts, faces, colors)
+        return verts, faces, colors
+
+
 def write_ply(path, vertices, faces, colors=None):
     """Writes a binary little-endian PLY: float x, y, z per vertex (and uchar red, green, blue from colors in [0, 1],
     rounded), and the faces as uchar-counted int lists.  Arrays may be tensors on any device or numpy."""

@@ -4,15 +4,18 @@ already fused, track its camera when it has no pose, integrate it into a TSDF vo
 extracted mesh as a PLY:
 
     python reconstruct.py --img_path DIR [--pose_path DIR [--track]] --intrinsics FX,FY,CX,CY --voxel V
-                          --bounds X0,Y0,Z0,X1,Y1,Z1 --out mesh.ply [--pose_out DIR]
+                          [--bounds X0,Y0,Z0,X1,Y1,Z1] --out mesh.ply [--pose_out DIR]
                           [--checkpoint CKPT | --synthetic_weights] [--backbone ...] [--precision {fp32,bf16,fp8}]
                           [--mode {tiled,direct,guided}] [--tile 384 --overlap 64] [--guided_size HxW]
                           [--sparse_path DIR [--depth_scale 1000]] [--trunc T] [--color] [--photometric LAMBDA]
                           [--loop_closure [--place_recognition]]
 
 Frames are the images of --img_path (PNG / JPEG) in file-name order.  Each has a pose, the 4 x 4 camera-to-world matrix
-as text (ScanNet's pose/<stem>.txt), in --pose_path by file stem.  The intrinsics are in pixels of the images.  The grid
-covers --bounds with points every --voxel metres (write `--bounds=-1,...` when X0 is negative).
+as text (ScanNet's pose/<stem>.txt), in --pose_path by file stem.  The intrinsics are in pixels of the images.  With
+--bounds a dense grid (`TSDFVolume`) covers that box with points every --voxel metres (write `--bounds=-1,...` when X0
+is negative).  Without it the volume is sparse (`SparseTSDFVolume`, DESIGN.md §3 "Sparse TSDF volumes"): blocks of 8^3
+points every --voxel metres from the world's zero are allocated where frames see depth, so the scene needs no box and
+memory goes to observed surfaces only; the summary then reports `blocks` and the allocated `bounds` instead of `dims`.
 
 Per frame: the depth model predicts at the image's size (evaluate.py's predictor and preprocessing; `--mode`, `--tile`,
 `--overlap`, `--guided_size`).  `SparseDepthAligner(grid=(1, 1), robust=0.05)` then fits one scale and shift (Huber IRLS, so that
@@ -20,15 +23,15 @@ rays that pass through not-yet-observed space and hit a surface behind it do not
 frame's sparse depths when --sparse_path has a file for it (16-bit PNG / --depth_scale units per metre, or a `.npy` in
 metres; 0 is no measurement).  Otherwise it is the volume's own raycast at the frame's pose, so each frame is aligned
 to what is already fused.  Frame 0 must have sparse depths: they fix the scene's metric scale.  The aligned depth is
-integrated (`TSDFVolume`).  A frame whose fit fails (fewer than two target pixels, a flat prediction) is skipped and
+integrated.  A frame whose fit fails (fewer than two target pixels, a flat prediction) is skipped and
 named in the summary.
 
 Without --pose_path the cameras are tracked (`FrameTracker`, point-to-plane ICP against the volume).  This mode and
 --track are experimental: tracking against the fused model drifts (on the analytic test scene at 12.5 mm voxels, 13.5
 mm over 48 frames, and refined poses end a mean 6.8 mm from the truth when given 20 mm off; with --photometric 1e-2 on
 its textured version 3.4 mm and 1.45 mm; DESIGN.md §6).  Frame 0's pose is
-the identity, so --bounds are in frame 0's camera coordinates (x right, y down, z forward); frame 0 still needs sparse
-depths.  Every later frame starts from the last tracked pose: the volume is raycast there, one scale and shift is fitted
+the identity, so --bounds (when given) are in frame 0's camera coordinates (x right, y down, z forward); frame 0 still
+needs sparse depths.  Every later frame starts from the last tracked pose: the volume is raycast there, one scale and shift is fitted
 as above (to the frame's sparse depths when it has them, then the aligned metres are tracked with the pose alone;
 otherwise to that raycast, then the scale and shift are tracked with the pose), and the frame is integrated at the
 tracked pose.  A frame whose fit or tracking fails is skipped and named with its status; the next frame starts from the
@@ -57,7 +60,8 @@ tracking from that pose (raycast, fit, tracking against the model, integration).
 skipped with status "relocalise: failed".  So a covered lens, a fast turn or a cut in the video no longer loses the
 rest of it.  Relocalisation starts only from a failure: a frame that tracks to a wrong pose is not detected.
 
-Prints one JSON line: frames used and skipped, vertices, faces and seconds (with --loop_closure also the keyframes,
+Prints one JSON line: frames used and skipped, vertices, faces, the grid's dims (without --bounds the blocks and the
+allocated bounds) and seconds (with --loop_closure also the keyframes,
 the accepted loops as (frame i, frame j) index pairs of the used frames, and the number of re-fusions; with
 --place_recognition also the names of the relocalised frames).  Runs on cuda:0; there is no CPU path.
 """
@@ -114,8 +118,8 @@ def parse_args(argv=None):
     ap.add_argument("--intrinsics", required=True, type=evaluate._intrinsics, metavar="FX,FY,CX,CY",
                     help="camera intrinsics in pixels of the frames")
     ap.add_argument("--voxel", required=True, type=float, help="grid spacing in metres")
-    ap.add_argument("--bounds", required=True, type=_floats(6, "X0,Y0,Z0,X1,Y1,Z1"), metavar="X0,Y0,Z0,X1,Y1,Z1",
-                    help="world-space box the grid covers")
+    ap.add_argument("--bounds", default=None, type=_floats(6, "X0,Y0,Z0,X1,Y1,Z1"), metavar="X0,Y0,Z0,X1,Y1,Z1",
+                    help="world-space box a dense grid covers (default: a sparse volume, no box)")
     ap.add_argument("--out", required=True, help="output mesh (binary PLY)")
     w = ap.add_mutually_exclusive_group(required=True)
     w.add_argument("--checkpoint", default=None)
@@ -144,14 +148,17 @@ def parse_args(argv=None):
     args = ap.parse_args(argv)
     if not (math.isfinite(args.voxel) and args.voxel > 0):
         ap.error(f"--voxel must be finite and > 0, got {args.voxel}")
-    lo, hi = args.bounds[:3], args.bounds[3:]
-    if not all(h > l for l, h in zip(lo, hi)):
-        ap.error(f"--bounds must have X1 > X0, Y1 > Y0 and Z1 > Z0, got {args.bounds}")
-    args.origin = tuple(lo)
-    args.dims = tuple(int(math.floor((h - l) / args.voxel + 1e-9)) + 1 for l, h in zip(lo, hi))
-    if not all(2 <= d <= MAX_DIM for d in args.dims) or math.prod(args.dims) > MAX_POINTS:
-        ap.error(f"--bounds / --voxel give a {args.dims} grid; each dimension must lie in [2, {MAX_DIM}] and the "
-                 f"grid hold at most {MAX_POINTS} points")
+    if args.bounds is None:
+        args.origin, args.dims = (0.0, 0.0, 0.0), None
+    else:
+        lo, hi = args.bounds[:3], args.bounds[3:]
+        if not all(h > l for l, h in zip(lo, hi)):
+            ap.error(f"--bounds must have X1 > X0, Y1 > Y0 and Z1 > Z0, got {args.bounds}")
+        args.origin = tuple(lo)
+        args.dims = tuple(int(math.floor((h - l) / args.voxel + 1e-9)) + 1 for l, h in zip(lo, hi))
+        if not all(2 <= d <= MAX_DIM for d in args.dims) or math.prod(args.dims) > MAX_POINTS:
+            ap.error(f"--bounds / --voxel give a {args.dims} grid; each dimension must lie in [2, {MAX_DIM}] and the "
+                     f"grid hold at most {MAX_POINTS} points")
     if args.sparse_path is None:
         ap.error("--sparse_path is required: frame 0's sparse depths fix the scene's metric scale")
     if not (math.isfinite(args.depth_scale) and args.depth_scale > 0):
@@ -259,7 +266,7 @@ def reconstruct(args) -> dict:
     from omnidata_b200.loop import LoopClosure
     from omnidata_b200.sparse import STATUS, SparseDepthAligner
     from omnidata_b200.track import FrameTracker
-    from omnidata_b200.volume import TSDFVolume, write_ply
+    from omnidata_b200.volume import SparseTSDFVolume, TSDFVolume, write_ply
     t0 = time.perf_counter()
     device = torch.device("cuda:0")
     images = sorted(p for p in Path(args.img_path).iterdir() if p.suffix.lower() in evaluate.IMAGE_EXT)
@@ -271,7 +278,10 @@ def reconstruct(args) -> dict:
     model = evaluate.build_model("depth", args.backbone, args.checkpoint, args.synthetic_weights, args.precision,
                                  device)
     guided = (args.guided_size, 4, 1e-3) if args.mode == "guided" else None
-    volume = TSDFVolume(args.origin, args.voxel, args.dims, trunc=args.trunc, color=args.color, device=device)
+    if args.dims is None:
+        volume = SparseTSDFVolume(args.voxel, trunc=args.trunc, color=args.color, origin=args.origin, device=device)
+    else:
+        volume = TSDFVolume(args.origin, args.voxel, args.dims, trunc=args.trunc, color=args.color, device=device)
     aligner = SparseDepthAligner(grid=(1, 1), robust=ROBUST)
     tracking = args.track or not posed
     lam = 0.0 if args.photometric is None else args.photometric
@@ -325,8 +335,13 @@ def reconstruct(args) -> dict:
     vertices, faces, colors = volume.extract_mesh()
     write_ply(args.out, vertices, faces, colors)
     result = {"frames": len(images), "frames_used": len(used), "frames_skipped": skipped,
-              "vertices": int(vertices.shape[0]), "faces": int(faces.shape[0]), "dims": list(args.dims),
-              "voxel": args.voxel, "out": str(args.out), "seconds": round(time.perf_counter() - t0, 3)}
+              "vertices": int(vertices.shape[0]), "faces": int(faces.shape[0])}
+    if args.dims is None:
+        bounds = volume.bounds()
+        result.update(blocks=volume.blocks, bounds=None if bounds is None else [list(bounds[0]), list(bounds[1])])
+    else:
+        result["dims"] = list(args.dims)
+    result.update(voxel=args.voxel, out=str(args.out), seconds=round(time.perf_counter() - t0, 3))
     if loop is not None:
         result.update(keyframes=len(loop.keyframes), loops=[list(pair) for pair in loop.loops],
                       refusions=loop.refusions)
