@@ -1095,6 +1095,77 @@ int odb_guided_apply(const float* image, const float* coef, int32_t b, int32_t c
                      int32_t W, const int32_t* bounds_h, const float* weights_h, int32_t ksize_h,
                      const int32_t* bounds_v, const float* weights_v, int32_t ksize_v, float* out, void* stream);
 
+/* ---- Mesh metrics (omnidata_b200/mesh.py, omnidata_b200/metrics.py MeshMetrics) -----------------------------------
+ *
+ * No reference counterpart.  Measures a reconstructed mesh against a ground-truth mesh: both are sampled the same way,
+ * optionally culled to what the cameras saw, and compared by exact nearest neighbours.  Definitions in DESIGN.md §3
+ * "Mesh metrics"; oracle/mesh_oracle.py restates them in float64.  Point sets are fp32 [n][3] with n <=
+ * ODB_MESH_MAX_POINTS; every fp64 step below is one round-to-nearest operation in the stated order.
+ *
+ * odb_mesh_sample_count + odb_mesh_sample_emit: vertices fp32 [nv][3], faces int32 [nf][3], density rho finite > 0
+ * (points per m^2).  Draws u(t, j) = (x >> 11) 2^-53 with x = splitmix64(splitmix64(key ^ t) ^ j), key =
+ * splitmix64(splitmix64(seed) ^ rng_stream).  Face t = (a, b, c): A = 0.5 |(b - a) x (c - a)|, n_t = floor(A rho +
+ * u(t, 0)).  Sample k of face t: r1 = u(t, 2k + 1), r2 = u(t, 2k + 2), s = sqrt(r1), p = ((1 - s) a + (s (1 - r2)) b)
+ * + (s r2) c, rounded to fp32; samples are ordered by (face, k).  count: writes info int64 [2] = (total, flags) on the
+ * device; flags bit 0: a face index outside [0, nv), bit 1: a non-finite vertex used by a face (such faces count 0);
+ * workspace odb_mesh_sample_workspace_bytes(nf), 8-byte aligned.  emit: after count on the same workspace, out fp32
+ * [total][3]; the caller reads info and refuses flagged meshes and totals above ODB_MESH_MAX_POINTS before emitting.
+ *
+ * odb_nn_bounds + odb_nn_build + odb_nn_query: for each query q of query fp32 [m][3], distance fp64 [m] = sqrt(d2) and
+ * index int32 [m] = the smallest reference index at the minimal d2 = (dx dx + dy dy) + dz dz, dx = (double) q.x -
+ * (double) r.x; +inf and -1 when n_ref = 0.  bounds: box int32 [7] = the reference set's order-preserving min keys
+ * (x, y, z), max keys, and flags (bit 0: a non-finite reference coordinate, bit 1: a non-finite query coordinate); a
+ * float x has the key bits(x) when bits(x) >= 0 as int32, else bits(x) ^ 0x7FFFFFFF.  grid: a HOST array of 7 doubles
+ * (lo x, y, z, hi x, y, z, h): finite, lo <= hi, h > 0, n_a = floor((hi_a - lo_a) / h) + 1 cells per axis and at most
+ * ODB_NN_MAX_CELLS cells.  A point's cell along axis a is clamp(floor((p_a - lo_a) / h), 0, n_a - 1), for reference
+ * points and queries alike.  build: workspace odb_nn_workspace_bytes(n_ref, grid), 16-byte aligned; query: after build
+ * on the same workspace and grid.  The cell size changes the time, never an output bit.
+ *
+ * odb_frustum_mask: mask uint8 [n] = 1 when one of the frames sees the point: cam_to_world a DEVICE array fp64
+ * [frames][16] of row-major camera-to-world matrices (checked by the caller), Xc = R^T (X - t), 0 < z <= max_depth and
+ * the pixel (floor(fx x / z + cx + 0.5), floor(fy y / z + cy + 0.5)) in the h x w image (odb_tsdf_integrate's
+ * projection).  odb_compact_points: out fp32 [count][3] = the points with mask != 0 in order, count int64 [1] on the
+ * device; workspace odb_compact_workspace_bytes(n), 8-byte aligned.
+ *
+ * odb_mesh_metrics_update: one scene from dist_pred fp64 [n_pred] (prediction samples to the ground truth) and dist_gt
+ * fp64 [n_gt] (ground truth to the prediction), thresholds a HOST array of 1..ODB_MESH_MAX_THRESHOLDS finite values >
+ * 0.  Sums over fixed slabs of 4096 distances, combined in a fixed order; counts of d < t exact.  record fp64
+ * [ODB_MESH_RECORD] = (n_pred, n_gt, accuracy, completion, chamfer, then (precision, recall, F) per threshold), NaN
+ * where undefined; accuracy = mean dist_pred, completion = mean dist_gt, chamfer = (accuracy + completion) / 2,
+ * precision = #(dist_pred < t) / n_pred (0 when n_pred = 0), recall = #(dist_gt < t) / n_gt, F = (2 P R) / (P + R), 0
+ * when P + R = 0.  The state: state_counts int64 [7] += (1, n_gt = 0, n_pred = 0 < n_gt, n_pred, n_gt, pred_culled,
+ * gt_culled); with n_gt > 0, state_sums fp64 [3 + 3 ODB_MESH_MAX_THRESHOLDS] += (P, R, F) per threshold at [3 + 3k..],
+ * and with n_pred > 0 also (accuracy, completion, chamfer) at [0..2].  Workspace
+ * odb_mesh_metrics_workspace_bytes(n_pred, n_gt), 8-byte aligned.
+ *
+ * No floating-point atomics; integer atomics only in the box, the grid's counts, the scatter (no output depends on
+ * the order within a cell) and the flags.  Every output is bit-reproducible. */
+#define ODB_MESH_MAX_POINTS 268435456
+#define ODB_NN_MAX_CELLS 67108864
+#define ODB_MESH_MAX_THRESHOLDS 4
+#define ODB_MESH_RECORD 17
+int64_t odb_mesh_sample_workspace_bytes(int64_t faces);
+int odb_mesh_sample_count(const float* vertices, int64_t nv, const int32_t* faces, int64_t nf, double density,
+                          int64_t seed, int64_t rng_stream, void* workspace, int64_t* info, void* stream);
+int odb_mesh_sample_emit(const float* vertices, int64_t nv, const int32_t* faces, int64_t nf, int64_t seed,
+                         int64_t rng_stream, const void* workspace, int64_t total, float* out, void* stream);
+int odb_nn_bounds(const float* reference, int64_t n_ref, const float* query, int64_t n_query, int32_t* box,
+                  void* stream);
+int64_t odb_nn_workspace_bytes(int64_t n_ref, const double* grid);
+int odb_nn_build(const float* reference, int64_t n_ref, const double* grid, void* workspace, void* stream);
+int odb_nn_query(const float* query, int64_t n_query, int64_t n_ref, const double* grid, const void* workspace,
+                 double* distance, int32_t* index, void* stream);
+int odb_frustum_mask(const float* points, int64_t n, const double* cam_to_world, int32_t frames, int32_t h, int32_t w,
+                     double fx, double fy, double cx, double cy, double max_depth, uint8_t* mask, void* stream);
+int64_t odb_compact_workspace_bytes(int64_t n);
+int odb_compact_points(const float* points, const uint8_t* mask, int64_t n, void* workspace, float* out,
+                       int64_t* count, void* stream);
+int64_t odb_mesh_metrics_workspace_bytes(int64_t n_pred, int64_t n_gt);
+int odb_mesh_metrics_update(const double* dist_pred, int64_t n_pred, const double* dist_gt, int64_t n_gt,
+                            const double* thresholds, int32_t n_thresholds, int64_t pred_culled, int64_t gt_culled,
+                            void* workspace, double* record, double* state_sums, int64_t* state_counts,
+                            void* stream);
+
 /* Introspection (no GPU needed). */
 int odb_abi_version(void);
 const char* odb_last_error(void);

@@ -39,6 +39,10 @@ FERN_GRID = (60, 80)                            # ODB_FERN_GRID_ROWS, ODB_FERN_G
 FERN_MAX_FERNS = 4096                           # ODB_FERN_MAX_FERNS
 FERN_MAX_K = 1024                               # ODB_FERN_MAX_K
 FERN_MAX_ENTRIES = 1 << 28                      # ODB_FERN_MAX_ENTRIES
+MESH_MAX_POINTS = 1 << 28                       # ODB_MESH_MAX_POINTS
+NN_MAX_CELLS = 1 << 26                          # ODB_NN_MAX_CELLS
+MESH_MAX_THRESHOLDS = 4                         # ODB_MESH_MAX_THRESHOLDS
+MESH_RECORD = 17                                # ODB_MESH_RECORD
 
 
 class OdbError(RuntimeError):
@@ -293,6 +297,22 @@ _SIGNATURES = {
     "odb_fern_encode": (C.c_int, [C.c_int32] * 3 + [C.c_void_p] * 2 + [C.c_int32] + [C.c_void_p] * 5),
     "odb_fern_query_workspace_bytes": (C.c_int64, [C.c_int32]),
     "odb_fern_query": (C.c_int, [C.c_int32] * 2 + [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 4),
+    "odb_mesh_sample_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "odb_mesh_sample_count": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_double, C.c_int64,
+                                        C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "odb_mesh_sample_emit": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p] + [C.c_int64] * 3 + [C.c_void_p, C.c_int64,
+                                                                                              C.c_void_p, C.c_void_p]),
+    "odb_nn_bounds": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "odb_nn_workspace_bytes": (C.c_int64, [C.c_int64, C.c_void_p]),
+    "odb_nn_build": (C.c_int, [C.c_void_p, C.c_int64] + [C.c_void_p] * 3),
+    "odb_nn_query": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 5),
+    "odb_frustum_mask": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p] + [C.c_int32] * 3 + [C.c_double] * 5 +
+                         [C.c_void_p] * 2),
+    "odb_compact_workspace_bytes": (C.c_int64, [C.c_int64]),
+    "odb_compact_points": (C.c_int, [C.c_void_p] * 2 + [C.c_int64] + [C.c_void_p] * 4),
+    "odb_mesh_metrics_workspace_bytes": (C.c_int64, [C.c_int64] * 2),
+    "odb_mesh_metrics_update": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
+                                          C.c_int64, C.c_int64] + [C.c_void_p] * 5),
     "odb_abi_version": (C.c_int, []),
     "odb_last_error": (C.c_char_p, []),
     "odb_launch_count": (C.c_int64, []),

@@ -18,7 +18,7 @@ LIB_PATH = LIB_DIR / "libomnidata_b200.so"
 SOURCES = ["api.cu", "conv_gemm.cu", "ops.cu", "attention_tc.cu", "fp32_path.cu", "bwd_ops.cu", "bgemm.cu", "bgemm_tc.cu", "loss.cu",
            "imageproc.cu", "optim.cu", "refocus.cu", "tiled.cu", "metrics.cu",
            "ensemble.cu", "guided.cu", "boundary.cu", "sparse.cu", "fusion.cu", "volume.cu", "track.cu",
-           "posegraph.cu", "places.cu", "sparse_volume.cu"]
+           "posegraph.cu", "places.cu", "sparse_volume.cu", "mesh_metrics.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

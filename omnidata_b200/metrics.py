@@ -16,6 +16,10 @@
   in the ground truth) with a masked Canny detector; accuracy is the mean distance in pixels from predicted edges to
   true ones (those within max_dist), completeness the mean distance from true edges to predicted ones.  Csrc:
   boundary.cu.
+- MeshMetrics: reconstructed meshes against ground-truth meshes, both sampled alike: accuracy (mean distance from the
+  prediction to the truth), completion (the reverse), Chamfer-L1, and precision, recall and F-score at distance
+  thresholds, optionally culled to what the cameras saw.  Csrc: mesh_metrics.cu.  Unlike the others its `update`
+  synchronises (sample counts, bounding boxes).
 
 Definitions: DESIGN.md §3 "Evaluation metrics" and include/omnidata_b200.h; oracle/metrics_oracle.py restates them in
 float64.  The state lives in fixed device tensors.  `update` neither synchronises the host nor allocates after its first
@@ -239,4 +243,85 @@ class BoundaryMetrics(_Metrics):
         acc, comp = st["sums"].tolist()
         out = {"dbe_acc": acc / n if n else math.nan, "dbe_comp": comp / n if n else math.nan}
         out.update(zip(BOUNDARY_COUNTS, counts))
+        return out
+
+
+MESH_COUNTS = ("scenes", "no_gt", "empty_pred", "pred_points", "gt_points", "pred_culled", "gt_culled")
+
+
+class MeshMetrics(_Metrics):
+    """Accuracy, completion, Chamfer-L1, precision, recall and F-score of reconstructed meshes against ground-truth
+    meshes (DESIGN.md §3 "Mesh metrics"; csrc/mesh_metrics.cu).  Both meshes are sampled alike (`mesh.sample_surface`
+    at density points per m^2, streams 0 and 1 of seed), so vertex density does not bias the result; thresholds (1 to
+    4, metres) are the distances at which a point counts as matched (5 cm is the usual indoor value; density 1e4,
+    about 1 cm spacing, is not tuned)."""
+
+    _STATE = {"sums": ((3 + 3 * _capi.MESH_MAX_THRESHOLDS,), torch.float64), "counts": ((7,), torch.int64)}
+
+    def __init__(self, thresholds=(0.05,), density: float = 1e4, seed: int = 0):
+        super().__init__()
+        try:
+            self.thresholds = tuple(float(t) for t in ops.check_thresholds("MeshMetrics", thresholds))
+        except _capi.OdbError as e:
+            raise ValueError(str(e)) from None
+        density = float(density)
+        if not (math.isfinite(density) and density > 0):
+            raise ValueError(f"MeshMetrics: density must be finite and > 0, got {density}")
+        if not (isinstance(seed, int) and 0 <= seed < 2 ** 63):
+            raise ValueError(f"MeshMetrics: seed must be an integer in [0, 2^63), got {seed!r}")
+        self.density, self.seed = density, seed
+
+    @_capi.on_tensor_device
+    @torch.no_grad()
+    def update(self, pred_vertices: torch.Tensor, pred_faces: torch.Tensor, gt_vertices: torch.Tensor,
+               gt_faces: torch.Tensor, views=None, return_distances: bool = False):
+        """Adds one scene: the predicted and the true mesh (vertices fp32 [V,3], faces int32 [F,3], on one device).
+        views = (intrinsics, (h, w), poses [n,4,4] camera-to-world, host or device) culls both sample sets to what
+        those cameras see (`mesh.frustum_mask`, max_depth 10 m, occlusion not modelled).  Returns the scene's record
+        fp64 [1, MESH_RECORD] (include/omnidata_b200.h odb_mesh_metrics_update); with return_distances also a dict of
+        the culled samples and their distances to the other mesh: pred_points fp32 [P,3], pred_distance fp64 [P],
+        gt_points, gt_distance.  Synchronises: to read the sample counts, the kept counts and the bounding boxes."""
+        from . import mesh
+        dev = pred_vertices.device
+        st = self._state_on(dev)
+        P = mesh.sample_surface(pred_vertices, pred_faces, self.density, self.seed, 0)
+        G = mesh.sample_surface(gt_vertices, gt_faces, self.density, self.seed, 1)
+        culled = [0, 0]
+        if views is not None:
+            intrinsics, size, poses = views
+            T = mesh.device_poses("MeshMetrics.update", poses, dev)
+            kept = []
+            for q, X in enumerate((P, G)):
+                m = torch.empty(X.shape[0], dtype=torch.uint8, device=dev)
+                mesh._value_error(ops.frustum_mask, X, intrinsics, size, T, 10.0, m)
+                Y = mesh.compact(X, m)
+                culled[q] = X.shape[0] - Y.shape[0]
+                kept.append(Y)
+            P, G = kept
+        dp, _ = mesh.nearest(P, G)
+        dg, _ = mesh.nearest(G, P)
+        ws = self._buf("workspace", (max(1, ops.mesh_metrics_workspace_bytes(P.shape[0], G.shape[0]) // 8),),
+                       torch.float64, dev)
+        rec = torch.empty(_capi.MESH_RECORD, dtype=torch.float64, device=dev)
+        ops.mesh_metrics_update(dp, dg, self.thresholds, culled[0], culled[1], ws, rec, st["sums"], st["counts"])
+        rec = rec.unsqueeze(0)
+        if return_distances:
+            return rec, {"pred_points": P, "pred_distance": dp, "gt_points": G, "gt_distance": dg}
+        return rec
+
+    def compute(self) -> dict:
+        """The means over scenes of accuracy, completion and chamfer (metres; over the scenes with both samples),
+        and of precision@t, recall@t and fscore@t per threshold t (over the scenes with ground-truth samples; an
+        empty prediction scores 0); NaN before any such scene.  Counts: scenes, no_gt (no ground-truth samples:
+        excluded), empty_pred (no predicted samples), pred_points, gt_points (kept samples), pred_culled, gt_culled."""
+        st = self._host_state()
+        counts = [int(c) for c in st["counts"].tolist()]
+        sums = st["sums"].tolist()
+        n_prf = counts[0] - counts[1]
+        n_dist = n_prf - counts[2]
+        out = {k: (s / n_dist if n_dist else math.nan) for k, s in zip(("accuracy", "completion", "chamfer"), sums)}
+        for q, t in enumerate(self.thresholds):
+            for j, k in enumerate(("precision", "recall", "fscore")):
+                out[f"{k}@{t:g}"] = sums[3 + 3 * q + j] / n_prf if n_prf else math.nan
+        out.update(zip(MESH_COUNTS, counts))
         return out

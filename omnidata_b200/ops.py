@@ -1647,3 +1647,193 @@ def fern_query(db_codes, code, limit: int, k: int, out_index, out_distance, work
     _call(name, {"bytes": int(limit) * f}, lib().odb_fern_query,
           _same_device(db_codes, code, out_index, out_distance, workspace), n_db, f, db_codes.data_ptr(),
           code.data_ptr(), int(limit), int(k), out_index.data_ptr(), out_distance.data_ptr(), workspace.data_ptr())
+
+
+# ---------------------------------------------------------------- mesh metrics (csrc/mesh_metrics.cu)
+def check_points(name: str, t, what: str = "points") -> int:
+    """The point count of a contiguous fp32 [N,3] CUDA tensor; OdbError otherwise or beyond MESH_MAX_POINTS."""
+    _need(t, torch.float32, what)
+    if t.dim() != 2 or t.shape[1] != 3 or not t.is_contiguous():
+        raise _capi.OdbError(f"{name}: {what} must be a contiguous fp32 [N,3] tensor, got {tuple(t.shape)}")
+    if t.shape[0] > _capi.MESH_MAX_POINTS:
+        raise _capi.OdbError(f"{name}: {t.shape[0]} {what}, at most {_capi.MESH_MAX_POINTS}")
+    return int(t.shape[0])
+
+
+def check_mesh(name: str, vertices, faces) -> Tuple[int, int]:
+    """(V, F) of vertices fp32 [V,3] and faces int32 [F,3] (contiguous, on one CUDA device)."""
+    _need(vertices, torch.float32, "vertices")
+    _need(faces, torch.int32, "faces")
+    for t, n in ((vertices, "vertices"), (faces, "faces")):
+        if t.dim() != 2 or t.shape[1] != 3 or not t.is_contiguous():
+            raise _capi.OdbError(f"{name}: {n} must be a contiguous [N,3] tensor, got {tuple(t.shape)}")
+        if t.shape[0] >= 2 ** 31:
+            raise _capi.OdbError(f"{name}: {t.shape[0]} {n}, at most 2^31 - 1")
+    _same_device(vertices, faces)
+    return int(vertices.shape[0]), int(faces.shape[0])
+
+
+def _check_seed(name: str, seed: int, stream: int):
+    if not (isinstance(seed, numbers.Integral) and isinstance(stream, numbers.Integral) and 0 <= seed < 2 ** 63 and
+            0 <= stream < 2 ** 63):
+        raise _capi.OdbError(f"{name}: seed and stream must be integers in [0, 2^63), got {seed!r}, {stream!r}")
+
+
+def mesh_sample_workspace_bytes(nf: int) -> int:
+    return int(lib().odb_mesh_sample_workspace_bytes(nf))
+
+
+def mesh_sample_count(vertices, faces, density: float, seed: int, stream: int, workspace, info):
+    """info int64 [2] = (samples, flags) of the surface sampling of the mesh; fills workspace for mesh_sample_emit
+    (include/omnidata_b200.h odb_mesh_sample_count)."""
+    name = "mesh_sample_count"
+    nv, nf = check_mesh(name, vertices, faces)
+    if not (math.isfinite(density) and density > 0):
+        raise _capi.OdbError(f"{name}: density must be finite and > 0, got {density}")
+    _check_seed(name, seed, stream)
+    _check_workspace(name, workspace, mesh_sample_workspace_bytes(nf))
+    _need_shape(info, (2,), torch.int64, "info")
+    _call(name, {"bytes": 48 * nf}, lib().odb_mesh_sample_count, _same_device(vertices, faces, workspace, info),
+          vertices.data_ptr(), nv, faces.data_ptr(), nf, float(density), int(seed), int(stream), workspace.data_ptr(),
+          info.data_ptr())
+
+
+def mesh_sample_emit(vertices, faces, seed: int, stream: int, workspace, out):
+    """out fp32 [N,3] = the samples counted by mesh_sample_count on the same workspace (N its total)."""
+    name = "mesh_sample_emit"
+    nv, nf = check_mesh(name, vertices, faces)
+    _check_seed(name, seed, stream)
+    _check_workspace(name, workspace, mesh_sample_workspace_bytes(nf))
+    n = check_points(name, out, "out")
+    _call(name, {"bytes": 12 * n}, lib().odb_mesh_sample_emit, _same_device(vertices, faces, workspace, out),
+          vertices.data_ptr(), nv, faces.data_ptr(), nf, int(seed), int(stream), workspace.data_ptr(), n,
+          out.data_ptr())
+
+
+def nn_bounds(reference, query, box):
+    """box int32 [7] = the reference set's order-preserving min / max keys and the non-finite flags
+    (include/omnidata_b200.h odb_nn_bounds)."""
+    name = "nn_bounds"
+    nr, nq = check_points(name, reference, "reference"), check_points(name, query, "query")
+    _need_shape(box, (7,), torch.int32, "box")
+    _call(name, {"bytes": 12 * (nr + nq)}, lib().odb_nn_bounds, _same_device(reference, query, box),
+          reference.data_ptr(), nr, query.data_ptr(), nq, box.data_ptr())
+
+
+def nn_grid_cells(grid) -> int:
+    """The number of cells of the grid (lo[3], hi[3], h): prod over axes of floor((hi - lo) / h) + 1."""
+    return math.prod(int(math.floor((grid[3 + a] - grid[a]) / grid[6])) + 1 for a in range(3))
+
+
+def _nn_grid(name: str, grid) -> np.ndarray:
+    g = np.ascontiguousarray(grid, dtype=np.float64)
+    if g.shape != (7,) or not np.isfinite(g).all() or not (g[6] > 0) or not (g[:3] <= g[3:6]).all() or \
+            nn_grid_cells(g) > _capi.NN_MAX_CELLS:
+        raise _capi.OdbError(f"{name}: grid must be finite (lo[3], hi[3], h) with lo <= hi, h > 0 and at most "
+                             f"{_capi.NN_MAX_CELLS} cells, got {grid!r}")
+    return g
+
+
+def nn_workspace_bytes(n_ref: int, grid) -> int:
+    g = _nn_grid("nn_workspace_bytes", grid)
+    return int(lib().odb_nn_workspace_bytes(n_ref, g.ctypes.data))
+
+
+def nn_build(reference, grid, workspace):
+    """Sorts reference fp32 [N,3] into the uniform grid (lo[3], hi[3], h) (host) in workspace
+    (include/omnidata_b200.h odb_nn_build)."""
+    name = "nn_build"
+    nr = check_points(name, reference, "reference")
+    g = _nn_grid(name, grid)
+    _check_workspace(name, workspace, nn_workspace_bytes(nr, g))
+    _call(name, {"bytes": 40 * nr}, lib().odb_nn_build, _same_device(reference, workspace), reference.data_ptr(), nr,
+          g.ctypes.data, workspace.data_ptr())
+
+
+def nn_query(query, n_ref: int, grid, workspace, distance, index):
+    """distance fp64 [M] and index int32 [M] of each query's nearest reference point, from nn_build's workspace and
+    grid (include/omnidata_b200.h odb_nn_query); n_ref = 0 needs neither."""
+    name = "nn_query"
+    nq = check_points(name, query, "query")
+    g = None
+    if n_ref:
+        g = _nn_grid(name, grid)
+        _check_workspace(name, workspace, nn_workspace_bytes(n_ref, g))
+    _need_shape(distance, (nq,), torch.float64, "distance")
+    _need_shape(index, (nq,), torch.int32, "index")
+    _call(name, {"bytes": 24 * nq}, lib().odb_nn_query, _same_device(query, workspace, distance, index),
+          query.data_ptr(), nq, int(n_ref), None if g is None else g.ctypes.data, _ptr(workspace),
+          distance.data_ptr(), index.data_ptr())
+
+
+def frustum_mask(points, intrinsics, size: Tuple[int, int], poses, max_depth: float, mask):
+    """mask uint8 [N] = 1 where one of the cameras poses (a DEVICE fp64 [n,16] tensor of checked camera-to-world
+    matrices, see check_poses) sees the point (include/omnidata_b200.h odb_frustum_mask)."""
+    name = "frustum_mask"
+    n = check_points(name, points)
+    fx, fy, cx, cy = check_intrinsics(name, intrinsics)
+    h, w = (int(v) for v in size)
+    _check_planes(name, 1, h, w)
+    if not (math.isfinite(max_depth) and max_depth > 0):
+        raise _capi.OdbError(f"{name}: max_depth must be finite and > 0, got {max_depth}")
+    _need(poses, torch.float64, "poses")
+    if poses.dim() != 2 or poses.shape[1] != 16 or poses.shape[0] < 1 or poses.shape[0] >= 2 ** 31 or \
+            not poses.is_contiguous():
+        raise _capi.OdbError(f"{name}: poses must be a contiguous fp64 [n,16] tensor, got {tuple(poses.shape)}")
+    _need_shape(mask, (n,), torch.uint8, "mask")
+    _call(name, {"bytes": 13 * n}, lib().odb_frustum_mask, _same_device(points, poses, mask), points.data_ptr(), n,
+          poses.data_ptr(), int(poses.shape[0]), h, w, fx, fy, cx, cy, float(max_depth), mask.data_ptr())
+
+
+def compact_workspace_bytes(n: int) -> int:
+    return int(lib().odb_compact_workspace_bytes(n))
+
+
+def compact_points(points, mask, workspace, out, count):
+    """out fp32 [>= K,3] starts with the K points of points fp32 [N,3] where mask uint8 [N] != 0, in order; count int64
+    [1] = K on the device (include/omnidata_b200.h odb_compact_points)."""
+    name = "compact_points"
+    n = check_points(name, points)
+    _need_shape(mask, (n,), torch.uint8, "mask")
+    _check_workspace(name, workspace, compact_workspace_bytes(n))
+    _need(out, torch.float32, "out")
+    if out.dim() != 2 or out.shape[1] != 3 or out.shape[0] < n or not out.is_contiguous():
+        raise _capi.OdbError(f"{name}: out must be a contiguous fp32 [>= {n}, 3] tensor, got {tuple(out.shape)}")
+    _need_shape(count, (1,), torch.int64, "count")
+    _call(name, {"bytes": 29 * n}, lib().odb_compact_points, _same_device(points, mask, workspace, out, count),
+          points.data_ptr(), mask.data_ptr(), n, workspace.data_ptr(), out.data_ptr(), count.data_ptr())
+
+
+def check_thresholds(name: str, thresholds) -> np.ndarray:
+    try:
+        t = np.asarray([float(v) for v in thresholds], dtype=np.float64)
+    except (TypeError, ValueError):
+        raise _capi.OdbError(f"{name}: thresholds must be a sequence of numbers, got {thresholds!r}") from None
+    if not 1 <= len(t) <= _capi.MESH_MAX_THRESHOLDS or not (np.isfinite(t) & (t > 0)).all():
+        raise _capi.OdbError(f"{name}: 1 to {_capi.MESH_MAX_THRESHOLDS} finite thresholds > 0, got {thresholds!r}")
+    return t
+
+
+def mesh_metrics_workspace_bytes(n_pred: int, n_gt: int) -> int:
+    return int(lib().odb_mesh_metrics_workspace_bytes(n_pred, n_gt))
+
+
+def mesh_metrics_update(dist_pred, dist_gt, thresholds, pred_culled: int, gt_culled: int, workspace, record, sums,
+                        counts):
+    """Folds one scene (dist_pred fp64 [N_p], dist_gt fp64 [N_g]) into sums fp64 [15] and counts int64 [7]; record
+    fp64 [MESH_RECORD] (include/omnidata_b200.h odb_mesh_metrics_update)."""
+    name = "mesh_metrics_update"
+    t = check_thresholds(name, thresholds)
+    for d, n in ((dist_pred, "dist_pred"), (dist_gt, "dist_gt")):
+        _need(d, torch.float64, n)
+        if d.dim() != 1 or not d.is_contiguous():
+            raise _capi.OdbError(f"{name}: {n} must be a contiguous fp64 [N] tensor, got {tuple(d.shape)}")
+    n_p, n_g = int(dist_pred.shape[0]), int(dist_gt.shape[0])
+    _check_workspace(name, workspace, mesh_metrics_workspace_bytes(n_p, n_g))
+    _need_shape(record, (_capi.MESH_RECORD,), torch.float64, "record")
+    _need_shape(sums, (3 + 3 * _capi.MESH_MAX_THRESHOLDS,), torch.float64, "sums")
+    _need_shape(counts, (7,), torch.int64, "counts")
+    _call(name, {"bytes": 8 * (n_p + n_g)}, lib().odb_mesh_metrics_update,
+          _same_device(dist_pred, dist_gt, workspace, record, sums, counts), dist_pred.data_ptr(), n_p,
+          dist_gt.data_ptr(), n_g, t.ctypes.data, len(t), int(pred_culled), int(gt_culled), workspace.data_ptr(),
+          record.data_ptr(), sums.data_ptr(), counts.data_ptr())

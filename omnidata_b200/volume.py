@@ -464,3 +464,170 @@ def write_ply(path, vertices, faces, colors=None):
         fh.write(("\n".join(header) + "\n").encode("ascii"))
         fh.write(vrec.tobytes())
         fh.write(frec.tobytes())
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
+              "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4",
+              "float32": "f4", "double": "f8", "float64": "f8"}
+
+
+def read_ply(path):
+    """Reads a triangle or polygon mesh PLY (binary little-endian or ascii): (vertices fp32 [V,3], faces int32 [F,3],
+    colors fp32 [V,3] in [0, 1] or None) as numpy arrays.  Vertex x, y, z may be float or double; other vertex
+    properties of any scalar type are skipped except red, green, blue (uchar read as q / 255).  Faces are a list of
+    int / uint indices with a uchar, ushort, int or uint count; polygons are fan-triangulated ((v0, v_i, v_i+1)), so
+    Replica's quads read as two triangles each.  Other elements must have scalar properties only and are skipped.
+    ValueError, naming the file, for big-endian files, missing x / y / z, indices outside the vertices, polygons of
+    fewer than 3 vertices and truncated files.  Reads what write_ply writes exactly."""
+    path = Path(path)
+
+    def bad(msg):
+        return ValueError(f"read_ply: {path}: {msg}")
+
+    data = path.read_bytes()
+
+    def parse():
+        end = data.find(b"end_header")
+        if not data.startswith(b"ply") or end < 0:
+            raise bad("not a PLY file")
+        nl = data.find(b"\n", end)
+        if nl < 0:
+            raise bad("truncated header")
+        body = nl + 1
+        fmt, elements = None, []
+        for line in data[:end].decode("ascii", errors="replace").splitlines()[1:]:
+            tok = line.split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "format":
+                fmt = tok[1] if len(tok) > 1 else None
+            elif tok[0] == "element" and len(tok) == 3:
+                if int(tok[2]) < 0:
+                    raise bad(f"negative element count in {line!r}")
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property" and elements:
+                if tok[1] == "list" and len(tok) == 5:
+                    if tok[2] not in _PLY_TYPES or tok[3] not in _PLY_TYPES:
+                        raise bad(f"unknown property type in {line!r}")
+                    elements[-1][2].append((tok[4], "list", _PLY_TYPES[tok[2]], _PLY_TYPES[tok[3]]))
+                elif len(tok) == 3 and tok[1] in _PLY_TYPES:
+                    elements[-1][2].append((tok[2], _PLY_TYPES[tok[1]]))
+                else:
+                    raise bad(f"cannot parse {line!r}")
+            else:
+                raise bad(f"cannot parse {line!r}")
+        if fmt == "binary_big_endian":
+            raise bad("big-endian PLY is not supported")
+        if fmt not in ("binary_little_endian", "ascii"):
+            raise bad(f"unknown format {fmt!r}")
+        ascii_ = fmt == "ascii"
+        tokens = data[body:].split() if ascii_ else None
+        pos = 0                                                   # byte offset (binary) or token index (ascii)
+        verts = colors = faces = None
+        for name, count, props in elements:
+            lists = [p for p in props if p[1] == "list"]
+            if name == "face":
+                if len(props) != 1 or not lists or lists[0][0] not in ("vertex_indices", "vertex_index"):
+                    raise bad("faces must have exactly one list property vertex_indices")
+                _, _, ct, it = lists[0]
+                if ct not in ("u1", "u2", "i4", "u4") or it not in ("i4", "u4"):
+                    raise bad("face lists need a uchar / ushort / int / uint count and int / uint indices")
+                polys, pos = _ply_lists(tokens, data, pos, count, ct, it, ascii_, bad)
+                faces = _fan(polys, bad)
+                continue
+            if lists:
+                raise bad(f"element {name!r} has a list property; only faces may")
+            dt = np.dtype([(p[0], "<" + p[1]) for p in props])
+            if ascii_:
+                if pos + count * len(props) > len(tokens):
+                    raise bad(f"truncated element {name!r}")
+                cols = np.asarray(tokens[pos:pos + count * len(props)], dtype=np.float64).reshape(count, len(props))
+                pos += count * len(props)
+                rec = {p[0]: cols[:, q] for q, p in enumerate(props)}
+            else:
+                if pos + count * dt.itemsize > len(data) - body:
+                    raise bad(f"truncated element {name!r}")
+                arr = np.frombuffer(data, dtype=dt, count=count, offset=body + pos)
+                pos += count * dt.itemsize
+                rec = {p[0]: arr[p[0]] for p in props}
+            if name == "vertex":
+                types = {p[0]: p[1] for p in props}
+                if not all(types.get(k) in ("f4", "f8") for k in "xyz"):
+                    raise bad("vertices need float or double x, y, z")
+                verts = np.stack([np.asarray(rec[k]).astype(np.float32) for k in "xyz"], 1)
+                if all(k in types for k in ("red", "green", "blue")):
+                    scale = {"u1": 255.0, "u2": 65535.0}.get(types["red"], 1.0)
+                    colors = np.stack([(np.asarray(rec[k], np.float64) / scale).astype(np.float32)
+                                       for k in ("red", "green", "blue")], 1)
+        if verts is None:
+            raise bad("no vertex element")
+        if faces is None:
+            faces = np.zeros((0, 3), np.int64)
+        if faces.size and (faces.min() < 0 or faces.max() >= len(verts)):
+            raise bad("a face index lies outside the vertices")
+        return np.ascontiguousarray(verts), faces.astype(np.int32).reshape(-1, 3), colors
+
+    try:
+        return parse()
+    except (ValueError, IndexError, OverflowError) as e:   # a malformed number or count: name the file
+        if str(path) in str(e):
+            raise
+        raise bad(f"malformed file ({e})") from None
+
+
+def _ply_lists(tokens, data, pos, count, ct, it, ascii_, bad):
+    """The polygons of a face element: a list of int64 arrays [n_i] (all of one length: an array [F, n])."""
+    if ascii_:
+        polys = []
+        for _ in range(count):
+            if pos >= len(tokens):
+                raise bad("truncated faces")
+            n = int(tokens[pos])
+            if pos + 1 + n > len(tokens):
+                raise bad("truncated faces")
+            polys.append(np.asarray(tokens[pos + 1:pos + 1 + n], dtype=np.int64))
+            pos += 1 + n
+        return polys, pos
+    body = data.index(b"\n", data.find(b"end_header")) + 1
+    cs, isz = np.dtype(ct).itemsize, np.dtype(it).itemsize
+    if count == 0:
+        return np.zeros((0, 3), np.int64), pos
+    if body + pos + cs > len(data):
+        raise bad("truncated faces")
+    n0 = int(np.frombuffer(data, dtype="<" + ct, count=1, offset=body + pos)[0])
+    # Read at the stride of n0-gons.  Exact whenever every count read so equals n0: record r's count is read at its
+    # true offset as long as records 0..r-1 are n0-gons, so the first polygon of another size is read where it lies
+    # and fails the check; no misaligned field is ever compared.
+    uniform = np.dtype([("n", "<" + ct), ("i", "<" + it, (n0,))])
+    if body + pos + count * uniform.itemsize <= len(data):
+        arr = np.frombuffer(data, dtype=uniform, count=count, offset=body + pos)
+        if (arr["n"] == n0).all():
+            return arr["i"].astype(np.int64).reshape(count, n0), pos + count * uniform.itemsize
+    polys = []                                                # mixed polygon sizes: one at a time
+    for _ in range(count):
+        if body + pos + cs > len(data):
+            raise bad("truncated faces")
+        n = int(np.frombuffer(data, dtype="<" + ct, count=1, offset=body + pos)[0])
+        if body + pos + cs + n * isz > len(data):
+            raise bad("truncated faces")
+        polys.append(np.frombuffer(data, dtype="<" + it, count=n, offset=body + pos + cs).astype(np.int64))
+        pos += cs + n * isz
+    return polys, pos
+
+
+def _fan(polys, bad) -> np.ndarray:
+    """Fan triangulation (v0, v_i, v_i+1), i = 1 .. n - 2, of each polygon, in polygon order."""
+    if isinstance(polys, np.ndarray):
+        n = polys.shape[1] if polys.ndim == 2 else 3
+        if len(polys) and n < 3:
+            raise bad(f"a face has {n} vertices")
+        if not len(polys):
+            return np.zeros((0, 3), np.int64)
+        return np.stack([np.stack([polys[:, 0], polys[:, i], polys[:, i + 1]], 1) for i in range(1, n - 1)],
+                        1).reshape(-1, 3)
+    out = []
+    for p in polys:
+        if len(p) < 3:
+            raise bad(f"a face has {len(p)} vertices")
+        out.extend((p[0], p[i], p[i + 1]) for i in range(1, len(p) - 1))
+    return np.asarray(out, np.int64).reshape(-1, 3)

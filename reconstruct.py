@@ -60,6 +60,12 @@ tracking from that pose (raycast, fit, tracking against the model, integration).
 skipped with status "relocalise: failed".  So a covered lens, a fast turn or a cut in the video no longer loses the
 rest of it.  Relocalisation starts only from a failure: a frame that tracks to a wrong pose is not detected.
 
+--gt_mesh PLY evaluates the extracted mesh against a ground-truth mesh in the world frame of --pose_path (so it needs
+--pose_path) with `MeshMetrics` (DESIGN.md §3 "Mesh metrics"): both meshes sampled at --eval_density points per m^2,
+accuracy, completion, Chamfer-L1 and precision / recall / F-score at --eval_thresholds metres.  --gt_cull keeps only
+what the used frames' cameras see (their final poses, after loop closure), without modelling occlusion.  The result is
+the `mesh_metrics` key of the JSON line.
+
 Prints one JSON line: frames used and skipped, vertices, faces, the grid's dims (without --bounds the blocks and the
 allocated bounds) and seconds (with --loop_closure also the keyframes,
 the accepted loops as (frame i, frame j) index pairs of the used frames, and the number of re-fusions; with
@@ -95,6 +101,16 @@ def _floats(n: int, what: str):
             raise argparse.ArgumentTypeError(f"expected {what} ({n} finite numbers), got {text!r}")
         return v
     return parse
+
+
+def _float_list(text: str):
+    try:
+        v = tuple(float(x) for x in text.split(","))
+    except ValueError:
+        v = ()
+    if not v or not all(math.isfinite(x) for x in v):
+        raise argparse.ArgumentTypeError(f"expected comma-separated finite numbers, got {text!r}")
+    return v
 
 
 def load_pose(path: Path) -> np.ndarray:
@@ -145,6 +161,14 @@ def parse_args(argv=None):
     ap.add_argument("--place_recognition", action="store_true",
                     help="experimental: with --loop_closure, find loops by appearance and relocalise frames whose "
                          "tracking fails")
+    ap.add_argument("--gt_mesh", default=None, metavar="PLY",
+                    help="evaluate the mesh against this ground-truth mesh (world frame of --pose_path)")
+    ap.add_argument("--gt_cull", action="store_true",
+                    help="with --gt_mesh, keep only surface the used frames' cameras see (final poses)")
+    ap.add_argument("--eval_density", type=float, default=1e4,
+                    help="with --gt_mesh, surface samples per m^2 of both meshes (default 1e4, about 1 cm apart)")
+    ap.add_argument("--eval_thresholds", type=_float_list, default=(0.05,), metavar="T1,...",
+                    help="with --gt_mesh, the precision / recall distances in metres (1 to 4; default 0.05)")
     args = ap.parse_args(argv)
     if not (math.isfinite(args.voxel) and args.voxel > 0):
         ap.error(f"--voxel must be finite and > 0, got {args.voxel}")
@@ -183,6 +207,16 @@ def parse_args(argv=None):
         ap.error("--place_recognition needs --loop_closure (it keeps the keyframes it looks up)")
     if args.pose_out is not None and Path(args.pose_out).exists() and not Path(args.pose_out).is_dir():
         ap.error(f"--pose_out must be a directory, got the file {args.pose_out}")
+    if args.gt_mesh is None:
+        if args.gt_cull:
+            ap.error("--gt_cull culls the ground truth of --gt_mesh")
+    elif args.pose_path is None:
+        ap.error("--gt_mesh needs --pose_path: without it the world frame is frame 0's camera, not the ground truth's "
+                 "frame")
+    if not (math.isfinite(args.eval_density) and args.eval_density > 0):
+        ap.error(f"--eval_density must be finite and > 0, got {args.eval_density}")
+    if not 1 <= len(args.eval_thresholds) <= 4 or not all(t > 0 for t in args.eval_thresholds):
+        ap.error(f"--eval_thresholds takes 1 to 4 distances > 0, got {args.eval_thresholds}")
     if args.mode == "guided":
         if args.guided_size is None:
             ap.error("--mode guided needs --guided_size HxW")
@@ -290,7 +324,7 @@ def reconstruct(args) -> dict:
         Path(args.pose_out).mkdir(parents=True, exist_ok=True)
     loop = None
     last = np.eye(4)                                  # the last good pose: frame 0's without --pose_path
-    used, skipped, relocalised = [], [], []
+    used, used_poses, skipped, relocalised = [], [], [], []
     for q, (p, pose) in enumerate(zip(images, poses)):
         image = evaluate.image_tensor(p, "rgb")                   # [1,3,H,W] in [0, 1]
         x = ((image - 0.5) / 0.5).to(device)                       # image_tensor(p, "depth")'s normalisation
@@ -324,6 +358,7 @@ def reconstruct(args) -> dict:
             failure = None if int(rec[1]) == 0 else STATUS[int(rec[1])]
         if failure is None:
             used.append(p)
+            used_poses.append(pose)
             last = pose
             if args.pose_out is not None and loop is None:
                 np.savetxt(Path(args.pose_out) / (p.stem + ".txt"), pose)
@@ -348,7 +383,26 @@ def reconstruct(args) -> dict:
         if args.place_recognition:
             result["relocalised"] = relocalised
         result["seconds"] = round(time.perf_counter() - t0, 3)
+    if args.gt_mesh is not None:
+        # every used frame is stored in the loop closure, whose poses are the final ones
+        final = None if not used else loop.poses if loop is not None else np.stack(used_poses)
+        result["mesh_metrics"] = evaluate_mesh(args, vertices, faces, final, tuple(pred.shape[-2:]))
+        result["seconds"] = round(time.perf_counter() - t0, 3)
     return result
+
+
+def evaluate_mesh(args, vertices, faces, poses, size) -> dict:
+    """MeshMetrics of the extracted mesh against --gt_mesh; with --gt_cull both sides are culled to the frustums of
+    the used frames' final poses (host float64 [F,4,4], None when no frame was used: then nothing is culled) at the
+    prediction's size and intrinsics."""
+    from omnidata_b200.metrics import MeshMetrics
+    from omnidata_b200.volume import read_ply
+    gv, gf, _ = read_ply(args.gt_mesh)
+    dev = vertices.device
+    metric = MeshMetrics(thresholds=args.eval_thresholds, density=args.eval_density)
+    views = (args.intrinsics, size, poses) if args.gt_cull and poses is not None else None
+    metric.update(vertices, faces, torch.from_numpy(gv).to(dev), torch.from_numpy(gf).to(dev), views=views)
+    return metric.compute()
 
 
 def main(argv=None) -> dict:
